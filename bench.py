@@ -12,9 +12,11 @@ all_gather, inside the timed region).  Prints ONE JSON line (rank 0).
   value ...... env-steps/s, inputs resident in HBM, device-timed (CUDA events, max over ranks)
   e2e ........ same metric through the public API with pinned HOST tensors (H2D + D2H inside)
   roofline ... DUNE kernel (the dominant launch): algorithmic GEMM FLOPs / CUDA-event duration
-  cpu_baseline the CPU oracle (port of the reference path) on the box's host cores, bounded sample
+  cpu_baseline the CPU oracle (port of the reference path) on the machine's host cores, bounded sample
 
 --impl reference times that CPU path alone, on all host cores (rank 0 only).
+--dump-outputs DIR writes what the last timed step returned (S, U, D, min_distance of every environment) as DIR/<name>.npy;
+the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -42,13 +44,13 @@ def peaks():
     if os.path.exists(path):
         z = json.load(open(path))
         return dict(hbm_gbs=z["hbm_gbs"], tflops=z["bf16_tflops_sustained"], which="measured (MEASURED_PEAKS.json, sustained bf16)")
-    return dict(hbm_gbs=6650.0, tflops=1400.0, which="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, tflops=989.0, which="H100 SXM data sheet (dense fp16, 700 W), not a measured peak")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region, plus the card's name and power limit (part of every number)."""
 
-    Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+    Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit,name"
 
     def __init__(self, index: int):
         self.rows, self.proc, self.index = [], None, index
@@ -69,11 +71,15 @@ class ClockSampler:
         if self.proc is None:
             return dict(sm_mhz=None, sm_max_mhz=None, reasons=["nvidia-smi unavailable"])
         self.proc.terminate()
+        self.proc.wait()
         sm = [float(r[0]) for r in self.rows if len(r) >= 7 and r[0].replace(".", "").isdigit()]
         mx = [float(r[1]) for r in self.rows if len(r) >= 7 and r[1].replace(".", "").isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = sorted({names[i] for r in self.rows if len(r) >= 7 for i in range(4) if r[3 + i].lower().startswith("active")})
-        return dict(sm_mhz=float(np.median(sm)) if sm else None, sm_max_mhz=max(mx) if mx else None, reasons=reasons, samples=len(sm))
+        lim = [float(r[7]) for r in self.rows if len(r) >= 9 and r[7].replace(".", "").isdigit()]
+        gpu = next((r[8] for r in self.rows if len(r) >= 9), None)
+        return dict(gpu=gpu, power_limit_w=max(lim) if lim else None, sm_mhz=float(np.median(sm)) if sm else None, sm_max_mhz=max(mx) if mx else None,
+                    reasons=reasons, samples=len(sm))
 
 
 # --------------------------------------------------------------------------------------------
@@ -198,14 +204,14 @@ CPU_WHAT = ("oracle/pan.py: the reference's torch-CPU DUNE code restated (pinned
 
 def run_reference(args):
     """--impl reference: the CPU path alone on all usable host cores.  A step = 8 environments per core (one full pass of the
-    hot path, K PAN iterations, per environment); at most 4 timed steps so that the driver's --steps 20 ends within minutes."""
+    hot path, K PAN iterations, per environment); --steps of them are timed (each takes seconds)."""
     from helpers import CONFIGS
 
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
     cfg = CONFIGS[args.workload]
-    steps = max(1, min(args.steps, 4))
+    steps = max(1, args.steps)
     summ, runs = cpu_sample(args.workload, cfg.K, args.iter_threshold, steps, 8)
     ms = 1e3 * summ["wall_s"] / steps
     value = summ["value"]
@@ -246,10 +252,11 @@ class PanBench:
             sets.append({k: (None if v is None else torch.from_numpy(v)) for k, v in inp.items()})
         self.dsets = [{k: (None if v is None else v.to(dev)) for k, v in s_.items()} for s_ in sets]
         self.hsets = [{k: (None if v is None else v.pin_memory()) for k, v in s_.items()} for s_ in sets]
-        self.flush = flush if flush is not None else torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+        self.flush = flush if flush is not None else torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
         self.pan = make_pan(cfg, K=cfg.K, iter_threshold=iter_threshold, max_envs=B_local, overlap=args.overlap, dune_kernel=args.dune_kernel, nrmp_warm=args.nrmp_warm)
         self.sp = ShardedPAN(self.pan, total)
         self.lib = _lib.load()
+        self.last = None  # what the last timed step returned
 
     def step(self, i, host=False):
         d = (self.hsets if host else self.dsets)[i % self.n_sets]
@@ -284,7 +291,7 @@ class PanBench:
         for i in range(steps):
             self.flush.zero_()  # L2 flush, outside the per-step events
             ev[i][0].record()
-            self.step(i)
+            self.last = self.step(i)
             ev[i][1].record()
         self.barrier()
         launches = (self.lib.nb_launch_count() - l0) // max(1, steps)
@@ -310,6 +317,15 @@ class PanBench:
 
     def close(self):
         self.pan.close()
+
+
+def dump_outputs(out_dir, packed, T):
+    """The last timed step's result as the caller receives it, unpacked: S (B, 3, T+1), U (B, 2, T), D (B, 1, T), min_distance (B,)."""
+    from neupan_b200.parallel import unpack_results
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, v in zip(("S", "U", "D", "min_distance"), unpack_results(packed, T)):
+        np.save(os.path.join(out_dir, f"{name}.npy"), v.detach().cpu().numpy().astype(np.float32))
 
 
 def run_ours(args):
@@ -345,7 +361,9 @@ def run_ours(args):
     clocks = sampler.stop() if rank == 0 else None
     status_bad = int((hb.pan.status != 0).sum().item())
     iters_mean = float(hb.pan.iterations.float().mean().item())
-    e2e_ms = hb.time_e2e(max(2, min(args.steps, 5)))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, hb.last, T)
+    e2e_ms = hb.time_e2e(args.steps)
     h2d, d2h = hb.bytes_per_step()
     pan, flush, dsets = hb.pan, hb.flush, hb.dsets
 
@@ -375,30 +393,26 @@ def run_ours(args):
         pk = peaks()
         ach = flops / (dune_ms * 1e-3) / 1e12
         alg_bytes = 4.0 * B * ((2 * N) * (2 if cfg.dynamic else 1) + 3 * (T + 1)) + 4.0 * B * (T + 1) * cfg.M * 9
-        # executed tensor work (3 passes of the fp16 hi/lo split): per 128-point tile 4 layers x 6 UMMA (128x32x16) + head 6 UMMA (128x16x16)
+        # executed tensor work (3 passes of the fp16 hi/lo split): per 128-point tile and layer a bias product + 6 MMAs of 128x32x16
         if args.dune_kernel == 4:
             tiles = B * (T + 1) * ((N + 127) // 128)
-            exec_flops = tiles * 5 * 3 * 2.0 * 128 * 32 * 16  # screening pass: bias product + one fp16 pass (2 UMMA 128x32x16) per layer; + ~7 % for the refined candidates
+            exec_flops = tiles * 5 * 3 * 2.0 * 128 * 32 * 16  # screening pass: bias product + one fp16 pass (2 MMAs 128x32x16) per layer; + a few % for the refined candidates
             kname = ("dune_screen_mma_kernel + dune_refine_kernel + dune_tcp_kernel (single-pass fp16 interval screening of all points on mma.sync m16n8k16 with "
-                     "the activations in registers; tcgen05.mma kind::f16 fp16 hi/lo 3-pass exact network for the <= 32 candidates per item and the full kernel "
-                     "for the items the screen cannot narrow down; bit-identical selection to the full kernel; SASS HMMA.16816 / MUFU.TANH, UTCHMMA / LDTM / STTM)")
+                     "the activations in registers; wgmma m64n32k16 fp16 hi/lo 3-pass exact network for the <= 32 candidates per item and the full kernel "
+                     "for the items the screen cannot narrow down; bit-identical selection to the full kernel)")
         elif args.dune_kernel == 3:
             tiles = B * (T + 1) * ((N + 127) // 128)
             exec_flops = tiles * 5 * 7 * 2.0 * 128 * 32 * 16
-            kname = "dune_tc8_kernel (tcgen05.mma kind::f16, A from TMEM, fp16 hi/lo split, 3 passes + bias product; two threads per point = 8 warps per 128-point tile, two tiles in flight per CTA; SASS UTCHMMA / LDTM / STTM)"
+            kname = "dune_tc8_kernel (wgmma m64n32k16, fp16 hi/lo split, 3 passes + bias product; two threads per point = 8 warps per 128-point tile, two tiles per CTA)"
         elif args.dune_kernel == 2:
             tiles = B * (T + 1) * ((N + 127) // 128)
-            exec_flops = tiles * 5 * 7 * 2.0 * 128 * 32 * 16  # 5 dense layers x (bias product + 6 UMMA 128x32x16)
-            kname = "dune_tcp_kernel (tcgen05.mma kind::f16, A from TMEM, fp16 hi/lo split, 3 passes + bias product; two tiles in flight per CTA; FFMA2/FHFMA epilogues; SASS UTCHMMA / LDTM / STTM)"
+            exec_flops = tiles * 5 * 7 * 2.0 * 128 * 32 * 16  # 5 dense layers x (bias product + 6 MMAs 128x32x16)
+            kname = "dune_tcp_kernel (wgmma m64n32k16, A and D in a shared-memory tile, fp16 hi/lo split, 3 passes + bias product; two tiles per CTA)"
         else:
             tiles = B * (T + 1) * ((N + 31) // 32 * 2 + 1)
             exec_flops = tiles * (4 * 24 + 6) * 2.0 * 16 * 8 * 16
             kname = "dune_mma_kernel (mma.sync m16n8k16 f16, hi/lo split, 3 passes; SASS HMMA.16816.F32)" if args.dune_kernel == 1 else "dune_kernel (all-FP32 FFMA reference variant)"
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "dune_traffic.json")
-        if os.path.exists(tpath):
-            traffic = json.load(open(tpath)).get(args.workload)
-        roof = dict(bound="tensor", achieved=ach, peak=pk["tflops"], unit="TFLOP/s", frac=ach / pk["tflops"], traffic=traffic,
+        roof = dict(bound="tensor", achieved=ach, peak=pk["tflops"], unit="TFLOP/s", frac=ach / pk["tflops"], traffic=None,
                     kernel=kname, kernel_ms=dune_ms,
                     # a full launch (all T+1 steps) is timed; inside a control step the launches of PAN iterations k > 0 skip the step-0 items
                     share_of_step=(1.0 + max(0.0, iters_mean - 1.0) * (T / (T + 1.0) if args.dune_kernel == 4 else 1.0)) * dune_ms / ms, peak_source=pk["which"],
@@ -410,17 +424,17 @@ def run_ours(args):
     del hb, pan, dsets
 
     # ---- what BASELINE.json asks for beside the headline (VERDICT r1 item 3) --------------------------------------
-    def side(cname, total, thr=0.0, steps=5, warmup=3, e2e=False):
+    def side(cname, total, thr=0.0, e2e=False):
         """ms/step and env-steps/s of `total` environments of config cname split over all ranks (strong split when world > 1)."""
         lo, hi = shard_range(total, rank, world)
         sb = PanBench(cname, hi - lo, lo, dev, world, total, args, iter_threshold=thr, flush=flush)
-        m, l = sb.time_device(steps, warmup)
+        m, l = sb.time_device(args.steps, args.warmup)
         out = dict(workload=f"{cname} {sb.cfg.name}", global_batch=total, envs_per_gpu=[shard_range(total, r, world)[1] - shard_range(total, r, world)[0] for r in range(world)],
                    T=sb.cfg.T, N=sb.cfg.N, K=sb.cfg.K, iter_threshold=thr, ms_per_step=m, env_steps_per_s=total / (m * 1e-3), gpu_launches=l,
                    pan_iterations_mean=sb.reduce_max(float(sb.pan.iterations.float().mean().item())),
                    envs_with_solver_status=int(sb.reduce_max(float((sb.pan.status != 0).sum().item()))))
         if e2e:
-            em = sb.time_e2e(3)
+            em = sb.time_e2e(args.steps)
             out["e2e_ms_per_step"], out["e2e_env_steps_per_s"] = em, total / (em * 1e-3)
         sb.close()
         return out
@@ -449,7 +463,7 @@ def run_ours(args):
     if rank == 0:
         value = world * B / (ms * 1e-3)
         line = dict(metric=METRIC, value=value, unit=UNIT, n_gpus=world, steps=args.steps, warmup=args.warmup, ms_per_step=ms,
-                    higher_is_better=True, scaling="weak", vs_baseline=None, dtype="f32-accurate fp16 hi/lo split on tcgen05 tensor cores (ObsPointNet) / f64 (NRMP interior point)",
+                    higher_is_better=True, scaling="weak", vs_baseline=None, dtype="f32-accurate fp16 hi/lo split on tensor cores (ObsPointNet) / f64 (NRMP interior point)",
                     data="synthetic",
                     config=dict(workload=f"{args.workload} {cfg.name}: B={B}/GPU T={T} N={N} K={K} M={cfg.M} dyn={cfg.dynamic}" + (f" iter_threshold={args.iter_threshold} (early stop active)" if args.iter_threshold > 0 else ""), global_batch=world * B,
                                 parallelism=f"env-sharded x{world}, one all_gather of {per_env} floats/env per step (inside the timed region, device-resident and e2e)",
@@ -710,7 +724,7 @@ def run_control(args):
     e2e_ms = (time.perf_counter() - t0) * 1e3 / args.steps
     print(json.dumps(dict(metric="robot control steps/sec (initial path + scan -> points + PAN, batched envs)", value=B / (ms * 1e-3), unit="env-steps/s", n_gpus=1,
                           steps=args.steps, warmup=args.warmup, ms_per_step=ms, higher_is_better=True, scaling="weak", vs_baseline=None,
-                          dtype="f64 (path, scan) / fp16 hi-lo tcgen05 (ObsPointNet) / f64 (NRMP)", data="synthetic",
+                          dtype="f64 (path, scan) / fp16 hi-lo tensor cores (ObsPointNet) / f64 (NRMP)", data="synthetic",
                           config=dict(workload=f"control: C4 robot, B={B}, T={cfg.T}, K={cfg.K}, scans of R={R} beams -> N={N} points, velocities on", global_batch=B,
                                       l2="L2 flushed between timed iterations"),
                           gpu_launches=int(launches), clocks=clocks,
@@ -745,7 +759,7 @@ def run_train(args):
     label_s = time.perf_counter() - t0
     n = int(n_total * 0.8)
     data = (pts[:n], mu[:n], dist[:n])
-    steps = max(1, min(args.steps, 2)) if reference else args.steps
+    steps = max(1, args.steps)
     for _ in range(1 if reference else args.warmup):
         tr.train_one_epoch(data, batch, False)
     l0 = _lib.load().nb_launch_count() if not reference else 0
@@ -781,12 +795,15 @@ def main():
     ap.add_argument("--envs", type=int, default=0, help="override B per GPU")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-sides", action="store_true", help="skip the side measurements (other BASELINE configs / strong split / iter_threshold=0.1)")
-    ap.add_argument("--dune-kernel", type=int, default=4, help="NB_OPT_DUNE_KERNEL: 0 fp32 ffma, 1 mma.sync, 2 tcgen05 (every point exactly), 3 tcgen05 (two threads per point), 4 tcgen05 with screening (default)")
+    ap.add_argument("--dune-kernel", type=int, default=4, help="NB_OPT_DUNE_KERNEL: 0 fp32 ffma, 1 mma.sync, 2 wgmma (every point exactly), 3 wgmma (two threads per point), 4 wgmma with screening (default)")
     ap.add_argument("--iter-threshold", type=float, default=0.0, help="PAN stop criterion (pan.py:243); 0 forces exactly K iterations (the headline), the reference default is 0.1")
     ap.add_argument("--nrmp-warm", type=int, default=0, help="NB_OPT_NRMP_WARM: 1 = NRMP solves of PAN iterations k > 0 start from iteration k-1's solution")
     ap.add_argument("--overlap", type=int, default=2, help="env sub-batches pipelined on internal streams (NB_OPT_OVERLAP)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy (PAN workloads)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
+    if args.dump_outputs and (args.impl != "ours" or args.workload in ("train", "control", "ipath", "scan")):
+        ap.error("--dump-outputs writes the outputs of the PAN workloads (C1..C5) with --impl ours")
     if args.workload == "train":
         run_train(args)
     elif args.workload == "control" and args.impl == "ours":

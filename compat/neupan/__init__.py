@@ -1,5 +1,5 @@
 """`import neupan` shim: put this directory's parent (``compat/``) on PYTHONPATH and the reference's
-entry script runs unchanged on the B200 implementation:
+entry script runs unchanged on the CUDA implementation:
 
     PYTHONPATH=/path/to/repo:/path/to/repo/compat python example/run_exp.py -e corridor -d diff
 

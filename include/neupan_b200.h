@@ -1,5 +1,5 @@
 /*
- * neupan_b200 -- C ABI of the B200-native PAN hot path (libneupan_b200.so).
+ * neupan_b200 -- C ABI of the H100-native (sm_90a) PAN hot path (libneupan_b200.so).
  *
  * The reference (hanruihua/NeuPAN) has no FFI: its boundary for this path is the Python class
  * neupan.blocks.PAN (neupan/blocks/pan.py:27-147), constructed at neupan/neupan.py:84 and called
@@ -55,7 +55,10 @@ typedef struct {
   int32_t iter_num;       /* K            pan.py:48                                  */
   int32_t nrmp_max_num;   /* M (0 => no_obs, pan.py:85); receding <= 32, M <= 32 and receding * M <= 256 */
   int32_t max_envs;       /* capacity: largest B of any later call                   */
-  int32_t max_points;     /* capacity: largest N of any later call (after decimation) */
+  int32_t max_points;     /* capacity: largest N of any later call (after decimation).  The exact and warpgroup screening DUNE
+                             kernels hold the operand image, two 16 KB tiles and per-point keys / mu in shared memory: on an H100
+                             (227 KB per block) N up to ~7000 at E = 4, ~4000 at E = 8; a larger N fails at launch with
+                             NB_ERR_CUDA ("N=... needs ... B of shared memory"). */
   int32_t device;         /* CUDA device ordinal                                     */
   float iter_threshold;   /* pan.py:52; <= 0 never stops early                       */
   /* Python floats in the reference (float64 constants of the convex program): */
@@ -122,26 +125,27 @@ int nb_pan_set_adjust(nb_pan_t* pan, const float q_s[3], float p_u, float eta, f
 int nb_pan_set_iteration(nb_pan_t* pan, int32_t iter_num, float iter_threshold);
 
 /* Implementation switches (no reference counterpart).  NB_OPT_DUNE_KERNEL: 2 (the handle's initial value; the Python mirror selects 4) =
- * tcgen05 DUNE kernel (UMMA with TMEM accumulators, fp16 hi/lo split, fp32 accumulate); 1 = the same arithmetic on warp-level mma.sync;
+ * warpgroup DUNE kernel (wgmma with a shared-memory operand / output tile, fp16 hi/lo split, fp32 accumulate); 1 = the same arithmetic on
+ * warp-level mma.sync;
  * 0 = all-FP32 FFMA kernel, kept as the in-tree numerical reference of the same contract (needs the edge count
  * compiled in).
  * NB_OPT_OVERLAP: 1..4 = number of environment sub-batches pipelined on internal streams so that the DUNE kernels
  * of one sub-batch share the SMs with the NRMP kernel of another (results are identical; envs are independent; batches with
  * fewer than 64 environments per part are not split).  The handle starts with 2: the straggler tail of one half's NRMP launch
- * and the small kernels between the big ones run under the other half's DUNE pass (C4: 20.6 -> 19.3 ms per step; 3 and 4 lose again).
+ * and the small kernels between the big ones run under the other half's DUNE pass.
  * NB_OPT_NRMP_WARM: 1 = inside one nb_pan_forward the NRMP solve of PAN iteration k > 0 starts from the solution of
  * iteration k-1 of the same environment (fewer interior point iterations on average, same optimum to the solver tolerance;
  * a warm start that is not converging by its 12th iteration is abandoned for a cold one); 0 (default) = every solve starts
  * cold.  The first solve of every call is always cold, so results never depend on earlier calls.
- * NB_OPT_DUNE_KERNEL also takes 3 = tcgen05 with two threads per point (8 warps per 128-point tile; measured slower, kept for A/B)
- * and 4 = tcgen05 with screening: a single-pass fp16 interval pass over all points, the exact network only for the <= 32 points
+ * NB_OPT_DUNE_KERNEL also takes 3 = wgmma with two threads per point (8 warps per 128-point tile, kept for A/B)
+ * and 4 = wgmma with screening: a single-pass fp16 interval pass over all points, the exact network only for the <= 32 points
  * per (environment, step) that can be among the M closest, the exact kernel for the items the screen cannot narrow down -- the same
  * selection and values as 2, bit for bit (csrc/dune_screen_kernel.cuh).
  * NB_OPT_DIFFERENTIABLE: 1 = every NRMP solve of nb_pan_forward also stores what nb_pan_backward needs (one extra factorisation
  * at the optimum + ~5 KB per environment and iteration); 0 (default) = inference only.
  * NB_OPT_DUNE_SCREEN_MMA (with NB_OPT_DUNE_KERNEL = 4): 1 (default) = the screening pass runs on warp-level mma.sync with the
- * activations in registers (csrc/dune_screen_mma_kernel.cuh; clouds of at most 1024 points, larger ones take the tcgen05 pass), 0 = on
- * tcgen05 (csrc/dune_screen_kernel.cuh).  Same candidate contract, same final results (the refine / exact kernels are tcgen05 either way).
+ * activations in registers (csrc/dune_screen_mma_kernel.cuh; clouds of at most 1024 points, larger ones take the wgmma pass), 0 = on
+ * wgmma (csrc/dune_screen_kernel.cuh).  Same candidate contract, same final results (the refine / exact kernels are wgmma either way).
  * NB_OPT_DUNE_SKIP_T0 (with NB_OPT_DUNE_KERNEL = 4): 1 (default) = PAN iterations k > 0 of one nb_pan_forward do not re-evaluate the
  * step-0 items: nom_s[:, 0] is the fixed initial state (robot.py:234), so their inputs and results are those of iteration 0, which
  * stand in the selection buffers; 0 = evaluate them in every iteration (identical results). */

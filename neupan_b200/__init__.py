@@ -1,4 +1,4 @@
-"""neupan_b200 -- B200-native implementation of NeuPAN's PAN hot path.
+"""neupan_b200 -- H100-native implementation of NeuPAN's PAN hot path.
 
 Mirrors the reference's public names for this path (``neupan.blocks.PAN`` / ``DUNE`` / ``NRMP`` /
 ``ObsPointNet``, ``neupan.robot.robot``, ``neupan.configuration``, ``neupan.util``) on top of a

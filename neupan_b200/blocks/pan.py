@@ -3,7 +3,7 @@
 Same constructor and ``forward(nom_s, nom_u, ref_s, ref_us, obs_points=None, point_velocities=None)
 -> (nom_s, nom_u, nom_distance)`` as the reference; every tensor may carry a leading batch axis B
 of independent environments (the reference is the unbatched case).  All computation is done by
-libneupan_b200.so (sm_100a CUDA) through its C ABI -- there is no torch / CPU compute path:
+libneupan_b200.so (sm_90a CUDA) through its C ABI -- there is no torch / CPU compute path:
 
 * CUDA tensors in  -> ``nb_pan_forward`` on torch's current stream, CUDA tensors out (no sync);
 * CPU tensors in   -> ``nb_pan_forward_host`` (H2D, compute, D2H in one call), CPU tensors out,
@@ -101,13 +101,13 @@ class PAN(torch.nn.Module):
         self.device = torch.device("cuda", dev.index if dev.index is not None else 0)
         self._handle = None
         # env sub-batches pipelined on internal streams (1 = off; batches below 64 per part are never split): the stragglers of one half's NRMP
-        # launch and the small kernels between the big ones run under the other half's DUNE pass -- 20.6 -> 19.3 ms per C4 step at 2, 3 and 4 lose again
+        # launch and the small kernels between the big ones run under the other half's DUNE pass
         self.overlap = int(kwargs.get("overlap", 2))
         self.nrmp_warm = int(kwargs.get("nrmp_warm", 0))  # 1 = NRMP solves of PAN iterations k > 0 start from iteration k-1's solution (fewer IPM iterations on average, but stragglers: DESIGN.md 3.2)
-        # 4 = screening pipeline (default: interval pass + exact tcgen05 network on the candidates, bit-identical to 2, ~35 % less DUNE time), 2 = tcgen05 on every point, 3 = two threads per
+        # 4 = screening pipeline (default: interval pass + exact wgmma network on the candidates, bit-identical to 2), 2 = wgmma on every point, 3 = two threads per
         # point (experiment), 1 = mma.sync, 0 = all-FP32 FFMA
         self.dune_kernel = int(kwargs.get("dune_kernel", 4))
-        # with dune_kernel = 4: the screening pass on mma.sync (1, default; clouds of <= 1024 points) or tcgen05 (0); PAN iterations k > 0
+        # with dune_kernel = 4: the screening pass on mma.sync (1, default; clouds of <= 1024 points) or wgmma (0); PAN iterations k > 0
         # keep the step-0 items of iteration 0 (1, default: nom_s[:, 0] is the fixed initial state) or re-evaluate them (0).  Same results.
         self.dune_screen_mma = int(kwargs.get("dune_screen_mma", 1))
         self.dune_skip_t0 = int(kwargs.get("dune_skip_t0", 1))

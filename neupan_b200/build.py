@@ -1,11 +1,10 @@
-"""Builds libneupan_b200.so in-tree with nvcc for sm_100a (no torch involved).
+"""Builds libneupan_b200.so in-tree with nvcc for sm_90a (H100; no torch involved).
 
     python -m neupan_b200.build            # all edge counts 3..8
     NB_EDGE_DIMS=4 python -m neupan_b200.build   # quick developer build
 
 The DUNE kernel is instantiated once per polygon edge count E; each instantiation is its own
-translation unit so they compile in parallel.  The .so lands in neupan_b200/lib/ (git-ignored,
-but it travels to the GPU box with the repo snapshot).
+translation unit so they compile in parallel.  The .so lands in neupan_b200/lib/ (git-ignored).
 """
 from __future__ import annotations
 
@@ -20,7 +19,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libneupan_b200.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 

@@ -1,7 +1,7 @@
 """Process-wide defaults mirroring neupan/configuration/__init__.py:25-57.
 
 The reference keeps ``device`` / ``time_print`` / ``tensor_dtype`` as mutable module globals
-(set from the yaml at neupan/neupan.py:68-69).  They are kept for API compatibility; the B200
+(set from the yaml at neupan/neupan.py:68-69).  They are kept for API compatibility; this
 build additionally carries the device per PAN instance, so two planners on different GPUs can
 coexist (the globals only provide the default for helpers called without an instance).
 """

@@ -1,4 +1,4 @@
-// Shared definitions of the PAN hot-path kernels (sm_100a).
+// Shared definitions of the PAN hot-path kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

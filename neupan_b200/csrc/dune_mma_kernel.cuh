@@ -1,12 +1,11 @@
 // DUNE kernel, tensor-core version: same contract as dune_kernel.cuh, ObsPointNet's dense layers on
 // the tensor pipe.
 //
-// Variant 1 of NB_OPT_DUNE_KERNEL (the default is the tcgen05 kernel, dune_tc_kernel.cuh).  The network is a
+// Variant 1 of NB_OPT_DUNE_KERNEL (the exact default arithmetic is the wgmma kernel, dune_tc_kernel.cuh).  The network is a
 // chain of 32x32 GEMM slices separated by per-row LayerNorm/tanh/ReLU.  With warp-level m16n8k16 the
 // accumulator fragment of layer l *is* the A-operand fragment of layer l+1 (same lane <-> (row, column-pair)
-// mapping), so 32 points travel through all six layers inside one warp's registers -- no shared-memory or TMEM
-// round trip, no barrier.  Measured at C4: 2.82 ms per launch against 2.49 ms for the tcgen05 kernel, whose
-// thread-per-row layout needs no shuffles / fragment moves (DESIGN.md 3.1).
+// mapping), so 32 points travel through all six layers inside one warp's registers -- no shared-memory
+// round trip, no barrier.
 //
 // Precision: every fp32 operand is split x = hi + lo into two fp16 values (22 significant bits) and
 // the product is formed as lo_x*hi_w + hi_x*lo_w + hi_x*hi_w with fp32 accumulation (3 HMMA passes),

@@ -2,16 +2,16 @@
 // points that can be among the M closest.
 //
 // Only the M (= 10) smallest of the N (= 500) distances of an (environment, step) item are ever consumed (dune.py:100-104,
-// nrmp.py:243-259), but dune_tcp_kernel pays the full fp32-accurate network -- fp16 hi/lo split, 3 MMA passes, exp2 + rcp tanh:
-// 1,730 instructions per point -- for every point.  Here:
+// nrmp.py:243-259), but dune_tcp_kernel pays the full fp32-accurate network -- fp16 hi/lo split, 3 MMA passes, exp2 + rcp tanh --
+// for every point.  Here:
 //
 //  1. screening pass       (dune_screen_mma_kernel.cuh for clouds of <= 1024 points -- the default --, dune_screen_kernel below
 //     otherwise or with NB_OPT_DUNE_SCREEN_MMA = 0): every point through a SINGLE-pass fp16 network (activations and weights rounded
-//     to fp16 once, fp32 accumulation, tanh by MUFU.TANH: ~45 % of the instructions, 40 % of the MUFU work, a third of the MMAs), giving an
+//     to fp16 once, fp32 accumulation, tanh by MUFU.TANH: a third of the MMAs and fewer MUFU operations per point), giving an
 //     approximate distance d~ and a per-point error radius eps = c_mu sum_e |G_e p0 - h_e| + 1e-4 (d is linear in mu, |mu~ - mu|
 //     <= c_mu).  With tau = the M-th smallest upper bound d~ + eps, a point whose lower bound d~ - eps exceeds tau cannot be among
 //     the M smallest EXACT distances; the others (typically 11-16 of 500) are the item's candidates.
-//  2. dune_refine_kernel   the candidates through exactly the arithmetic of dune_tcp_kernel (same helpers, same MMA structure;
+//  2. dune_refine_kernel   the candidates through exactly the arithmetic of dune_tcp_kernel (same helpers, same wgmma sequence;
 //     rows of an MMA tile are independent, so a point's mu / distance are bit-identical to what the full kernel computes for it);
 //     work lists by candidate count (filled by the screening kernels): an item with 17..32 candidates takes a warp, two items with
 //     <= 16 share one; 8 units per two-slot pass; rank-based selection inside the group, output rows.
@@ -30,15 +30,11 @@ namespace nb {
 
 namespace tc {
 
-// bias product + the two K-steps of A_hi . B_hi (single fp16 pass) + commit
-__device__ __forceinline__ void issue_layer_screen(uint32_t tD, uint32_t dw, uint32_t done, int layer, uint32_t bar) {
-  using I = TcImage;
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  mma_f16_ss(tD, mk_desc(done), mk_desc(dw + (I::kBiasBOff >> 4) + layer * (1024 >> 4)), kIdescN32, 0u);
-  const uint32_t w = dw + layer * (I::kLayerStride >> 4);
-  mma_f16(tD, tD + 32, mk_desc(w), kIdescN32, 1u);
-  mma_f16(tD, tD + 40, mk_desc(w + (1024 >> 4)), kIdescN32, 1u);
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// the thread's activations (single fp16 pass) -> the hi half of its A row
+__device__ __forceinline__ void st_a_hi(unsigned char* tile, int p, const uint32_t (&hi)[16]) {
+#pragma unroll
+  for (int q = 0; q < 4; ++q)
+    *reinterpret_cast<uint4*>(tile + chunk_off(p, q)) = make_uint4(hi[4 * q], hi[4 * q + 1], hi[4 * q + 2], hi[4 * q + 3]);
 }
 
 // LayerNorm (centred inputs, eps 1e-5) + tanh by MUFU.TANH; g / be are the checkpoint's plain gain / offset
@@ -115,23 +111,24 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 
 }  // namespace tc
 
-// shared memory of the screen kernel: operand image | UB keys (N x 8) | lower bounds (N x 4) | d~ (N x 4) | per-warp candidates (4 M x 8)
+// shared memory of the screen kernel: operand image | two tiles | UB keys (N x 8) | lower bounds (N x 4) | d~ (N x 4) |
+// per-warp candidates (4 M x 8)
 __host__ __device__ inline size_t dune_screen_smem_bytes(int N, int M) {
-  return TcImage::kBytes + (size_t)N * 16 + (size_t)4 * M * 8 + 64;
+  return TcImage::kBytes + 2 * (size_t)tc::kTileBytes + (size_t)N * 16 + (size_t)4 * M * 8 + 64;
 }
 
 template <int kDummy>
-__global__ void __launch_bounds__(128, 4) dune_screen_kernel(const DuneParams prm, const unsigned char* __restrict__ image) {
+__global__ void __launch_bounds__(128) dune_screen_kernel(const DuneParams prm, const unsigned char* __restrict__ image) {
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   using I = TcImage;
   unsigned char* simg = smem_dyn;
+  unsigned char* tiles = simg + I::kBytes;
   const float* fl = reinterpret_cast<const float*>(simg + I::kFloatOff);
-  unsigned long long* keys = reinterpret_cast<unsigned long long*>(simg + I::kBytes);  // (orderable(UB) << 32) | index
-  float* lbv = reinterpret_cast<float*>(simg + I::kBytes + (size_t)prm.N * 8);
+  unsigned char* tail = tiles + 2 * tc::kTileBytes;
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(tail);  // (orderable(UB) << 32) | index
+  float* lbv = reinterpret_cast<float*>(tail + (size_t)prm.N * 8);
   float* dtv = lbv + prm.N;
-  unsigned long long* cands = reinterpret_cast<unsigned long long*>(simg + I::kBytes + (size_t)prm.N * 16);
-  __shared__ __align__(8) unsigned long long mbar[2];
-  __shared__ uint32_t tmem_base_s;
+  unsigned long long* cands = reinterpret_cast<unsigned long long*>(tail + (size_t)prm.N * 16);
   __shared__ uint32_t tau_s;
   __shared__ int cnt_s;
   __shared__ int list_s[kCandMax];
@@ -139,43 +136,18 @@ __global__ void __launch_bounds__(128, 4) dune_screen_kernel(const DuneParams pr
   __shared__ float2 xy_s[2][128];  // robot-frame coordinates of the points in flight (stage 0 -> head)
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int prow = tc::tile_row(tid);
   for (int i = tid; i < I::kBytes / 16; i += 128) reinterpret_cast<uint4*>(simg)[i] = reinterpret_cast<const uint4*>(image)[i];
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(tc::smem_u32(&mbar[0])));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(tc::smem_u32(&mbar[1])));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 128;" ::"r"(tc::smem_u32(&tmem_base_s)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tbase = tmem_base_s;
-  const uint32_t trow = tbase + ((uint32_t)(warp * 32) << 16);
   const uint32_t simg_u = tc::smem_u32(simg);
-  const uint32_t bar0 = tc::smem_u32(&mbar[0]);
-  const uint32_t desc_w = tc::desc_lo(simg_u, 512), desc_ones = tc::desc_lo(simg_u + I::kOnesOff, 2048);
-  uint32_t phases = 0;
 
   auto publish = [&](const uint32_t (&hi)[16], int slot, int layer) {
-    tc::st16(trow + 64 * slot + 32, hi);
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    const int issuer = (layer + slot + (int)blockIdx.x) & 3;
+    unsigned char* tile = tiles + slot * tc::kTileBytes;
+    tc::st_a_hi(tile, prow, hi);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
-    if (warp == issuer) {
-      uint32_t elected;
-      asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(elected));
-      if (elected) tc::issue_layer_screen(tbase + 64 * slot, desc_w, desc_ones, layer, bar0 + 8 * slot);
-    }
-  };
-  auto acquire = [&](int slot) {
-    tc::mbar_wait(bar0 + 8 * slot, (phases >> slot) & 1u);
-    phases ^= 1u << slot;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    tc::layer_mma<false>(tile, simg_u, layer, warp, lane);
   };
 
   const int T1 = prm.T + 1, N = prm.N, M = prm.M, E = prm.geo.E;
@@ -265,16 +237,8 @@ __global__ void __launch_bounds__(128, 4) dune_screen_kernel(const DuneParams pr
           y0 = fmaf(fr.cs, dy, -(fr.sn * dx));
         }
         xy_s[sl][tid] = make_float2(x0, y0);
-        const tc::f2 x2 = tc::pk(x0, x0), y2 = tc::pk(y0, y0);
         tc::f2 hp[16];
-#pragma unroll
-        for (int c = 0; c < 16; c += 2) {
-          const ulonglong2 wx = *reinterpret_cast<const ulonglong2*>(fl + I::W0X + 2 * c);
-          const ulonglong2 wy = *reinterpret_cast<const ulonglong2*>(fl + I::W0Y + 2 * c);
-          const ulonglong2 bb = *reinterpret_cast<const ulonglong2*>(fl + I::B0 + 2 * c);
-          hp[c] = tc::fma2(wy.x, y2, tc::fma2(wx.x, x2, bb.x));
-          hp[c + 1] = tc::fma2(wy.y, y2, tc::fma2(wx.y, x2, bb.y));
-        }
+        tc::layer0(fl, x0, y0, 0, hp);
         uint32_t hi[16];
         tc::ln_tanh_screen(hp, fl + I::G1, fl + I::BE1, hi);
         publish(hi, sl, 0);
@@ -288,8 +252,7 @@ __global__ void __launch_bounds__(128, 4) dune_screen_kernel(const DuneParams pr
         for (int sl = 0; sl < nslots; ++sl) {
           tc::f2 hp[16];
           uint32_t hi[16];
-          acquire(sl);
-          tc::ld32p(trow + 64 * sl, hp);
+          tc::ld32p(tiles + sl * tc::kTileBytes, prow, hp);
           if (st & 1) tc::relu_screen(hp, hi);
           else tc::ln_tanh_screen(hp, fl + I::G1 + 32 * st, fl + I::BE1 + 32 * st, hi);
           publish(hi, sl, st);
@@ -298,8 +261,7 @@ __global__ void __launch_bounds__(128, 4) dune_screen_kernel(const DuneParams pr
 #pragma unroll 1
       for (int sl = 0; sl < nslots; ++sl) {  // head: approximate distance and its error radius
         float mu[8];
-        acquire(sl);
-        tc::ld8(trow + 64 * sl, mu);
+        tc::ld8(tiles + sl * tc::kTileBytes, prow, mu);
         const int i = base + sl * 128 + tid;
         uint32_t kub = 0xFFFFFFFFu;
         float lbi = __int_as_float(0x7f800000), dti = 0.f;
@@ -419,10 +381,6 @@ __global__ void __launch_bounds__(128, 4) dune_screen_kernel(const DuneParams pr
     }
     __syncthreads();  // keys / lbv / list are reused by the next item
   }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 128;" ::"r"(tbase) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------------------------------
@@ -431,54 +389,26 @@ __global__ void __launch_bounds__(128, 4) dune_screen_kernel(const DuneParams pr
 // paired form nearly halves the number of 128-row tiles.  8 units per two-slot pass (slot s, warp w -> unit 8 g + 4 s + w), lane =
 // candidate.  Rows of an MMA tile are independent, so where a candidate sits does not change its mu / distance by a bit.
 template <bool kFast>
-__global__ void __launch_bounds__(128, 4) dune_refine_kernel(const DuneParams prm, const unsigned char* __restrict__ image) {
+__global__ void __launch_bounds__(128) dune_refine_kernel(const DuneParams prm, const unsigned char* __restrict__ image) {
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   using I = TcImage;
   unsigned char* simg = smem_dyn;
+  unsigned char* tiles = simg + I::kBytes;
   const float* fl = reinterpret_cast<const float*>(simg + I::kFloatOff);
-  __shared__ __align__(8) unsigned long long mbar[2];
-  __shared__ uint32_t tmem_base_s;
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int prow = tc::tile_row(tid);
   for (int i = tid; i < I::kBytes / 16; i += 128) reinterpret_cast<uint4*>(simg)[i] = reinterpret_cast<const uint4*>(image)[i];
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(tc::smem_u32(&mbar[0])));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(tc::smem_u32(&mbar[1])));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 128;" ::"r"(tc::smem_u32(&tmem_base_s)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tbase = tmem_base_s;
-  const uint32_t trow = tbase + ((uint32_t)(warp * 32) << 16);
   const uint32_t simg_u = tc::smem_u32(simg);
-  const uint32_t bar0 = tc::smem_u32(&mbar[0]);
-  const uint32_t desc_w = tc::desc_lo(simg_u, 512), desc_ones = tc::desc_lo(simg_u + I::kOnesOff, 2048);
-  uint32_t phases = 0;
 
   auto publish = [&](const uint32_t (&hi)[16], const uint32_t (&lo)[16], int slot, int layer) {
-    const uint32_t tS = trow + 64 * slot;
-    tc::st16(tS + 32, hi);
-    tc::st16(tS + 48, lo);
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    const int issuer = (layer + slot + (int)blockIdx.x) & 3;
+    unsigned char* tile = tiles + slot * tc::kTileBytes;
+    tc::st_a(tile, prow, hi, lo);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
-    if (warp == issuer) {
-      uint32_t elected;
-      asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(elected));
-      if (elected) tc::issue_layer_bias(tbase + 64 * slot, desc_w, desc_ones, layer, bar0 + 8 * slot);
-    }
-  };
-  auto acquire = [&](int slot) {
-    tc::mbar_wait(bar0 + 8 * slot, (phases >> slot) & 1u);
-    phases ^= 1u << slot;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    tc::layer_mma<true>(tile, simg_u, layer, warp, lane);
   };
 
   const int T1 = prm.T + 1, M = prm.M, E = prm.geo.E;
@@ -511,16 +441,8 @@ __global__ void __launch_bounds__(128, 4) dune_refine_kernel(const DuneParams pr
       const tc::ItemFrame fr = tc::item_frame(prm, it / T1, it % T1);
       float x0, y0;
       fr.local(myidx[sl], x0, y0);
-      const tc::f2 x2 = tc::pk(x0, x0), y2 = tc::pk(y0, y0);
       tc::f2 hp[16];
-#pragma unroll
-      for (int c = 0; c < 16; c += 2) {
-        const ulonglong2 wx = *reinterpret_cast<const ulonglong2*>(fl + I::W0X + 2 * c);
-        const ulonglong2 wy = *reinterpret_cast<const ulonglong2*>(fl + I::W0Y + 2 * c);
-        const ulonglong2 bb = *reinterpret_cast<const ulonglong2*>(fl + I::B0 + 2 * c);
-        hp[c] = tc::fma2(wy.x, y2, tc::fma2(wx.x, x2, bb.x));
-        hp[c + 1] = tc::fma2(wy.y, y2, tc::fma2(wx.y, x2, bb.y));
-      }
+      tc::layer0(fl, x0, y0, 0, hp);
       uint32_t hi[16], lo[16];
       tc::ln_tanh_split<kFast>(hp, fl + I::G1, fl + I::BE1, hi, lo);
       publish(hi, lo, sl, 0);
@@ -531,8 +453,7 @@ __global__ void __launch_bounds__(128, 4) dune_refine_kernel(const DuneParams pr
       for (int sl = 0; sl < 2; ++sl) {
         tc::f2 hp[16];
         uint32_t hi[16], lo[16];
-        acquire(sl);
-        tc::ld32p(trow + 64 * sl, hp);
+        tc::ld32p(tiles + sl * tc::kTileBytes, prow, hp);
         if (st & 1) tc::relu_split(hp, hi, lo);
         else tc::ln_tanh_split<kFast>(hp, fl + I::G1 + 32 * st, fl + I::BE1 + 32 * st, hi, lo);
         publish(hi, lo, sl, st);
@@ -541,8 +462,7 @@ __global__ void __launch_bounds__(128, 4) dune_refine_kernel(const DuneParams pr
 #pragma unroll 1
     for (int sl = 0; sl < 2; ++sl) {  // head, selection inside the lane's group (warp or half warp), output rows
       float mu[8];
-      acquire(sl);
-      tc::ld8(trow + 64 * sl, mu);
+      tc::ld8(tiles + sl * tc::kTileBytes, prow, mu);
       const int u = 8 * g + 4 * sl + warp;
       if (u >= units) continue;  // warp-uniform
       const bool whole = u < nB;  // warp-uniform
@@ -619,10 +539,6 @@ __global__ void __launch_bounds__(128, 4) dune_refine_kernel(const DuneParams pr
     }
     __syncthreads();  // D of both slots has been read before the next group's operands arrive
   }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 128;" ::"r"(tbase) : "memory");
 }
 
 }  // namespace nb

@@ -2,15 +2,12 @@
 // candidate lists and the same operand image as dune_screen_kernel (dune_screen_kernel.cuh), different execution shape.
 //
 // Why a second shape for this one pass.  The screening network is SINGLE-pass fp16 (no hi/lo split): per 32-wide layer and 128
-// points it needs 3 tcgen05.mma of 128x32x16 -- the tensor pipe is 1 % busy -- but pays the full tcgen05 round trip five times
-// per tile: tcgen05.st of the A operand, block barrier, elected issue, mbarrier wait, tcgen05.ld of 32 fp32 columns per point
-// (544 B per point through the 64 B/clk TMEM read port).  ncu of dune_screen_kernel: 16 warps/SM, issue slots 53 % busy, no
-// pipe above 40 %, and two thirds of a warp's time spent in those variable waits.  With mma.sync m16n8k16 the accumulator
-// fragment of layer l IS the A fragment of layer l+1 (same lane <-> (row, column pair) map), so 32 points travel through all
-// six layers inside one warp's registers: no TMEM, no mbarrier, no block barrier inside the network, warps drift freely and the
-// MUFU (tanh), FMA, ALU and tensor phases of the four warps of a scheduler overlap.  The single fp16 pass costs 68 HMMA per 32
-// points (585 clk of the legacy tensor pipe per scheduler) against 792 clk of MUFU.TANH -- the exact path (3 passes, 204 HMMA)
-// is the one that needs tcgen05, and keeps it (dune_refine_kernel / dune_tcp_kernel).
+// points it needs 3 wgmma of 64x32x16 per half tile -- a tiny amount of tensor work -- but dune_screen_kernel pays a round trip
+// through shared memory five times per tile: operand store, block barrier, MMA wait, fp32 row load.  With mma.sync m16n8k16 the
+// accumulator fragment of layer l IS the A fragment of layer l+1 (same lane <-> (row, column pair) map), so 32 points travel
+// through all six layers inside one warp's registers: no shared-memory tile, no block barrier inside the network, warps drift
+// freely and the MUFU (tanh), FMA, ALU and tensor phases of the four warps of a scheduler overlap.  The exact path (3 passes)
+// keeps the warpgroup kernels (dune_refine_kernel / dune_tcp_kernel).
 //
 // Mapping (clouds of up to 1024 points; see the kP template parameter): CTA = 4 warps = one (environment, step) item at a time; pass p, warp w: points [128 p + 32 w, +32) as two m16 tiles.
 // Lane (g = lane >> 2, tq = lane & 3) holds rows g, g+8 (tile 0), g, g+8 (tile 1) -- "row slots" 0..3 = local points g + 8 r --
@@ -163,7 +160,7 @@ __host__ __device__ inline size_t dune_screen_mma_smem_bytes(int N, int M) {
 }
 
 #ifndef NB_SMMA_BLOCKS
-#define NB_SMMA_BLOCKS 5  // CTAs per SM the register allocation is made for: 96 registers, 12 B of spills (4: 21.57, 5: 21.37, 6: 21.81 ms per C4 step)
+#define NB_SMMA_BLOCKS 5  // CTAs per SM the register allocation is made for: 96 registers, 12 B of spills (NB_SMMA_BLOCKS is a tuning knob: time 4, 5 and 6 with bench.py)
 #endif
 // kP = the most 128-point passes an item can need: every thread keeps the bounds of its <= kP points in registers, with the point's
 // index in the low kIdxBits bits of the key.  kP = 4: N <= 512 (96 registers, 5 CTAs per SM); kP = 8: N <= 1024 (4 CTAs per SM).  The
@@ -182,7 +179,7 @@ __global__ void __launch_bounds__(128, kP <= 4 ? NB_SMMA_BLOCKS : 4) dune_screen
   __shared__ float ldt_s[kCandMax];
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, tq = lane & 3;
-  // ---- operand staging: the screen image of dune_screen_kernel (K-major UMMA layout, hi halves) re-ordered into mma.sync B fragments
+  // ---- operand staging: the screen image of dune_screen_kernel (K-major wgmma layout, hi halves) re-ordered into mma.sync B fragments
   {
     uint32_t* wf = reinterpret_cast<uint32_t*>(wfrag);
     for (int x = tid; x < sm::kFragBytes / 4; x += 128) {

@@ -1,4 +1,4 @@
-// Translation unit of the tcgen05 DUNE kernel: host-side operand image + launcher.
+// Translation unit of the warpgroup (wgmma) DUNE kernels: host-side operand image + launchers.
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -19,7 +19,7 @@ static inline void split_half_tc(float v, uint16_t& hi, uint16_t& lo) {
   memcpy(&lo, &l, 2);
 }
 
-// packed checkpoint (WeightLayout order, E outputs) -> TcImage bytes (canonical K-major / no-swizzle UMMA layout)
+// packed checkpoint (WeightLayout order, E outputs) -> TcImage bytes (canonical K-major / no-swizzle wgmma layout)
 // returns flags: bit 0 = every tanh argument of the network is bounded by 30 in exp2 units (|LN(x)_j| <= sqrt(32)), which
 // allows the kernel's shared-reciprocal tanh (ln_tanh_split<true>)
 // screen = true: the image of the screening network (dune_screen_kernel.cuh): the same layout, but tanh is NOT folded into the
@@ -115,6 +115,17 @@ int build_tc_image(const float* w, int E, std::vector<unsigned char>& out, bool 
   return amax <= 30.0 ? 1 : 0;
 }
 
+// persistent grid: as many CTAs as fit on every SM, at most `work` (0: the kernel does not fit at all)
+template <typename K>
+static cudaError_t resident_grid(K kern, int threads, size_t smem, int sm_count, int work, int& grid) {
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  int per_sm = 0;
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem);
+  grid = sm_count * (per_sm < 1 ? 1 : per_sm);
+  if (grid > work) grid = work;
+  return e;
+}
+
 int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const unsigned char* d_screen_image, int image_flags, int variant, int sm_count,
                    int max_smem_optin, cudaStream_t st, char* err, size_t errlen) {
   DuneParams prm = prm_in;
@@ -126,61 +137,44 @@ int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const
       return -1;
     }
     const int items_ = prm.B * (prm.T + 1);
-    const size_t pad4 = (size_t)(233472 / 5) - 2048 + 512;  // never more than 4 CTAs (128 TMEM columns each) per SM
-    size_t smem_s = dune_screen_smem_bytes(prm.N, prm.M);
+    const size_t smem_s = dune_screen_smem_bytes(prm.N, prm.M);
     if ((long long)smem_s > max_smem_optin) {
       snprintf(err, errlen, "N=%d needs %zu B of shared memory (limit %d)", prm.N, smem_s, max_smem_optin);
       return -3;
     }
-    if (smem_s < pad4) smem_s = pad4;
-    size_t smem_r = TcImage::kBytes + 64;
-    if (smem_r < pad4) smem_r = pad4;
-    int per_s = (int)(233472 / (smem_s + 2048));
-    per_s = per_s > 4 ? 4 : (per_s < 1 ? 1 : per_s);
+    const size_t smem_r = TcImage::kBytes + 2 * (size_t)tc::kTileBytes;
     const int screen_mma = prm.screen_mma;
     cudaError_t e = cudaMemsetAsync(prm.flag_count, 0, 3 * sizeof(int32_t), st);
     const size_t smem_m = dune_screen_mma_smem_bytes(prm.N, prm.M);
-    if (screen_mma && prm.N <= 1024 && (long long)smem_m <= max_smem_optin) {  // larger clouds: the tcgen05 screen kernel (key arrays in shared memory)
-      // no TMEM in this kernel: residency is whatever registers and shared memory admit
-      auto go = [&](auto kern, int& per_m, size_t& per_m_smem) {
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_m);
-        if (e == cudaSuccess && (per_m < 0 || per_m_smem != smem_m)) {
-          e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_m, kern, 128, smem_m);
-          per_m_smem = smem_m;
-          if (per_m < 1) per_m = 1;
-        }
+    int grid = 0;
+    if (screen_mma && prm.N <= 1024 && (long long)smem_m <= max_smem_optin) {  // larger clouds: the warpgroup screen kernel (key arrays in shared memory)
+      auto go = [&](auto kern) {
+        if (e == cudaSuccess) e = resident_grid(kern, 128, smem_m, sm_count, items_, grid);
         if (e == cudaSuccess) {
           static int cap = -1;  // NB_SCREEN_CTA_CAP (developer switch): fewer CTAs per SM, to leave room for a kernel of another stream (NB_OPT_OVERLAP)
           if (cap < 0) {
             const char* v = getenv("NB_SCREEN_CTA_CAP");
             cap = v ? atoi(v) : 0;
           }
-          int grid = sm_count * ((cap > 0 && cap < per_m) ? cap : per_m);
-          if (grid > items_) grid = items_;
+          if (cap > 0 && grid > sm_count * cap) grid = sm_count * cap;
           kern<<<grid, 128, smem_m, st>>>(prm, d_screen_image);
           e = cudaGetLastError();
         }
       };
-      static int per4 = -1, per8 = -1;
-      static size_t smem4 = 0, smem8 = 0;
-      if (prm.N <= 512) go(dune_screen_mma_kernel<4>, per4, smem4);
-      else go(dune_screen_mma_kernel<8>, per8, smem8);
+      if (prm.N <= 512) go(dune_screen_mma_kernel<4>);
+      else go(dune_screen_mma_kernel<8>);
     } else {
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(dune_screen_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_s);
+      if (e == cudaSuccess) e = resident_grid(dune_screen_kernel<0>, 128, smem_s, sm_count, items_, grid);
       if (e == cudaSuccess) {
-        int grid = sm_count * per_s;
-        if (grid > items_) grid = items_;
         dune_screen_kernel<0><<<grid, 128, smem_s, st>>>(prm, d_screen_image);
         e = cudaGetLastError();
       }
     }
     const bool fast_r = (image_flags & 1) != 0;
-    if (e == cudaSuccess) e = fast_r ? cudaFuncSetAttribute(dune_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_r)
-                                      : cudaFuncSetAttribute(dune_refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_r);
+    const int groups = (items_ + 7) / 8;  // the number of work units is only known on the device: a persistent grid sized for the worst case
+    if (e == cudaSuccess) e = fast_r ? resident_grid(dune_refine_kernel<true>, 128, smem_r, sm_count, groups, grid)
+                                      : resident_grid(dune_refine_kernel<false>, 128, smem_r, sm_count, groups, grid);
     if (e == cudaSuccess) {
-      int grid = sm_count * 4;  // the number of work units is only known on the device: a persistent grid sized for the worst case
-      const int groups = (items_ + 7) / 8;
-      if (grid > groups) grid = groups;
       if (fast_r) dune_refine_kernel<true><<<grid, 128, smem_r, st>>>(prm, d_image);
       else dune_refine_kernel<false><<<grid, 128, smem_r, st>>>(prm, d_image);
       e = cudaGetLastError();
@@ -192,43 +186,28 @@ int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const
     prm.only_flagged = 1;
     variant = 2;
   }
-  size_t smem = variant == 3 ? dune_tc8_smem_bytes(prm.N, prm.geo.E, prm.M) : dune_tc_smem_bytes(prm.N, prm.geo.E, prm.M);
+  const size_t smem = variant == 3 ? dune_tc8_smem_bytes(prm.N, prm.geo.E, prm.M) : dune_tc_smem_bytes(prm.N, prm.geo.E, prm.M);
   if ((long long)smem > max_smem_optin) {
     snprintf(err, errlen, "N=%d needs %zu B of shared memory (limit %d)", prm.N, smem, max_smem_optin);
     return -3;
   }
   const int items = prm.B * (prm.T + 1);
-  static int force = -1;  // NB_DUNE_TC: developer switch, 1 = first (single-slot, scalar math) kernel, 2 = mbarrier hand-off
+  static int force = -1;  // NB_DUNE_TC=4 (developer switch): plain reciprocals instead of the shared-reciprocal tanh
   if (force < 0) {
     const char* v = getenv("NB_DUNE_TC");
     force = v ? atoi(v) : 0;
   }
-  static int blocks8 = -1;  // NB_DUNE_TC8_BLOCKS: CTAs per SM of the 8-warp kernel (3: <= 85 registers, 4: <= 64 registers)
+  static int blocks8 = -1;  // NB_DUNE_TC8_BLOCKS: minimum CTAs per SM the 8-warp kernel is compiled for (3: <= 85 registers, 4: <= 64 registers)
   if (blocks8 < 0) {
     const char* v = getenv("NB_DUNE_TC8_BLOCKS");
     blocks8 = v ? atoi(v) : 3;
     if (blocks8 != 4) blocks8 = 3;
   }
-  const bool single = force == 1 && variant != 3;
-  const bool barrier_sync = force != 2;  // default: block barrier between operand stores and MMAs (2.19 ms vs 2.29 ms with the mbarrier hand-off)
-  // TMEM columns are held by a CTA for its whole (persistent) lifetime: 512 / columns-per-CTA CTAs may share an SM, one
-  // more would sit in tcgen05.alloc until another CTA exits, and the block scheduler knows nothing about TMEM
-  // (observed: a 5th CTA with 128 columns landing on an SM turned 2.7 ms into 4.3 ms per launch).  The shared-memory
-  // request is therefore padded so that never more CTAs fit than registers and TMEM admit.
-  const int want = variant == 3 ? blocks8 : (single ? 5 : 4);  // two-slot kernel: 128 columns -> 4 CTAs;  single slot: 64 columns, 96 registers -> 5 CTAs
-  // smallest request that keeps a (want+1)-th CTA out (anything larger only shrinks the L1 cache: 44 KB instead of 38 KB
-  // per CTA cost 2.49 -> 3.50 ms per launch of the single-slot kernel)
-  const size_t pad = (size_t)(233472 / (want + 1)) - 2048 + 512;
-  if (smem < pad) smem = pad;
-  const bool fast = (image_flags & 1) != 0 && force != 4;  // NB_DUNE_TC=4: plain reciprocals
+  const bool fast = (image_flags & 1) != 0 && force != 4;
   auto run = [&](auto kern, int threads) -> cudaError_t {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    int grid = 0;
+    cudaError_t e = resident_grid(kern, threads, smem, sm_count, items, grid);
     if (e != cudaSuccess) return e;
-    int per_sm = (int)(233472 / (smem + 2048));
-    if (per_sm > want) per_sm = want;
-    if (per_sm < 1) per_sm = 1;
-    int grid = sm_count * per_sm;
-    if (grid > items) grid = items;
     kern<<<grid, threads, smem, st>>>(prm, d_image);
     return cudaGetLastError();
   };
@@ -236,9 +215,9 @@ int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const
   if (variant == 3) {
     if (blocks8 == 4) e = fast ? run(dune_tc8_kernel<true, 4>, 256) : run(dune_tc8_kernel<false, 4>, 256);
     else e = fast ? run(dune_tc8_kernel<true, 3>, 256) : run(dune_tc8_kernel<false, 3>, 256);
-  } else if (single) e = run(dune_tc_kernel, 128);
-  else if (barrier_sync) e = fast ? run(dune_tcp_kernel<0, true>, 128) : run(dune_tcp_kernel<0, false>, 128);
-  else e = fast ? run(dune_tcp_kernel<1, true>, 128) : run(dune_tcp_kernel<1, false>, 128);
+  } else {
+    e = fast ? run(dune_tcp_kernel<true>, 128) : run(dune_tcp_kernel<false>, 128);
+  }
   if (e != cudaSuccess) {
     snprintf(err, errlen, "dune_tc kernel launch failed: %s", cudaGetErrorString(e));
     return -2;

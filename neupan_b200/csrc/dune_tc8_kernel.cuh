@@ -1,42 +1,39 @@
-// DUNE kernel, tcgen05 version with TWO THREADS PER POINT (8 warps per 128-point tile).
+// DUNE kernel with TWO THREADS PER POINT (8 warps per 128-point tile).
 //
-// Why: the two-slot kernel of dune_tc_kernel.cuh (one thread per point, 123 registers, 16 warps per SM) is bound by
-// dependent-issue latency -- issue slots 60 % busy, no pipe above 36 %, stalls per issue: fixed-latency wait 1.64, TMEM
-// scoreboard 0.60, barrier 0.55 (profiles/r01_dune_tc_v4_final_ncu.txt).  Registers and TMEM pin it at 4 warps per scheduler.
-// Here every point is shared by two threads that own 16 of the 32 features each: half the per-thread state (<= 80
-// registers), twice the warps per tile, same TMEM footprint (128 columns per CTA: 2 slots x {D 32 | A_hi 16 | A_lo 16}).
+// Every point is shared by two threads that own 16 of the 32 features each: half the per-thread state of dune_tcp_kernel,
+// twice the warps per tile, the same two 16 KB tiles per CTA.
 //
-//   thread (row r = tid & 127, half hf = tid >> 7): warps w and w + 4 address the same 32 TMEM lanes (lane quarter w & 3)
-//   and split the columns: D columns [16 hf, 16 hf + 16), A_hi columns 32 + [8 hf, 8 hf + 8), A_lo columns 48 + [8 hf, ..).
-//   LayerNorm needs the sum of squares over all 32 features: both threads read the other half as well (one extra
-//   tcgen05.ld.x16 + 8 FFMA2) and add the two half sums -- the same two numbers, so both get the same bits (a + b = b + a)
-//   without any exchange through shared memory.  Layer 0 (2 -> 32, FMA pipe) is evaluated in full by both threads.
-//   The head epilogue (mu, distance, sort key) of slot s is done by the threads with hf == s.
-// Everything else -- operand image, descriptors, bias product, centred LayerNorm, folded tanh map, packed FP32 math,
-// shared-reciprocal tanh, elect.sync issue, rank-merge top-M -- is the contract of dune_tcp_kernel.
+//   thread (row r = tid & 127, half hf = tid >> 7): warps w and w + 4 own the same tile rows and split the columns: D features
+//   [16 hf, 16 hf + 16), A K range [16 hf, 16 hf + 16).  The first warpgroup issues the layer's MMAs; a block barrier hands D to
+//   both halves.  LayerNorm needs the sum of squares over all 32 features: both threads read the other half as well and add
+//   the two half sums -- the same two numbers, so both get the same bits (a + b = b + a) without any exchange.  Layer 0
+//   (2 -> 32, FMA pipe) is evaluated in full by both threads.  The head epilogue (mu, distance, sort key) of slot s is done by
+//   the threads with hf == s.
+// Everything else -- operand image, bias product, centred LayerNorm, folded tanh map, shared-reciprocal tanh, rank-merge
+// top-M -- is the contract of dune_tcp_kernel.
 #pragma once
 #include "dune_tc_kernel.cuh"
 
 namespace nb {
 namespace tc {
 
-__device__ __forceinline__ void st8(uint32_t taddr, const uint32_t (&a)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]),
-               "r"(a[4]), "r"(a[5]), "r"(a[6]), "r"(a[7])
-               : "memory");
+// the thread's half of the A row (K 16 hf .. 16 hf + 15): chunks 2 hf, 2 hf + 1 of hi and of lo
+__device__ __forceinline__ void st_a_half(unsigned char* tile, int p, int hf, const uint32_t (&hi)[8], const uint32_t (&lo)[8]) {
+#pragma unroll
+  for (int q = 0; q < 2; ++q) {
+    *reinterpret_cast<uint4*>(tile + chunk_off(p, 2 * hf + q)) = make_uint4(hi[4 * q], hi[4 * q + 1], hi[4 * q + 2], hi[4 * q + 3]);
+    *reinterpret_cast<uint4*>(tile + chunk_off(p, 4 + 2 * hf + q)) = make_uint4(lo[4 * q], lo[4 * q + 1], lo[4 * q + 2], lo[4 * q + 3]);
+  }
 }
 
-__device__ __forceinline__ void ld16p(uint32_t taddr, f2 (&hp)[8]) {
-  uint32_t d[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3]), "=r"(d[4]), "=r"(d[5]), "=r"(d[6]), "=r"(d[7]), "=r"(d[8]), "=r"(d[9]), "=r"(d[10]),
-        "=r"(d[11]), "=r"(d[12]), "=r"(d[13]), "=r"(d[14]), "=r"(d[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// features 16 half .. 16 half + 15 of the row's D as 8 pairs
+__device__ __forceinline__ void ld16p(const unsigned char* tile, int p, int half, f2 (&hp)[8]) {
 #pragma unroll
-  for (int c = 0; c < 8; ++c) hp[c] = pku(d[2 * c], d[2 * c + 1]);
+  for (int c = 0; c < 4; ++c) {
+    const uint4 v = *reinterpret_cast<const uint4*>(tile + chunk_off(p, 4 * half + c));
+    hp[2 * c] = pku(v.x, v.y);
+    hp[2 * c + 1] = pku(v.z, v.w);
+  }
 }
 
 // sum of squares of 16 features held as 8 packed pairs; fixed association (two chains, then lanes) so that the two threads of a
@@ -94,17 +91,13 @@ __device__ __forceinline__ void tanh_split16(const f2 (&hp)[8], float r, const f
 }
 
 __device__ __forceinline__ void relu_split16(const f2 (&hp)[8], uint32_t (&hi)[8], uint32_t (&lo)[8]) {
-  const unsigned short m1 = 0xBC00;  // -1.0h
 #pragma unroll
   for (int c = 0; c < 8; ++c) {
-    float a0, a1, l0, l1;
+    float a0, a1;
     upk(hp[c], a0, a1);
     asm("cvt.rz.relu.f16x2.f32 %0, %1, %2;" : "=r"(hi[c]) : "f"(a1), "f"(a0));
-    unsigned short h0, h1;
-    asm("mov.b32 {%0,%1}, %2;" : "=h"(h0), "=h"(h1) : "r"(hi[c]));
-    asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(l0) : "h"(h0), "h"(m1), "f"(a0));
-    asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(l1) : "h"(h1), "h"(m1), "f"(a1));
-    asm("cvt.rn.relu.f16x2.f32 %0, %1, %2;" : "=r"(lo[c]) : "f"(l1), "f"(l0));
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi[c]));
+    asm("cvt.rn.relu.f16x2.f32 %0, %1, %2;" : "=r"(lo[c]) : "f"(__fsub_rn(a1, f.y)), "f"(__fsub_rn(a0, f.x)));
   }
 }
 
@@ -228,9 +221,9 @@ __device__ __forceinline__ void select_and_write8(const DuneParams& prm, const I
 
 }  // namespace tc
 
-// shared memory: operand image | keys (N x 8 B, generic path) | smu (N x E floats) | candidates (8 warps x M)
+// shared memory: operand image | two tiles | keys (N x 8 B, generic path) | smu (N x E floats) | candidates (8 warps x M)
 __host__ __device__ inline size_t dune_tc8_smem_bytes(int N, int E, int M) {
-  return TcImage::kBytes + (size_t)N * 8 + (((size_t)N * E * 4 + 7) / 8) * 8 + (size_t)8 * M * 8 + 64;
+  return TcImage::kBytes + 2 * (size_t)tc::kTileBytes + (size_t)N * 8 + (((size_t)N * E * 4 + 7) / 8) * 8 + (size_t)8 * M * 8 + 64;
 }
 
 template <bool kFast, int kMinBlocks>
@@ -238,54 +231,32 @@ __global__ void __launch_bounds__(256, kMinBlocks) dune_tc8_kernel(const DunePar
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   using I = TcImage;
   unsigned char* simg = smem_dyn;
+  unsigned char* tiles = simg + I::kBytes;
   const float* fl = reinterpret_cast<const float*>(simg + I::kFloatOff);
-  unsigned long long* keys = reinterpret_cast<unsigned long long*>(simg + I::kBytes);
-  float* smu = reinterpret_cast<float*>(simg + I::kBytes + (size_t)prm.N * 8);
-  unsigned long long* cands = reinterpret_cast<unsigned long long*>(simg + I::kBytes + (size_t)prm.N * 8 + (((size_t)prm.N * prm.geo.E * 4 + 7) / 8) * 8);
-  __shared__ __align__(8) unsigned long long mbar[2];  // D of slot 0 / 1 ready (tcgen05.commit)
-  __shared__ uint32_t tmem_base_s;
+  unsigned char* tail = tiles + 2 * tc::kTileBytes;
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(tail);
+  float* smu = reinterpret_cast<float*>(tail + (size_t)prm.N * 8);
+  unsigned long long* cands = reinterpret_cast<unsigned long long*>(tail + (size_t)prm.N * 8 + (((size_t)prm.N * prm.geo.E * 4 + 7) / 8) * 8);
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int row = tid & 127, hf = tid >> 7;  // hf is warp-uniform
+  const int prow = tc::tile_row(row);
   for (int i = tid; i < I::kBytes / 16; i += 256) reinterpret_cast<uint4*>(simg)[i] = reinterpret_cast<const uint4*>(image)[i];
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(tc::smem_u32(&mbar[0])));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(tc::smem_u32(&mbar[1])));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 128;" ::"r"(tc::smem_u32(&tmem_base_s)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tbase = tmem_base_s;
-  const uint32_t trow = tbase + ((uint32_t)((warp & 3) * 32) << 16);  // warps w and w + 4 share a TMEM lane quarter
   const uint32_t simg_u = tc::smem_u32(simg);
-  const uint32_t bar0 = tc::smem_u32(&mbar[0]);
-  const uint32_t desc_w = tc::desc_lo(simg_u, 512), desc_ones = tc::desc_lo(simg_u + I::kOnesOff, 2048);
-  uint32_t phases = 0;
 
+  // both halves store their operands; the first warpgroup runs the MMAs; the block barrier after them hands D to both halves.
+  // The barrier before the stores: a row's operands overwrite that row's D, which BOTH of its threads read (each needs the other
+  // half's features for the LayerNorm), so neither may store until its partner has finished reading.
   auto publish = [&](const uint32_t (&hi)[8], const uint32_t (&lo)[8], int slot, int layer) {
-    const uint32_t tS = trow + 64 * slot;
-    tc::st8(tS + 32 + 8 * hf, hi);
-    tc::st8(tS + 48 + 8 * hf, lo);
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    const int issuer = (layer + slot + (int)blockIdx.x) & 7;  // rotate over the 8 warps (two per scheduler)
+    unsigned char* tile = tiles + slot * tc::kTileBytes;
     __syncthreads();
-    if (warp == issuer) {
-      uint32_t elected;
-      asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(elected));
-      if (elected) tc::issue_layer_bias(tbase + 64 * slot, desc_w, desc_ones, layer, bar0 + 8 * slot);
-    }
-  };
-  auto acquire = [&](int slot) {
-    tc::mbar_wait(bar0 + 8 * slot, (phases >> slot) & 1u);
-    phases ^= 1u << slot;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    tc::st_a_half(tile, prow, hf, hi, lo);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    if (hf == 0) tc::layer_mma<true>(tile, simg_u, layer, warp, lane);
+    __syncthreads();
   };
 
   const int T1 = prm.T + 1, N = prm.N, M = prm.M, E = prm.geo.E;
@@ -314,29 +285,13 @@ __global__ void __launch_bounds__(256, kMinBlocks) dune_tc8_kernel(const DunePar
         i = i < n ? i : n - 1;
         float x0, y0;
         fr.local(i, x0, y0);
-        const tc::f2 x2 = tc::pk(x0, x0), y2 = tc::pk(y0, y0);
         tc::f2 own[8];
         float qo, qw;
         {
           tc::f2 oth[8];
-          const int oo = 16 * (1 - hf), ow = 16 * hf;
-#pragma unroll
-          for (int c = 0; c < 8; c += 2) {
-            const ulonglong2 wx = *reinterpret_cast<const ulonglong2*>(fl + I::W0X + oo + 2 * c);
-            const ulonglong2 wy = *reinterpret_cast<const ulonglong2*>(fl + I::W0Y + oo + 2 * c);
-            const ulonglong2 bb = *reinterpret_cast<const ulonglong2*>(fl + I::B0 + oo + 2 * c);
-            oth[c] = tc::fma2(wy.x, y2, tc::fma2(wx.x, x2, bb.x));
-            oth[c + 1] = tc::fma2(wy.y, y2, tc::fma2(wx.y, x2, bb.y));
-          }
+          tc::layer0(fl, x0, y0, 16 * (1 - hf), oth);
           qo = tc::sumsq16(oth);
-#pragma unroll
-          for (int c = 0; c < 8; c += 2) {
-            const ulonglong2 wx = *reinterpret_cast<const ulonglong2*>(fl + I::W0X + ow + 2 * c);
-            const ulonglong2 wy = *reinterpret_cast<const ulonglong2*>(fl + I::W0Y + ow + 2 * c);
-            const ulonglong2 bb = *reinterpret_cast<const ulonglong2*>(fl + I::B0 + ow + 2 * c);
-            own[c] = tc::fma2(wy.x, y2, tc::fma2(wx.x, x2, bb.x));
-            own[c + 1] = tc::fma2(wy.y, y2, tc::fma2(wx.y, x2, bb.y));
-          }
+          tc::layer0(fl, x0, y0, 16 * hf, own);
           qw = tc::sumsq16(own);
         }
         float r;
@@ -351,19 +306,18 @@ __global__ void __launch_bounds__(256, kMinBlocks) dune_tc8_kernel(const DunePar
         for (int sl = 0; sl < nslots; ++sl) {
           tc::f2 own[8];
           uint32_t hi[8], lo[8];
-          acquire(sl);
-          const uint32_t tD = trow + 64 * sl;
+          const unsigned char* tile = tiles + sl * tc::kTileBytes;
           if (st & 1) {
-            tc::ld16p(tD + 16 * hf, own);
+            tc::ld16p(tile, prow, hf, own);
             tc::relu_split16(own, hi, lo);
           } else {
             float qo;
             {
               tc::f2 oth[8];
-              tc::ld16p(tD + 16 * (1 - hf), oth);
+              tc::ld16p(tile, prow, 1 - hf, oth);
               qo = tc::sumsq16(oth);
             }
-            tc::ld16p(tD + 16 * hf, own);
+            tc::ld16p(tile, prow, hf, own);
             const float qw = tc::sumsq16(own);
             float r;
             asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(fmaf(qw + qo, 1.0f / 32, 1e-5f)));
@@ -372,11 +326,10 @@ __global__ void __launch_bounds__(256, kMinBlocks) dune_tc8_kernel(const DunePar
           publish(hi, lo, sl, st);
         }
       }
-      // head epilogue: slot s by the threads with hf == s (every thread waits for its own slot only)
+      // head epilogue: slot s by the threads with hf == s
       if (hf < nslots) {
         float mu[8];
-        acquire(hf);
-        tc::ld8(trow + 64 * hf, mu);
+        tc::ld8(tiles + hf * tc::kTileBytes, prow, mu);
         int i = base + hf * 128 + row;
         const bool valid = i < n;
         i = valid ? i : n - 1;
@@ -386,20 +339,13 @@ __global__ void __launch_bounds__(256, kMinBlocks) dune_tc8_kernel(const DunePar
         if (base == 0) k0 = key;
         else if (base == 256) k1 = key;
       }
-      // the other half's phase bookkeeping: the slot it did not wait for completed one more phase
-      if (nslots == 2) phases ^= 1u << (1 - hf);
-      else if (hf == 1) phases ^= 1u;
-      __syncthreads();  // D of both slots has been read before the next pass (or item) overwrites the operands / D
+      __syncthreads();  // D of both slots has been read before the next pass (or item) overwrites the tiles
     }
     // ---- top-M and the output rows -----------------------------------------------------------------------------------
     if (reg_keys) tc::select_and_write_reg8(prm, fr, b, t, n, cnt, tid, k0, k1, smu, cands);
     else tc::select_and_write8(prm, fr, b, t, n, cnt, warp, lane, keys, smu, cands);
     __syncthreads();  // smu / cands (and keys) are reused by the next item
   }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 128;" ::"r"(tbase) : "memory");
 }
 
 }  // namespace nb

@@ -1,18 +1,14 @@
-// DUNE kernels, tcgen05 versions (Blackwell 5th-gen tensor cores, accumulators and A operand in TMEM).
+// DUNE kernels, warpgroup versions (Hopper wgmma: B operand from shared memory, accumulators in registers).
 //
-// Same contract as dune_mma_kernel.cuh / dune_kernel.cuh.  Mapping: CTA = 128 threads = 128 TMEM lanes;
-// thread r owns point r of a 128-point tile for the whole network, so LayerNorm statistics, tanh, ReLU
-// and the distance are thread-local (no shuffles, no fragment bookkeeping).  Per dense layer:
-//   registers --split x = hi + lo (fp16)--> tcgen05.st (A operand, TMEM)              [all threads]
-//   D[128 x 32] = ONES.BIASB + A_lo.B_hi + A_hi.B_lo + A_hi.B_hi                       [one elected lane, tcgen05.mma,
-//                                                      B (and ONES) from shared memory via UMMA descriptors]
-//   tcgen05.commit -> mbarrier -> tcgen05.ld (32 fp32 columns = the thread's row)      [all threads]
-// Layouts / descriptors were verified in isolation with tools/tc05_probe.cu.
+// Same contract as dune_mma_kernel.cuh / dune_kernel.cuh.  Mapping: CTA = 128 threads = one warpgroup; thread r owns point r
+// of a 128-point tile for the whole network, so LayerNorm statistics, tanh, ReLU and the distance are thread-local (no
+// shuffles, no fragment bookkeeping).  Per dense layer:
+//   registers --split x = hi + lo (fp16)--> shared-memory tile (A operand, canonical K-major layout)   [all threads]
+//   D[128 x 32] = ONES.BIASB + A_lo.B_hi + A_hi.B_lo + A_hi.B_hi                                    [the warpgroup, wgmma
+//                                                      m64n32k16 per 64-row half, B and ONES from shared memory]
+//   accumulator fragments -> the same tile -> 32 fp32 columns = the thread's row                      [all threads]
 //
-// dune_tcp_kernel (default): two 128-point tiles ("slots") per CTA, 128 TMEM columns = 2 x {D [0,32) | A_hi [32,48) |
-//   A_lo [48,64)}; the epilogue of one slot overlaps the MMAs of the other; packed FP32 / FHFMA epilogue math.
-// dune_tc_kernel (NB_DUNE_TC=1): the first version -- one slot (64 columns), bias row written into D by tcgen05.st,
-//   scalar epilogue math, every layer waits for its MMAs.
+// dune_tcp_kernel: two 128-point tiles ("slots") per CTA, each with its own 16 KB tile, interleaved by the same 128 threads.
 #pragma once
 #include <cuda_fp16.h>
 
@@ -21,7 +17,7 @@
 
 namespace nb {
 
-// Weight image built on the host (dune_tc.cu): canonical K-major / no-swizzle UMMA operand layout
+// Weight image built on the host (dune_tc.cu): canonical K-major / no-swizzle wgmma operand layout
 // (core matrix = 8 rows x 16 B; SBO = 128 B between 8-row groups; LBO between the two 8-half K groups).
 struct TcImage {
   static constexpr int kLayerStride = 4096;  // per dense layer (4 hidden + head, all N = 32): W_hi 2048 | W_lo 2048
@@ -29,198 +25,168 @@ struct TcImage {
   static constexpr int kFloatOff = kLayers * kLayerStride;  // 20480
   // float section (offsets in floats): W0 (32x2, row-major), b0, LayerNorm gain/offset pre-multiplied by 2*log2(e),
   // the biases of the five dense layers (already including the folded tanh map; head zero padded to 32), and W0
-  // again as two columns (W0X[j] = W0[j][0], W0Y[j] = W0[j][1]) for the packed-FP32 layer 0
+  // again as two columns (W0X[j] = W0[j][0], W0Y[j] = W0[j][1]) for the layer-0 loop
   static constexpr int W0 = 0, B0 = 64, G1 = 96, BE1 = 128, G6 = 160, BE6 = 192, G11 = 224, BE11 = 256, BH = 288, W0X = 448, W0Y = 480,
                        kFloats = 512;
   // bias by tensor core: D = ONES[128 x 16] . BIASB[layer][32 x 16] with ONES(m, 0..2) = 1 and BIASB(n, 0..2) = the three
-  // fp16 pieces of the bias (hi, lo, lo2: exact to fp32) -- the first MMA of a layer, replaces 8 LDS.128 + a 32-column
-  // tcgen05.st per thread and layer.  Both are K-major / no-swizzle core-matrix images like the weights.
+  // fp16 pieces of the bias (hi, lo, lo2) -- the first MMA of a layer, so that the accumulators need no initialisation from
+  // shared memory.  Both are K-major / no-swizzle core-matrix images like the weights.
   static constexpr int kOnesOff = kFloatOff + kFloats * 4;   // 22528, 4096 B  (LBO 2048)
   static constexpr int kBiasBOff = kOnesOff + 4096;          // 26624, 5 x 1024 B (LBO 512)
-  static constexpr int kBytes = kBiasBOff + kLayers * 1024;  // 31744
+  static constexpr int kBytes = kBiasBOff + kLayers * 1024;  // 31744 (a multiple of 1024: the tiles that follow stay aligned)
 };
 
 namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-constexpr uint32_t kIdescN32 = (1u << 4) | (4u << 17) | (8u << 24);  // D f32, A/B f16 K-major, N = 32, M = 128
+// ---- the 128-row tile ------------------------------------------------------------------------------------------------
+// A operand of a layer: 128 rows x 32 K, fp16 hi at bytes [0, 8192), lo at [8192, 16384), each in the canonical K-major /
+// no-swizzle layout (row p, K group q of 8 halves at q * 2048 + p * 16: LBO 2048, SBO 128, 4096 B per K step of 16).
+// Once the layer's MMAs have completed, the same 16 KB hold its fp32 output D: features 4c..4c+3 of row p lie in the
+// 16 bytes of A's chunk c (c = 0..7) of the same row, so every row's output replaces exactly that row's operands.
+constexpr int kTileBytes = 16384;
+__device__ __forceinline__ int chunk_off(int p, int c) { return c * 2048 + p * 16; }
 
-__device__ __forceinline__ uint64_t b_desc(uint32_t saddr, uint32_t lbo_bytes) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(128 >> 4) << 32) | (1ull << 46);
+// Row of the tile that thread r of the warpgroup owns.  wgmma gives warp w the accumulators of rows 16w..16w+15 of each
+// 64-row half; placing lanes 0-15 of warp w in the first half and lanes 16-31 in the second makes the warp's accumulators
+// exactly its own 32 rows, so D reaches its owners through shared memory with a warp barrier only.
+__device__ __forceinline__ int tile_row(int r) { return ((r & 16) << 2) | ((r >> 5) << 4) | (r & 15); }
+
+// the thread's activations (K 0..31 as 16 fp16 pairs, hi and lo) -> its row of the A operand
+__device__ __forceinline__ void st_a(unsigned char* tile, int p, const uint32_t (&hi)[16], const uint32_t (&lo)[16]) {
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    *reinterpret_cast<uint4*>(tile + chunk_off(p, q)) = make_uint4(hi[4 * q], hi[4 * q + 1], hi[4 * q + 2], hi[4 * q + 3]);
+    *reinterpret_cast<uint4*>(tile + chunk_off(p, 4 + q)) = make_uint4(lo[4 * q], lo[4 * q + 1], lo[4 * q + 2], lo[4 * q + 3]);
+  }
 }
 
-__device__ __forceinline__ void mma_f16(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// wgmma shared-memory descriptor, no swizzle: start address, LBO, SBO = 128 B (all operands lie in the first 256 KB)
+__device__ __forceinline__ uint64_t desc(uint32_t saddr, uint32_t lbo_bytes) {
+  return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(128u >> 4) << 32);
+}
+
+// D[64 x 32] += A[64 x 16] . B[32 x 16]^T, fp16 operands, fp32 accumulators
+__device__ __forceinline__ void wgmma32(float (&d)[16], uint64_t da, uint64_t db) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, 1, 1, 1, 0, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+        "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db)
       : "memory");
 }
 
-// A and B from shared memory (both through descriptors); used for the bias product that initialises D
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 32] = A[64 x 16] . B[32 x 16]^T (scale-d = 0: D is written, not read)
+__device__ __forceinline__ void wgmma32_first(float (&d)[16], uint64_t da, uint64_t db) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, 0, 1, 1, 0, 0;"
+      : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]), "=f"(d[9]), "=f"(d[10]),
+        "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15])
+      : "l"(da), "l"(db)
       : "memory");
 }
 
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-#pragma unroll 1
-  for (int i = 0; i < (1 << 26); ++i) {
-    uint32_t ok;
-    // the suspend-time hint lets the hardware park the thread until the phase completes (or the time limit passes)
-    // instead of returning immediately: fewer polling instructions competing for issue slots
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\tselp.b32 %0, 1, 0, p;\n\t}"
-                 : "=r"(ok)
-                 : "r"(bar), "r"(parity), "r"(20000u)
-                 : "memory");
-    if (ok) return;
+// One dense layer of the tile, issued by the 128 threads of a warpgroup after a barrier that made every row of A visible
+// to the async proxy (st_a + fence.proxy.async + barrier):
+//   kLo = true:  D = ONES.BIASB[layer] + A_lo.B_hi + A_hi.B_lo + A_hi.B_hi   (3-pass fp16 split, fp32 accuracy)
+//   kLo = false: D = ONES.BIASB[layer] + A_hi.B_hi                           (single pass: the screening network)
+// then D replaces A in the tile.  `img` is the shared-memory address of the operand image.
+template <bool kLo>
+__device__ __forceinline__ void layer_mma(unsigned char* tile, uint32_t img, int layer, int warp, int lane) {
+  using I = TcImage;
+  const uint32_t ta = smem_u32(tile);
+  float d[2][16];
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+  const uint64_t ones = desc(img + I::kOnesOff, 2048), biasb = desc(img + I::kBiasBOff + layer * 1024, 512);
+  const uint32_t w = img + layer * I::kLayerStride;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {  // rows 64 h .. 64 h + 63: 8 row groups of 128 B further
+    const uint32_t a = ta + h * 1024;
+    wgmma32_first(d[h], ones, biasb);
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      const uint64_t bhi = desc(w + s * 1024, 512), ahi = desc(a + s * 4096, 2048);
+      if (kLo) {
+        wgmma32(d[h], desc(a + 8192 + s * 4096, 2048), bhi);  // A_lo . B_hi (small terms first)
+        wgmma32(d[h], ahi, desc(w + 2048 + s * 1024, 512));   // A_hi . B_lo
+      }
+      wgmma32(d[h], ahi, bhi);  // A_hi . B_hi
+    }
   }
-  __trap();  // never hang the device on a protocol error
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+  asm volatile("bar.sync 1, 128;" ::: "memory");  // every warp's MMAs have read A before any D overwrites it
+  // accumulator i of half h: row 16 warp + g + 8 ((i >> 1) & 1) of the half, column 8 (i >> 2) + 2 tq + (i & 1)
+  const int g = lane >> 2, tq = lane & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < 16; i += 2) {
+      const int p = 64 * h + 16 * warp + g + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * tq;
+      *reinterpret_cast<float2*>(tile + chunk_off(p, col >> 2) + (col & 3) * 4) = make_float2(d[h][i], d[h][i + 1]);
+    }
+  __syncwarp();
 }
 
-__device__ __forceinline__ void st16(uint32_t taddr, const uint32_t (&a)[16]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr), "r"(a[0]),
-               "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(a[4]), "r"(a[5]), "r"(a[6]), "r"(a[7]), "r"(a[8]), "r"(a[9]), "r"(a[10]), "r"(a[11]), "r"(a[12]),
-               "r"(a[13]), "r"(a[14]), "r"(a[15])
-               : "memory");
-}
-
-// every thread writes the same 32-float row (the layer's bias) into its TMEM lane: D := bias
-__device__ __forceinline__ void st_bias32(uint32_t taddr, const float* __restrict__ b) {
-  uint32_t v[32];
-#pragma unroll
-  for (int j4 = 0; j4 < 8; ++j4) {
-    const uint4 q = *reinterpret_cast<const uint4*>(b + 4 * j4);
-    v[4 * j4] = q.x; v[4 * j4 + 1] = q.y; v[4 * j4 + 2] = q.z; v[4 * j4 + 3] = q.w;
-  }
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]),
-      "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]),
-      "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void ld32(uint32_t taddr, float (&h)[32]) {
-  uint32_t d[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3]), "=r"(d[4]), "=r"(d[5]), "=r"(d[6]), "=r"(d[7]), "=r"(d[8]), "=r"(d[9]), "=r"(d[10]),
-        "=r"(d[11]), "=r"(d[12]), "=r"(d[13]), "=r"(d[14]), "=r"(d[15]), "=r"(d[16]), "=r"(d[17]), "=r"(d[18]), "=r"(d[19]), "=r"(d[20]), "=r"(d[21]),
-        "=r"(d[22]), "=r"(d[23]), "=r"(d[24]), "=r"(d[25]), "=r"(d[26]), "=r"(d[27]), "=r"(d[28]), "=r"(d[29]), "=r"(d[30]), "=r"(d[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int j = 0; j < 32; ++j) h[j] = __uint_as_float(d[j]);
-}
-
-__device__ __forceinline__ void ld8(uint32_t taddr, float (&h)[8]) {
-  uint32_t d[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3]), "=r"(d[4]), "=r"(d[5]), "=r"(d[6]), "=r"(d[7])
-               : "r"(taddr)
-               : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int j = 0; j < 8; ++j) h[j] = __uint_as_float(d[j]);
-}
-
-// x = hi + lo (fp16 each), packed two values per 32-bit TMEM column (even k in the low half)
-__device__ __forceinline__ void split32(const float (&h)[32], uint32_t (&hi)[16], uint32_t (&lo)[16]) {
-#pragma unroll
-  for (int c = 0; c < 16; ++c) {
-    const __half2 hh = __floats2half2_rn(h[2 * c], h[2 * c + 1]);
-    const float2 f = __half22float2(hh);
-    const __half2 ll = __floats2half2_rn(h[2 * c] - f.x, h[2 * c + 1] - f.y);
-    hi[c] = *reinterpret_cast<const uint32_t*>(&hh);
-    lo[c] = *reinterpret_cast<const uint32_t*>(&ll);
-  }
-}
-
-// r = 1/(exp2(a) + 1) with a = 2*log2(e)*y; tanh(y) = 1 - 2r.  The affine map 1 - 2r is folded into the weights and
-// bias of the layer that follows (W' = -2W, b' = b + rowsum(W), built on the host), so r itself is the activation.
-__device__ __forceinline__ float tanh_r(float a) {
-  float e, r;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(a));
-  const float d = e + 1.0f;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(d));
-  return r;
-}
-
-// thread-local LayerNorm (eps 1e-5, biased variance) + tanh; g / be pre-scaled by 2*log2(e)
-__device__ __forceinline__ void ln_tanh32(float (&h)[32], const float* __restrict__ g, const float* __restrict__ be) {
-  float s = 0.f;
-#pragma unroll
-  for (int j = 0; j < 32; ++j) s += h[j];
-  const float mean = s * (1.0f / 32);
-  float q = 0.f;
-#pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    h[j] -= mean;
-    q = fmaf(h[j], h[j], q);
-  }
-  const float r = rsqrtf(fmaf(q, 1.0f / 32, 1e-5f));
-#pragma unroll
-  for (int j4 = 0; j4 < 8; ++j4) {
-    const float4 gg = *reinterpret_cast<const float4*>(g + 4 * j4);
-    const float4 bb = *reinterpret_cast<const float4*>(be + 4 * j4);
-    h[4 * j4 + 0] = tanh_r(fmaf(h[4 * j4 + 0] * r, gg.x, bb.x));
-    h[4 * j4 + 1] = tanh_r(fmaf(h[4 * j4 + 1] * r, gg.y, bb.y));
-    h[4 * j4 + 2] = tanh_r(fmaf(h[4 * j4 + 2] * r, gg.z, bb.z));
-    h[4 * j4 + 3] = tanh_r(fmaf(h[4 * j4 + 3] * r, gg.w, bb.w));
-  }
-}
-
-// ---- packed FP32 (FFMA2 / FADD2 / FMUL2: one issue slot, two lanes) and mixed f16*f16+f32 (FHFMA) -----------------
-using f2 = unsigned long long;  // two floats in an aligned register pair (low word = even feature)
+// ---- packed pairs of FP32 values (two features per 64-bit register pair, low word = even feature) ----------------------
+// Each operation is two correctly rounded scalar operations; the explicit _rn intrinsics keep the compiler from contracting
+// a multiply and an add into one FMA, so every result has the bits the formula states.
+using f2 = unsigned long long;
 __device__ __forceinline__ f2 pk(float lo, float hi) { f2 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
 __device__ __forceinline__ f2 pku(uint32_t lo, uint32_t hi) { f2 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "r"(lo), "r"(hi)); return r; }
 __device__ __forceinline__ void upk(f2 v, float& lo, float& hi) { asm("mov.b64 {%0,%1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { f2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
-__device__ __forceinline__ f2 add2(f2 a, f2 b) { f2 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) { f2 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
+__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) {
+  float a0, a1, b0, b1, c0, c1;
+  upk(a, a0, a1); upk(b, b0, b1); upk(c, c0, c1);
+  return pk(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
+}
+__device__ __forceinline__ f2 add2(f2 a, f2 b) {
+  float a0, a1, b0, b1;
+  upk(a, a0, a1); upk(b, b0, b1);
+  return pk(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
+}
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) {
+  float a0, a1, b0, b1;
+  upk(a, a0, a1); upk(b, b0, b1);
+  return pk(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
+}
 
-// (a0, a1) -> hi = fp16x2(a), lo = fp16x2(a - hi): F2FP, 2 x FHFMA (a - hi*1 in one instruction), F2FP
+// the thread's row of D (32 fp32 features) as 16 pairs / the first 8 features (the head)
+__device__ __forceinline__ void ld32p(const unsigned char* tile, int p, f2 (&hp)[16]) {
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {
+    const uint4 v = *reinterpret_cast<const uint4*>(tile + chunk_off(p, c));
+    hp[2 * c] = pku(v.x, v.y);
+    hp[2 * c + 1] = pku(v.z, v.w);
+  }
+}
+__device__ __forceinline__ void ld8(const unsigned char* tile, int p, float (&h)[8]) {
+#pragma unroll
+  for (int c = 0; c < 2; ++c) {
+    const float4 v = *reinterpret_cast<const float4*>(tile + chunk_off(p, c));
+    h[4 * c] = v.x; h[4 * c + 1] = v.y; h[4 * c + 2] = v.z; h[4 * c + 3] = v.w;
+  }
+}
+
+// (a0, a1) -> hi = fp16x2(a), lo = fp16x2(a - hi)  (a - hi is exact to one rounding, like a fused a + hi * -1)
 __device__ __forceinline__ void split_pair(float a0, float a1, uint32_t& hi, uint32_t& lo) {
   const __half2 hh = __floats2half2_rn(a0, a1);
   hi = *reinterpret_cast<const uint32_t*>(&hh);
-  unsigned short h0, h1;
-  asm("mov.b32 {%0,%1}, %2;" : "=h"(h0), "=h"(h1) : "r"(hi));
-  const unsigned short m1 = 0xBC00;  // -1.0h
-  float l0, l1;
-  asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(l0) : "h"(h0), "h"(m1), "f"(a0));
-  asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(l1) : "h"(h1), "h"(m1), "f"(a1));
-  const __half2 ll = __floats2half2_rn(l0, l1);
+  const float2 f = __half22float2(hh);
+  const __half2 ll = __floats2half2_rn(__fsub_rn(a0, f.x), __fsub_rn(a1, f.y));
   lo = *reinterpret_cast<const uint32_t*>(&ll);
 }
 
-__device__ __forceinline__ void ld32p(uint32_t taddr, f2 (&hp)[16]) {
-  uint32_t d[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3]), "=r"(d[4]), "=r"(d[5]), "=r"(d[6]), "=r"(d[7]), "=r"(d[8]), "=r"(d[9]), "=r"(d[10]),
-        "=r"(d[11]), "=r"(d[12]), "=r"(d[13]), "=r"(d[14]), "=r"(d[15]), "=r"(d[16]), "=r"(d[17]), "=r"(d[18]), "=r"(d[19]), "=r"(d[20]), "=r"(d[21]),
-        "=r"(d[22]), "=r"(d[23]), "=r"(d[24]), "=r"(d[25]), "=r"(d[26]), "=r"(d[27]), "=r"(d[28]), "=r"(d[29]), "=r"(d[30]), "=r"(d[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int c = 0; c < 16; ++c) hp[c] = pku(d[2 * c], d[2 * c + 1]);
-}
-
-// LayerNorm (eps 1e-5, biased variance) + r = 1/(exp2(.)+1) + fp16 split, two features per instruction where the ISA
-// allows it (squares, scale/offset, +1); MUFU.EX2 / MUFU.RCP stay scalar.  The inputs arrive CENTRED: the layer that
+// LayerNorm (eps 1e-5, biased variance) + r = 1/(exp2(.)+1) + fp16 split.  The inputs arrive CENTRED: the layer that
 // produces them has W - colmean(W), b - mean(b) (host image), so mean(h) = 0 up to rounding and only the variance is left.
-// kFast: one MUFU.RCP serves four features: with d_i = exp2(a_i) + 1,  t = 1/(d0 d1 d2 d3),  1/d0 = t d1 d2 d3, ...  (three
-// packed and three scalar multiplies instead of three MUFUs; the host enables it only if the checkpoint's LayerNorm
-// gains/offsets bound every a_i by 30, so that the product of four stays below 2^124)
+// tanh(y) = 1 - 2r with r = 1/(exp2(a) + 1), a = 2*log2(e)*y; the affine map 1 - 2r is folded into the weights and bias of
+// the layer that follows (W' = -2W, b' = b + rowsum(W), built on the host), so r itself is the activation.
+// kFast: one MUFU.RCP serves four features: with d_i = exp2(a_i) + 1,  t = 1/(d0 d1 d2 d3),  1/d0 = t d1 d2 d3, ...  (the
+// host enables it only if the checkpoint's LayerNorm gains/offsets bound every a_i by 30, so that the product of four stays
+// below 2^124)
 template <bool kFast>
 __device__ __forceinline__ void ln_tanh_split(f2 (&hp)[16], const float* __restrict__ g, const float* __restrict__ be, uint32_t (&hi)[16],
                                               uint32_t (&lo)[16]) {
@@ -275,24 +241,21 @@ __device__ __forceinline__ void ln_tanh_split(f2 (&hp)[16], const float* __restr
 // relu + split without a max: hi = fp16x2(relu(a)) rounded TOWARDS ZERO (cvt.rz.relu), so that a - hi is >= 0 for a > 0
 // and equals a < 0 for a <= 0 (hi = 0); lo = fp16x2(relu(a - hi)) then drops exactly the negative inputs
 __device__ __forceinline__ void relu_split(const f2 (&hp)[16], uint32_t (&hi)[16], uint32_t (&lo)[16]) {
-  const unsigned short m1 = 0xBC00;  // -1.0h
 #pragma unroll
   for (int c = 0; c < 16; ++c) {
-    float a0, a1, l0, l1;
+    float a0, a1;
     upk(hp[c], a0, a1);
     asm("cvt.rz.relu.f16x2.f32 %0, %1, %2;" : "=r"(hi[c]) : "f"(a1), "f"(a0));  // d = {hi half: first source, lo half: second}
-    unsigned short h0, h1;
-    asm("mov.b32 {%0,%1}, %2;" : "=h"(h0), "=h"(h1) : "r"(hi[c]));
-    asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(l0) : "h"(h0), "h"(m1), "f"(a0));
-    asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(l1) : "h"(h1), "h"(m1), "f"(a1));
-    asm("cvt.rn.relu.f16x2.f32 %0, %1, %2;" : "=r"(lo[c]) : "f"(l1), "f"(l0));
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi[c]));
+    asm("cvt.rn.relu.f16x2.f32 %0, %1, %2;" : "=r"(lo[c]) : "f"(__fsub_rn(a1, f.y)), "f"(__fsub_rn(a0, f.x)));
   }
 }
 
 }  // namespace tc
 
+// shared memory: operand image | two tiles | keys (N x 8 B, n > 512) | smu (N x E floats) | candidates (4 warps x M)
 __host__ __device__ inline size_t dune_tc_smem_bytes(int N, int E, int M) {
-  return TcImage::kBytes + (size_t)N * 8 + (((size_t)N * E * 4 + 7) / 8) * 8 + (size_t)4 * M * 8 + 64;
+  return TcImage::kBytes + 2 * (size_t)tc::kTileBytes + (size_t)N * 8 + (((size_t)N * E * 4 + 7) / 8) * 8 + (size_t)4 * M * 8 + 64;
 }
 
 namespace tc {
@@ -331,6 +294,21 @@ __device__ __forceinline__ ItemFrame item_frame(const DuneParams& prm, int b, in
   f.vx = prm.velocities ? prm.velocities + (size_t)b * 2 * prm.N : nullptr;
   f.vy = f.vx ? f.vx + prm.N : nullptr;
   return f;
+}
+
+// layer 0 (2 -> 32, FMA pipe) of the point (x0, y0), features `off` .. `off` + 2 cnt - 1 as pairs
+template <int kPairs>
+__device__ __forceinline__ void layer0(const float* __restrict__ fl, float x0, float y0, int off, f2 (&hp)[kPairs]) {
+  using I = TcImage;
+  const f2 x2 = pk(x0, x0), y2 = pk(y0, y0);
+#pragma unroll
+  for (int c = 0; c < kPairs; c += 2) {
+    const ulonglong2 wx = *reinterpret_cast<const ulonglong2*>(fl + I::W0X + off + 2 * c);
+    const ulonglong2 wy = *reinterpret_cast<const ulonglong2*>(fl + I::W0Y + off + 2 * c);
+    const ulonglong2 bb = *reinterpret_cast<const ulonglong2*>(fl + I::B0 + off + 2 * c);
+    hp[c] = fma2(wy.x, y2, fma2(wx.x, x2, bb.x));
+    hp[c + 1] = fma2(wy.y, y2, fma2(wx.y, x2, bb.y));
+  }
 }
 
 // mu = relu(head), dist = mu^T (G p0 - h)   (dune.py:119-122); publishes mu and the sortable key of the point
@@ -416,41 +394,6 @@ __device__ __forceinline__ void select_and_write(const DuneParams& prm, const It
   }
 }
 
-// the six MMAs of one dense layer (3-pass fp16 split, K = 32 as two K = 16 steps) + commit to an mbarrier; one thread
-__device__ __forceinline__ void issue_layer(uint32_t tD, uint32_t wsmem, uint32_t bar) {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-  for (int s = 0; s < 2; ++s) {
-    const uint64_t bhi = b_desc(wsmem + s * 1024, 512), blo = b_desc(wsmem + 2048 + s * 1024, 512);
-    mma_f16(tD, tD + 48 + 8 * s, bhi, kIdescN32, 1u);  // A_lo . B_hi
-    mma_f16(tD, tD + 32 + 8 * s, blo, kIdescN32, 1u);  // A_hi . B_lo
-    mma_f16(tD, tD + 32 + 8 * s, bhi, kIdescN32, 1u);  // A_hi . B_hi
-  }
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// same, but D is initialised by the bias product ONES . BIASB[layer] instead of a tcgen05.st of the bias row.
-// The descriptors are linear in the operand address (all operands are 16-byte multiples inside one 1024-aligned image and
-// shared memory addresses fit the 14-bit field), so they are formed by adding constants to two precomputed low words:
-//   dw = descriptor low word of the image base with LBO 512 (weights, BIASB), done = same for ONES (LBO 2048)
-constexpr uint32_t kDescHi = (128u >> 4) | (1u << 14);  // SBO = 128 B, descriptor version bit 46
-__device__ __forceinline__ uint32_t desc_lo(uint32_t saddr, uint32_t lbo_bytes) { return ((saddr >> 4) & 0x3FFFu) | ((lbo_bytes >> 4) << 16); }
-__device__ __forceinline__ uint64_t mk_desc(uint32_t lo) { return ((uint64_t)kDescHi << 32) | lo; }
-__device__ __forceinline__ void issue_layer_bias(uint32_t tD, uint32_t dw, uint32_t done, int layer, uint32_t bar) {
-  using I = TcImage;
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  mma_f16_ss(tD, mk_desc(done), mk_desc(dw + (I::kBiasBOff >> 4) + layer * (1024 >> 4)), kIdescN32, 0u);
-  const uint32_t w = dw + layer * (I::kLayerStride >> 4);
-#pragma unroll
-  for (int s = 0; s < 2; ++s) {
-    const uint64_t bhi = mk_desc(w + s * (1024 >> 4)), blo = mk_desc(w + (2048 >> 4) + s * (1024 >> 4));
-    mma_f16(tD, tD + 48 + 8 * s, bhi, kIdescN32, 1u);  // A_lo . B_hi
-    mma_f16(tD, tD + 32 + 8 * s, blo, kIdescN32, 1u);  // A_hi . B_lo
-    mma_f16(tD, tD + 32 + 8 * s, bhi, kIdescN32, 1u);  // A_hi . B_hi
-  }
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
 // Selection for n <= 512 with the thread's own (<= 4) distance keys in registers (thread tid owns points tid + 128 j):
 // per-warp REDUX rounds produce each warp's cnt smallest in ascending order, then every candidate computes its rank among
 // the 4 x cnt candidates (all four warps in parallel, no serial merge) and the lanes of rank < cnt write the output rows.
@@ -509,78 +452,35 @@ __device__ __forceinline__ void select_and_write_reg(const DuneParams& prm, cons
 }  // namespace tc
 
 // ------------------------------------------------------------------------------------------------------
-// Default kernel: two 128-point tiles ("slots") per CTA, interleaved by the same 128 threads.  Thread r owns point r of
-// both tiles.  While the threads run the epilogue of one slot (tcgen05.ld -> LayerNorm/tanh or ReLU -> fp16 split ->
-// tcgen05.st), the tensor core works on the other slot, so the mbarrier wait that follows is already satisfied: no
-// polling, no MMA latency on the critical path, no dedicated issuer warp.
-//   TMEM per CTA: 128 columns = 2 slots x {D [0,32) | A_hi [32,48) | A_lo [48,64)};  4 CTAs per SM.
-//   Element-wise math is packed two features per instruction (FFMA2/FADD2/FMUL2) and the fp16 split uses FHFMA.
-// kSync = 0: a block barrier between the operand stores of a slot and its MMAs;  kSync = 1: the four warps arrive on an
-// mbarrier instead and only warp 0 (whose lane 0 issues the MMAs) waits for it, so warps 1-3 run ahead into the other slot.
-template <int kSync, bool kFast>
-__global__ void __launch_bounds__(128, 4) dune_tcp_kernel(const DuneParams prm, const unsigned char* __restrict__ image) {
-  extern __shared__ __align__(1024) unsigned char smem_dyn[];  // the attribute aligns the dynamic segment (UMMA operands need 128 B)
+// Exact kernel: two 128-point tiles ("slots") per CTA, interleaved by the same 128 threads; thread r owns point r of both
+// tiles.  Per stage and slot: read the slot's D row -> LayerNorm/tanh or ReLU -> fp16 split -> A row -> barrier -> the
+// warpgroup's MMAs for the slot.
+template <bool kFast>
+__global__ void __launch_bounds__(128) dune_tcp_kernel(const DuneParams prm, const unsigned char* __restrict__ image) {
+  extern __shared__ __align__(1024) unsigned char smem_dyn[];
   using I = TcImage;
   unsigned char* simg = smem_dyn;
+  unsigned char* tiles = simg + I::kBytes;
   const float* fl = reinterpret_cast<const float*>(simg + I::kFloatOff);
-  unsigned long long* keys = reinterpret_cast<unsigned long long*>(simg + I::kBytes);
-  float* smu = reinterpret_cast<float*>(simg + I::kBytes + (size_t)prm.N * 8);
-  unsigned long long* cands = reinterpret_cast<unsigned long long*>(simg + I::kBytes + (size_t)prm.N * 8 + (((size_t)prm.N * prm.geo.E * 4 + 7) / 8) * 8);
-  __shared__ __align__(8) unsigned long long mbar[4];  // [0,1]: D of slot 0/1 ready (tcgen05.commit);  [2,3]: operands of slot 0/1 stored
-  __shared__ uint32_t tmem_base_s;
+  unsigned char* tail = tiles + 2 * tc::kTileBytes;
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(tail);
+  float* smu = reinterpret_cast<float*>(tail + (size_t)prm.N * 8);
+  unsigned long long* cands = reinterpret_cast<unsigned long long*>(tail + (size_t)prm.N * 8 + (((size_t)prm.N * prm.geo.E * 4 + 7) / 8) * 8);
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int prow = tc::tile_row(tid);
   for (int i = tid; i < I::kBytes / 16; i += 128) reinterpret_cast<uint4*>(simg)[i] = reinterpret_cast<const uint4*>(image)[i];
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(tc::smem_u32(&mbar[0])));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(tc::smem_u32(&mbar[1])));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 4;" ::"r"(tc::smem_u32(&mbar[2])));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 4;" ::"r"(tc::smem_u32(&mbar[3])));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // operand image -> visible to the tensor core (async proxy)
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 128;" ::"r"(tc::smem_u32(&tmem_base_s)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tbase = tmem_base_s;
-  const uint32_t trow = tbase + ((uint32_t)(warp * 32) << 16);  // this warp's 32 TMEM lanes
   const uint32_t simg_u = tc::smem_u32(simg);
-  const uint32_t bar0 = tc::smem_u32(&mbar[0]);
-  const uint32_t desc_w = tc::desc_lo(simg_u, 512), desc_ones = tc::desc_lo(simg_u + I::kOnesOff, 2048);
-  uint32_t phases = 0;  // bit sl: parity of the next completion of mbar[sl];  bit 2 + sl: same for mbar[2 + sl]
 
-  // activations (already split) of `slot` -> TMEM, then one thread starts the layer's MMAs (bias product first)
+  // activations (already split) of `slot` -> the slot's tile, then the warpgroup runs the layer's MMAs on it
   auto publish = [&](const uint32_t (&hi)[16], const uint32_t (&lo)[16], int slot, int layer) {
-    const uint32_t tS = trow + 64 * slot;
-    tc::st16(tS + 32, hi);
-    tc::st16(tS + 48, lo);
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    // The issuing warp rotates: warp w of every CTA lives on scheduler w of its SM, so a fixed issuer would put the ~100
-    // issue instructions (and, with kSync = 1, the waiting) of all resident CTAs on one of the four schedulers.
-    const int issuer = (layer + slot + (int)blockIdx.x) & 3;
-    if (kSync == 0) {
-      __syncthreads();
-    } else {
-      __syncwarp();
-      if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar0 + 16 + 8 * slot) : "memory");
-      if (warp == issuer) tc::mbar_wait(bar0 + 16 + 8 * slot, (phases >> (2 + slot)) & 1u);
-      phases ^= 4u << slot;  // every warp tracks the parity, only the issuer waits
-    }
-    if (warp == issuer) {  // warp-uniform branch; elect.sync picks the issuing lane (no divergent-branch waterfall around UTCHMMA)
-      uint32_t elected;
-      asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(elected));
-      if (elected) tc::issue_layer_bias(tbase + 64 * slot, desc_w, desc_ones, layer, bar0 + 8 * slot);
-    }
-  };
-  auto acquire = [&](int slot) {
-    tc::mbar_wait(bar0 + 8 * slot, (phases >> slot) & 1u);
-    phases ^= 1u << slot;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    unsigned char* tile = tiles + slot * tc::kTileBytes;
+    tc::st_a(tile, prow, hi, lo);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    tc::layer_mma<true>(tile, simg_u, layer, warp, lane);
   };
 
   const int T1 = prm.T + 1, N = prm.N, M = prm.M, E = prm.geo.E;
@@ -612,16 +512,8 @@ __global__ void __launch_bounds__(128, 4) dune_tcp_kernel(const DuneParams prm, 
         i = i < n ? i : n - 1;
         float x0, y0;
         fr.local(i, x0, y0);
-        const tc::f2 x2 = tc::pk(x0, x0), y2 = tc::pk(y0, y0);
         tc::f2 hp[16];
-#pragma unroll
-        for (int c = 0; c < 16; c += 2) {
-          const ulonglong2 wx = *reinterpret_cast<const ulonglong2*>(fl + I::W0X + 2 * c);
-          const ulonglong2 wy = *reinterpret_cast<const ulonglong2*>(fl + I::W0Y + 2 * c);
-          const ulonglong2 bb = *reinterpret_cast<const ulonglong2*>(fl + I::B0 + 2 * c);
-          hp[c] = tc::fma2(wy.x, y2, tc::fma2(wx.x, x2, bb.x));
-          hp[c + 1] = tc::fma2(wy.y, y2, tc::fma2(wx.y, x2, bb.y));
-        }
+        tc::layer0(fl, x0, y0, 0, hp);
         uint32_t hi[16], lo[16];
         tc::ln_tanh_split<kFast>(hp, fl + I::G1, fl + I::BE1, hi, lo);
         publish(hi, lo, sl, 0);
@@ -632,8 +524,7 @@ __global__ void __launch_bounds__(128, 4) dune_tcp_kernel(const DuneParams prm, 
         for (int sl = 0; sl < nslots; ++sl) {
           tc::f2 hp[16];
           uint32_t hi[16], lo[16];
-          acquire(sl);
-          tc::ld32p(trow + 64 * sl, hp);
+          tc::ld32p(tiles + sl * tc::kTileBytes, prow, hp);
           if (st & 1) tc::relu_split(hp, hi, lo);
           else tc::ln_tanh_split<kFast>(hp, fl + I::G1 + 32 * st, fl + I::BE1 + 32 * st, hi, lo);  // st = 2: G6/BE6, st = 4: G11/BE11
           publish(hi, lo, sl, st);
@@ -642,8 +533,7 @@ __global__ void __launch_bounds__(128, 4) dune_tcp_kernel(const DuneParams prm, 
 #pragma unroll 1
       for (int sl = 0; sl < nslots; ++sl) {  // head epilogue
         float mu[8];
-        acquire(sl);
-        tc::ld8(trow + 64 * sl, mu);
+        tc::ld8(tiles + sl * tc::kTileBytes, prow, mu);
         int i = base + sl * 128 + tid;
         const bool valid = i < n;
         i = valid ? i : n - 1;
@@ -663,120 +553,6 @@ __global__ void __launch_bounds__(128, 4) dune_tcp_kernel(const DuneParams prm, 
     else tc::select_and_write(prm, fr, b, t, n, cnt, warp, lane, keys, smu, cands);
     __syncthreads();  // smu / cands (and keys) are reused by the next item
   }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 128;" ::"r"(tbase) : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------------
-// First tcgen05 version, kept for A/B measurements (NB_DUNE_TC=1): one 128-point tile per CTA at a time, 64 TMEM columns,
-// 5 CTAs per SM, scalar FP32 element-wise math; every layer exposes the MMA latency behind an mbarrier poll.
-__global__ void __launch_bounds__(128, 5) dune_tc_kernel(const DuneParams prm, const unsigned char* __restrict__ image) {
-  extern __shared__ __align__(1024) unsigned char smem_dyn[];
-  using I = TcImage;
-  unsigned char* simg = smem_dyn;
-  const float* fl = reinterpret_cast<const float*>(simg + I::kFloatOff);
-  unsigned long long* keys = reinterpret_cast<unsigned long long*>(simg + I::kBytes);
-  float* smu = reinterpret_cast<float*>(simg + I::kBytes + (size_t)prm.N * 8);
-  unsigned long long* cands = reinterpret_cast<unsigned long long*>(simg + I::kBytes + (size_t)prm.N * 8 + (((size_t)prm.N * prm.geo.E * 4 + 7) / 8) * 8);
-  __shared__ __align__(8) unsigned long long mbar;
-  __shared__ uint32_t tmem_base_s;
-
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (int i = tid; i < I::kBytes / 16; i += 128) reinterpret_cast<uint4*>(simg)[i] = reinterpret_cast<const uint4*>(image)[i];
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(tc::smem_u32(&mbar)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 64;" ::"r"(tc::smem_u32(&tmem_base_s)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tbase = tmem_base_s;
-  const uint32_t trow = tbase + ((uint32_t)(warp * 32) << 16);
-  const uint32_t simg_u = tc::smem_u32(simg);
-  const uint32_t bar = tc::smem_u32(&mbar);
-  uint32_t phase = 0;
-
-  // one dense layer on the tensor core: h (activations) -> D (pre-activations incl. bias), left in TMEM
-  auto dense = [&](const float (&h)[32], int layer) {
-    uint32_t hi[16], lo[16];
-    tc::split32(h, hi, lo);
-    tc::st16(trow + 32, hi);
-    tc::st16(trow + 48, lo);
-    tc::st_bias32(trow, fl + I::BH + 32 * layer);
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (tid == 0) tc::issue_layer(tbase, simg_u + layer * I::kLayerStride, bar);
-    tc::mbar_wait(bar, phase);
-    phase ^= 1u;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  };
-
-  const int T1 = prm.T + 1, N = prm.N, M = prm.M, E = prm.geo.E;
-  const int items = prm.B * T1;
-  for (int item = blockIdx.x; item < items; item += gridDim.x) {
-    const int b = item / T1, t = item - b * T1;
-    if (prm.active && prm.active[b] == 0) continue;
-    int n = prm.num_points ? prm.num_points[b] : N;
-    n = n < 0 ? 0 : (n > N ? N : n);
-    const int cnt = n < M ? n : M;
-    if (t == 0 && tid == 0) {
-      prm.sel_count[b] = cnt;
-      if (n == 0 && prm.min_dist) prm.min_dist[b] = __int_as_float(0x7f800000);
-    }
-    if (n == 0) continue;
-    const tc::ItemFrame fr = tc::item_frame(prm, b, t);
-
-#pragma unroll 1
-    for (int tile = 0; tile * 128 < n; ++tile) {
-      int i = tile * 128 + tid;
-      const bool valid = i < n;
-      i = valid ? i : n - 1;
-      float x0, y0;
-      fr.local(i, x0, y0);
-      float h[32];
-#pragma unroll
-      for (int j2 = 0; j2 < 16; ++j2) {  // layer 0 on the FMA pipe
-        const float4 w = *reinterpret_cast<const float4*>(fl + I::W0 + 4 * j2);  // W0[2j][0..1], W0[2j+1][0..1]
-        const float2 bb = *reinterpret_cast<const float2*>(fl + I::B0 + 2 * j2);
-        h[2 * j2] = fmaf(w.y, y0, fmaf(w.x, x0, bb.x));
-        h[2 * j2 + 1] = fmaf(w.w, y0, fmaf(w.z, x0, bb.y));
-      }
-      tc::ln_tanh32(h, fl + I::G1, fl + I::BE1);
-      dense(h, 0);
-      tc::ld32(trow, h);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) h[j] = fmaxf(h[j], 0.f);
-      dense(h, 1);
-      tc::ld32(trow, h);
-      tc::ln_tanh32(h, fl + I::G6, fl + I::BE6);
-      dense(h, 2);
-      tc::ld32(trow, h);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) h[j] = fmaxf(h[j], 0.f);
-      dense(h, 3);
-      tc::ld32(trow, h);
-      tc::ln_tanh32(h, fl + I::G11, fl + I::BE11);
-      dense(h, 4);
-      float mu[8];
-      tc::ld8(trow, mu);
-      tc::finish_point(prm, mu, x0, y0, i, valid, E, smu, keys);
-    }
-    __syncthreads();
-    tc::select_and_write(prm, fr, b, t, n, cnt, warp, lane, keys, smu, cands);
-    __syncthreads();
-  }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 64;" ::"r"(tbase) : "memory");
 }
 
 }  // namespace nb

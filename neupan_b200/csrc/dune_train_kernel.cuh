@@ -13,7 +13,7 @@
 //
 // Shape of the work: 4,644 parameters, 256 points per optimiser step, and the steps are strictly sequential (every batch sees the
 // weights the previous one produced): 20 MFLOP per step.  That is a latency problem, not a throughput problem -- tensor cores
-// (128-row tiles, fp16 operands) would add split/TMEM traffic to a step that is bound by its ~20 block barriers -- so ONE persistent
+// (128-row tiles, fp16 operands) would add split / operand-tile traffic to a step that is bound by its ~20 block barriers -- so ONE persistent
 // CTA keeps the weights in shared memory for the whole epoch and runs thread-per-point FP32 forward/backward passes; the weight
 // gradients  dW = delta' a  are small GEMMs over the batch done cooperatively from shared memory (each thread owns four entries per
 // layer and, afterwards, the Adam update of exactly those entries).  Pre-activations are recomputed in the backward pass instead of

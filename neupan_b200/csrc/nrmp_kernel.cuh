@@ -225,7 +225,7 @@ __device__ __forceinline__ void nrmp_stop_env(const NrmpParams& prm, const int b
 // instructions were integer address arithmetic.
 // Residency: the (10, 10) specialisation is built for 7 CTAs (14 warps) per SM -- 128 registers with ~200 B of spills and
 // 29 KB of shared memory per CTA.  At B = 4096 that is 2072 resident solves = two full rounds instead of 2.3 rounds of
-// 1776; measured 1.39 -> 1.25 ms per launch.  (__maxnreg__(144) instead of the min-blocks bound spills more and is slower.)
+// 1776.  (__maxnreg__(144) instead of the min-blocks bound makes ptxas spill more.)
 template <int HPL, bool SMALL, int TT, int MM>
 __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int b, double* wsp, const unsigned short* __restrict__ ptab, const int lane) {
   const int T = TT > 0 ? TT : prm.T, M = TT > 0 ? MM : prm.M, T1 = T + 1;
@@ -1189,7 +1189,7 @@ __global__ void __launch_bounds__(128) nrmp_adjoint_kernel(const NrmpAdjParams p
 // work_counter == nullptr: one environment per warp (b = blockIdx.x * warps + warp), the grid covers the batch.
 template <int HPL, bool SMALL, int TT, int MM>
 #ifndef NB_NRMP_WPC
-#define NB_NRMP_WPC 3  // warps per CTA of the (10, 10) specialisation: 3 x 5 CTAs = 15 warps per SM (2 x 7 = 14: 29.29 vs 29.02 ms per step; 1 x 14: 29.64)
+#define NB_NRMP_WPC 3  // warps per CTA of the (10, 10) specialisation: 3 x 5 CTAs = 15 warps per SM (NB_NRMP_WPC is a tuning knob: 2 x 7 and 1 x 14 are the alternatives to time with bench.py)
 #endif
 __global__ void __launch_bounds__((TT == 10 && MM == 10) ? 32 * NB_NRMP_WPC : 64, (TT == 10 && MM == 10) ? (NB_NRMP_WPC == 3 ? 5 : (NB_NRMP_WPC == 1 ? 14 : 7)) : (HPL <= 4 ? 6 : 4))
     nrmp_kernel(const NrmpParams prm, int warps_per_cta, int warp_doubles_rt) {

@@ -86,7 +86,7 @@ struct nb_pan {
   // device buffers
   float* d_weights = nullptr;
   unsigned char* d_image = nullptr;  // fragment-ordered fp16 hi/lo weight image of the mma.sync DUNE kernel
-  unsigned char* d_tc_image = nullptr;  // UMMA operand image of the tcgen05 DUNE kernel
+  unsigned char* d_tc_image = nullptr;  // wgmma operand image of the warpgroup DUNE kernels
   int tc_flags = 0;                     // build_tc_image(): bit 0 = bounded tanh arguments
   unsigned char* d_tc_screen = nullptr; // operand image of the screening network (NB_OPT_DUNE_KERNEL = 4)
   int32_t *cand_idx = nullptr, *cand_cnt = nullptr, *flag_list = nullptr, *flag_count = nullptr, *refine_list = nullptr;
@@ -96,7 +96,7 @@ struct nb_pan {
                                         // measured for THIS checkpoint and polygon (NB_SCREEN_CMU overrides; DESIGN.md 3.1)
   bool screen_calibrated = false;
   float screen_cal_ratio = 0.f;
-  int dune_variant = 2;              // NB_OPT_DUNE_KERNEL: 0 = FP32 FFMA, 1 = mma.sync tensor-core, 2 = tcgen05 tensor-core kernel
+  int dune_variant = 2;              // NB_OPT_DUNE_KERNEL: 0 = FP32 FFMA, 1 = mma.sync tensor-core, 2 = wgmma tensor-core kernel
   int overlap = 1;                   // NB_OPT_OVERLAP: number of env sub-batches pipelined on internal streams
   cudaStream_t streams[4] = {nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t ev_fork = nullptr, ev_join[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -116,7 +116,7 @@ struct nb_pan {
   int32_t* adj_valid = nullptr;
   int* work_counters = nullptr;     // dynamic env -> warp assignment of the NRMP kernel, one counter per internal stream
   int dune_skip_t0 = 1;             // NB_OPT_DUNE_SKIP_T0: PAN iterations k > 0 keep the step-0 items of iteration 0 (screening variant)
-  int screen_mma = 1;               // NB_OPT_DUNE_SCREEN_MMA: screening pass on mma.sync (N <= 512) instead of tcgen05
+  int screen_mma = 1;               // NB_OPT_DUNE_SCREEN_MMA: screening pass on mma.sync (N <= 1024) instead of wgmma
   int nrmp_defer_stop_min = 256;    // NB_NRMP_DEFER_STOP_MIN (developer switch, read at create): smallest batch whose stop criterion runs as its own kernel
   int nrmp_dynamic = 1;             // NB_NRMP_STATIC=1 (developer switch, read at create) turns the persistent-warp schedule off
   float* warm = nullptr;            // NRMP warm-start records, nrmp_warm_floats(T, M) per environment
@@ -305,7 +305,7 @@ int calibrate_screen(nb_pan* p, cudaStream_t st) {
     prm.B = Bc; prm.N = N; prm.T = c.receding; prm.M = c.nrmp_max_num; prm.dt = (float)c.step_time; prm.geo = p->geo;
     prm.cand_idx = p->cand_idx; prm.cand_cnt = p->cand_cnt; prm.cand_dt = p->cand_dt; prm.screen_stats = p->screen_stats; prm.c_mu = p->c_mu;
     prm.flag_list = p->flag_list; prm.flag_count = p->flag_count; prm.refine_list = p->refine_list; prm.calibrate = 1;
-    for (int shape = 0; shape < 2 && rc == NB_OK; ++shape) {  // both screening kernels (tcgen05 / mma.sync): the bound holds whichever option is set later
+    for (int shape = 0; shape < 2 && rc == NB_OK; ++shape) {  // both screening kernels (wgmma / mma.sync): the bound holds whichever option is set later
       prm.screen_mma = shape;
       rc = launch_dune(p, prm, st);
       if (rc == NB_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = fail(NB_ERR_CUDA, "calibrate_screen: kernel failed");
@@ -493,7 +493,7 @@ int nb_pan_set_option(nb_pan_t* p, int32_t option, int32_t value) {
   if (!p) return fail(NB_ERR_INVALID, "null handle");
   if (option == NB_OPT_DUNE_KERNEL) {
     if (value < 0 || value > 4)
-      return fail(NB_ERR_INVALID, "NB_OPT_DUNE_KERNEL takes 0 (fp32 ffma), 1 (mma.sync), 2 (tcgen05), 3 (tcgen05, two threads per point) or 4 (tcgen05 with screening)");
+      return fail(NB_ERR_INVALID, "NB_OPT_DUNE_KERNEL takes 0 (fp32 ffma), 1 (mma.sync), 2 (wgmma), 3 (wgmma, two threads per point) or 4 (wgmma with screening)");
     p->dune_variant = value;
     if (value == 4 && !p->screen_calibrated && p->d_tc_screen) {
       NB_CUDA(cudaSetDevice(p->cfg.device));
@@ -708,7 +708,7 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
     NB_CUDA(cudaEventRecord(p->ev_fork, st));
     for (int i = 0; i < parts; ++i) NB_CUDA(cudaStreamWaitEvent(p->streams[i], p->ev_fork, 0));
     // enqueue order: iteration by iteration, alternating the streams (every sub-batch starts at once; NB_PAN_INTERLEAVE=0, a developer
-    // switch, enqueues all K iterations of one sub-batch before the next: 19.29 vs 19.30-19.7 ms per C4 step)
+    // switch, enqueues all K iterations of one sub-batch before the next)
     static int interleave = -1;
     if (interleave < 0) {
       const char* v = getenv("NB_PAN_INTERLEAVE");

@@ -2,7 +2,7 @@
 split into contiguous blocks, one process per GPU; the single exchange of a control step is the
 gather of the packed per-environment result [S 3(T+1) | U 2T | D T | min_distance 1].
 
-Works with any torch.distributed backend (NCCL over NVLink on the B200 box, gloo in the CPU tests).
+Works with any torch.distributed backend (NCCL over NVLink between GPUs, gloo in the CPU tests).
 """
 from __future__ import annotations
 

@@ -431,6 +431,24 @@ class Canonical:
         self.n, self.quads, self.hinges, self.l, self.const = n, quads, hinges, l, const
         self.E, self.e, self.G, self.g, self.soc, self.lb = E, e, G, g, soc, lb
 
+    # -- storage: the program as a flat dict of arrays (fixtures of programs built by the reference's own code)
+    def to_arrays(self, prefix):
+        if self.soc:
+            raise NotImplementedError("cone rows are not stored")
+        out = {f"{prefix}.{k}": np.asarray(v, np.float64) for k, v in dict(l=self.l, const=self.const, E=self.E, e=self.e, G=self.G, g=self.g, lb=self.lb).items()}
+        for name, terms in (("quad", self.quads), ("hinge", self.hinges)):
+            out[f"{prefix}.{name}_c"] = np.array([c for c, _ in terms], np.float64)
+            for j, (_, a) in enumerate(terms):
+                out[f"{prefix}.{name}{j}_A"], out[f"{prefix}.{name}{j}_b"] = np.asarray(a.A, np.float64), np.asarray(a.b, np.float64)
+        return out
+
+    @classmethod
+    def from_arrays(cls, z, prefix):
+        g = lambda k: np.asarray(z[f"{prefix}.{k}"])
+        terms = lambda name: [(float(c), _Aff(g(f"{name}{j}_A"), g(f"{name}{j}_b"), (len(g(f"{name}{j}_b")),))) for j, c in enumerate(g(f"{name}_c"))]
+        l = g("l")
+        return cls(len(l), terms("quad"), terms("hinge"), l, float(g("const")), g("E"), g("e"), g("G"), g("g"), [], g("lb"))
+
     # -- evaluation
     def objective(self, x):
         v = self.const + self.l @ x

@@ -11,7 +11,7 @@ active-set polish) -- the solver is NOT ECOS, the program is the reference's.
 
 Used by ``tests/golden/make_golden.py`` (fixture generation) and by the not-gpu tests
 that validate ``oracle/dune.py`` against the reference.  /root/reference does not
-exist on the GPU box: everything that calls this must skip when it is absent.
+exist on every machine: everything that calls this must skip when it is absent.
 """
 import os
 import sys

@@ -10,7 +10,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -27,7 +27,7 @@ def pytest_collection_modifyitems(config, items):
         raise pytest.UsageError(f"CUDA device present but {lib} is missing: run `python -m neupan_b200.build` (no CPU fallback)")
     if have_gpu:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200 box, -m gpu)")
+    skip = pytest.mark.skip(reason="needs a CUDA device (H100, -m gpu)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -25,17 +25,9 @@ def run_pan(pan, inp, cuda=True):
 
 
 def record(name: str, **values):
-    """Observed parity margins (pass fractions, max errors) of a -m gpu run: printed and appended to
-    gpurun_out/parity_observed.jsonl so that the thresholds in the tests can be ratcheted to what is observed."""
+    """Observed parity margins (pass fractions, max errors) of a -m gpu run, printed as one `OBSERVED` JSON line so that the
+    thresholds in the tests can be ratcheted to what is observed (pytest -s shows them)."""
     import json
-    import os
 
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     line = json.dumps(dict(test=name, **{k: (float(v) if isinstance(v, (int, float, np.floating, np.integer)) else v) for k, v in values.items()}))
     print("OBSERVED", line)
-    try:
-        os.makedirs(os.path.join(root, "gpurun_out"), exist_ok=True)
-        with open(os.path.join(root, "gpurun_out", "parity_observed.jsonl"), "a") as f:
-            f.write(line + "\n")
-    except OSError:
-        pass

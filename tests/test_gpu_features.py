@@ -11,7 +11,7 @@ from oracle import pan as op
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
-STOP_SAME_MIN = 0.9  # observed 12/12 on the B200 in both calls; fraction of envs that must stop at the oracle's iteration count (ratcheted from the observed value)
+STOP_SAME_MIN = 0.9  # observed 12/12 in both calls; fraction of envs that must stop at the oracle's iteration count (ratcheted from the observed value)
 
 
 def _cmp(got, ref, tol=TOL):
@@ -339,11 +339,9 @@ def test_generic_horizon_and_hinge_counts(T, M):
     assert (pan.status.cpu().numpy() == 0).all()
 
 
-@pytest.mark.parametrize("variant", ["1", "2", "4"])
-def test_tcgen05_kernel_variants_in_subprocess(variant):
-    """NB_DUNE_TC (read at process start) selects the other tcgen05 kernels: 1 = first single-slot kernel with scalar
-    math, 2 = two-slot kernel with the mbarrier hand-off instead of the block barrier, 4 = plain reciprocals instead of
-    the shared-reciprocal tanh.  Each must agree with the mma.sync kernel."""
+def test_plain_reciprocal_tanh_in_subprocess():
+    """NB_DUNE_TC=4 (read at process start) makes the warpgroup kernels use plain reciprocals instead of the shared-reciprocal
+    tanh.  The result must agree with the mma.sync kernel."""
     import os
     import subprocess
     import sys
@@ -360,5 +358,5 @@ def test_tcgen05_kernel_variants_in_subprocess(variant):
         "assert np.allclose(sa['points'].cpu().numpy(), sb['points'].cpu().numpy(), atol=1e-6)\n"
         "print('variant ok')\n")
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-c", code], cwd=root, env=dict(os.environ, NB_DUNE_TC=variant), capture_output=True, text=True, timeout=300)
+    r = subprocess.run([sys.executable, "-c", code], cwd=root, env=dict(os.environ, NB_DUNE_TC="4"), capture_output=True, text=True, timeout=300)
     assert r.returncode == 0 and "variant ok" in r.stdout, r.stdout + r.stderr

@@ -1,7 +1,7 @@
 """Differentiable NRMP (SURVEY 8f row 3; LON, example/LON/LON_corridor.py:94 `loss.backward()`): the gradients that
 ``loss.backward()`` delivers to NRMP.adjust_parameters through neupan_b200.PAN (native adjoint solves, nb_pan_backward) against
 the float64 oracle ``oracle/nrmp_grad.backward_chain`` -- itself validated against finite differences
-(tests/test_oracle_nrmp_grad.py).  Tolerance: 1e-3 of the gradient's scale, every environment (observed on the B200: <= 1.3e-4 on C2, <= 1e-5 on C1/C4/C5; the
+(tests/test_oracle_nrmp_grad.py).  Tolerance: 1e-3 of the gradient's scale, every environment (the
 oracle differentiates the exact active-set system, the kernel the barrier system with capped weights -- independent formulations)."""
 import numpy as np
 import pytest

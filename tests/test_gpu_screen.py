@@ -56,7 +56,7 @@ def test_screened_equals_full_kernel_bitwise(cname, scene):
 @pytest.mark.parametrize("screen_mma,skip_t0", [(0, 0), (0, 1), (1, 0)])
 @pytest.mark.parametrize("cname", ["C2", "C4", "C5"])
 def test_screen_shapes_and_step0_reuse_equal_full_kernel_bitwise(cname, screen_mma, skip_t0):
-    """The non-default combinations of NB_OPT_DUNE_SCREEN_MMA (screening pass on tcgen05 / mma.sync) and NB_OPT_DUNE_SKIP_T0 (step-0
+    """The non-default combinations of NB_OPT_DUNE_SCREEN_MMA (screening pass on wgmma / mma.sync) and NB_OPT_DUNE_SKIP_T0 (step-0
     items of PAN iterations k > 0 re-evaluated / kept): same bits as the full kernel, like the defaults in the tests above."""
     cfg = CONFIGS[cname]
     inp = make_inputs(cfg, B=12 if cname != "C5" else 6, scene="obstacles" if cname == "C2" else "annulus")

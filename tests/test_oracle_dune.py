@@ -1,6 +1,9 @@
-"""Pins oracle/dune.py (the CPU restatement of the DUNE half) against the reference's own code:
-golden vectors produced by that code (tests/golden/ref_dune_*.npz, made by make_golden.py) and,
-when /root/reference is present, the live import."""
+"""Pins oracle/dune.py (the CPU restatement of the DUNE half) against the reference's own code: golden vectors produced by
+that code (tests/golden/ref_dune_*.npz, made by make_golden.py; ref_dune_flow.npz, made by make_golden_dune_flow.py) and,
+where the reference checkout is present, a check that those vectors are current."""
+import importlib.util
+import os
+
 import numpy as np
 import pytest
 import torch
@@ -8,6 +11,10 @@ import torch
 from helpers import GOLDEN, weights_path
 from oracle import dune as od
 from oracle.refload import reference_available
+
+_spec = importlib.util.spec_from_file_location("make_golden_dune_flow", os.path.join(GOLDEN, "make_golden_dune_flow.py"))
+mgf = importlib.util.module_from_spec(_spec)
+_spec.loader.exec_module(mgf)
 
 
 @pytest.mark.parametrize("model", ["diff", "acker", "polygon"])
@@ -36,32 +43,28 @@ def test_dune_matches_reference_golden(model, case):
         assert torch.equal(d_ref, d_stb)
 
 
-@pytest.mark.skipif(not reference_available(), reason="/root/reference not present on this machine")
+def test_dune_matches_reference_point_flow_fixture():
+    """The reference's own point flow + DUNE (acker checkpoint, 200 moving points; tests/golden/make_golden_dune_flow.py) vs
+    oracle/dune.py on the same inputs: bit for bit."""
+    z = np.load(f"{GOLDEN}/ref_dune_flow.npz")
+    T, dt, n = mgf.T, mgf.DT, mgf.DUNE_MAX_NUM
+    nom_s, pts, vel = torch.from_numpy(z["nom_s"]), torch.from_numpy(z["points"]), torch.from_numpy(z["vel"])
+    p0, R, pl = od.point_flow(nom_s, pts, vel, T, dt, n)
+    mu, lam, sp, md, _ = od.dune_forward(od.load_weights(weights_path("acker")), torch.from_numpy(z["G"]).float(), torch.from_numpy(z["h"]).float(),
+                                         p0, R, pl, stable=False)
+    assert np.array_equal(torch.stack(mu).numpy(), z["mu"])
+    assert np.array_equal(torch.stack(lam).numpy(), z["lam"])
+    assert np.array_equal(torch.stack(sp).numpy(), z["sorted_points"])
+    assert np.float32(md) == z["min_distance"]
+
+
+@pytest.mark.skipif(not reference_available(), reason="needs the reference checkout")
 def test_dune_matches_live_reference():
-    import types
+    """The fixture above is current: the reference's code reproduces it, and the weights fixture equals its checkpoint."""
+    from oracle.refload import REFERENCE_ROOT
 
-    from oracle.refload import REFERENCE_ROOT, load_reference
-
-    load_reference()
-    from neupan.blocks import DUNE, PAN
-    from neupan.robot import robot as RefRobot
-
-    rr = RefRobot(10, 0.1, kinematics="acker", length=4.6, width=1.6, wheelbase=3)
-    ck = f"{REFERENCE_ROOT}/example/model/acker_robot_default/model_5000.pth"
-    dune = DUNE(10, ck, rr, 80, {})
-    fake = types.SimpleNamespace(T=10, dt=0.1, dune_max_num=80, printed=True, print_once=lambda *_: None)
-    fake.point_state_transform = types.MethodType(PAN.point_state_transform, fake)
-    g = torch.Generator().manual_seed(3)
-    nom_s = torch.randn(3, 11, generator=g); pts = 6 * torch.randn(2, 200, generator=g); vel = torch.randn(2, 200, generator=g)
-    pf, Rl, pl = PAN.generate_point_flow(fake, nom_s, pts, vel)
-    mu_r, lam_r, sp_r = dune(pf, Rl, pl)
-    w = od.load_weights(ck)
-    p0, R, pl2 = od.point_flow(nom_s, pts, vel, 10, 0.1, 80)
-    mu, lam, sp, md, _ = od.dune_forward(w, torch.from_numpy(rr.G).float(), torch.from_numpy(rr.h).float(), p0, R, pl2, stable=False)
-    assert all(torch.equal(a, b) for a, b in zip(mu, mu_r))
-    assert all(torch.equal(a, b) for a, b in zip(lam, lam_r))
-    assert all(torch.equal(a, b) for a, b in zip(sp, sp_r))
-    assert float(md) == float(dune.min_distance)
-    # weights fixture == checkpoint
-    wz = od.load_weights(weights_path("acker"))
+    fresh, z = mgf.reference_dune_flow(), np.load(f"{GOLDEN}/ref_dune_flow.npz")
+    for k, v in fresh.items():
+        assert np.array_equal(np.asarray(v), z[k]), k
+    w, wz = od.load_weights(f"{REFERENCE_ROOT}/example/model/acker_robot_default/model_5000.pth"), od.load_weights(weights_path("acker"))
     assert all(torch.equal(w[k], wz[k]) for k in w)

@@ -1,5 +1,5 @@
 """CPU check of the index logic of dune_screen_mma_kernel (csrc/dune_screen_mma_kernel.cuh), transcribed to numpy: the re-ordering of
-the tcgen05 operand image (K-major core matrices) into mma.sync m16n8k16 B fragments, the permuted fp32 vectors, the bias fragments,
+the wgmma operand image (K-major core matrices) into mma.sync m16n8k16 B fragments, the permuted fp32 vectors, the bias fragments,
 the accumulator -> A-fragment hand-over between layers (row slots, column pairs), the lane <-> point ownership and the transposing quad
 reduction -- one warp's 32 points through the whole screening network equal the plain matrix form of the same network.
 (The arithmetic itself -- HMMA, MUFU.TANH, the candidate logic -- is covered on the GPU by tests/test_gpu_screen.py.)"""

@@ -2,7 +2,7 @@
 
     # here (no GPU): build the default library plus variants that differ by -D flags on one translation unit
     python tools/ab_bench.py build  nrmp7:pan_api.cu:-DNB_SOME_FLAG=1  tcx:dune_tc.cu:-DNB_OTHER=2
-    # on the GPU box (inside a gpurun command): time the default and every built variant with bench.py
+    # on the GPU machine: time the default and every built variant with bench.py
     python tools/ab_bench.py run --steps 6 --warmup 3
 
 Variants are written to neupan_b200/lib/variants/<name>.so (git-ignored like every built .so; they travel with the snapshot)
