@@ -148,8 +148,14 @@ int nb_pan_set_iteration(nb_pan_t* pan, int32_t iter_num, float iter_threshold);
  * wgmma (csrc/dune_screen_kernel.cuh).  Same candidate contract, same final results (the refine / exact kernels are wgmma either way).
  * NB_OPT_DUNE_SKIP_T0 (with NB_OPT_DUNE_KERNEL = 4): 1 (default) = PAN iterations k > 0 of one nb_pan_forward do not re-evaluate the
  * step-0 items: nom_s[:, 0] is the fixed initial state (robot.py:234), so their inputs and results are those of iteration 0, which
- * stand in the selection buffers; 0 = evaluate them in every iteration (identical results). */
-enum { NB_OPT_DUNE_KERNEL = 1, NB_OPT_OVERLAP = 2, NB_OPT_NRMP_WARM = 3, NB_OPT_DIFFERENTIABLE = 4, NB_OPT_DUNE_SCREEN_MMA = 5, NB_OPT_DUNE_SKIP_T0 = 6 };
+ * stand in the selection buffers; 0 = evaluate them in every iteration (identical results).
+ * NB_OPT_DUNE_SCREEN_TABLE (with NB_OPT_DUNE_KERNEL = 4 and the mma.sync screen): 1 (default) = the screen looks each point's distance
+ * and error radius up in a table of the network's distance over the robot frame, built once per handle when both are first selected
+ * (csrc/dune_table_kernel.cuh; points outside the table take the network; a table less than twice as accurate as the handle's
+ * bound c_mu is not kept, and the network screens every point); 0 = every point runs the single-pass fp16 network.  Same final
+ * results, bit for bit. */
+enum { NB_OPT_DUNE_KERNEL = 1, NB_OPT_OVERLAP = 2, NB_OPT_NRMP_WARM = 3, NB_OPT_DIFFERENTIABLE = 4, NB_OPT_DUNE_SCREEN_MMA = 5, NB_OPT_DUNE_SKIP_T0 = 6,
+       NB_OPT_DUNE_SCREEN_TABLE = 7 };
 int nb_pan_set_option(nb_pan_t* pan, int32_t option, int32_t value);
 
 /* Replaces the backward pass of the reference's differentiable solve (CvxpyLayer, nrmp.py:144; used by LON,
@@ -181,6 +187,10 @@ int nb_pan_read_selection(nb_pan_t* pan, int32_t B, float* sel_mu, float* sel_la
  * (4 x the error measured at calibration, when NB_OPT_DUNE_KERNEL = 4 is first selected), [2] = that calibration measurement;
  * counts[0] = items sent to the exact kernel, counts[1] = candidates refined, counts[2] = items screened. */
 int nb_pan_read_screen_stats(nb_pan_t* pan, float* max_error_ratio, int32_t* counts, int32_t reset);
+/* The screen's distance table (all zero while none is built): info[0] = cell side h (m), [1] = half-width of the covered square (m),
+ * [2] = device bytes (0: built, but not kept: [4] > c_mu / 2), [3] = build time (ms, host clock around the synchronised build), [4] = the largest |table - network| /
+ * sum_e |G_e p - h_e| on the 4 x 4 sub-grid of every cell. */
+int nb_pan_read_screen_table(nb_pan_t* pan, float info[5]);
 
 /* Diagnostics of the last executed NRMP solve: interior point iterations per env (B) int32. */
 int nb_pan_read_diagnostics(nb_pan_t* pan, int32_t B, int32_t* ipm_iterations, void* stream);

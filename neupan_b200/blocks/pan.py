@@ -111,6 +111,9 @@ class PAN(torch.nn.Module):
         # keep the step-0 items of iteration 0 (1, default: nom_s[:, 0] is the fixed initial state) or re-evaluate them (0).  Same results.
         self.dune_screen_mma = int(kwargs.get("dune_screen_mma", 1))
         self.dune_skip_t0 = int(kwargs.get("dune_skip_t0", 1))
+        # with the mma.sync screen: look the screened distances up in the handle's distance table (1) or run the screening network on every
+        # point (0).  Same results.  None keeps the handle's default (1, or NB_SCREEN_TABLE=0/1).
+        self.dune_screen_table = kwargs.get("dune_screen_table")
         self._cap = (max(1, int(kwargs.get("max_envs", 1))), max(1, int(kwargs.get("max_points", max(1, dune_max_num)))))
         self._forward_id = 0
         self._differentiable = None  # last NB_OPT_DIFFERENTIABLE value pushed to the handle
@@ -167,6 +170,8 @@ class PAN(torch.nn.Module):
                                      None if G is None else G.ctypes.data, None if h is None else h.ctypes.data, C.byref(handle)))
         self._handle, self._cap = handle, (cap_b, cap_n)
         if not self.no_obs:
+            if self.dune_screen_table is not None:  # before the kernel: selecting the screening pipeline builds the table when it is on
+                _lib.check(lib.nb_pan_set_option(handle, _lib.OPT_DUNE_SCREEN_TABLE, int(self.dune_screen_table)))
             _lib.check(lib.nb_pan_set_option(handle, _lib.OPT_DUNE_KERNEL, int(self.dune_kernel)))
             _lib.check(lib.nb_pan_set_option(handle, _lib.OPT_DUNE_SCREEN_MMA, int(self.dune_screen_mma)))
             _lib.check(lib.nb_pan_set_option(handle, _lib.OPT_DUNE_SKIP_T0, int(self.dune_skip_t0)))
@@ -319,6 +324,14 @@ class PAN(torch.nn.Module):
         r, c = (C.c_float * 3)(), (C.c_int32 * 3)()
         _lib.check(_lib.load().nb_pan_read_screen_stats(self._handle, C.byref(r), C.byref(c), int(reset)))
         return dict(max_error_ratio=float(r[0]), c_mu=float(r[1]), calibration_ratio=float(r[2]), exact_items=int(c[0]), candidates=int(c[1]), screened_items=int(c[2]))
+
+    def screen_table(self):
+        """The screen's distance table: dict(h, half, bytes, build_ms, max_error_ratio); all zero while none is built."""
+        if self._handle is None or self.no_obs:
+            return None
+        r = (C.c_float * 5)()
+        _lib.check(_lib.load().nb_pan_read_screen_table(self._handle, C.byref(r)))
+        return dict(h=float(r[0]), half=float(r[1]), bytes=int(r[2]), build_ms=float(r[3]), max_error_ratio=float(r[4]))
 
     def read_selection(self):
         """The M closest points per (env, step) of the last executed iteration, ascending distance:

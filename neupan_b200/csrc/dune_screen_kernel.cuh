@@ -132,7 +132,7 @@ __global__ void __launch_bounds__(128) dune_screen_kernel(const DuneParams prm, 
   __shared__ uint32_t tau_s;
   __shared__ int cnt_s;
   __shared__ int list_s[kCandMax];
-  __shared__ float ldt_s[kCandMax];
+  __shared__ float ldt_s[kCandMax], lrad_s[kCandMax];
   __shared__ float2 xy_s[2][128];  // robot-frame coordinates of the points in flight (stage 0 -> head)
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -352,7 +352,7 @@ __global__ void __launch_bounds__(128) dune_screen_kernel(const DuneParams prm, 
       auto take = [&](uint32_t k, float lb, float dt, int j) {
         if (k != 0xFFFFFFFFu && orderable(lb) <= tau) {
           const int pos = atomicAdd(&cnt_s, 1);
-          if (pos < kCandMax) { list_s[pos] = tid + 128 * j; ldt_s[pos] = dt; }
+          if (pos < kCandMax) { list_s[pos] = tid + 128 * j; ldt_s[pos] = dt; lrad_s[pos] = dt - lb; }
         }
       };
       take(k0, l0, d0, 0); take(k1, l1, d1, 1); take(k2, l2, d2, 2); take(k3, l3, d3, 3);
@@ -360,14 +360,14 @@ __global__ void __launch_bounds__(128) dune_screen_kernel(const DuneParams prm, 
       for (int i = tid; i < n; i += 128) {
         if (orderable(lbv[i]) <= tau) {
           const int pos = atomicAdd(&cnt_s, 1);
-          if (pos < kCandMax) { list_s[pos] = i; ldt_s[pos] = dtv[i]; }
+          if (pos < kCandMax) { list_s[pos] = i; ldt_s[pos] = dtv[i]; lrad_s[pos] = dtv[i] - lbv[i]; }
         }
       }
     }
     __syncthreads();
     const int nc = cnt_s;
     if (nc <= kCandMax) {
-      if (tid < nc) { out_idx[tid] = list_s[tid]; out_dt[tid] = ldt_s[tid]; }
+      if (tid < nc) { out_idx[tid] = list_s[tid]; out_dt[tid] = ldt_s[tid]; prm.cand_rad[(size_t)item * kCandMax + tid] = lrad_s[tid]; }
       if (tid == 0) {
         prm.cand_cnt[item] = nc;
         tc::refine_append(prm, item, nc);
@@ -491,7 +491,7 @@ __global__ void __launch_bounds__(128) dune_refine_kernel(const DuneParams prm, 
         const bool screened = valid && dt == dt;
         const float err = screened ? fabsf(dt - d) : 0.f;
         float ratio = screened ? err / fmaxf(sa, 1e-6f) : 0.f;
-        const bool viol = screened && !prm.calibrate && err > 0.5f * fmaf(prm.c_mu, sa, 1e-4f);
+        const bool viol = screened && !prm.calibrate && err > 0.5f * prm.cand_rad[(size_t)it * kCandMax + myli[sl]];
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) ratio = fmaxf(ratio, __shfl_xor_sync(0xffffffffu, ratio, o));
         if (lane == 0 && ratio > 0.f) atomicMax(&prm.screen_stats[0], __float_as_uint(ratio));

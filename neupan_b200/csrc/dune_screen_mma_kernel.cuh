@@ -176,7 +176,7 @@ __global__ void __launch_bounds__(128, kP <= 4 ? NB_SMMA_BLOCKS : 4) dune_screen
   uint32_t* c32 = reinterpret_cast<uint32_t*>(raw + (size_t)4 * prm.N);
   __shared__ int cnt_s[2];
   __shared__ int list_s[kCandMax];
-  __shared__ float ldt_s[kCandMax];
+  __shared__ float ldt_s[kCandMax], lrad_s[kCandMax];
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, tq = lane & 3;
   // ---- operand staging: the screen image of dune_screen_kernel (K-major wgmma layout, hi halves) re-ordered into mma.sync B fragments
@@ -298,53 +298,62 @@ __global__ void __launch_bounds__(128, kP <= 4 ? NB_SMMA_BLOCKS : 4) dune_screen
         x0 = fmaf(fr.cs, dx, fr.sn * dy);
         y0 = fmaf(fr.cs, dy, -(fr.sn * dx));
       }
-      float xr[4], yr[4];
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        xr[r] = __shfl_sync(0xffffffffu, x0, (lane & ~3) | r);
-        yr[r] = __shfl_sync(0xffffffffu, y0, (lane & ~3) | r);
-      }
-      sm::f2 acc[4][4];
-      uint32_t a[2][2][4];
-      {  // layer 0 (2 -> 32) on the FMA pipe, directly in accumulator layout
-        const ulonglong2 wx01 = *reinterpret_cast<const ulonglong2*>(vq + 32 * sm::V_W0X), wx23 = *reinterpret_cast<const ulonglong2*>(vq + 32 * sm::V_W0X + 4);
-        const ulonglong2 wy01 = *reinterpret_cast<const ulonglong2*>(vq + 32 * sm::V_W0Y), wy23 = *reinterpret_cast<const ulonglong2*>(vq + 32 * sm::V_W0Y + 4);
-        const ulonglong2 b01 = *reinterpret_cast<const ulonglong2*>(vq + 32 * sm::V_B0), b23 = *reinterpret_cast<const ulonglong2*>(vq + 32 * sm::V_B0 + 4);
-        const sm::f2 wx[4] = {wx01.x, wx01.y, wx23.x, wx23.y}, wy[4] = {wy01.x, wy01.y, wy23.x, wy23.y}, bb[4] = {b01.x, b01.y, b23.x, b23.y};
+      // the distance table where it covers the point (rows beyond n need nothing); the warp runs the network on its tile when any
+      // of its points lies outside the table, or when there is no table
+      float d = 0.f, eps = 0.f;
+      const bool hit = prm.tab_cell != nullptr && (i >= n || table_lookup(prm, x0, y0, d, eps));
+      if (!__all_sync(0xffffffffu, hit)) {
+        float xr[4], yr[4];
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
-          const sm::f2 x2 = tc::pk(xr[r], xr[r]), y2 = tc::pk(yr[r], yr[r]);
+          xr[r] = __shfl_sync(0xffffffffu, x0, (lane & ~3) | r);
+          yr[r] = __shfl_sync(0xffffffffu, y0, (lane & ~3) | r);
+        }
+        sm::f2 acc[4][4];
+        uint32_t a[2][2][4];
+        {  // layer 0 (2 -> 32) on the FMA pipe, directly in accumulator layout
+          const ulonglong2 wx01 = *reinterpret_cast<const ulonglong2*>(vq + 32 * sm::V_W0X), wx23 = *reinterpret_cast<const ulonglong2*>(vq + 32 * sm::V_W0X + 4);
+          const ulonglong2 wy01 = *reinterpret_cast<const ulonglong2*>(vq + 32 * sm::V_W0Y), wy23 = *reinterpret_cast<const ulonglong2*>(vq + 32 * sm::V_W0Y + 4);
+          const ulonglong2 b01 = *reinterpret_cast<const ulonglong2*>(vq + 32 * sm::V_B0), b23 = *reinterpret_cast<const ulonglong2*>(vq + 32 * sm::V_B0 + 4);
+          const sm::f2 wx[4] = {wx01.x, wx01.y, wx23.x, wx23.y}, wy[4] = {wy01.x, wy01.y, wy23.x, wy23.y}, bb[4] = {b01.x, b01.y, b23.x, b23.y};
 #pragma unroll
-          for (int j = 0; j < 4; ++j) acc[r][j] = tc::fma2(wy[j], y2, tc::fma2(wx[j], x2, bb[j]));
+          for (int r = 0; r < 4; ++r) {
+            const sm::f2 x2 = tc::pk(xr[r], xr[r]), y2 = tc::pk(yr[r], yr[r]);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[r][j] = tc::fma2(wy[j], y2, tc::fma2(wx[j], x2, bb[j]));
+          }
+        }
+        sm::ln_tanh_frag(acc, vq + 32 * sm::V_G1, vq + 32 * sm::V_BE1, lane, a);
+        sm::dense_frag<4>(wl + 0 * 128, bqq + 16 * 0, a, acc);
+        sm::relu_frag(acc, a);
+        sm::dense_frag<4>(wl + 1 * 128, bqq + 16 * 1, a, acc);
+        sm::ln_tanh_frag(acc, vq + 32 * sm::V_G6, vq + 32 * sm::V_BE6, lane, a);
+        sm::dense_frag<4>(wl + 2 * 128, bqq + 16 * 2, a, acc);
+        sm::relu_frag(acc, a);
+        sm::dense_frag<4>(wl + 3 * 128, bqq + 16 * 3, a, acc);
+        sm::ln_tanh_frag(acc, vq + 32 * sm::V_G11, vq + 32 * sm::V_BE11, lane, a);
+        sm::f2 mu[4][1];
+        sm::dense_frag<1>(wl + 4 * 128, bqq + 16 * 4, a, mu);
+
+        // head: d~ = relu(mu)^T (G p0 - h): partial over the lane's two channels for each row slot, transposing quad reduction
+        float dp[4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          float m0, m1;
+          tc::upk(mu[r][0], m0, m1);
+          const float ge0 = fmaf(gy0, yr[r], gx0 * xr[r]) - h0, ge1 = fmaf(gy1, yr[r], gx1 * xr[r]) - h1;
+          dp[r] = fmaf(fmaxf(m1, 0.f), ge1, fmaxf(m0, 0.f) * ge0);
+        }
+        const float dn = sm::quad_transpose_sum(dp, tq);  // the lane's own point
+        if (!hit) {
+          float sa = 0.f;
+#pragma unroll
+          for (int e = 0; e < kMaxEdges; ++e)
+            if (e < E) sa += fabsf(fmaf(prm.geo.G[e][1], y0, prm.geo.G[e][0] * x0) - prm.geo.h[e]);
+          d = dn;
+          eps = fmaf(prm.c_mu, sa, 1e-4f);
         }
       }
-      sm::ln_tanh_frag(acc, vq + 32 * sm::V_G1, vq + 32 * sm::V_BE1, lane, a);
-      sm::dense_frag<4>(wl + 0 * 128, bqq + 16 * 0, a, acc);
-      sm::relu_frag(acc, a);
-      sm::dense_frag<4>(wl + 1 * 128, bqq + 16 * 1, a, acc);
-      sm::ln_tanh_frag(acc, vq + 32 * sm::V_G6, vq + 32 * sm::V_BE6, lane, a);
-      sm::dense_frag<4>(wl + 2 * 128, bqq + 16 * 2, a, acc);
-      sm::relu_frag(acc, a);
-      sm::dense_frag<4>(wl + 3 * 128, bqq + 16 * 3, a, acc);
-      sm::ln_tanh_frag(acc, vq + 32 * sm::V_G11, vq + 32 * sm::V_BE11, lane, a);
-      sm::f2 mu[4][1];
-      sm::dense_frag<1>(wl + 4 * 128, bqq + 16 * 4, a, mu);
-
-      // head: d~ = relu(mu)^T (G p0 - h): partial over the lane's two channels for each row slot, transposing quad reduction
-      float dp[4];
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        float m0, m1;
-        tc::upk(mu[r][0], m0, m1);
-        const float ge0 = fmaf(gy0, yr[r], gx0 * xr[r]) - h0, ge1 = fmaf(gy1, yr[r], gx1 * xr[r]) - h1;
-        dp[r] = fmaf(fmaxf(m1, 0.f), ge1, fmaxf(m0, 0.f) * ge0);
-      }
-      const float d = sm::quad_transpose_sum(dp, tq);  // the lane's own point
-      float sa = 0.f;
-#pragma unroll
-      for (int e = 0; e < kMaxEdges; ++e)
-        if (e < E) sa += fabsf(fmaf(prm.geo.G[e][1], y0, prm.geo.G[e][0] * x0) - prm.geo.h[e]);
-      const float eps = fmaf(prm.c_mu, sa, 1e-4f);
 #pragma unroll
       for (int j = kP - 1; j > 0; --j) { kk[j] = kk[j - 1]; ll[j] = ll[j - 1]; dd[j] = dd[j - 1]; }
       kk[0] = i < n ? unique_key(orderable(d + eps), i) : 0xFFFFFFFFu;
@@ -396,7 +405,7 @@ __global__ void __launch_bounds__(128, kP <= 4 ? NB_SMMA_BLOCKS : 4) dune_screen
     auto take = [&](uint32_t k, float lb, float dt) {
       if (k != 0xFFFFFFFFu && orderable(lb) <= tau) {
         const int pos = atomicAdd(&cnt_s[par], 1);
-        if (pos < kCandMax) { list_s[pos] = (int)(k & kIdxMask); ldt_s[pos] = dt; }
+        if (pos < kCandMax) { list_s[pos] = (int)(k & kIdxMask); ldt_s[pos] = dt; lrad_s[pos] = dt - lb; }
       }
     };
 #pragma unroll
@@ -404,7 +413,7 @@ __global__ void __launch_bounds__(128, kP <= 4 ? NB_SMMA_BLOCKS : 4) dune_screen
     __syncthreads();
     const int nc = cnt_s[par];
     if (nc <= kCandMax) {
-      if (tid < nc) { out_idx[tid] = list_s[tid]; out_dt[tid] = ldt_s[tid]; }
+      if (tid < nc) { out_idx[tid] = list_s[tid]; out_dt[tid] = ldt_s[tid]; prm.cand_rad[(size_t)item * kCandMax + tid] = lrad_s[tid]; }
       if (tid == 0) {
         prm.cand_cnt[item] = nc;
         tc::refine_append(prm, item, nc);

@@ -132,7 +132,7 @@ int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const
   if (variant == 4) {
     // screening: (1) interval pass over all points, (2) exact evaluation of the candidates, (3) the exact kernel for the items the
     // screen could not narrow down to 32 candidates (below, with only_flagged)
-    if (!d_screen_image || !prm.cand_idx || !prm.cand_cnt || !prm.cand_dt || !prm.screen_stats || !prm.flag_list || !prm.flag_count || !prm.refine_list) {
+    if (!d_screen_image || !prm.cand_idx || !prm.cand_cnt || !prm.cand_dt || !prm.cand_rad || !prm.screen_stats || !prm.flag_list || !prm.flag_count || !prm.refine_list) {
       snprintf(err, errlen, "screening buffers are not allocated");
       return -1;
     }

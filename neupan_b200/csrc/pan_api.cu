@@ -6,6 +6,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
+#include <chrono>
 #include <cstring>
 #include <new>
 
@@ -15,6 +16,7 @@
 #include "scan_kernel.cuh"
 #include "ipath_kernel.cuh"
 #include "dune_train_kernel.cuh"
+#include "dune_table_kernel.cuh"
 
 #include <vector>
 
@@ -90,12 +92,19 @@ struct nb_pan {
   int tc_flags = 0;                     // build_tc_image(): bit 0 = bounded tanh arguments
   unsigned char* d_tc_screen = nullptr; // operand image of the screening network (NB_OPT_DUNE_KERNEL = 4)
   int32_t *cand_idx = nullptr, *cand_cnt = nullptr, *flag_list = nullptr, *flag_count = nullptr, *refine_list = nullptr;
-  float* cand_dt = nullptr;
+  float *cand_dt = nullptr, *cand_rad = nullptr;
   unsigned* screen_stats = nullptr;
   float c_mu = 0.012f;                  // bound on the screening network's |mu~ - mu|: set by calibrate_screen() to 4 x the largest error
                                         // measured for THIS checkpoint and polygon (NB_SCREEN_CMU overrides; DESIGN.md 3.1)
   bool screen_calibrated = false;
   float screen_cal_ratio = 0.f;
+  bool cmu_override = false;            // NB_SCREEN_CMU is set: every point gets the radius c_mu sum_e |G_e p0 - h_e| + 1e-4 (network screen)
+  int screen_table = 1;                 // NB_OPT_DUNE_SCREEN_TABLE: the mma.sync screen looks distances up in the table below
+  float4* tab_cell = nullptr;           // distance table (dune_table_kernel.cuh), built once per handle by build_screen_table()
+  float* tab_rad = nullptr;
+  int tab_n = 0;
+  float tab_h = 0.f, tab_half = 0.f, tab_ratio = 0.f, tab_ms = 0.f;
+  bool tab_built = false;               // built (and kept, or freed as not accurate enough: tab_cell == nullptr)
   int dune_variant = 2;              // NB_OPT_DUNE_KERNEL: 0 = FP32 FFMA, 1 = mma.sync tensor-core, 2 = wgmma tensor-core kernel
   int overlap = 1;                   // NB_OPT_OVERLAP: number of env sub-batches pipelined on internal streams
   cudaStream_t streams[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -303,7 +312,7 @@ int calibrate_screen(nb_pan* p, cudaStream_t st) {
     prm.weights = p->d_weights; prm.nom_s = d_ns; prm.points = d_pts;
     prm.sel_mu = p->sel_mu; prm.sel_lam = p->sel_lam; prm.sel_pts = p->sel_pts; prm.sel_dist = p->sel_dist; prm.sel_count = p->sel_count; prm.min_dist = d_md;
     prm.B = Bc; prm.N = N; prm.T = c.receding; prm.M = c.nrmp_max_num; prm.dt = (float)c.step_time; prm.geo = p->geo;
-    prm.cand_idx = p->cand_idx; prm.cand_cnt = p->cand_cnt; prm.cand_dt = p->cand_dt; prm.screen_stats = p->screen_stats; prm.c_mu = p->c_mu;
+    prm.cand_idx = p->cand_idx; prm.cand_cnt = p->cand_cnt; prm.cand_dt = p->cand_dt; prm.cand_rad = p->cand_rad; prm.screen_stats = p->screen_stats; prm.c_mu = p->c_mu;
     prm.flag_list = p->flag_list; prm.flag_count = p->flag_count; prm.refine_list = p->refine_list; prm.calibrate = 1;
     for (int shape = 0; shape < 2 && rc == NB_OK; ++shape) {  // both screening kernels (wgmma / mma.sync): the bound holds whichever option is set later
       prm.screen_mma = shape;
@@ -326,6 +335,63 @@ int calibrate_screen(nb_pan* p, cudaStream_t st) {
   cudaMemcpy(p->screen_stats, saved, sizeof(saved), cudaMemcpyHostToDevice);
   cudaFree(d_pts); cudaFree(d_ns); cudaFree(d_md);
   return rc;
+}
+
+// The distance table of the mma.sync screen (dune_table_kernel.cuh): cells of h metres over [-half, half]^2 of the robot frame,
+// rounded up to whole cells.  The defaults h = 0.04, half = 16.384 cover clouds of up to 10 m around the start, a robot displacement of
+// up to ~4 m and a point flow of up to 1.5 m over the horizon in 13.4 MB; points outside take the screening network.
+// NB_SCREEN_TABLE_GRID="h,half" (metres) overrides both.  The table is kept only where it is at least twice as accurate as the
+// handle's screening bound: largest |table - network| / sum_e |G_e p - h_e| on the fine samples <= c_mu / 2, so that the statistic
+// nb_pan_read_screen_stats compares with c_mu keeps its margin.  Otherwise (at 4 cm: the acker and polygon checkpoints, whose ReLU
+// kinks near the polygon give 7e-3 and 1e-2) it is freed and the handle keeps the network screen.
+int build_screen_table(nb_pan* p) {
+  float h = 0.04f, half = 16.384f;
+  if (const char* e = getenv("NB_SCREEN_TABLE_GRID"))
+    if (sscanf(e, "%f,%f", &h, &half) != 2 || !(h >= 1e-3f) || !(half > 0.f) || !(half < 1e3f))
+      return fail(NB_ERR_INVALID, "NB_SCREEN_TABLE_GRID takes \"h,half\" in metres, h >= 0.001 (got \"%s\")", e);
+  const long long n = (long long)ceilf(2.f * half / h);
+  if (n > 4096) return fail(NB_ERR_INVALID, "NB_SCREEN_TABLE_GRID: %lld cells per side (at most 4096)", n);
+  half = 0.5f * (float)n * h;
+  const long long m = nb::kTableSub * n + 1;
+  const auto t0 = std::chrono::steady_clock::now();
+  NB_CUDA(cudaDeviceSynchronize());
+  float* fine = nullptr;
+  unsigned* d_ratio = nullptr;
+  NB_CUDA(dalloc(&fine, (size_t)(m * m)));
+  NB_CUDA(dalloc(&d_ratio, (size_t)1));
+  if (!p->tab_cell) NB_CUDA(dalloc(&p->tab_cell, (size_t)(n * n)));
+  if (!p->tab_rad) NB_CUDA(dalloc(&p->tab_rad, (size_t)(n * n)));
+  NB_CUDA(cudaMemset(d_ratio, 0, sizeof(unsigned)));
+  const float hs = h / nb::kTableSub;
+  nb::dune_table_sample_kernel<<<p->sm_count * 16, 128>>>(p->d_weights, p->geo, (int)m, half, hs, fine);
+  nb::dune_table_cell_kernel<<<p->sm_count * 8, 128>>>(fine, (int)n, half, hs, p->geo, p->tab_cell, p->tab_rad, d_ratio);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  unsigned r = 0;
+  if (e == cudaSuccess) e = cudaMemcpy(&r, d_ratio, sizeof(r), cudaMemcpyDeviceToHost);
+  cudaFree(fine);
+  cudaFree(d_ratio);
+  if (e != cudaSuccess) return fail(NB_ERR_CUDA, "build_screen_table: %s", cudaGetErrorString(e));
+  memcpy(&p->tab_ratio, &r, 4);
+  p->tab_n = (int)n; p->tab_h = h; p->tab_half = half; p->tab_built = true;
+  if (!(2.f * p->tab_ratio <= p->c_mu)) {
+    cudaFree(p->tab_cell);
+    cudaFree(p->tab_rad);
+    p->tab_cell = nullptr;
+    p->tab_rad = nullptr;
+  }
+  p->tab_ms = (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  return NB_OK;
+}
+
+// the table goes to the screen only where it is meant to be used; without it every point runs the screening network
+void set_screen_table(const nb_pan* p, nb::DuneParams& prm) {
+  const bool on = p->screen_table && !p->cmu_override && p->tab_cell;
+  prm.tab_cell = on ? p->tab_cell : nullptr;
+  prm.tab_rad = p->tab_rad;
+  prm.tab_n = p->tab_n;
+  prm.tab_half = p->tab_half;
+  prm.tab_inv_h = on ? 1.f / p->tab_h : 0.f;
 }
 
 __global__ void init_run_kernel(int B, int32_t* active, int32_t* iters, int32_t* status, float* min_dist, int32_t* sel_count, int32_t* warm_valid) {
@@ -407,13 +473,14 @@ int nb_pan_create(const nb_pan_config* cfg, const float* weights, int64_t n_weig
     NB_CUDA(cudaMemcpy(p->d_tc_screen, image.data(), image.size(), cudaMemcpyHostToDevice));
     NB_CUDA(dalloc(&p->cand_idx, (size_t)cfg->max_envs * (cfg->receding + 1) * nb::kCandMax));
     NB_CUDA(dalloc(&p->cand_dt, (size_t)cfg->max_envs * (cfg->receding + 1) * nb::kCandMax));
+    NB_CUDA(dalloc(&p->cand_rad, (size_t)cfg->max_envs * (cfg->receding + 1) * nb::kCandMax));
     NB_CUDA(dalloc(&p->cand_cnt, (size_t)cfg->max_envs * (cfg->receding + 1)));
     NB_CUDA(dalloc(&p->flag_list, (size_t)cfg->max_envs * (cfg->receding + 1)));
     NB_CUDA(dalloc(&p->flag_count, (size_t)32));  // 4 words per internal stream: flagged items, the two refine list lengths
     NB_CUDA(dalloc(&p->refine_list, (size_t)2 * cfg->max_envs * (cfg->receding + 1)));
     NB_CUDA(dalloc(&p->screen_stats, (size_t)4));
     NB_CUDA(cudaMemset(p->screen_stats, 0, 4 * sizeof(unsigned)));
-    if (const char* e = getenv("NB_SCREEN_CMU")) p->c_mu = (float)atof(e);
+    if (const char* e = getenv("NB_SCREEN_CMU")) { p->c_mu = (float)atof(e); p->cmu_override = true; }
   }
   NB_CUDA(dalloc(&p->sel_mu, B * T1 * M * E));
   NB_CUDA(dalloc(&p->sel_lam, B * T1 * M * 2));
@@ -440,6 +507,7 @@ int nb_pan_create(const nb_pan_config* cfg, const float* weights, int64_t n_weig
   if (const char* e = getenv("NB_H2D_CHUNKS")) { p->h2d_chunks = atoi(e); if (p->h2d_chunks < 1) p->h2d_chunks = 1; if (p->h2d_chunks > nb_pan::kMaxChunks) p->h2d_chunks = nb_pan::kMaxChunks; }
   if (const char* e = getenv("NB_DUNE_SKIP_T0")) p->dune_skip_t0 = atoi(e) != 0;  // developer overrides of the option defaults
   if (const char* e = getenv("NB_SCREEN_MMA")) p->screen_mma = atoi(e) != 0;
+  if (const char* e = getenv("NB_SCREEN_TABLE")) p->screen_table = atoi(e) != 0;
   if (const char* e = getenv("NB_NRMP_RESTART_IT")) p->warm_check_it = atoi(e);
   if (const char* e = getenv("NB_NRMP_RESTART_GAP")) p->warm_check_gap = atof(e);
   NB_CUDA(cudaMemset(p->warm_valid, 0, B * sizeof(int32_t)));
@@ -469,7 +537,7 @@ int nb_pan_destroy(nb_pan_t* p) {
     if (e) cudaEventDestroy(e);
   void* bufs[] = {p->d_tc_image, p->d_image, p->d_weights, p->sel_mu, p->sel_lam, p->sel_pts, p->sel_dist, p->sel_count, p->prev_s, p->prev_u, p->prev_mu,
                   p->prev_lam, p->prev_count, p->prev_valid, p->active, p->iters, p->status, p->ipm_it, p->min_dist, p->h_in, p->h_out, p->h_np, p->h_io,
-                  p->d_tc_screen, p->cand_idx, p->cand_cnt, p->cand_dt, p->screen_stats, p->flag_list, p->flag_count, p->refine_list, p->warm, p->warm_valid, p->work_counters, p->adj_rec, p->adj_gs, p->adj_gu, p->adj_gd, p->adj_gtheta, p->adj_valid};
+                  p->d_tc_screen, p->cand_idx, p->cand_cnt, p->cand_dt, p->cand_rad, p->tab_cell, p->tab_rad, p->screen_stats, p->flag_list, p->flag_count, p->refine_list, p->warm, p->warm_valid, p->work_counters, p->adj_rec, p->adj_gs, p->adj_gu, p->adj_gd, p->adj_gtheta, p->adj_valid};
   for (void* b : bufs)
     if (b) cudaFree(b);
   delete p;
@@ -495,9 +563,20 @@ int nb_pan_set_option(nb_pan_t* p, int32_t option, int32_t value) {
     if (value < 0 || value > 4)
       return fail(NB_ERR_INVALID, "NB_OPT_DUNE_KERNEL takes 0 (fp32 ffma), 1 (mma.sync), 2 (wgmma), 3 (wgmma, two threads per point) or 4 (wgmma with screening)");
     p->dune_variant = value;
-    if (value == 4 && !p->screen_calibrated && p->d_tc_screen) {
+    if (value == 4 && p->d_tc_screen) {
       NB_CUDA(cudaSetDevice(p->cfg.device));
-      return calibrate_screen(p, nullptr);
+      if (!p->screen_calibrated)
+        if (int rc = calibrate_screen(p, nullptr)) return rc;
+      if (p->screen_table && !p->tab_built) return build_screen_table(p);
+    }
+    return NB_OK;
+  }
+  if (option == NB_OPT_DUNE_SCREEN_TABLE) {
+    if (value < 0 || value > 1) return fail(NB_ERR_INVALID, "NB_OPT_DUNE_SCREEN_TABLE takes 0 or 1");
+    p->screen_table = value;
+    if (value == 1 && p->dune_variant == 4 && p->d_tc_screen && !p->tab_built) {
+      NB_CUDA(cudaSetDevice(p->cfg.device));
+      return build_screen_table(p);
     }
     return NB_OK;
   }
@@ -559,6 +638,8 @@ int nb_dune_forward(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, const
   prm.B = B; prm.N = N; prm.T = p->cfg.receding; prm.M = p->cfg.nrmp_max_num; prm.dt = (float)p->cfg.step_time; prm.geo = p->geo;
   prm.cand_idx = p->cand_idx; prm.cand_cnt = p->cand_cnt; prm.cand_dt = p->cand_dt; prm.screen_stats = p->screen_stats; prm.c_mu = p->c_mu;
   prm.flag_list = p->flag_list; prm.flag_count = p->flag_count; prm.refine_list = p->refine_list; prm.screen_mma = p->screen_mma;
+  prm.cand_rad = p->cand_rad;
+  set_screen_table(p, prm);
   return launch_dune(p, prm, (cudaStream_t)stream);
 }
 
@@ -648,6 +729,8 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
         d.cand_cnt = p->cand_cnt + (size_t)lo * T1s; d.screen_stats = p->screen_stats; d.c_mu = p->c_mu;
         d.flag_list = p->flag_list + (size_t)lo * T1s; d.flag_count = p->flag_count + 4 * counter_slot; d.refine_list = p->refine_list + (size_t)2 * lo * T1s;
         d.screen_mma = p->screen_mma;
+        d.cand_rad = p->cand_rad + (size_t)lo * T1s * nb::kCandMax;
+        set_screen_table(p, d);
         d.skip_t0 = (k > 0 && p->dune_skip_t0) ? 1 : 0;  // the step-0 items of iteration 0 stand (DuneParams::skip_t0)
         if (k == 0 && plan && plan->n > 1) {
           // the first DUNE pass of this range chunk by chunk, each as soon as its points have landed: the upload of chunk c+1 overlaps the
@@ -667,7 +750,7 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
             dc.min_dist = d.min_dist + off;
             dc.B = chi - clo;
             dc.cand_idx = d.cand_idx + off * T1s * nb::kCandMax; dc.cand_dt = d.cand_dt + off * T1s * nb::kCandMax;
-            dc.cand_cnt = d.cand_cnt + off * T1s;
+            dc.cand_cnt = d.cand_cnt + off * T1s; dc.cand_rad = d.cand_rad + off * T1s * nb::kCandMax;
             dc.flag_list = d.flag_list + off * T1s; dc.refine_list = d.refine_list + (size_t)2 * off * T1s;
             if (int rc = launch_dune(p, dc, s, dune_cta_limit)) return rc;
           }
@@ -818,6 +901,16 @@ int nb_pan_read_screen_stats(nb_pan_t* p, float* max_error_ratio, int32_t* count
   max_error_ratio[2] = p->screen_cal_ratio;
   counts[0] = (int32_t)h[1]; counts[1] = (int32_t)h[2]; counts[2] = (int32_t)h[3];
   if (reset) NB_CUDA(cudaMemset(p->screen_stats, 0, sizeof(h)));
+  return NB_OK;
+}
+
+int nb_pan_read_screen_table(nb_pan_t* p, float* info) {
+  if (!p || !info) return fail(NB_ERR_INVALID, "nb_pan_read_screen_table: null argument");
+  info[0] = p->tab_h;
+  info[1] = p->tab_half;
+  info[2] = p->tab_cell ? (float)((double)p->tab_n * p->tab_n * (sizeof(float4) + sizeof(float))) : 0.f;
+  info[3] = p->tab_ms;
+  info[4] = p->tab_ratio;
   return NB_OK;
 }
 
