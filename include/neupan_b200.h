@@ -283,6 +283,70 @@ int nb_ipath_reset_async(nb_ipath_t* ip, void* stream);   /* ordered with the st
 int nb_ipath_read_state(nb_ipath_t* ip, int32_t B, int32_t* curve_index, int32_t* point_index, int32_t* arrive_flag,
                         double* points_host, void* stream);
 
+/* ---- batched 2-D world: lidar scans, moving obstacles and collisions for closed-loop runs ------------------------------ */
+
+/* What the reference's simulator (IR-SIM, example/run_exp.py:27-56, configured by example/<scenario>/<kin>/env.yaml) provides around
+ * the planner, for B environments on the device.  The robot is a convex polygon (the planner's robot.vertices, neupan_b200/robot.py);
+ * the lidar is the `lidar2d` sensor without noise. */
+typedef struct nb_world_config {
+  int32_t kinematics;              /* NB_KIN_*: diff (v, omega), acker (v, steering phi), omni (vx, vy)                           */
+  int32_t num_beams;               /* R >= 1                                                                                    */
+  int32_t max_envs;
+  int32_t device;
+  int32_t robot_num_vertices;      /* 3..8 */
+  int32_t reserved_;
+  double step_time;                /* dt of one nb_world_step */
+  double wheelbase;                /* robot.L, acker only */
+  double angle_min, angle_max;     /* beam i sits at linspace(angle_min, angle_max, R)[i] in the sensor frame                   */
+  double range_max;                /* a beam with no crossing closer than range_max reports range_max                          */
+  double scan_offset[3];           /* sensor pose in the robot frame                                                            */
+  double robot_vertices[16];       /* x0, y0, x1, y1, ...: the convex robot polygon in its own frame                            */
+} nb_world_config;
+
+typedef struct nb_world nb_world_t;  /* opaque; owns the scenes, robot states and flags of B environments */
+
+int nb_world_create(const nb_world_config* cfg, nb_world_t** out);
+int nb_world_destroy(nb_world_t* w);
+
+/* The scene of every environment (the obstacle, robot and goal sections of env.yaml), HOST arrays, ragged like nb_ipath_set_paths:
+ *   obs_begin (B+1) int32   offsets into the obstacle rows; at most 256 obstacles and 2048 polygon edges per environment
+ *   obstacles (O,5) float64 rows [cx, cy, vx, vy, radius]: centre, constant world-frame velocity, circle radius (> 0; unused for
+ *                           polygons).  An obstacle whose velocity component is non-zero must start inside its rectangle, and
+ *                           |v| * step_time must be smaller than the rectangle's extent on that axis.
+ *   vert_begin (O+1) int32  offsets into vertices; an empty range is a circle, otherwise a convex polygon of 3..8 vertices
+ *   vertices (V,2) float64  polygon vertices relative to the obstacle's centre (motion moves the centre only)
+ *   envs (B,10) float64     rows [xmin, ymin, xmax, ymax, start_x, start_y, start_theta, goal_x, goal_y, goal_threshold]: the
+ *                           rectangle in which moving obstacles bounce, the robot's initial state and its goal
+ * nb_world_check_scenes performs every check of nb_world_set_scenes on the host (NB_ERR_INVALID) without a handle or a device.
+ * nb_world_set_scenes (IR-SIM's make_env / env.reset) uploads the scenes, places the robots at their starts and clears the
+ * collided / arrived flags; it synchronises the device. */
+int nb_world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles,
+                          const int32_t* vert_begin, const double* vertices, const double* envs);
+int nb_world_set_scenes(nb_world_t* w, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                        const double* vertices, const double* envs);
+
+/* env.get_lidar_scan() for every environment (the dict's `ranges` and per-beam `velocity`), DEVICE outputs:
+ *   ranges (B,R) float32: the first crossing t > 0 of beam i with an obstacle boundary (circle: the quadratic; polygon: every edge);
+ *     range_max when there is none closer; the robot's own body is not seen; a sensor inside an obstacle sees the exit crossing
+ *   velocity (B,2,R) float32 or NULL: world-frame velocity of the obstacle a beam hit, zero on a miss (neupan.py:252 consumes it)
+ *   hit (B,R) int32 or NULL: index of that obstacle within its environment, -1 on a miss; equal t: the lower index
+ * FP64 arithmetic, float32 at the store; ranges and velocity are exactly what nb_scan_to_points takes. */
+int nb_world_scan(nb_world_t* w, int32_t B, float* ranges, float* velocity, int32_t* hit, void* stream);
+
+/* env.step(action) + env.done() for every environment: obstacles move by v * dt (a moving centre that leaves its rectangle is mirrored
+ * back and that velocity component reversed); a robot that has not collided integrates action (B,2) float32 DEVICE with the motion
+ * models of initial_path.py:401-444 (diff: (v cos th, v sin th, omega); acker: (v cos th, v sin th, v tan phi / L); omni: (vx, vy), the
+ * velocities PlannerBatch returns), FP64 state.  Then the exact Euclidean clearance between the robot polygon and every obstacle
+ * (0 when they overlap) and the sticky flags: collided = clearance <= 0 (the robot stops for good: collision_mode 'stop'),
+ * arrived = distance to the goal < goal_threshold.  DEVICE outputs, any may be NULL: collided, arrived (B) int32, clearance (B)
+ * float32 (min over the obstacles; +inf without obstacles). */
+int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collided, int32_t* arrived, float* clearance, void* stream);
+
+/* env.get_robot_state() and the obstacle states, DEVICE outputs, any may be NULL: states (B,3) float64 [x, y, theta],
+ * obstacles (O,5) float64 (the rows of nb_world_set_scenes with the current centres and velocities), collided, arrived (B) int32.
+ * Enqueued on `stream` without synchronising. */
+int nb_world_read_state(nb_world_t* w, int32_t B, double* states, double* obstacles, int32_t* collided, int32_t* arrived, void* stream);
+
 /* ---- DUNE training on the device (SURVEY 8f "next" row 4) ------------------------------------------------------------ */
 
 /* DUNETrain.generate_data_set / prob_solve (neupan/blocks/dune_train.py:100-140): labels of n sampled points -- the solution of the

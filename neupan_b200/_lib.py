@@ -56,6 +56,16 @@ class IpathConfig(C.Structure):
     ]
 
 
+class WorldConfig(C.Structure):
+    """struct nb_world_config (include/neupan_b200.h)."""
+    _fields_ = [
+        ("kinematics", C.c_int32), ("num_beams", C.c_int32), ("max_envs", C.c_int32), ("device", C.c_int32),
+        ("robot_num_vertices", C.c_int32), ("reserved_", C.c_int32),
+        ("step_time", C.c_double), ("wheelbase", C.c_double), ("angle_min", C.c_double), ("angle_max", C.c_double),
+        ("range_max", C.c_double), ("scan_offset", C.c_double * 3), ("robot_vertices", C.c_double * 16),
+    ]
+
+
 _FP = C.c_void_p  # device or host float* / int32*: passed as raw addresses
 
 # name -> (restype, argtypes); every symbol include/neupan_b200.h declares
@@ -86,6 +96,13 @@ SYMBOLS = {
     "nb_ipath_reset": (C.c_int, [C.c_void_p]),
     "nb_ipath_reset_async": (C.c_int, [C.c_void_p, C.c_void_p]),
     "nb_ipath_read_state": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, _FP, C.c_void_p]),
+    "nb_world_create": (C.c_int, [C.POINTER(WorldConfig), C.POINTER(C.c_void_p)]),
+    "nb_world_destroy": (C.c_int, [C.c_void_p]),
+    "nb_world_check_scenes": (C.c_int, [C.POINTER(WorldConfig), C.c_int32, _FP, _FP, _FP, _FP, _FP]),
+    "nb_world_set_scenes": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, _FP, _FP]),
+    "nb_world_scan": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, C.c_void_p]),
+    "nb_world_step": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, _FP, C.c_void_p]),
+    "nb_world_read_state": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, _FP, C.c_void_p]),
     "nb_dune_labels": (C.c_int, [C.c_int32, _FP, _FP, C.c_int64, _FP, _FP, _FP, _FP, C.c_void_p]),
     "nb_dune_train_create": (C.c_int, [C.c_int32, _FP, _FP, _FP, C.c_int64, C.c_int32, C.POINTER(C.c_void_p)]),
     "nb_dune_train_destroy": (C.c_int, [C.c_void_p]),

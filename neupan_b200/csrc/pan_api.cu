@@ -17,7 +17,9 @@
 #include "ipath_kernel.cuh"
 #include "dune_train_kernel.cuh"
 #include "dune_table_kernel.cuh"
+#include "world_kernel.cuh"
 
+#include <algorithm>
 #include <vector>
 
 namespace nb {
@@ -55,6 +57,100 @@ cudaError_t dalloc(T** p, size_t n) {
   return cudaMalloc((void**)p, (n ? n : 1) * sizeof(T));
 }
 
+// A convex polygon of n vertices (x0, y0, x1, y1, ...): every vertex off an edge lies strictly on the same side of it
+// (rejects repeated and collinear vertices, reflex corners and self-intersecting stars).
+bool world_convex(const double* v, int n) {
+  double sign = 0.0;
+  for (int k = 0; k < n; ++k) {
+    const int k1 = (k + 1) % n;
+    const double ex = v[2 * k1] - v[2 * k], ey = v[2 * k1 + 1] - v[2 * k + 1];
+    for (int i = 0; i < n; ++i) {
+      if (i == k || i == k1) continue;
+      const double c = ex * (v[2 * i + 1] - v[2 * k + 1]) - ey * (v[2 * i] - v[2 * k]);
+      if (!(c != 0.0) || (sign != 0.0 && (c > 0.0) != (sign > 0.0))) return false;
+      sign = c;
+    }
+  }
+  return true;
+}
+
+bool world_finite(const double* a, size_t n) {
+  for (size_t i = 0; i < n; ++i)
+    if (!std::isfinite(a[i])) return false;
+  return true;
+}
+
+int world_check_config(const nb_world_config* cfg) {
+  if (!cfg) return fail(NB_ERR_INVALID, "nb_world: null config");
+  if (cfg->kinematics < 0 || cfg->kinematics > 2) return fail(NB_ERR_INVALID, "kinematics currently only supports diff, acker or omni");
+  if (cfg->num_beams < 1) return fail(NB_ERR_INVALID, "the lidar needs R >= 1 beams (got %d)", cfg->num_beams);
+  if (cfg->max_envs < 1) return fail(NB_ERR_INVALID, "max_envs must be positive");
+  if (!(cfg->step_time > 0) || !std::isfinite(cfg->step_time)) return fail(NB_ERR_INVALID, "step_time must be positive");
+  if (cfg->kinematics == NB_KIN_ACKER && !(cfg->wheelbase > 0)) return fail(NB_ERR_INVALID, "acker needs a positive wheelbase");
+  if (!(cfg->range_max > 0) || !std::isfinite(cfg->range_max)) return fail(NB_ERR_INVALID, "range_max must be positive and finite");
+  if (!std::isfinite(cfg->angle_min) || !std::isfinite(cfg->angle_max) || !world_finite(cfg->scan_offset, 3))
+    return fail(NB_ERR_INVALID, "lidar angles and scan_offset must be finite");
+  const int nr = cfg->robot_num_vertices;
+  if (nr < 3 || nr > nb::kWorldMaxVertices) return fail(NB_ERR_INVALID, "the robot polygon needs 3..%d vertices (got %d)", nb::kWorldMaxVertices, nr);
+  if (!world_finite(cfg->robot_vertices, 2 * nr) || !world_convex(cfg->robot_vertices, nr)) return fail(NB_ERR_INVALID, "the robot polygon is not convex");
+  return NB_OK;
+}
+
+// Every check of nb_world_set_scenes, on the host.  Fills the per-obstacle slots (circle rank / first edge index within the
+// environment), the per-environment (circles, edges) counts and the largest counts of any environment when asked to.
+int world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obs, const int32_t* vert_begin,
+                       const double* vertices, const double* envs, std::vector<int32_t>* slot, std::vector<int32_t>* counts, int* max_circ,
+                       int* max_edges) {
+  if (int rc = world_check_config(cfg)) return rc;
+  if (!obs_begin || !vert_begin || !envs) return fail(NB_ERR_INVALID, "nb_world scenes: null argument");
+  if (B < 1 || B > cfg->max_envs) return fail(NB_ERR_INVALID, "B = %d outside [1, max_envs = %d]", B, cfg->max_envs);
+  if (obs_begin[0] != 0) return fail(NB_ERR_INVALID, "obs_begin[0] must be 0");
+  for (int b = 0; b < B; ++b) {
+    const int n = obs_begin[b + 1] - obs_begin[b];
+    if (n < 0) return fail(NB_ERR_INVALID, "obs_begin is not ascending at environment %d", b);
+    if (n > nb::kWorldMaxObstacles) return fail(NB_ERR_INVALID, "environment %d has %d obstacles (at most %d)", b, n, nb::kWorldMaxObstacles);
+  }
+  const int O = obs_begin[B];
+  if (O > 0 && !obs) return fail(NB_ERR_INVALID, "nb_world scenes: null obstacles");
+  if (vert_begin[0] != 0) return fail(NB_ERR_INVALID, "vert_begin[0] must be 0");
+  for (int o = 0; o < O; ++o) {
+    const int nv = vert_begin[o + 1] - vert_begin[o];
+    if (nv != 0 && (nv < 3 || nv > nb::kWorldMaxVertices))
+      return fail(NB_ERR_INVALID, "obstacle %d has %d vertices (0 for a circle, 3..%d for a polygon)", o, nv, nb::kWorldMaxVertices);
+  }
+  const int V = vert_begin[O];
+  if (V > 0 && !vertices) return fail(NB_ERR_INVALID, "nb_world scenes: null vertices");
+  if (!world_finite(envs, (size_t)B * nb::kWorldEnvCols) || !world_finite(obs, (size_t)O * nb::kWorldObsCols) || !world_finite(vertices, (size_t)V * 2))
+    return fail(NB_ERR_INVALID, "nb_world scenes: non-finite value");
+  if (slot) { slot->assign(O, 0); counts->assign(2 * (size_t)B, 0); *max_circ = 0; *max_edges = 0; }
+  const double dt = cfg->step_time;
+  for (int b = 0; b < B; ++b) {
+    const double* e = envs + (size_t)nb::kWorldEnvCols * b;
+    if (!(e[0] < e[2]) || !(e[1] < e[3])) return fail(NB_ERR_INVALID, "environment %d: the rectangle needs xmin < xmax and ymin < ymax", b);
+    if (!(e[9] >= 0)) return fail(NB_ERR_INVALID, "environment %d: goal_threshold must be >= 0", b);
+    int nc = 0, ne = 0;
+    for (int o = obs_begin[b]; o < obs_begin[b + 1]; ++o) {
+      const double* r = obs + (size_t)nb::kWorldObsCols * o;
+      const int nv = vert_begin[o + 1] - vert_begin[o];
+      if (nv == 0 && !(r[4] > 0)) return fail(NB_ERR_INVALID, "obstacle %d: a circle needs a positive radius", o);
+      if (nv > 0 && !world_convex(vertices + 2 * (size_t)vert_begin[o], nv)) return fail(NB_ERR_INVALID, "obstacle %d is not a convex polygon", o);
+      for (int a = 0; a < 2; ++a) {
+        if (r[2 + a] == 0.0) continue;
+        const double lo = e[a], hi = e[2 + a];
+        if (r[a] < lo || r[a] > hi) return fail(NB_ERR_INVALID, "obstacle %d moves but its centre starts outside the rectangle of environment %d", o, b);
+        if (!(std::fabs(r[2 + a]) * dt < hi - lo)) return fail(NB_ERR_INVALID, "obstacle %d: |v| * step_time exceeds the rectangle of environment %d", o, b);
+      }
+      if (slot) (*slot)[o] = nv == 0 ? nc : ne;
+      if (nv == 0) ++nc; else ne += nv;
+    }
+    if (slot) {
+      (*counts)[2 * b] = nc; (*counts)[2 * b + 1] = ne;
+      *max_circ = std::max(*max_circ, nc); *max_edges = std::max(*max_edges, ne);
+    }
+  }
+  return NB_OK;
+}
+
 }  // namespace
 
 struct nb_ipath {
@@ -68,6 +164,17 @@ struct nb_ipath {
   int32_t* d_curve_index = nullptr;
   int32_t* d_point_index = nullptr;
   int32_t* d_arrive_flag = nullptr;
+};
+
+struct nb_world {
+  nb_world_config cfg;
+  int B = 0, O = 0, V = 0;
+  int max_circ = 0, max_edges = 0, scan_threads = 0, scan_grid = 0;
+  size_t scan_smem = 0;
+  int32_t *d_obs_begin = nullptr, *d_vert_begin = nullptr, *d_slot = nullptr, *d_counts = nullptr;
+  int32_t *d_collided = nullptr, *d_arrived = nullptr;
+  double *d_vertices = nullptr, *d_env = nullptr, *d_obs = nullptr, *d_states = nullptr;
+  double* d_beam_cs = nullptr;  // (R, 2), fixed at creation
 };
 
 struct nb_dune_train {
@@ -1261,6 +1368,168 @@ int nb_ipath_read_state(nb_ipath_t* p, int32_t B, int32_t* curve_index, int32_t*
     NB_CUDA(cudaMemcpyAsync(points_host, p->d_pts, sizeof(double) * 4 * p->P, cudaMemcpyDeviceToHost, st));
     NB_CUDA(cudaStreamSynchronize(st));
   }
+  return NB_OK;
+}
+
+// ---- batched 2-D world ----------------------------------------------------------------------------------------------------
+int nb_world_create(const nb_world_config* cfg, nb_world_t** out) {
+  if (!out) return fail(NB_ERR_INVALID, "nb_world_create: null argument");
+  *out = nullptr;
+  if (int rc = world_check_config(cfg)) return rc;
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cfg->device < 0 || cfg->device >= ndev)
+    return fail(NB_ERR_NO_DEVICE, "no CUDA device available: neupan_b200 has no CPU fallback");
+  NB_CUDA(cudaSetDevice(cfg->device));
+  nb_world* w = new (std::nothrow) nb_world();
+  if (!w) return fail(NB_ERR_INVALID, "out of host memory");
+  w->cfg = *cfg;
+  // cos / sin of the beam angles a_i = numpy.linspace(angle_min, angle_max, R)[i] (i * step + start, the last one = stop)
+  const int R = cfg->num_beams;
+  const double step = R > 1 ? (cfg->angle_max - cfg->angle_min) / (double)(R - 1) : 0.0;
+  std::vector<double> cs(2 * (size_t)R);
+  for (int i = 0; i < R; ++i) {
+    const double a = R == 1 ? cfg->angle_min : (i == R - 1 ? cfg->angle_max : (double)i * step + cfg->angle_min);
+    cs[2 * i] = std::cos(a);
+    cs[2 * i + 1] = std::sin(a);
+  }
+  cudaError_t e = dalloc(&w->d_beam_cs, cs.size());
+  if (e == cudaSuccess) e = cudaMemcpy(w->d_beam_cs, cs.data(), sizeof(double) * cs.size(), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    nb_world_destroy(w);
+    return fail(NB_ERR_CUDA, "nb_world_create: %s", cudaGetErrorString(e));
+  }
+  *out = w;
+  return NB_OK;
+}
+
+int nb_world_destroy(nb_world_t* w) {
+  if (!w) return NB_OK;
+  cudaSetDevice(w->cfg.device);
+  void* bufs[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs, w->d_states,
+                  w->d_beam_cs};
+  for (void* b : bufs)
+    if (b) cudaFree(b);
+  delete w;
+  return NB_OK;
+}
+
+int nb_world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                          const double* vertices, const double* envs) {
+  return world_check_scenes(cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, nullptr, nullptr, nullptr, nullptr);
+}
+
+int nb_world_set_scenes(nb_world_t* w, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                        const double* vertices, const double* envs) {
+  if (!w) return fail(NB_ERR_INVALID, "nb_world_set_scenes: null handle");
+  std::vector<int32_t> slot, counts;
+  int max_circ = 0, max_edges = 0;
+  if (int rc = world_check_scenes(&w->cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, &slot, &counts, &max_circ, &max_edges)) return rc;
+  const int O = obs_begin[B], V = vert_begin[O];
+  std::vector<double> states(3 * (size_t)B);
+  for (int b = 0; b < B; ++b)
+    for (int k = 0; k < 3; ++k) states[3 * b + k] = envs[(size_t)nb::kWorldEnvCols * b + 4 + k];
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  void* old[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs, w->d_states};
+  for (void* b : old)
+    if (b) cudaFree(b);
+  w->d_obs_begin = w->d_vert_begin = w->d_slot = w->d_counts = w->d_collided = w->d_arrived = nullptr;
+  w->d_vertices = w->d_env = w->d_obs = w->d_states = nullptr;
+  w->B = 0;
+  NB_CUDA(dalloc(&w->d_obs_begin, (size_t)B + 1));
+  NB_CUDA(dalloc(&w->d_vert_begin, (size_t)O + 1));
+  NB_CUDA(dalloc(&w->d_slot, (size_t)O));
+  NB_CUDA(dalloc(&w->d_counts, 2 * (size_t)B));
+  NB_CUDA(dalloc(&w->d_collided, (size_t)B));
+  NB_CUDA(dalloc(&w->d_arrived, (size_t)B));
+  NB_CUDA(dalloc(&w->d_vertices, 2 * (size_t)V));
+  NB_CUDA(dalloc(&w->d_env, (size_t)nb::kWorldEnvCols * B));
+  NB_CUDA(dalloc(&w->d_obs, (size_t)nb::kWorldObsCols * O));
+  NB_CUDA(dalloc(&w->d_states, 3 * (size_t)B));
+  NB_CUDA(cudaMemcpy(w->d_obs_begin, obs_begin, sizeof(int32_t) * (B + 1), cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_vert_begin, vert_begin, sizeof(int32_t) * (O + 1), cudaMemcpyHostToDevice));
+  if (O) NB_CUDA(cudaMemcpy(w->d_slot, slot.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_counts, counts.data(), sizeof(int32_t) * 2 * B, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemset(w->d_collided, 0, sizeof(int32_t) * B));
+  NB_CUDA(cudaMemset(w->d_arrived, 0, sizeof(int32_t) * B));
+  if (V) NB_CUDA(cudaMemcpy(w->d_vertices, vertices, sizeof(double) * 2 * V, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_env, envs, sizeof(double) * nb::kWorldEnvCols * B, cudaMemcpyHostToDevice));
+  if (O) NB_CUDA(cudaMemcpy(w->d_obs, obstacles, sizeof(double) * nb::kWorldObsCols * O, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_states, states.data(), sizeof(double) * 3 * B, cudaMemcpyHostToDevice));
+  // scan launch shape: the largest environment's circles and edges in shared memory, one thread per beam (at most 256)
+  w->max_circ = max_circ; w->max_edges = max_edges;
+  w->scan_smem = (size_t)max_circ * (3 * sizeof(double) + sizeof(int32_t)) + (size_t)max_edges * (4 * sizeof(double) + sizeof(int32_t));
+  w->scan_threads = std::min(256, std::max(32, (w->cfg.num_beams + 31) / 32 * 32));
+  // the occupancy query sees the kernel's current limit; nb_world_scan sets it again before every launch
+  NB_CUDA(cudaFuncSetAttribute(nb::world_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
+  int per_sm = 0, sms = 0;
+  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_scan_kernel, w->scan_threads, w->scan_smem));
+  NB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->cfg.device));
+  if (per_sm < 1) return fail(NB_ERR_CUDA, "world_scan_kernel: %zu B of shared memory do not fit", w->scan_smem);
+  w->scan_grid = std::min(B, per_sm * sms);
+  w->B = B; w->O = O; w->V = V;
+  NB_CUDA(cudaDeviceSynchronize());
+  return NB_OK;
+}
+
+}  // extern "C"
+
+namespace {
+nb::WorldParams world_params(const nb_world* w) {
+  nb::WorldParams prm;
+  const nb_world_config& c = w->cfg;
+  prm.B = w->B; prm.R = c.num_beams; prm.kinematics = c.kinematics; prm.robot_nv = c.robot_num_vertices;
+  prm.dt = c.step_time; prm.L = c.wheelbase; prm.range_max = c.range_max; prm.beam_cs = w->d_beam_cs;
+  prm.off_x = c.scan_offset[0]; prm.off_y = c.scan_offset[1]; prm.off_th = c.scan_offset[2];
+  for (int i = 0; i < 2 * nb::kWorldMaxVertices; ++i) prm.robot_v[i] = c.robot_vertices[i];
+  prm.obs_begin = w->d_obs_begin; prm.vert_begin = w->d_vert_begin; prm.slot = w->d_slot; prm.counts = w->d_counts;
+  prm.vertices = w->d_vertices; prm.env = w->d_env; prm.obs = w->d_obs; prm.states = w->d_states;
+  prm.collided = w->d_collided; prm.arrived = w->d_arrived;
+  return prm;
+}
+
+int world_ready(const nb_world* w, int32_t B, const char* what) {
+  if (!w) return fail(NB_ERR_INVALID, "%s: null handle", what);
+  if (!w->B) return fail(NB_ERR_INVALID, "%s: no scenes set (nb_world_set_scenes)", what);
+  if (B != w->B) return fail(NB_ERR_INVALID, "%s: B = %d but the scenes were set for %d environments", what, B, w->B);
+  return NB_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int nb_world_scan(nb_world_t* w, int32_t B, float* ranges, float* velocity, int32_t* hit, void* stream) {
+  if (int rc = world_ready(w, B, "nb_world_scan")) return rc;
+  if (!ranges) return fail(NB_ERR_INVALID, "nb_world_scan: null ranges");
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  // the dynamic shared-memory limit is an attribute of the kernel, shared by every handle of the process: set this handle's
+  // size before each launch (another handle's nb_world_set_scenes may have set a smaller one)
+  NB_CUDA(cudaFuncSetAttribute(nb::world_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
+  nb::world_scan_kernel<<<w->scan_grid, w->scan_threads, w->scan_smem, (cudaStream_t)stream>>>(world_params(w), w->max_circ, w->max_edges, ranges,
+                                                                                               velocity, hit);
+  ++g_launches;
+  NB_CUDA(cudaGetLastError());
+  return NB_OK;
+}
+
+int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collided, int32_t* arrived, float* clearance, void* stream) {
+  if (int rc = world_ready(w, B, "nb_world_step")) return rc;
+  if (!action) return fail(NB_ERR_INVALID, "nb_world_step: null action");
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  nb::world_step_kernel<<<(B + nb::kWorldStepWarps - 1) / nb::kWorldStepWarps, 32 * nb::kWorldStepWarps, 0, (cudaStream_t)stream>>>(
+      world_params(w), action, collided, arrived, clearance);
+  ++g_launches;
+  NB_CUDA(cudaGetLastError());
+  return NB_OK;
+}
+
+int nb_world_read_state(nb_world_t* w, int32_t B, double* states, double* obstacles, int32_t* collided, int32_t* arrived, void* stream) {
+  if (int rc = world_ready(w, B, "nb_world_read_state")) return rc;
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (states) NB_CUDA(cudaMemcpyAsync(states, w->d_states, sizeof(double) * 3 * B, cudaMemcpyDeviceToDevice, st));
+  if (obstacles && w->O) NB_CUDA(cudaMemcpyAsync(obstacles, w->d_obs, sizeof(double) * nb::kWorldObsCols * w->O, cudaMemcpyDeviceToDevice, st));
+  if (collided) NB_CUDA(cudaMemcpyAsync(collided, w->d_collided, sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
+  if (arrived) NB_CUDA(cudaMemcpyAsync(arrived, w->d_arrived, sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
   return NB_OK;
 }
 

@@ -1,0 +1,242 @@
+"""Batched 2-D world on the device: lidar scans, moving obstacles and collisions for closed-loop runs of B planners.
+
+The reference evaluates its planner in IR-SIM, one robot at a time in host Python (example/run_exp.py:27-56):
+``env.get_robot_state()`` -> ``env.get_lidar_scan()`` -> ``planner(...)`` -> ``env.step(action)`` -> ``env.done()``.
+``WorldBatch`` is that loop's world for B environments at once (``nb_world_*``, csrc/world_kernel.cuh), so that a
+``PlannerBatch`` runs closed loop without its state ever leaving the GPU; ``rollout`` is the loop itself.
+
+A scene (one environment) is a dict with the sections of an ``env.yaml``:
+
+    obstacles       list of dicts: {"center": (x, y), "radius": r} (circle) or {"center": (x, y), "vertices": [[dx, dy], ...]}
+                    (convex polygon, 3..8 vertices relative to the centre), each with an optional "velocity": (vx, vy) in the
+                    world frame (constant; default still).  At most 256 obstacles and 2048 polygon edges per environment.
+    bounds          (xmin, ymin, xmax, ymax): a moving obstacle whose centre leaves this rectangle is mirrored back into it and
+                    that velocity component is reversed
+    start           (x, y, theta) of the robot
+    goal            (x, y); goal_threshold: the robot has arrived when it is closer than this to the goal
+    path            optional (n, 4) rows [x, y, theta, gear]: an initial path for the planner (the scene builders add one)
+
+There is no CPU implementation here: the CUDA library is the product (oracle/world.py restates it for the tests).
+"""
+from __future__ import annotations
+
+import ctypes as C
+import math
+
+import numpy as np
+import torch
+
+from . import _lib
+
+ENV_COLS = 10  # xmin, ymin, xmax, ymax, start x, y, theta, goal x, y, goal threshold
+
+
+def make_config(robot, lidar: dict, step_time: float, max_envs: int, device: int = 0) -> _lib.WorldConfig:
+    """struct nb_world_config from the planner's robot (its ``vertices`` (2, n), ``kinematics`` and ``L``) and a lidar dict with
+    ``angle_min``, ``angle_max``, ``range_max``, ``number`` (R) and optionally ``scan_offset`` (sensor pose in the robot frame)."""
+    verts = np.asarray(robot.vertices, dtype=np.float64)
+    if verts.ndim != 2 or verts.shape[0] != 2 or verts.shape[1] > 8:
+        raise ValueError("robot.vertices must be (2, n) with n <= 8")
+    rv = np.zeros(16)
+    rv[:2 * verts.shape[1]] = verts.T.reshape(-1)
+    return _lib.WorldConfig(kinematics=_lib.NB_KIN[robot.kinematics], num_beams=int(lidar["number"]), max_envs=int(max_envs), device=int(device),
+                            robot_num_vertices=verts.shape[1], step_time=float(step_time), wheelbase=float(robot.L or 0.0),
+                            angle_min=float(lidar["angle_min"]), angle_max=float(lidar["angle_max"]), range_max=float(lidar["range_max"]),
+                            scan_offset=(C.c_double * 3)(*[float(v) for v in lidar.get("scan_offset", (0.0, 0.0, 0.0))]),
+                            robot_vertices=(C.c_double * 16)(*rv))
+
+
+def pack_scenes(scenes):
+    """Scenes -> the ragged host arrays of nb_world_set_scenes: obs_begin (B+1) int32, obstacles (O,5) float64 rows
+    [cx, cy, vx, vy, radius], vert_begin (O+1) int32, vertices (V,2) float64, envs (B,10) float64."""
+    obs_begin, rows, vert_begin, verts, envs = [0], [], [0], [], []
+    for sc in scenes:
+        for ob in sc["obstacles"]:
+            vel = ob.get("velocity", (0.0, 0.0))
+            if "vertices" in ob:
+                v = np.asarray(ob["vertices"], dtype=np.float64).reshape(-1, 2)
+                verts.append(v)
+                vert_begin.append(vert_begin[-1] + v.shape[0])
+                rows.append((*ob["center"], *vel, 0.0))
+            else:
+                vert_begin.append(vert_begin[-1])
+                rows.append((*ob["center"], *vel, ob["radius"]))
+        obs_begin.append(len(rows))
+        envs.append((*sc["bounds"], *sc["start"], *sc["goal"], sc["goal_threshold"]))
+    return (np.asarray(obs_begin, np.int32), np.ascontiguousarray(np.asarray(rows, np.float64).reshape(-1, 5)),
+            np.asarray(vert_begin, np.int32), np.ascontiguousarray(np.vstack(verts) if verts else np.zeros((0, 2))),
+            np.ascontiguousarray(np.asarray(envs, np.float64).reshape(-1, ENV_COLS)))
+
+
+def _host_ptrs(packed):
+    return [C.c_void_p(a.ctypes.data) for a in packed]
+
+
+class WorldBatch:
+    """B environments of one robot type and one lidar.  ``lidar``: angle_min, angle_max, range_min, range_max, number (R),
+    optional scan_offset.  ``scan`` / ``step`` enqueue on the current stream and never synchronise the host."""
+
+    def __init__(self, num_envs: int, robot, lidar: dict, step_time: float, device=None):
+        if not torch.cuda.is_available():
+            raise RuntimeError("neupan_b200.WorldBatch needs a CUDA device (no CPU fallback)")
+        self.B, self.dt, self.R = int(num_envs), float(step_time), int(lidar["number"])
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.scan_offset = tuple(float(v) for v in lidar.get("scan_offset", (0.0, 0.0, 0.0)))
+        self.scan_dict = dict(angle_min=float(lidar["angle_min"]), angle_max=float(lidar["angle_max"]),
+                              range_min=float(lidar.get("range_min", 0.0)), range_max=float(lidar["range_max"]))
+        self.config = make_config(robot, lidar, step_time, self.B, self.device.index or 0)
+        self._handle = C.c_void_p()
+        _lib.check(_lib.load().nb_world_create(C.byref(self.config), C.byref(self._handle)))
+        self.O = 0
+
+    def close(self):
+        if getattr(self, "_handle", None):
+            _lib.load().nb_world_destroy(self._handle)
+            self._handle = None
+
+    __del__ = close
+
+    def _stream(self):
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def set_scenes(self, scenes):
+        """Uploads B scenes, puts every robot at its start and clears the flags (env.reset)."""
+        if len(scenes) != self.B:
+            raise ValueError(f"expected {self.B} scenes, got {len(scenes)}")
+        packed = pack_scenes(scenes)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nb_world_set_scenes(self._handle, self.B, *_host_ptrs(packed)))
+        self.O = int(packed[0][-1])
+
+    def _read(self, states=None, obstacles=None, collided=None, arrived=None):
+        p = lambda t: C.c_void_p(0 if t is None else t.data_ptr())
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nb_world_read_state(self._handle, self.B, p(states), p(obstacles), p(collided), p(arrived), self._stream()))
+
+    @property
+    def states(self) -> torch.Tensor:
+        """(B,3) float64 [x, y, theta] on the device (env.get_robot_state for every robot): a copy, enqueued on the current stream."""
+        s = torch.empty((self.B, 3), dtype=torch.float64, device=self.device)
+        self._read(states=s)
+        return s
+
+    def obstacles(self) -> torch.Tensor:
+        """(O,5) float64 rows [cx, cy, vx, vy, radius] with the current centres and velocities, environments back to back."""
+        o = torch.empty((self.O, 5), dtype=torch.float64, device=self.device)
+        self._read(obstacles=o)
+        return o
+
+    def flags(self):
+        """(collided, arrived) (B,) int32, sticky since set_scenes."""
+        c, a = (torch.empty(self.B, dtype=torch.int32, device=self.device) for _ in range(2))
+        self._read(collided=c, arrived=a)
+        return c, a
+
+    def scan(self, hit: bool = False):
+        """env.get_lidar_scan() for every robot: (ranges (B,R) f32, velocity (B,2,R) f32, scan dict) -- the arguments of
+        PlannerBatch.forward(states, ranges, scan, scan_offset=world.scan_offset, scan_velocity=velocity).  With ``hit``, also the
+        index of the obstacle each beam hit within its environment, -1 on a miss (B,R) int32.  Passing ``velocity`` selects
+        scan_to_point_velocity, which applies the sensor offset inversely (neupan.py:271-273): with a non-zero ``scan_offset`` its
+        points do not land on the obstacles (the reference's behaviour); without velocities, or at a zero offset, they do."""
+        ranges = torch.empty((self.B, self.R), dtype=torch.float32, device=self.device)
+        vel = torch.empty((self.B, 2, self.R), dtype=torch.float32, device=self.device)
+        hits = torch.empty((self.B, self.R), dtype=torch.int32, device=self.device) if hit else None
+        p = lambda t: C.c_void_p(0 if t is None else t.data_ptr())
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nb_world_scan(self._handle, self.B, p(ranges), p(vel), p(hits), self._stream()))
+        return (ranges, vel, dict(self.scan_dict), hits) if hit else (ranges, vel, dict(self.scan_dict))
+
+    def step(self, action):
+        """env.step(action) + env.done(): action (B,2) [v, omega] (diff), [v, steering] (acker) or [vx, vy] (omni).
+        Returns (collided (B,) int32, arrived (B,) int32, clearance (B,) f32) on the device."""
+        action = torch.as_tensor(action).reshape(self.B, 2).to(device=self.device, dtype=torch.float32).contiguous()
+        col, arr = (torch.empty(self.B, dtype=torch.int32, device=self.device) for _ in range(2))
+        clear = torch.empty(self.B, dtype=torch.float32, device=self.device)
+        p = lambda t: C.c_void_p(t.data_ptr())
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nb_world_step(self._handle, self.B, p(action), p(col), p(arr), p(clear), self._stream()))
+        return col, arr, clear
+
+
+def rollout(planner, world: WorldBatch, steps: int, blind: bool = False):
+    """The loop of example/run_exp.py for B robots: scan -> planner.forward -> step, ``steps`` times, all on the device and without
+    a host synchronisation of its own.  ``blind``: the planner gets all-range_max scans (it sees nothing) -- the baseline that shows
+    what the scans are worth.  Returns per-environment collided, arrived (bool), steps_to_arrive (int32, -1 = not arrived) and
+    min_clearance (float32, the smallest clearance after any step)."""
+    B, dev = world.B, world.device
+    steps_to_arrive = torch.full((B,), -1, dtype=torch.int32, device=dev)
+    min_clear = torch.full((B,), math.inf, dtype=torch.float32, device=dev)
+    if blind:
+        blind_ranges = torch.full((B, world.R), world.scan_dict["range_max"], dtype=torch.float32, device=dev)
+        blind_vel = torch.zeros((B, 2, world.R), dtype=torch.float32, device=dev)
+        blind_scan = dict(world.scan_dict)
+    for k in range(steps):
+        ranges, vel, scan = (blind_ranges, blind_vel, blind_scan) if blind else world.scan()
+        action, _ = planner.forward(world.states, ranges, scan, scan_offset=world.scan_offset, scan_velocity=vel)
+        _, arrived, clearance = world.step(action)
+        steps_to_arrive = torch.where((arrived != 0) & (steps_to_arrive < 0), k + 1, steps_to_arrive)
+        min_clear = torch.minimum(min_clear, clearance)
+    collided, arrived = world.flags()
+    return dict(collided=collided.bool(), arrived=arrived.bool(), steps_to_arrive=steps_to_arrive, min_clearance=min_clear)
+
+
+# ---- seeded scenes after the reference's examples -------------------------------------------------------------------------
+
+def _rng(seed: int, b: int) -> np.random.Generator:
+    """Environment b's own child stream (as synth.make_inputs): any sub-range of environments reproduces the same scenes."""
+    return np.random.Generator(np.random.PCG64(np.random.SeedSequence(seed, spawn_key=(b,))))
+
+
+def rectangle(length: float, width: float, theta: float = 0.0) -> np.ndarray:
+    """Vertices (4,2) of a length x width rectangle centred on its centre and turned by theta (IR-SIM's 'rectangle' shape)."""
+    c, s = math.cos(theta), math.sin(theta)
+    corners = np.array([[-length / 2, -width / 2], [length / 2, -width / 2], [length / 2, width / 2], [-length / 2, width / 2]])
+    return corners @ np.array([[c, s], [-s, c]])
+
+
+def line_path(start, goal, spacing: float = 0.1) -> np.ndarray:
+    """(n,4) rows [x, y, theta, gear = 1] along the segment start -> goal (the 'line' curve of two waypoints)."""
+    d = math.hypot(goal[0] - start[0], goal[1] - start[1])
+    n = max(2, int(math.ceil(d / spacing)) + 1)
+    s = np.linspace(0.0, 1.0, n)
+    th = math.atan2(goal[1] - start[1], goal[0] - start[0])
+    return np.stack([start[0] + s * (goal[0] - start[0]), start[1] + s * (goal[1] - start[1]), np.full(n, th), np.ones(n)], 1)
+
+
+def corridor(num_envs: int, seed: int = 0, circles: int = 4):
+    """example/corridor/diff/env.yaml: a 70 x 23 m world at offset (-3, 10), two 70 x 2 m walls centred at (30, 25) and (30, 15)
+    (a corridor 8 m wide around y = 20), goal threshold 0.3; the planner's path runs from (0, 20) to (60, 20)
+    (example/corridor/diff/planner.yaml).  Instead of the example's four turned blocks, ``circles`` static circles of radius
+    0.4..0.8 m stand in the corridor (x in 10..50 m, y in 17.5..22.5 m); the robot starts at (0, 20 +- 1, 0)."""
+    scenes = []
+    for b in range(num_envs):
+        rng = _rng(seed, b)
+        start = (0.0, 20.0 + rng.uniform(-1.0, 1.0), 0.0)
+        goal = (60.0, 20.0)
+        obs = [dict(center=(30.0, 25.0), vertices=rectangle(70.0, 2.0)), dict(center=(30.0, 15.0), vertices=rectangle(70.0, 2.0))]
+        for _ in range(circles):
+            obs.append(dict(center=(rng.uniform(10.0, 50.0), rng.uniform(17.5, 22.5)), radius=rng.uniform(0.4, 0.8)))
+        scenes.append(dict(obstacles=obs, bounds=(-3.0, 10.0, 67.0, 33.0), start=start, goal=goal, goal_threshold=0.3,
+                           path=line_path(start, goal)))
+    return scenes
+
+
+def dyna_obs(num_envs: int, seed: int = 0, count: int = 20):
+    """example/dyna_obs/diff/env.yaml: ``count`` (20) circles of radius 0.4..1.0 m placed at random in the box [10, 40]^2, each
+    moving at a constant speed of at most 0.5 m/s in a random direction and bouncing inside that box (the example's RVO 'wander'
+    behaviour is out of scope), goal threshold 0.4.  The robot crosses the box: it starts at (6, y0) facing the goal (44, y1),
+    y0, y1 in 15..35 m, on a straight path."""
+    scenes = []
+    for b in range(num_envs):
+        rng = _rng(seed, b)
+        y0, y1 = rng.uniform(15.0, 35.0, 2)
+        start = (6.0, y0, math.atan2(y1 - y0, 38.0))
+        goal = (44.0, y1)
+        c = rng.uniform(10.0, 40.0, (count, 2))
+        r = rng.uniform(0.4, 1.0, count)
+        speed, heading = rng.uniform(0.0, 0.5, count), rng.uniform(-math.pi, math.pi, count)
+        obs = [dict(center=(c[i, 0], c[i, 1]), radius=r[i], velocity=(speed[i] * math.cos(heading[i]), speed[i] * math.sin(heading[i])))
+               for i in range(count)]
+        scenes.append(dict(obstacles=obs, bounds=(10.0, 10.0, 40.0, 40.0), start=start, goal=goal, goal_threshold=0.4,
+                           path=line_path(start, goal)))
+    return scenes
