@@ -595,16 +595,17 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
 
       // (b) barrier weights; hinge rows publish omega for the per-step reductions
       __syncwarp();
-      // Differentiable mode, final pass: the weights of the factor that is saved for the adjoint come from the central path at
-      // mu_a = 1e-10 instead of the final mu = 1e-12 and are capped at 1e9.  With W = z/s = 1e13+ the information about the cost
-      // Hessian along an active RATE constraint (W (e_{i+2} - e_i)(e_{i+2} - e_i)' couples two controls) survives only through the
-      // cancellation of 1e14-sized entries: measured gradient errors of 1e-2 (C5, acceleration-limited) that grew to 3e-1 with a
-      // tighter gap; a pinned direction held by 1e9 instead of infinity moves the result by 1e-7.
-      //   active row (z >> s):  W = z^2 / mu_a;   inactive (s >> z):  W = mu_a / s^2;   smooth in between
+      // Differentiable mode, final pass: the factor that is saved for the adjoint is that of the active-set system.  A row whose
+      // multiplier exceeds its slack is active and held by W = 1e9; any other row keeps its barrier weight W = z/s (< 1).  With
+      // W = z/s = 1e13+ the information about the cost Hessian along an active RATE constraint (W (e_{i+2} - e_i)(e_{i+2} - e_i)'
+      // couples two controls) survives only through the cancellation of 1e14-sized entries: measured gradient errors of 1e-2 (C5,
+      // acceleration-limited) that grew to 3e-1 with a tighter gap; a pinned direction held by 1e9 instead of infinity moves the
+      // result by 1e-7.  A weight that grows with z instead (z^2 / 1e-10) leaves a row held by a small multiplier soft: z = 4e-4
+      // gave W = 1.6e3 and a 3.6e-2 error of the chain gradient (C4 `obstacles`, env 141 of 1024).
       NB_LL(k, mb) {
         if (finishing && enabled(k)) {
           const double sk = cs[k], zk = cz[k];
-          cis[k] = (float)(fmin((zk * zk + 1e-10) / (sk * sk + 1e-10), 1e9) / zk);
+          cis[k] = (float)(zk > sk ? 1e9 / zk : 1.0 / sk);
         } else {
           cis[k] = rcpf(cs[k]);
         }
@@ -613,7 +614,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
       for (int q_ = 0; q_ < HPL; ++q_) {
         const int k = lane + 32 * q_;
         if (k < TM) {
-          his[q_] = finishing ? (float)(fmin((hz[q_] * hz[q_] + 1e-10) / (hs[q_] * hs[q_] + 1e-10), 1e9) / hz[q_]) : rcpf(hs[q_]);
+          his[q_] = finishing ? (float)(hz[q_] > hs[q_] ? 1e9 / hz[q_] : 1.0 / hs[q_]) : rcpf(hs[q_]);
           const double Wr = hz[q_] * (double)his[q_];
           hih[q_] = rcp64(rho + Wr);
           tmpk[k] = Wr * rho * hih[q_];  // omega: the row's weight in the reduced Hessian (bounded by rho)

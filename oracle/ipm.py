@@ -156,7 +156,7 @@ def solve_ipm(p: NrmpProblem, max_iter: int = 60, tol: float = 1e-11, verbose: b
         if gap < 1e-9 and res < 1e-8:
             merit = max(gap, res * 1e-1)
             if best is None or merit < best[0]:
-                best = (merit, x.copy(), it)
+                best = (merit, x.copy(), it, z_b.copy(), sb_.copy())
             elif it - best[2] >= 3:  # three iterations without progress below the acceptance level: rounding floor
                 status = "stalled"
                 break
@@ -215,9 +215,10 @@ def solve_ipm(p: NrmpProblem, max_iter: int = 60, tol: float = 1e-11, verbose: b
     if status != "converged":
         if best is None:
             raise IpmFailure(f"interior point method ended with status {status} at iteration {it} (gap {gap:.2e}, rel. residual {res:.2e})")
-        x = best[1]
+        x, z_b, sb_ = best[1], best[3], best[4]
     if info is not None:
-        info.update(status=status, iterations=it, gap=float(gap), residual=float(res), scale=scale)
+        # z_b / s_b: multipliers and slacks of the rows Ab x <= bb at the returned iterate
+        info.update(status=status, iterations=it, gap=float(gap), residual=float(res), scale=scale, z_b=z_b, s_b=sb_)
     U = x[:nU].reshape(T, 2).T.copy()
     S = np.zeros((3, T + 1))
     S[:, 0] = p.nom_s[:, 0]

@@ -36,25 +36,37 @@ def with_theta(p: NrmpProblem, ref_s: np.ndarray, ref_us: np.ndarray, theta: np.
                                gamma_a=q.reshape(3, 1) * np.asarray(ref_s, np.float64), gamma_b=float(theta[3]) * np.asarray(ref_us, np.float64).reshape(-1))
 
 
+def _solve(p: NrmpProblem):
+    """solve_ipm plus the solver's final multipliers and slacks (for active_sets)."""
+    info = {}
+    S, U, D, _ = ipm.solve_ipm(p, info=info)
+    return S, U, D, info
+
+
 def _x_of(p: NrmpProblem, U, D):
     x = np.asarray(U, np.float64).T.reshape(-1)  # time-major (u_{0,0}, u_{1,0}, u_{0,1}, ...)
     return np.concatenate([x, np.asarray(D, np.float64).reshape(-1)]) if p.M > 0 else x
 
 
-def active_sets(p: NrmpProblem, x, tol=1e-7):
+def active_sets(p: NrmpProblem, x, tol=1e-7, info=None):
+    """Active rows of Ab x <= bb and hinge rows with positive argument at x.  With the solver's ``info`` (solve_ipm), a row whose
+    multiplier exceeds its slack is active too: a row held by a small multiplier ends the interior point iteration with a slack
+    of gap / z (C4 without obstacles: 2e-7 at z ~ 5e-5), above any fixed slack tolerance."""
     m = ipm.assemble(p)
     slack = m["bb"] - m["Ab"] @ x
     act = slack < tol * (1.0 + np.abs(m["bb"]))
+    if info is not None:
+        act |= info["z_b"] > info["s_b"]
     hinge = (m["J"] @ x + m["k"]) > tol if p.M > 0 else np.zeros(0, bool)
     return act, hinge
 
 
 def solution_sensitivity(p: NrmpProblem, ref_s, ref_us, tol=1e-7):
     """Returns dict(dS (7,3,T+1), dU (7,2,T), dD (7,T), active, hinge): derivatives of the optimal S, U, D w.r.t. THETA."""
-    S, U, D, _ = ipm.solve_ipm(p)
+    S, U, D, info = _solve(p)
     x = _x_of(p, U, D)
     m = ipm.assemble(p)
-    act, hinge = active_sets(p, x, tol)
+    act, hinge = active_sets(p, x, tol, info)
     A = m["Ab"][act]
     H = m["P"] + (m["rho"] * m["J"][hinge].T @ m["J"][hinge] if p.M > 0 else 0.0)
     n, na = m["n"], A.shape[0]
@@ -91,9 +103,9 @@ def finite_difference(p: NrmpProblem, ref_s, ref_us, i: int, rel_step=1e-5):
         th = th0.copy()
         th[i] += sgn * h
         q = with_theta(p, ref_s, ref_us, th)
-        S, U, D, _ = ipm.solve_ipm(q)
+        S, U, D, info = _solve(q)
         out.append((S, U, D[0] if p.M > 0 else np.zeros(p.T)))
-        sets.append(active_sets(q, _x_of(q, U, D)))
+        sets.append(active_sets(q, _x_of(q, U, D), info=info))
     same = np.array_equal(sets[0][0], sets[1][0]) and np.array_equal(sets[0][1], sets[1][1])
     return tuple((a - b) / (2 * h) for a, b in zip(out[0], out[1])), same
 
@@ -102,10 +114,10 @@ def backward(p: NrmpProblem, ref_s, ref_us, gS, gU, gD, tol=1e-7):
     """Adjoint form (what a backward kernel would do: ONE linear solve per environment instead of one per parameter):
     given the upstream gradients dL/dS (3,T+1), dL/dU (2,T), dL/dD (T) returns dL/dtheta (7).
         g_x = F' dL/dS + dL/dU (+ dL/dD);   K' z = [g_x; 0];   dL/dtheta_i = z' [-(dP_i x + dc_i); db_act_i]"""
-    S, U, D, _ = ipm.solve_ipm(p)
+    S, U, D, info = _solve(p)
     x = _x_of(p, U, D)
     m = ipm.assemble(p)
-    act, hinge = active_sets(p, x, tol)
+    act, hinge = active_sets(p, x, tol, info)
     A = m["Ab"][act]
     H = m["P"] + (m["rho"] * m["J"][hinge].T @ m["J"][hinge] if p.M > 0 else 0.0)
     n, na, nU, T = m["n"], A.shape[0], m["nU"], p.T
@@ -137,10 +149,10 @@ def backward_full(p: NrmpProblem, ref_s, ref_us, gS, gU, gD, tol=1e-7):
     solve, a tensor that carries its autograd history.  It enters the program through the proximal term only
     (0.5 bk |S - para_s|^2, nrmp.py:350); its first column also pins S[:, 0], but that column is the same constant in every
     iteration, so its gradient is not needed (returned as zero)."""
-    S, U, D, _ = ipm.solve_ipm(p)
+    S, U, D, info = _solve(p)
     x = _x_of(p, U, D)
     m = ipm.assemble(p)
-    act, hinge = active_sets(p, x, tol)
+    act, hinge = active_sets(p, x, tol, info)
     A = m["Ab"][act]
     H = m["P"] + (m["rho"] * m["J"][hinge].T @ m["J"][hinge] if p.M > 0 else 0.0)
     n, na, nU, T = m["n"], A.shape[0], m["nU"], p.T
