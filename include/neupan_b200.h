@@ -325,6 +325,19 @@ int nb_world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* 
 int nb_world_set_scenes(nb_world_t* w, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
                         const double* vertices, const double* envs);
 
+/* The same with obstacles of any shape: obs_kind (O) int32 HOST, or NULL (every kind 0: exactly nb_world_check_scenes /
+ * nb_world_set_scenes, whose checks, messages and uploaded bytes these are).
+ *   kind 0   a circle (empty vertex range) or a convex polygon of 3..8 vertices, as above
+ *   kind 1   an outline: any simple polygon of 3..16 vertices, convex or not, in either orientation (no zero-length edge, non-zero
+ *            area, no two edges that do not share a vertex intersect or touch; O(n^2) per outline).  Its edges are scanned like a
+ *            convex polygon's; its clearance is 0 when an outline edge meets a robot edge or either polygon contains the other's
+ *            vertex 0 (even-odd / sign tests), else the smallest vertex-edge distance both ways.
+ * At most 2048 polygon edges per environment, convex polygons and outlines together. */
+int nb_world_check_scenes_ex(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles,
+                             const int32_t* vert_begin, const double* vertices, const double* envs, const int32_t* obs_kind);
+int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                           const double* vertices, const double* envs, const int32_t* obs_kind);
+
 /* env.get_lidar_scan() for every environment (the dict's `ranges` and per-beam `velocity`), DEVICE outputs:
  *   ranges (B,R) float32: the first crossing t > 0 of beam i with an obstacle boundary (circle: the quadratic; polygon: every edge);
  *     range_max when there is none closer; the robot's own body is not seen; a sensor inside an obstacle sees the exit crossing

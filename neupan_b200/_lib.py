@@ -100,6 +100,8 @@ SYMBOLS = {
     "nb_world_destroy": (C.c_int, [C.c_void_p]),
     "nb_world_check_scenes": (C.c_int, [C.POINTER(WorldConfig), C.c_int32, _FP, _FP, _FP, _FP, _FP]),
     "nb_world_set_scenes": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, _FP, _FP]),
+    "nb_world_check_scenes_ex": (C.c_int, [C.POINTER(WorldConfig), C.c_int32, _FP, _FP, _FP, _FP, _FP, _FP]),
+    "nb_world_set_scenes_ex": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, _FP, _FP, _FP]),
     "nb_world_scan": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, C.c_void_p]),
     "nb_world_step": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, _FP, C.c_void_p]),
     "nb_world_read_state": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, _FP, C.c_void_p]),

@@ -74,6 +74,35 @@ bool world_convex(const double* v, int n) {
   return true;
 }
 
+// Closed segments p-q and a-b intersect or touch (orientation tests; a zero orientation counts inside the other's bounding box).
+bool world_segs_meet(const double* p, const double* q, const double* a, const double* b) {
+  auto orient = [](const double* u, const double* v, const double* w) { return (v[0] - u[0]) * (w[1] - u[1]) - (v[1] - u[1]) * (w[0] - u[0]); };
+  auto in_box = [](const double* u, const double* v, const double* w) {
+    return std::min(u[0], v[0]) <= w[0] && w[0] <= std::max(u[0], v[0]) && std::min(u[1], v[1]) <= w[1] && w[1] <= std::max(u[1], v[1]);
+  };
+  const double d1 = orient(a, b, p), d2 = orient(a, b, q), d3 = orient(p, q, a), d4 = orient(p, q, b);
+  if (((d1 > 0 && d2 < 0) || (d1 < 0 && d2 > 0)) && ((d3 > 0 && d4 < 0) || (d3 < 0 && d4 > 0))) return true;
+  return (d1 == 0 && in_box(a, b, p)) || (d2 == 0 && in_box(a, b, q)) || (d3 == 0 && in_box(p, q, a)) || (d4 == 0 && in_box(p, q, b));
+}
+
+// Why the outline of n vertices (x0, y0, x1, y1, ...) is not a simple polygon, or nullptr when it is one: every edge has a length,
+// the area is not zero, and no two non-adjacent edges intersect or touch.
+const char* world_outline_problem(const double* v, int n) {
+  double area2 = 0.0;
+  for (int k = 0; k < n; ++k) {
+    const int k1 = (k + 1) % n;
+    if (v[2 * k] == v[2 * k1] && v[2 * k + 1] == v[2 * k1 + 1]) return "has a zero-length edge";
+    area2 += v[2 * k] * v[2 * k1 + 1] - v[2 * k1] * v[2 * k + 1];
+  }
+  if (!(area2 != 0.0)) return "has zero area";
+  for (int i = 0; i < n; ++i)
+    for (int j = i + 2; j < n; ++j) {
+      if (i == 0 && j == n - 1) continue;  // adjacent through the closing vertex
+      if (world_segs_meet(v + 2 * i, v + 2 * ((i + 1) % n), v + 2 * j, v + 2 * ((j + 1) % n))) return "is not simple (two edges that do not share a vertex meet)";
+    }
+  return nullptr;
+}
+
 bool world_finite(const double* a, size_t n) {
   for (size_t i = 0; i < n; ++i)
     if (!std::isfinite(a[i])) return false;
@@ -96,11 +125,12 @@ int world_check_config(const nb_world_config* cfg) {
   return NB_OK;
 }
 
-// Every check of nb_world_set_scenes, on the host.  Fills the per-obstacle slots (circle rank / first edge index within the
-// environment), the per-environment (circles, edges) counts and the largest counts of any environment when asked to.
+// Every check of nb_world_set_scenes_ex, on the host (kind NULL: every obstacle is a circle or a convex polygon).  Fills the
+// per-obstacle slots (circle rank / first edge index within the environment), the per-environment (circles, edges) counts and the
+// largest counts of any environment when asked to.
 int world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obs, const int32_t* vert_begin,
-                       const double* vertices, const double* envs, std::vector<int32_t>* slot, std::vector<int32_t>* counts, int* max_circ,
-                       int* max_edges) {
+                       const double* vertices, const double* envs, const int32_t* kind, std::vector<int32_t>* slot, std::vector<int32_t>* counts,
+                       int* max_circ, int* max_edges) {
   if (int rc = world_check_config(cfg)) return rc;
   if (!obs_begin || !vert_begin || !envs) return fail(NB_ERR_INVALID, "nb_world scenes: null argument");
   if (B < 1 || B > cfg->max_envs) return fail(NB_ERR_INVALID, "B = %d outside [1, max_envs = %d]", B, cfg->max_envs);
@@ -115,6 +145,12 @@ int world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* obs
   if (vert_begin[0] != 0) return fail(NB_ERR_INVALID, "vert_begin[0] must be 0");
   for (int o = 0; o < O; ++o) {
     const int nv = vert_begin[o + 1] - vert_begin[o];
+    if (kind && kind[o] != 0) {
+      if (kind[o] != 1) return fail(NB_ERR_INVALID, "obstacle %d has kind %d (0: circle or convex polygon, 1: outline)", o, kind[o]);
+      if (nv < 3 || nv > nb::kWorldMaxOutlineVertices)
+        return fail(NB_ERR_INVALID, "obstacle %d: an outline needs 3..%d vertices (got %d)", o, nb::kWorldMaxOutlineVertices, nv);
+      continue;
+    }
     if (nv != 0 && (nv < 3 || nv > nb::kWorldMaxVertices))
       return fail(NB_ERR_INVALID, "obstacle %d has %d vertices (0 for a circle, 3..%d for a polygon)", o, nv, nb::kWorldMaxVertices);
   }
@@ -133,7 +169,11 @@ int world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* obs
       const double* r = obs + (size_t)nb::kWorldObsCols * o;
       const int nv = vert_begin[o + 1] - vert_begin[o];
       if (nv == 0 && !(r[4] > 0)) return fail(NB_ERR_INVALID, "obstacle %d: a circle needs a positive radius", o);
-      if (nv > 0 && !world_convex(vertices + 2 * (size_t)vert_begin[o], nv)) return fail(NB_ERR_INVALID, "obstacle %d is not a convex polygon", o);
+      if (kind && kind[o] == 1) {
+        if (const char* why = world_outline_problem(vertices + 2 * (size_t)vert_begin[o], nv)) return fail(NB_ERR_INVALID, "obstacle %d: the outline %s", o, why);
+      } else if (nv > 0 && !world_convex(vertices + 2 * (size_t)vert_begin[o], nv)) {
+        return fail(NB_ERR_INVALID, "obstacle %d is not a convex polygon", o);
+      }
       for (int a = 0; a < 2; ++a) {
         if (r[2 + a] == 0.0) continue;
         const double lo = e[a], hi = e[2 + a];
@@ -143,6 +183,8 @@ int world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* obs
       if (slot) (*slot)[o] = nv == 0 ? nc : ne;
       if (nv == 0) ++nc; else ne += nv;
     }
+    // the scan stages an environment's edges in shared memory; 256 convex polygons cannot exceed this, outlines can
+    if (ne > nb::kWorldMaxEdges) return fail(NB_ERR_INVALID, "environment %d has %d polygon edges (at most %d)", b, ne, nb::kWorldMaxEdges);
     if (slot) {
       (*counts)[2 * b] = nc; (*counts)[2 * b + 1] = ne;
       *max_circ = std::max(*max_circ, nc); *max_edges = std::max(*max_edges, ne);
@@ -171,7 +213,7 @@ struct nb_world {
   int B = 0, O = 0, V = 0;
   int max_circ = 0, max_edges = 0, scan_threads = 0, scan_grid = 0;
   size_t scan_smem = 0;
-  int32_t *d_obs_begin = nullptr, *d_vert_begin = nullptr, *d_slot = nullptr, *d_counts = nullptr;
+  int32_t *d_obs_begin = nullptr, *d_vert_begin = nullptr, *d_slot = nullptr, *d_counts = nullptr, *d_kind = nullptr;
   int32_t *d_collided = nullptr, *d_arrived = nullptr;
   double *d_vertices = nullptr, *d_env = nullptr, *d_obs = nullptr, *d_states = nullptr;
   double* d_beam_cs = nullptr;  // (R, 2), fixed at creation
@@ -1405,40 +1447,50 @@ int nb_world_create(const nb_world_config* cfg, nb_world_t** out) {
 int nb_world_destroy(nb_world_t* w) {
   if (!w) return NB_OK;
   cudaSetDevice(w->cfg.device);
-  void* bufs[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs, w->d_states,
-                  w->d_beam_cs};
+  void* bufs[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
+                  w->d_states, w->d_beam_cs};
   for (void* b : bufs)
     if (b) cudaFree(b);
   delete w;
   return NB_OK;
 }
 
-int nb_world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
-                          const double* vertices, const double* envs) {
-  return world_check_scenes(cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, nullptr, nullptr, nullptr, nullptr);
+int nb_world_check_scenes_ex(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                             const double* vertices, const double* envs, const int32_t* obs_kind) {
+  return world_check_scenes(cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, obs_kind, nullptr, nullptr, nullptr, nullptr);
 }
 
-int nb_world_set_scenes(nb_world_t* w, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
-                        const double* vertices, const double* envs) {
+int nb_world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                          const double* vertices, const double* envs) {
+  return nb_world_check_scenes_ex(cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, nullptr);
+}
+
+int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                           const double* vertices, const double* envs, const int32_t* obs_kind) {
   if (!w) return fail(NB_ERR_INVALID, "nb_world_set_scenes: null handle");
   std::vector<int32_t> slot, counts;
   int max_circ = 0, max_edges = 0;
-  if (int rc = world_check_scenes(&w->cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, &slot, &counts, &max_circ, &max_edges)) return rc;
+  if (int rc = world_check_scenes(&w->cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, obs_kind, &slot, &counts, &max_circ, &max_edges))
+    return rc;
   const int O = obs_begin[B], V = vert_begin[O];
   std::vector<double> states(3 * (size_t)B);
   for (int b = 0; b < B; ++b)
     for (int k = 0; k < 3; ++k) states[3 * b + k] = envs[(size_t)nb::kWorldEnvCols * b + 4 + k];
   NB_CUDA(cudaSetDevice(w->cfg.device));
-  void* old[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs, w->d_states};
+  void* old[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
+                 w->d_states};
   for (void* b : old)
     if (b) cudaFree(b);
-  w->d_obs_begin = w->d_vert_begin = w->d_slot = w->d_counts = w->d_collided = w->d_arrived = nullptr;
+  w->d_obs_begin = w->d_vert_begin = w->d_slot = w->d_counts = w->d_kind = w->d_collided = w->d_arrived = nullptr;
   w->d_vertices = w->d_env = w->d_obs = w->d_states = nullptr;
   w->B = 0;
   NB_CUDA(dalloc(&w->d_obs_begin, (size_t)B + 1));
   NB_CUDA(dalloc(&w->d_vert_begin, (size_t)O + 1));
   NB_CUDA(dalloc(&w->d_slot, (size_t)O));
   NB_CUDA(dalloc(&w->d_counts, 2 * (size_t)B));
+  NB_CUDA(dalloc(&w->d_kind, (size_t)O));
+  if (O && obs_kind) NB_CUDA(cudaMemcpy(w->d_kind, obs_kind, sizeof(int32_t) * O, cudaMemcpyHostToDevice));
+  else if (O) NB_CUDA(cudaMemset(w->d_kind, 0, sizeof(int32_t) * O));
   NB_CUDA(dalloc(&w->d_collided, (size_t)B));
   NB_CUDA(dalloc(&w->d_arrived, (size_t)B));
   NB_CUDA(dalloc(&w->d_vertices, 2 * (size_t)V));
@@ -1471,6 +1523,11 @@ int nb_world_set_scenes(nb_world_t* w, int32_t B, const int32_t* obs_begin, cons
   return NB_OK;
 }
 
+int nb_world_set_scenes(nb_world_t* w, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                        const double* vertices, const double* envs) {
+  return nb_world_set_scenes_ex(w, B, obs_begin, obstacles, vert_begin, vertices, envs, nullptr);
+}
+
 }  // extern "C"
 
 namespace {
@@ -1481,7 +1538,7 @@ nb::WorldParams world_params(const nb_world* w) {
   prm.dt = c.step_time; prm.L = c.wheelbase; prm.range_max = c.range_max; prm.beam_cs = w->d_beam_cs;
   prm.off_x = c.scan_offset[0]; prm.off_y = c.scan_offset[1]; prm.off_th = c.scan_offset[2];
   for (int i = 0; i < 2 * nb::kWorldMaxVertices; ++i) prm.robot_v[i] = c.robot_vertices[i];
-  prm.obs_begin = w->d_obs_begin; prm.vert_begin = w->d_vert_begin; prm.slot = w->d_slot; prm.counts = w->d_counts;
+  prm.obs_begin = w->d_obs_begin; prm.vert_begin = w->d_vert_begin; prm.slot = w->d_slot; prm.counts = w->d_counts; prm.kind = w->d_kind;
   prm.vertices = w->d_vertices; prm.env = w->d_env; prm.obs = w->d_obs; prm.states = w->d_states;
   prm.collided = w->d_collided; prm.arrived = w->d_arrived;
   return prm;

@@ -1,12 +1,14 @@
 // Batched 2-D world for closed-loop runs of B planners: what IR-SIM does between two planner calls (example/run_exp.py:27-56,
 // env.get_lidar_scan / env.step / env.done), for B environments at once and without leaving the device.
 //
-// Scene: per environment a ragged list of obstacles -- circles (centre, radius) and convex polygons (3..8 vertices stored relative
-// to the centre, so that motion only moves the centre) -- each with a constant world-frame velocity, an axis-aligned rectangle in
-// which moving obstacles bounce, the robot (the planner's robot polygon) and its goal.
+// Scene: per environment a ragged list of obstacles -- circles (centre, radius), convex polygons (3..8 vertices) and outlines (any
+// simple polygon of 3..16 vertices, convex or not; kind 1), vertices stored relative to the centre so that motion only moves the
+// centre -- each with a constant world-frame velocity, an axis-aligned rectangle in which moving obstacles bounce, the robot (the
+// planner's robot polygon) and its goal.
 //
-//   world_scan_kernel   one CTA per environment (grid-stride): the environment's circles and polygon edges are staged in shared
-//                       memory in world coordinates, then one thread per beam finds the first boundary crossing with t > 0
+//   world_scan_kernel   one CTA per environment (grid-stride): the environment's circles and polygon edges (convex and outline
+//                       alike) are staged in shared memory in world coordinates, then one thread per beam finds the first boundary
+//                       crossing with t > 0
 //   world_step_kernel   one warp per environment: obstacles move (reflecting at the rectangle), the robot integrates its action
 //                       unless it has collided, then the exact clearance robot polygon <-> every obstacle, reduced over the warp
 //
@@ -19,7 +21,9 @@
 namespace nb {
 
 constexpr int kWorldMaxObstacles = 256;  // per environment (staged in shared memory by the scan kernel)
-constexpr int kWorldMaxVertices = 8;     // per polygon (obstacles and the robot): at most 2048 polygon edges per environment
+constexpr int kWorldMaxVertices = 8;     // per convex polygon (obstacles and the robot)
+constexpr int kWorldMaxOutlineVertices = 16;
+constexpr int kWorldMaxEdges = 2048;     // polygon edges (convex and outline) per environment, staged in shared memory by the scan
 constexpr int kWorldObsCols = 5;         // obstacle row: cx, cy, vx, vy, radius (radius unused for polygons)
 constexpr int kWorldEnvCols = 10;        // env row: xmin, ymin, xmax, ymax, start x, y, theta, goal x, y, goal threshold
 constexpr int kWorldStepWarps = 4;
@@ -34,6 +38,7 @@ struct WorldParams {
   const int32_t* vert_begin;              // (O + 1) offsets into vertices; an empty range is a circle
   const int32_t* slot;                    // (O) circle: rank among the env's circles; polygon: index of its first edge in the env
   const int32_t* counts;                  // (B, 2) circles, polygon edges of the environment
+  const int32_t* kind;                    // (O) 0: circle or convex polygon, 1: outline
   const double* vertices;                 // (V, 2) relative to the obstacle's centre
   const double* env;                      // (B, kWorldEnvCols)
   double* obs;                            // (O, kWorldObsCols) -- centres and velocities change
@@ -182,6 +187,66 @@ __device__ __forceinline__ bool world_sat_separates(const PA& a, const PB& bp) {
   return false;
 }
 
+// p lies in the bounding box of the segment a-b (with a zero orientation: p lies on the closed segment)
+__device__ __forceinline__ bool world_in_box(double ax, double ay, double bx, double by, double px, double py) {
+  return fmin(ax, bx) <= px && px <= fmax(ax, bx) && fmin(ay, by) <= py && py <= fmax(ay, by);
+}
+
+// Do the closed segments p-q and a-b intersect or touch?  Orientation tests; a zero orientation (collinear, or an endpoint on the
+// other segment's line) counts when that endpoint lies within the other segment.
+__device__ __forceinline__ bool world_segs_meet(double px, double py, double qx, double qy, double ax, double ay, double bx, double by) {
+  const double ex = dsub(bx, ax), ey = dsub(by, ay), fx = dsub(qx, px), fy = dsub(qy, py);
+  const double d1 = dcross(ex, ey, dsub(px, ax), dsub(py, ay)), d2 = dcross(ex, ey, dsub(qx, ax), dsub(qy, ay));
+  const double d3 = dcross(fx, fy, dsub(ax, px), dsub(ay, py)), d4 = dcross(fx, fy, dsub(bx, px), dsub(by, py));
+  if (((d1 > 0.0 && d2 < 0.0) || (d1 < 0.0 && d2 > 0.0)) && ((d3 > 0.0 && d4 < 0.0) || (d3 < 0.0 && d4 > 0.0))) return true;
+  return (d1 == 0.0 && world_in_box(ax, ay, bx, by, px, py)) || (d2 == 0.0 && world_in_box(ax, ay, bx, by, qx, qy)) ||
+         (d3 == 0.0 && world_in_box(px, py, qx, qy, ax, ay)) || (d4 == 0.0 && world_in_box(px, py, qx, qy, bx, by));
+}
+
+// Robot (convex) <-> outline (any simple polygon): 0 when they overlap -- an outline edge meets a robot edge, robot vertex 0 lies
+// inside the outline, or outline vertex 0 lies inside the robot (the circle branch's sign test) -- else the smallest vertex-edge
+// distance both ways, in the convex branch's order (so a convex polygon given as an outline gets the same distance bit for bit).
+// The even-odd test of robot vertex 0 shares the edge loop of the segment tests (separate loops spill): an outline edge that
+// straddles the horizontal line through the vertex toggles it when it crosses that line to the vertex's right, which is the sign
+// of the cross product edge x (vertex - edge start) -- no division.
+__device__ __forceinline__ double world_outline_clearance(const WorldPoly& op, const double* rx, const double* ry, int nr) {
+  bool in = false;
+  for (int k = 0; k < op.nv; ++k) {
+    const int k1 = k + 1 < op.nv ? k + 1 : 0;
+    const double ax = op.vx(k), ay = op.vy(k), bx = op.vx(k1), by = op.vy(k1);
+    for (int i = 0; i < nr; ++i) {
+      const int i1 = i + 1 < nr ? i + 1 : 0;
+      if (world_segs_meet(rx[i], ry[i], rx[i1], ry[i1], ax, ay, bx, by)) return 0.0;
+    }
+    if ((ay > ry[0]) != (by > ry[0])) {
+      const double c = dcross(dsub(bx, ax), dsub(by, ay), dsub(rx[0], ax), dsub(ry[0], ay));
+      if (by > ay ? c > 0.0 : c < 0.0) in = !in;
+    }
+  }
+  if (in) return 0.0;
+  {
+    const double px = op.vx(0), py = op.vy(0);
+    bool pos = false, neg = false;
+    for (int k = 0; k < nr; ++k) {
+      const int k1 = k + 1 < nr ? k + 1 : 0;
+      const double cr = dcross(dsub(rx[k1], rx[k]), dsub(ry[k1], ry[k]), dsub(px, rx[k]), dsub(py, ry[k]));
+      pos |= cr > 0.0; neg |= cr < 0.0;
+    }
+    if (!(pos && neg)) return 0.0;
+  }
+  double d = INFINITY;
+  for (int k = 0; k < op.nv; ++k) {
+    const int k1 = k + 1 < op.nv ? k + 1 : 0;
+    const double ax = op.vx(k), ay = op.vy(k), bx = op.vx(k1), by = op.vy(k1);
+    for (int i = 0; i < nr; ++i) d = fmin(d, world_seg_dist(rx[i], ry[i], ax, ay, bx, by));
+  }
+  for (int k = 0; k < nr; ++k) {
+    const int k1 = k + 1 < nr ? k + 1 : 0;
+    for (int i = 0; i < op.nv; ++i) d = fmin(d, world_seg_dist(op.vx(i), op.vy(i), rx[k], ry[k], rx[k1], ry[k1]));
+  }
+  return d;
+}
+
 // ---- step -----------------------------------------------------------------------------------------------------------------
 
 __global__ void __launch_bounds__(32 * kWorldStepWarps) world_step_kernel(const WorldParams prm, const float* __restrict__ action,
@@ -255,6 +320,8 @@ __global__ void __launch_bounds__(32 * kWorldStepWarps) world_step_kernel(const 
         d = fmin(d, world_seg_dist(cx, cy, rx[k], ry[k], rx[k1], ry[k1]));
       }
       c = (pos && neg) ? dsub(d, row[4]) : 0.0;  // centre inside the robot: overlap
+    } else if (prm.kind[o] != 0) {
+      c = world_outline_clearance(WorldPoly{prm.vertices + 2 * (size_t)v0, cx, cy, nv}, rx, ry, nr);
     } else {        // convex polygon: 0 unless an edge normal separates them, then the smallest vertex-edge distance
       const WorldPoly op{prm.vertices + 2 * (size_t)v0, cx, cy, nv};
       const WorldRobot rp{rx, ry, nr};

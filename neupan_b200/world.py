@@ -7,9 +7,11 @@ The reference evaluates its planner in IR-SIM, one robot at a time in host Pytho
 
 A scene (one environment) is a dict with the sections of an ``env.yaml``:
 
-    obstacles       list of dicts: {"center": (x, y), "radius": r} (circle) or {"center": (x, y), "vertices": [[dx, dy], ...]}
-                    (convex polygon, 3..8 vertices relative to the centre), each with an optional "velocity": (vx, vy) in the
-                    world frame (constant; default still).  At most 256 obstacles and 2048 polygon edges per environment.
+    obstacles       list of dicts: {"center": (x, y), "radius": r} (circle), {"center": (x, y), "vertices": [[dx, dy], ...]}
+                    (convex polygon, 3..8 vertices relative to the centre) or {"center": (x, y), "outline": [[dx, dy], ...]} (any
+                    simple polygon, convex or not, either orientation, 3..16 vertices relative to the centre), each with an
+                    optional "velocity": (vx, vy) in the world frame (constant; default still; polygons do not rotate).  At most
+                    256 obstacles and 2048 polygon edges (convex and outline together) per environment.
     bounds          (xmin, ymin, xmax, ymax): a moving obstacle whose centre leaves this rectangle is mirrored back into it and
                     that velocity component is reversed
     start           (x, y, theta) of the robot
@@ -46,26 +48,41 @@ def make_config(robot, lidar: dict, step_time: float, max_envs: int, device: int
                             robot_vertices=(C.c_double * 16)(*rv))
 
 
-def pack_scenes(scenes):
-    """Scenes -> the ragged host arrays of nb_world_set_scenes: obs_begin (B+1) int32, obstacles (O,5) float64 rows
-    [cx, cy, vx, vy, radius], vert_begin (O+1) int32, vertices (V,2) float64, envs (B,10) float64."""
-    obs_begin, rows, vert_begin, verts, envs = [0], [], [0], [], []
+def pack_scenes_ex(scenes):
+    """Scenes -> the ragged host arrays of nb_world_set_scenes_ex: obs_begin (B+1) int32, obstacles (O,5) float64 rows
+    [cx, cy, vx, vy, radius], vert_begin (O+1) int32, vertices (V,2) float64, envs (B,10) float64, kinds (O) int32
+    (0: circle or convex polygon, 1: outline)."""
+    obs_begin, rows, vert_begin, verts, envs, kinds = [0], [], [0], [], [], []
     for sc in scenes:
         for ob in sc["obstacles"]:
             vel = ob.get("velocity", (0.0, 0.0))
-            if "vertices" in ob:
-                v = np.asarray(ob["vertices"], dtype=np.float64).reshape(-1, 2)
+            if "vertices" in ob and "outline" in ob:
+                raise ValueError("an obstacle has either 'vertices' (convex) or 'outline', not both")
+            shape = "vertices" if "vertices" in ob else ("outline" if "outline" in ob else None)
+            if shape:
+                v = np.asarray(ob[shape], dtype=np.float64).reshape(-1, 2)
                 verts.append(v)
                 vert_begin.append(vert_begin[-1] + v.shape[0])
                 rows.append((*ob["center"], *vel, 0.0))
             else:
                 vert_begin.append(vert_begin[-1])
                 rows.append((*ob["center"], *vel, ob["radius"]))
+            kinds.append(1 if shape == "outline" else 0)
         obs_begin.append(len(rows))
         envs.append((*sc["bounds"], *sc["start"], *sc["goal"], sc["goal_threshold"]))
     return (np.asarray(obs_begin, np.int32), np.ascontiguousarray(np.asarray(rows, np.float64).reshape(-1, 5)),
             np.asarray(vert_begin, np.int32), np.ascontiguousarray(np.vstack(verts) if verts else np.zeros((0, 2))),
-            np.ascontiguousarray(np.asarray(envs, np.float64).reshape(-1, ENV_COLS)))
+            np.ascontiguousarray(np.asarray(envs, np.float64).reshape(-1, ENV_COLS)), np.asarray(kinds, np.int32))
+
+
+def pack_scenes(scenes):
+    """Scenes of circles and convex polygons -> the ragged host arrays of nb_world_set_scenes: obs_begin (B+1) int32, obstacles
+    (O,5) float64 rows [cx, cy, vx, vy, radius], vert_begin (O+1) int32, vertices (V,2) float64, envs (B,10) float64.  Scenes with
+    outlines need the kinds of pack_scenes_ex."""
+    packed = pack_scenes_ex(scenes)
+    if packed[5].any():
+        raise ValueError("these scenes have outlines: use pack_scenes_ex (nb_world_set_scenes_ex)")
+    return packed[:5]
 
 
 def _host_ptrs(packed):
@@ -103,9 +120,9 @@ class WorldBatch:
         """Uploads B scenes, puts every robot at its start and clears the flags (env.reset)."""
         if len(scenes) != self.B:
             raise ValueError(f"expected {self.B} scenes, got {len(scenes)}")
-        packed = pack_scenes(scenes)
+        packed = pack_scenes_ex(scenes)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.load().nb_world_set_scenes(self._handle, self.B, *_host_ptrs(packed)))
+            _lib.check(_lib.load().nb_world_set_scenes_ex(self._handle, self.B, *_host_ptrs(packed)))
         self.O = int(packed[0][-1])
 
     def _read(self, states=None, obstacles=None, collided=None, arrived=None):
@@ -238,5 +255,79 @@ def dyna_obs(num_envs: int, seed: int = 0, count: int = 20):
         obs = [dict(center=(c[i, 0], c[i, 1]), radius=r[i], velocity=(speed[i] * math.cos(heading[i]), speed[i] * math.sin(heading[i])))
                for i in range(count)]
         scenes.append(dict(obstacles=obs, bounds=(10.0, 10.0, 40.0, 40.0), start=start, goal=goal, goal_threshold=0.4,
+                           path=line_path(start, goal)))
+    return scenes
+
+
+def random_outline(rng: np.random.Generator, avg_radius: float, irregularity: float, spikeyness: float, n_vertices: int) -> np.ndarray:
+    """Vertices (n,2) of a random star-shaped polygon around the centre (0, 0): this project's reading of IR-SIM's `random_shape`
+    polygons (the well-known random-polygon recipe; IR-SIM itself is not a dependency, so its polygons are not compared).
+
+    The angular steps are drawn from U(2 pi / n (1 - irregularity), 2 pi / n (1 + irregularity)) and normalised to sum to 2 pi,
+    from a random first angle; the radii from N(avg_radius, spikeyness * avg_radius), clipped to [0.1, 2] * avg_radius so that no
+    vertex collapses onto the centre.  Steps are drawn again while one of them reaches pi: with every step in (0, pi) the centre
+    sees the vertices in strictly increasing directions, each edge stays in its own sector, and the polygon is simple (usually not
+    convex)."""
+    n = int(n_vertices)
+    mean = 2.0 * math.pi / n
+    while True:
+        steps = rng.uniform(mean * (1.0 - irregularity), mean * (1.0 + irregularity), n)
+        steps *= 2.0 * math.pi / steps.sum()
+        if steps.max() < math.pi and steps.min() > 0.0:
+            break
+    angles = rng.uniform(0.0, 2.0 * math.pi) + np.concatenate([[0.0], np.cumsum(steps[:-1])])
+    r = np.clip(rng.normal(avg_radius, spikeyness * avg_radius, n), 0.1 * avg_radius, 2.0 * avg_radius)
+    return np.stack([r * np.cos(angles), r * np.sin(angles)], 1)
+
+
+def _example_outline(rng, avg_radius: float, irregularity: float) -> np.ndarray:
+    """An outline of the reference's `random_shape: true` obstacles: 4..9 vertices and spikeyness U(0, 1) (a stated choice: the
+    examples give only the radius and irregularity ranges)."""
+    spikeyness, n = rng.uniform(0.0, 1.0), int(rng.integers(4, 10))
+    return random_outline(rng, avg_radius, irregularity, spikeyness, n)
+
+
+def dyna_non_obs(num_envs: int, seed: int = 0):
+    """example/dyna_non_obs/diff/{env,planner}.yaml: 11 obstacles, each one of the example's four shapes drawn uniformly -- the
+    2 x 2 m square, a circle of r = 1.5, a circle of r = 1.0, or an outline of average radius U(0.5, 1.5) and irregularity 0.9 (how
+    IR-SIM assigns a 4-entry shape list to 11 obstacles is a stated choice here).  Centres uniform in [5, 45] x [15, 35], constant
+    velocities (vx, vy) in U(-1, 1)^2, bouncing in that box (the example's RVO 'wander' behaviour is out of scope).  The robot
+    starts at (-1, 25, 0) on the planner's line path to (50, 25), its goal, with threshold 0.4."""
+    square = [[-1.0, -1.0], [1.0, -1.0], [1.0, 1.0], [-1.0, 1.0]]
+    start, goal = (-1.0, 25.0, 0.0), (50.0, 25.0)
+    scenes = []
+    for b in range(num_envs):
+        rng = _rng(seed, b)
+        obs = []
+        for _ in range(11):
+            shape = int(rng.integers(0, 4))
+            ob = dict(center=tuple(rng.uniform((5.0, 15.0), (45.0, 35.0))), velocity=tuple(rng.uniform(-1.0, 1.0, 2)))
+            if shape == 0:
+                ob["vertices"] = square
+            elif shape in (1, 2):
+                ob["radius"] = 1.5 if shape == 1 else 1.0
+            else:
+                ob["outline"] = _example_outline(rng, rng.uniform(0.5, 1.5), 0.9)
+            obs.append(ob)
+        scenes.append(dict(obstacles=obs, bounds=(5.0, 15.0, 45.0, 35.0), start=start, goal=goal, goal_threshold=0.4,
+                           path=line_path(start, goal)))
+    return scenes
+
+
+# the first 11 `state` rows of example/non_obs/acker/env.yaml (its list has 12 for 11 obstacles; the repeated (16, 26) is kept)
+NON_OBS_CENTRES = ((20.0, 34.0), (31.0, 38.0), (10.0, 20.0), (41.0, 25.0), (18.8, 13.0), (16.0, 26.0), (10.0, 24.0), (15.0, 20.0),
+                   (16.0, 26.0), (19.0, 26.0), (11.0, 14.5))
+
+
+def non_obs(num_envs: int, seed: int = 0):
+    """example/non_obs/acker/{env,planner}.yaml: 11 static outlines at the example's positions, average radius U(0.5, 1.0) and
+    irregularity U(0.9, 1.0), different in every environment; the world's rectangle (-2, 5, 51, 47).  The robot starts at
+    (-1, 25, 0) with goal (50, 25) and threshold 0.3; the example's dubins curve between these two poses is the straight line."""
+    start, goal = (-1.0, 25.0, 0.0), (50.0, 25.0)
+    scenes = []
+    for b in range(num_envs):
+        rng = _rng(seed, b)
+        obs = [dict(center=c, outline=_example_outline(rng, rng.uniform(0.5, 1.0), rng.uniform(0.9, 1.0))) for c in NON_OBS_CENTRES]
+        scenes.append(dict(obstacles=obs, bounds=(-2.0, 5.0, 51.0, 47.0), start=start, goal=goal, goal_threshold=0.3,
                            path=line_path(start, goal)))
     return scenes

@@ -1,9 +1,10 @@
 """Times the batched world (csrc/world_kernel.cuh) against the planner it serves, on the device, and prints one JSON line.
 
-    python tools/world_bench.py [--envs 4096] [--beams 1080] [--steps 20] [--warmup 3]
+    python tools/world_bench.py [--scene dyna_obs|dyna_non_obs] [--envs 4096] [--beams 1080] [--steps 20] [--warmup 3]
 
-Scenes: seeded dyna_obs (20 moving circles per environment, neupan_b200.world.dyna_obs).  Planner: PlannerBatch with C4's robot,
-adjust values and K, the scans decimated to C4's N = 500 points.  Legs, each timed with CUDA events over --steps iterations after
+Scenes: seeded dyna_obs (20 moving circles per environment, neupan_b200.world.dyna_obs; the default) or dyna_non_obs (11 moving
+obstacles after example/dyna_non_obs: squares, circles and non-convex outlines, neupan_b200.world.dyna_non_obs).  Planner:
+PlannerBatch with C4's robot, adjust values and K, the scans decimated to C4's N = 500 points.  Legs, each timed with CUDA events over --steps iterations after
 --warmup: the world alone (scan + step), the planner alone (PlannerBatch.forward repeated on the initial states and scans, after a
 reset) and the closed-loop step (scan -> PlannerBatch.forward -> step, from the initial scenes after a reset), whose world and planner
 parts are also timed separately with events around each call.  The planner-alone leg repeats one input; in the closed loop the
@@ -33,6 +34,7 @@ def _card():
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--scene", choices=("dyna_obs", "dyna_non_obs"), default="dyna_obs")
     ap.add_argument("--envs", type=int, default=4096)
     ap.add_argument("--beams", type=int, default=1080)
     ap.add_argument("--steps", type=int, default=20)
@@ -45,14 +47,17 @@ def main():
 
     from helpers import CONFIGS, weights_path
     from neupan_b200 import PlannerBatch, WorldBatch
-    from neupan_b200.world import dyna_obs
+    from neupan_b200.world import dyna_non_obs, dyna_obs, pack_scenes_ex
 
     if not torch.cuda.is_available():
         raise SystemExit("world_bench.py needs a CUDA device")
     B, R = args.envs, args.beams
     cfg = CONFIGS["C4"]
     lidar = dict(angle_min=-math.pi, angle_max=math.pi, range_min=0.0, range_max=10.0, number=R)
-    scenes = dyna_obs(B, seed=2024)
+    scenes = (dyna_obs if args.scene == "dyna_obs" else dyna_non_obs)(B, seed=2024)
+    packed = pack_scenes_ex(scenes)
+    n_obs, n_edges = int(packed[0][-1]), int(packed[2][-1])
+    n_circles = int((packed[2][1:] == packed[2][:-1]).sum())
     pl = PlannerBatch(B, cfg.T, cfg.dt, 4.0, robot_kwargs=cfg.robot_kwargs, adjust_kwargs=dict(cfg.adjust),
                       pan_kwargs=dict(iter_num=cfg.K, dune_max_num=cfg.N, nrmp_max_num=cfg.M, dune_checkpoint=weights_path(cfg.model),
                                       iter_threshold=0.0, max_points=cfg.N))
@@ -105,8 +110,9 @@ def main():
     timed_steps = split[-args.steps:]  # the events of the timed window (all recorded and synchronised by timed())
     ms_loop_world = sum(e[0].elapsed_time(e[1]) + e[2].elapsed_time(e[3]) for e in timed_steps) / args.steps
     ms_loop_planner = sum(e[1].elapsed_time(e[2]) for e in timed_steps) / args.steps
-    tests = B * R * 20  # ray-obstacle tests of one scan (20 circles per environment)
-    print(json.dumps(dict(metric="batched world: scan + step vs PlannerBatch.forward", envs=B, beams=R, obstacles_per_env=20,
+    tests = R * (n_circles + n_edges)  # ray-boundary tests of one scan: every beam against every circle and polygon edge
+    print(json.dumps(dict(metric="batched world: scan + step vs PlannerBatch.forward", scene=args.scene, envs=B, beams=R,
+                          obstacles_per_env=n_obs / B, circles_per_env=n_circles / B, edges_per_env=n_edges / B,
                           steps=args.steps, warmup=args.warmup, ms_scan=ms_scan, ms_world_scan_step=ms_world, ms_planner_forward=ms_planner,
                           ms_closed_loop_step=ms_loop, ms_closed_loop_world=ms_loop_world, ms_closed_loop_planner=ms_loop_planner,
                           world_share_of_closed_loop=ms_loop_world / ms_loop,
