@@ -192,7 +192,7 @@ int nb_pan_read_screen_stats(nb_pan_t* pan, float* max_error_ratio, int32_t* cou
  * sum_e |G_e p - h_e| on the 4 x 4 sub-grid of every cell. */
 int nb_pan_read_screen_table(nb_pan_t* pan, float info[5]);
 
-/* Diagnostics of the last executed NRMP solve: interior point iterations per env (B) int32. */
+/* Diagnostics of the last executed NRMP solve (nb_pan_forward or nb_nrmp_forward): interior point iterations per env (B) int32. */
 int nb_pan_read_diagnostics(nb_pan_t* pan, int32_t B, int32_t* ipm_iterations, void* stream);
 
 /* ---- the two halves, exposed separately (parity tests, profiling) ------------------------ */

@@ -20,7 +20,8 @@
 // start: cold (u = 0, D mid-range) or WARM from the previous PAN iteration's solution of the same environment
 // (x pulled 5 % towards the centre, slacks recomputed from it, multipliers floored at mu0 / s): ~10 iterations.
 // Inside each Newton step the T*M hinge rows and the T distances D_t are eliminated analytically (both blocks are
-// diagonal), so the only factorisation is a dense 2T x 2T Cholesky in the warp's shared memory.
+// diagonal), so the only factorisation is a dense 2T x 2T Cholesky: blocked, in the registers of the tensor-pipe assembly, for
+// the compile-time (T, M) specialisations; in the warp's shared memory otherwise.
 //
 // Mapping: lanes own rows of the 2T x 2T system (triangular solves run in registers with
 // shuffles), lanes own HPL hinge rows each whose slack/multiplier state lives in registers, lanes
@@ -218,14 +219,79 @@ __device__ __forceinline__ void nrmp_stop_env(const NrmpParams& prm, const int b
   }
 }
 
+// Cholesky factor of the reduced Hessian held as the lower-triangular 8x8 tiles of the DMMA accumulators: tile (I, J), J <= I,
+// at w0/w1[I(I+1)/2 + J], lane 4g + q holding rows 8I + g, columns 8J + 2q (w0) and 8J + 2q + 1 (w1).  Rows nU..8NT-1 are
+// identity padding.  Right-looking by block columns: the diagonal tile and the panel below it column by column with quad
+// shuffles, then the trailing SYRK / GEMM updates on the FP64 tensor pipe, L_IJ -= L_IK L_JK' as two m8n8k4 k-steps.  Their
+// k-index runs over the columns in the order (2q | 2q + 1), which is the accumulator layout itself: the finished tiles are the
+// operands as they are.  L goes to the staircase H[hrow(i) + j] and 1/L_ii to `invd` of lane i, as the unblocked factorisation
+// leaves them.  Returns false at a pivot that is not positive (or NaN); the padding never reaches a pivot.
+template <int NT, int NU>
+__device__ __forceinline__ bool nrmp_block_cholesky(double (&w0)[NT * (NT + 1) / 2], double (&w1)[NT * (NT + 1) / 2], double* H, double& invd,
+                                                    const int lane) {
+  const int q = lane & 3, g = lane >> 2, quad = lane & ~3;
+#pragma unroll
+  for (int K = 0; K < NT; ++K) {
+    const int kd = K * (K + 1) / 2 + K;
+    const int ncol = NU - 8 * K < 8 ? NU - 8 * K : 8;  // padded columns of the last block are not factored
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      if (k >= ncol) break;
+      const int src = k >> 1;
+      const bool hi = (k & 1) != 0;
+      const double piv = __shfl_sync(0xffffffffu, hi ? w1[kd] : w0[kd], 4 * k + src);
+      const double c0 = __shfl_sync(0xffffffffu, hi ? w1[kd] : w0[kd], 8 * q + src);      // A_KK[2q][k]
+      const double c1 = __shfl_sync(0xffffffffu, hi ? w1[kd] : w0[kd], 8 * q + 4 + src);  // A_KK[2q + 1][k]
+      double own[NT];  // A_XK[g][k] of this lane's row in every tile of the block column
+#pragma unroll
+      for (int X = K; X < NT; ++X) {
+        const int xi = X * (X + 1) / 2 + K;
+        own[X] = __shfl_sync(0xffffffffu, hi ? w1[xi] : w0[xi], quad + src);
+      }
+      if (!(piv > 0.0)) return false;
+      const double ild = rsqrt64(piv);
+      if (lane == 8 * K + k) invd = ild;
+      const double l0 = c0 * ild, l1 = c1 * ild;  // L_KK[2q][k], L_KK[2q + 1][k]
+#pragma unroll
+      for (int X = K; X < NT; ++X) {
+        const int xi = X * (X + 1) / 2 + K;
+        const double l = own[X] * ild;  // L_XK[g][k]
+        if (q == src) {
+          if (hi) w1[xi] = l; else w0[xi] = l;
+        }
+        if (2 * q > k) w0[xi] = fma(-l, l0, w0[xi]);
+        if (2 * q + 1 > k) w1[xi] = fma(-l, l1, w1[xi]);
+      }
+    }
+#pragma unroll
+    for (int X = K; X < NT; ++X) {  // block column K is final
+      const int xi = X * (X + 1) / 2 + K, i = 8 * X + g, j = 8 * K + 2 * q;
+      if (i < NU && j <= i) H[((i * (i + 3)) >> 1) + j] = w0[xi];
+      if (i < NU && j + 1 <= i) H[((i * (i + 3)) >> 1) + j + 1] = w1[xi];
+    }
+#pragma unroll
+    for (int I = K + 1; I < NT; ++I) {
+      const int ik = I * (I + 1) / 2 + K;
+#pragma unroll
+      for (int J = K + 1; J <= I; ++J) {
+        const int ij = I * (I + 1) / 2 + J, jk = J * (J + 1) / 2 + K;
+        dmma884(w0[ij], w1[ij], -w0[ik], w0[jk]);
+        dmma884(w0[ij], w1[ij], -w1[ik], w1[jk]);
+      }
+    }
+  }
+  __syncwarp();
+  return true;
+}
+
 // SMALL: 2T <= 32, every lane owns at most one row of the reduced system (one register slot in the
 // triangular solves); the general version (T <= 32) carries a second slot.
 // TT, MM: compile-time horizon / hinge rows per step (0 = read them from the parameters).  With constants every
 // workspace offset, loop bound and row stride folds into immediates -- half of the generic kernel's
 // instructions were integer address arithmetic.
-// Residency: the (10, 10) specialisation is built for 7 CTAs (14 warps) per SM -- 128 registers with ~200 B of spills and
-// 29 KB of shared memory per CTA.  At B = 4096 that is 2072 resident solves = two full rounds instead of 2.3 rounds of
-// 1776.  (__maxnreg__(144) instead of the min-blocks bound makes ptxas spill more.)
+// Residency: the (10, 10) specialisation is built for 5 CTAs of 3 warps (15 warps) per SM (NB_NRMP_WPC) -- 128 registers with
+// ~240 B of spill stores, and ~43 KB of shared memory per CTA, which also caps the SM at 15 warps.  At B = 4096 that is 1980
+// resident solves on 132 SMs.  (__maxnreg__(144) instead of the min-blocks bound makes ptxas spill more.)
 template <int HPL, bool SMALL, int TT, int MM>
 __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int b, double* wsp, const unsigned short* __restrict__ ptab, const int lane) {
   const int T = TT > 0 ? TT : prm.T, M = TT > 0 ? MM : prm.M, T1 = T + 1;
@@ -243,9 +309,18 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
 #ifndef NB_NRMP_UNROLL_SOLVE
 #define NB_NRMP_UNROLL_SOLVE 1
 #endif
+#ifndef NB_NRMP_CHOL_TWICE
+#define NB_NRMP_CHOL_TWICE 0
+#endif
+#ifndef NB_NRMP_BLOCKCHOL
+#define NB_NRMP_BLOCKCHOL 1
+#endif
   constexpr int kUnrollSolve = (TT > 0 && NB_NRMP_UNROLL_SOLVE) ? 32 : 2;
   constexpr int kUnrollCholK = (TT > 0 && NB_NRMP_UNROLL_CHOL) ? 16 : 1, kUnrollCholP = (TT > 0 && NB_NRMP_UNROLL_CHOL) ? 32 : 4;
   const bool kDmma = NB_NRMP_DMMA != 0 && SMALL && TD > 0;  // Hessian assembly on the FP64 tensor pipe (2T <= 32, obstacles present)
+  // compile-time (T, M) with DMMA assembly: the Hessian tiles stay in the accumulators and are factored there (nrmp_block_cholesky)
+  constexpr bool kBlockChol = NB_NRMP_BLOCKCHOL != 0 && NB_NRMP_DMMA != 0 && SMALL && TT > 0 && MM > 0;
+  constexpr int kNT = TT > 0 ? (2 * TT + 7) / 8 : 1, kTiles = kNT * (kNT + 1) / 2;
 
   // ---- carve this warp's workspace -------------------------------------------------------
   const int FT = T * (T + 1);                      // packed size of one component of F / G
@@ -646,6 +721,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
         }
       }
       __syncwarp();
+      double tl0[kTiles], tl1[kTiles];  // kBlockChol: the Hessian tiles of (c), factored in place by (d)
       if (kDmma) {
         // V (packed like F, in the Gx | Gy scratch): row 2t = r00 Fx_t + r01 Fy_t, row 2t+1 = r11 Fy_t
         NB_LL(j, nU) {
@@ -685,6 +761,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int i = ia, j = j0 + 2 * q + e;
+              if constexpr (kBlockChol) (e ? tl1 : tl0)[I * (I + 1) / 2 + J] = i == j ? 1.0 : 0.0;  // padding: identity; diagonal tiles: 0 above
               if (i < nU && j <= i) {
                 double acc = Hc[(i * (i + 1) >> 1) + j] + (e ? c1 : c0);
                 if (i == j) {
@@ -694,7 +771,8 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
                 } else if (i == j + 2) {
                   acc -= cz[oRU + j] * (double)cis[oRU + j] + cz[oRL + j] * (double)cis[oRL + j];
                 }
-                H[hrow(i) + j] = acc;
+                if constexpr (kBlockChol) (e ? tl1 : tl0)[I * (I + 1) / 2 + J] = acc;
+                else H[hrow(i) + j] = acc;
               }
             }
           }
@@ -739,12 +817,34 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
       }
       }
       __syncwarp();
-      // (d) Cholesky, left-looking; lane owns rows lane, lane+32; inverse diagonal in registers.
-      //     SMALL: two columns per step (nU = 2T is even) -- row i is read once for both dot products, which are two
-      //     independent FMA chains; the second column then takes the rank-1 correction of the first.
+      // (d) Cholesky.  kBlockChol: blocked, on the tiles of (c) (nrmp_block_cholesky).  Otherwise left-looking; lane owns rows
+      //     lane, lane+32; inverse diagonal in registers.  SMALL: two columns per step (nU = 2T is even) -- row i is read once
+      //     for both dot products, which are two independent FMA chains; the second column then takes the rank-1 correction
+      //     of the first.
       bool bad = false;
+#if NB_NRMP_CHOL_TWICE
+      // timing only (NB_NRMP_CHOL_TWICE): (d) runs twice on the same Hessian -- the unblocked form restores H from `scratch`
+      // (dead here) in between; results and iteration counts are unchanged, so the difference in launch time is the cost of
+      // one factorisation (plus the copies)
+      if (!kBlockChol) {
+        NB_LL(p, nP) scratch[p] = H[hrow(ptab[p] >> 8) + (ptab[p] & 255)];
+        __syncwarp();
+      }
+#pragma unroll 1
+      for (int rep = 0; rep < 2; ++rep) {
+      if (rep == 1 && !kBlockChol) {
+        NB_LL(p, nP) H[hrow(ptab[p] >> 8) + (ptab[p] & 255)] = scratch[p];
+        __syncwarp();
+      }
+      bad = false;
+#endif
       invd0 = 0.0; invd1 = 0.0;
-      if (SMALL) {
+      if constexpr (kBlockChol) {
+        double w0[kTiles], w1[kTiles];
+#pragma unroll
+        for (int i = 0; i < kTiles; ++i) { w0[i] = tl0[i]; w1[i] = tl1[i]; }
+        bad = !nrmp_block_cholesky<kNT, 2 * TT>(w0, w1, H, invd0, lane);
+      } else if (SMALL) {
 #pragma unroll(kUnrollCholK)
         for (int k = 0; k < nU; k += 2) {
           const double* rowk = H + hrow(k);
@@ -805,6 +905,9 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
           __syncwarp();
         }
       }
+#if NB_NRMP_CHOL_TWICE
+      }
+#endif
       if (bad) {  // H lost definiteness: at barrier weights of 1e13+ that is rounding, and the iterate is already the optimum
         if (accept_gap) converged = true;
         else stat |= 2;

@@ -801,6 +801,7 @@ int nb_nrmp_forward(nb_pan_t* p, int32_t B, const float* nom_s, const float* nom
   nb::NrmpParams prm{};
   prm.nom_s = nom_s; prm.nom_u = nom_u; prm.ref_s = ref_s; prm.ref_us = ref_us; prm.fa = fa; prm.fb = fb;
   prm.out_s = out_s; prm.out_u = out_u; prm.out_d = out_d; prm.status = out_status;
+  prm.ipm_iters = p->ipm_it;  // nb_pan_read_diagnostics
   prm.B = B;
   return launch_nrmp(p, prm, (cudaStream_t)stream);
 }
