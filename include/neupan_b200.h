@@ -57,8 +57,8 @@ typedef struct {
   int32_t max_envs;       /* capacity: largest B of any later call                   */
   int32_t max_points;     /* capacity: largest N of any later call (after decimation).  The exact and warpgroup screening DUNE
                              kernels hold the operand image, two 16 KB tiles and per-point keys / mu in shared memory: on an H100
-                             (227 KB per block) N up to ~7000 at E = 4, ~4000 at E = 8; a larger N fails at launch with
-                             NB_ERR_CUDA ("N=... needs ... B of shared memory"). */
+                             (227 KB per block) N up to 6981 at E = 4, 4188 at E = 8 (M = 10); a larger N fails at launch with
+                             NB_ERR_CAPACITY ("N=... needs ... B of shared memory"). */
   int32_t device;         /* CUDA device ordinal                                     */
   float iter_threshold;   /* pan.py:52; <= 0 never stops early                       */
   /* Python floats in the reference (float64 constants of the convex program): */
