@@ -360,6 +360,30 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
  * Enqueued on `stream` without synchronising. */
 int nb_world_read_state(nb_world_t* w, int32_t B, double* states, double* obstacles, int32_t* collided, int32_t* arrived, void* stream);
 
+/* Obstacle behaviours: behaviors (O,13) float64 HOST rows
+ *   [kind (0 constant velocity, 1 rvo), vxmax, vymax, acce, factor, speed, wander (0 | 1), goal_x, goal_y (NaN, NaN: draw 0),
+ *    goal_threshold, neighbor_range, grid, min_speed]
+ * A kind-0 row keeps the obstacle's constant velocity (its other columns are not read).  A kind-1 obstacle is reactive: before every
+ * nb_world_step moves anything, it heads for its goal at `speed` and steers around the other obstacles and the robot with a
+ * reciprocal velocity obstacle, choosing from a grid of candidate velocities (this project's reading of IR-SIM's `rvo` behaviour,
+ * stated in full in csrc/world_rvo_kernel.cuh); with `wander` it draws a new goal in its rectangle on arrival, without it it parks.
+ * Goals are drawn from SplitMix64 streams keyed by (seed, environment, obstacle index within it, draw number).
+ * Checks (NB_ERR_INVALID, with the obstacle index): kind 0 or 1; finite values (a NaN goal requests draw 0); positive vxmax, vymax,
+ * acce, factor, speed, goal_threshold, neighbor_range, grid and min_speed >= 0; at most 64 candidates per axis
+ * (ceil(2 min(acce, vmax) / grid)); a reactive obstacle's centre inside its rectangle, vmax * step_time below the rectangle's extent,
+ * and an explicit goal inside the rectangle.
+ * nb_world_check_behaviors checks scenes and behaviours on the host without a handle or a device.  nb_world_set_behaviors applies
+ * them to the current state of a handle's scenes (their current centres) and synchronises the device; nb_world_set_scenes(_ex) makes
+ * every obstacle kind 0 again.  A world without a kind-1 obstacle launches nothing more per step than one without behaviours. */
+int nb_world_check_behaviors(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles,
+                             const int32_t* vert_begin, const double* vertices, const double* envs, const int32_t* obs_kind,
+                             const double* behaviors, uint64_t seed);
+int nb_world_set_behaviors(nb_world_t* w, int32_t B, const double* behaviors, uint64_t seed);
+
+/* The current goals (O,2) float64 and goal draw counters (O) int32 (the draws made so far), DEVICE outputs, either may be NULL;
+ * enqueued on `stream` without synchronising.  NB_ERR_INVALID before nb_world_set_behaviors. */
+int nb_world_read_behaviors(nb_world_t* w, int32_t B, double* goals, int32_t* draws, void* stream);
+
 /* ---- DUNE training on the device (SURVEY 8f "next" row 4) ------------------------------------------------------------ */
 
 /* DUNETrain.generate_data_set / prob_solve (neupan/blocks/dune_train.py:100-140): labels of n sampled points -- the solution of the

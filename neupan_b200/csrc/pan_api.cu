@@ -18,6 +18,7 @@
 #include "dune_train_kernel.cuh"
 #include "dune_table_kernel.cuh"
 #include "world_kernel.cuh"
+#include "world_rvo_kernel.cuh"
 
 #include <algorithm>
 #include <vector>
@@ -101,6 +102,12 @@ const char* world_outline_problem(const double* v, int n) {
       if (world_segs_meet(v + 2 * i, v + 2 * ((i + 1) % n), v + 2 * j, v + 2 * ((j + 1) % n))) return "is not simple (two edges that do not share a vertex meet)";
     }
   return nullptr;
+}
+
+// a * b rounded on its own: the host compiler may not fuse it into a following sum (the device's dmul / dadd order)
+double host_dmul(double a, double b) {
+  volatile double p = a * b;
+  return p;
 }
 
 bool world_finite(const double* a, size_t n) {
@@ -193,6 +200,45 @@ int world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* obs
   return NB_OK;
 }
 
+// Every check of nb_world_set_behaviors on the rows (kWorldBehCols) of valid scenes; obs holds the obstacles' current centres.
+int world_check_behaviors(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obs, const double* envs,
+                          const double* beh) {
+  if (!beh) return fail(NB_ERR_INVALID, "nb_world behaviors: null behaviors");
+  const double dt = cfg->step_time;
+  for (int b = 0; b < B; ++b) {
+    const double* e = envs + (size_t)nb::kWorldEnvCols * b;
+    for (int o = obs_begin[b]; o < obs_begin[b + 1]; ++o) {
+      const double* r = beh + (size_t)nb::kWorldBehCols * o;
+      if (r[0] == 0.0) continue;  // constant velocity: the other columns are not read
+      if (r[0] != 1.0) return fail(NB_ERR_INVALID, "obstacle %d has behaviour kind %g (0: constant velocity, 1: rvo)", o, r[0]);
+      for (int c = 1; c < nb::kWorldBehCols; ++c)
+        if (c != 7 && c != 8 && !std::isfinite(r[c])) return fail(NB_ERR_INVALID, "obstacle %d: behaviour column %d is not finite", o, c);
+      const bool draw = std::isnan(r[7]) && std::isnan(r[8]);
+      if (!draw && (!std::isfinite(r[7]) || !std::isfinite(r[8])))
+        return fail(NB_ERR_INVALID, "obstacle %d: the goal must be finite, or NaN in both coordinates (drawn)", o);
+      static const char* const names[] = {nullptr, "vxmax", "vymax", "acce", "factor", "speed", nullptr, nullptr, nullptr, "goal_threshold",
+                                          "neighbor_range", "grid"};
+      for (int c : {1, 2, 3, 4, 5, 9, 10, 11})
+        if (!(r[c] > 0)) return fail(NB_ERR_INVALID, "obstacle %d: %s must be positive", o, names[c]);
+      if (!(r[12] >= 0)) return fail(NB_ERR_INVALID, "obstacle %d: min_speed must be >= 0", o);
+      if (r[6] != 0.0 && r[6] != 1.0) return fail(NB_ERR_INVALID, "obstacle %d: wander must be 0 or 1", o);
+      for (int a = 0; a < 2; ++a) {
+        const double span = 2.0 * std::min(r[3], r[1 + a]), n = std::ceil(span / r[11]);
+        if (n > nb::kWorldRvoMaxAxis)
+          return fail(NB_ERR_INVALID, "obstacle %d: up to %.0f candidate velocities on an axis (at most %d)", o, n, nb::kWorldRvoMaxAxis);
+      }
+      for (int a = 0; a < 2; ++a) {
+        const double lo = e[a], hi = e[2 + a];
+        if (obs[(size_t)nb::kWorldObsCols * o + a] < lo || obs[(size_t)nb::kWorldObsCols * o + a] > hi)
+          return fail(NB_ERR_INVALID, "obstacle %d is reactive but its centre starts outside the rectangle of environment %d", o, b);
+        if (!(r[1 + a] * dt < hi - lo)) return fail(NB_ERR_INVALID, "obstacle %d: %s * step_time exceeds the rectangle of environment %d", o, names[1 + a], b);
+        if (!draw && (r[7 + a] < lo || r[7 + a] > hi)) return fail(NB_ERR_INVALID, "obstacle %d: its goal lies outside the rectangle of environment %d", o, b);
+      }
+    }
+  }
+  return NB_OK;
+}
+
 }  // namespace
 
 struct nb_ipath {
@@ -217,6 +263,18 @@ struct nb_world {
   int32_t *d_collided = nullptr, *d_arrived = nullptr;
   double *d_vertices = nullptr, *d_env = nullptr, *d_obs = nullptr, *d_states = nullptr;
   double* d_beam_cs = nullptr;  // (R, 2), fixed at creation
+  // host copies of the scene (nb_world_set_behaviors checks against them)
+  std::vector<int32_t> h_obs_begin, h_vert_begin;
+  std::vector<double> h_vertices, h_env;
+  // obstacle behaviours (nb_world_set_behaviors; nb_world_set_scenes clears them): has_rvo false -> nb_world_step launches only
+  // world_step_kernel
+  bool has_rvo = false;
+  uint64_t seed = 0;
+  int rvo_cap = 0, rvo_grid = 0;
+  size_t rvo_smem = 0;
+  double robot_r = 0.0;
+  double *d_beh = nullptr, *d_rad = nullptr, *d_goal = nullptr;
+  int32_t* d_draws = nullptr;
 };
 
 struct nb_dune_train {
@@ -1449,7 +1507,7 @@ int nb_world_destroy(nb_world_t* w) {
   if (!w) return NB_OK;
   cudaSetDevice(w->cfg.device);
   void* bufs[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
-                  w->d_states, w->d_beam_cs};
+                  w->d_states, w->d_beam_cs, w->d_beh, w->d_rad, w->d_goal, w->d_draws};
   for (void* b : bufs)
     if (b) cudaFree(b);
   delete w;
@@ -1479,12 +1537,17 @@ int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, c
     for (int k = 0; k < 3; ++k) states[3 * b + k] = envs[(size_t)nb::kWorldEnvCols * b + 4 + k];
   NB_CUDA(cudaSetDevice(w->cfg.device));
   void* old[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
-                 w->d_states};
+                 w->d_states, w->d_beh, w->d_rad, w->d_goal, w->d_draws};
   for (void* b : old)
     if (b) cudaFree(b);
-  w->d_obs_begin = w->d_vert_begin = w->d_slot = w->d_counts = w->d_kind = w->d_collided = w->d_arrived = nullptr;
-  w->d_vertices = w->d_env = w->d_obs = w->d_states = nullptr;
+  w->d_obs_begin = w->d_vert_begin = w->d_slot = w->d_counts = w->d_kind = w->d_collided = w->d_arrived = w->d_draws = nullptr;
+  w->d_vertices = w->d_env = w->d_obs = w->d_states = w->d_beh = w->d_rad = w->d_goal = nullptr;
   w->B = 0;
+  w->has_rvo = false;  // new scenes: every obstacle keeps a constant velocity until nb_world_set_behaviors
+  w->h_obs_begin.assign(obs_begin, obs_begin + B + 1);
+  w->h_vert_begin.assign(vert_begin, vert_begin + O + 1);
+  w->h_vertices.assign(vertices, vertices + 2 * (size_t)V);
+  w->h_env.assign(envs, envs + (size_t)nb::kWorldEnvCols * B);
   NB_CUDA(dalloc(&w->d_obs_begin, (size_t)B + 1));
   NB_CUDA(dalloc(&w->d_vert_begin, (size_t)O + 1));
   NB_CUDA(dalloc(&w->d_slot, (size_t)O));
@@ -1551,9 +1614,106 @@ int world_ready(const nb_world* w, int32_t B, const char* what) {
   if (B != w->B) return fail(NB_ERR_INVALID, "%s: B = %d but the scenes were set for %d environments", what, B, w->B);
   return NB_OK;
 }
+
+nb::WorldRvoParams world_rvo_params(const nb_world* w, const float* action) {
+  nb::WorldRvoParams rp;
+  rp.beh = w->d_beh; rp.radius = w->d_rad; rp.goal = w->d_goal; rp.draws = w->d_draws; rp.action = action;
+  rp.seed = w->seed; rp.robot_r = w->robot_r; rp.cap = w->rvo_cap;
+  return rp;
+}
 }  // namespace
 
 extern "C" {
+
+int nb_world_check_behaviors(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                             const double* vertices, const double* envs, const int32_t* obs_kind, const double* behaviors, uint64_t seed) {
+  (void)seed;  // every seed is valid: drawn goals lie in the rectangle by construction
+  if (int rc = world_check_scenes(cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, obs_kind, nullptr, nullptr, nullptr, nullptr)) return rc;
+  return world_check_behaviors(cfg, B, obs_begin, obstacles, envs, behaviors);
+}
+
+int nb_world_set_behaviors(nb_world_t* w, int32_t B, const double* behaviors, uint64_t seed) {
+  if (int rc = world_ready(w, B, "nb_world_set_behaviors")) return rc;
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  const int O = w->O;
+  std::vector<double> obs((size_t)nb::kWorldObsCols * O);
+  if (O) NB_CUDA(cudaMemcpy(obs.data(), w->d_obs, sizeof(double) * obs.size(), cudaMemcpyDeviceToHost));  // the current centres
+  if (int rc = world_check_behaviors(&w->cfg, B, w->h_obs_begin.data(), obs.data(), w->h_env.data(), behaviors)) return rc;
+  // radii (circle: its own; polygon: the largest vertex norm), initial goals (NaN: draw 0) and draw counters
+  std::vector<double> rad(O), goal(2 * (size_t)O, 0.0);
+  std::vector<int32_t> draws(O, 0);
+  bool any = false;
+  int max_n = 0;
+  for (int b = 0; b < B; ++b) {
+    const int o0 = w->h_obs_begin[b], o1 = w->h_obs_begin[b + 1];
+    const double* e = w->h_env.data() + (size_t)nb::kWorldEnvCols * b;
+    max_n = std::max(max_n, o1 - o0);
+    for (int o = o0; o < o1; ++o) {
+      const int v0 = w->h_vert_begin[o], v1 = w->h_vert_begin[o + 1];
+      double r = v0 == v1 ? obs[(size_t)nb::kWorldObsCols * o + 4] : 0.0;
+      for (int k = v0; k < v1; ++k) {
+        const double x = w->h_vertices[2 * k], y = w->h_vertices[2 * k + 1];
+        r = std::max(r, std::sqrt(host_dmul(x, x) + host_dmul(y, y)));
+      }
+      rad[o] = r;
+      const double* row = behaviors + (size_t)nb::kWorldBehCols * o;
+      if (row[0] != 1.0) continue;
+      any = true;
+      if (std::isnan(row[7])) {
+        const uint64_t key = nb::world_rvo_key(seed, b, o - o0);
+        goal[2 * o] = e[0] + host_dmul(nb::world_u01(nb::splitmix64_at(key, 0)), e[2] - e[0]);  // draw 0
+        goal[2 * o + 1] = e[1] + host_dmul(nb::world_u01(nb::splitmix64_at(key, 1)), e[3] - e[1]);
+        draws[o] = 1;
+      } else {
+        goal[2 * o] = row[7]; goal[2 * o + 1] = row[8];
+      }
+    }
+  }
+  double robot_r = 0.0;
+  for (int k = 0; k < w->cfg.robot_num_vertices; ++k) {
+    const double x = w->cfg.robot_vertices[2 * k], y = w->cfg.robot_vertices[2 * k + 1];
+    robot_r = std::max(robot_r, std::sqrt(host_dmul(x, x) + host_dmul(y, y)));
+  }
+  void* old[] = {w->d_beh, w->d_rad, w->d_goal, w->d_draws};
+  for (void* p : old)
+    if (p) cudaFree(p);
+  w->d_beh = w->d_rad = w->d_goal = nullptr;
+  w->d_draws = nullptr;
+  w->has_rvo = false;
+  NB_CUDA(dalloc(&w->d_beh, (size_t)nb::kWorldBehCols * O));
+  NB_CUDA(dalloc(&w->d_rad, (size_t)O));
+  NB_CUDA(dalloc(&w->d_goal, 2 * (size_t)O));
+  NB_CUDA(dalloc(&w->d_draws, (size_t)O));
+  if (O) {
+    NB_CUDA(cudaMemcpy(w->d_beh, behaviors, sizeof(double) * nb::kWorldBehCols * O, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemcpy(w->d_rad, rad.data(), sizeof(double) * O, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemcpy(w->d_goal, goal.data(), sizeof(double) * 2 * O, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemcpy(w->d_draws, draws.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice));
+  }
+  // launch shape: the largest environment's rows (+ the robot) and one cone list per warp in shared memory
+  w->seed = seed; w->robot_r = robot_r;
+  w->rvo_cap = max_n + 1;
+  w->rvo_smem = (size_t)w->rvo_cap * (5 * sizeof(double) + nb::kWorldRvoWarps * (6 * sizeof(double) + sizeof(int32_t)));
+  NB_CUDA(cudaFuncSetAttribute(nb::world_rvo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
+  int per_sm = 0, sms = 0;
+  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_rvo_kernel, 32 * nb::kWorldRvoWarps, w->rvo_smem));
+  NB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->cfg.device));
+  if (per_sm < 1) return fail(NB_ERR_CUDA, "world_rvo_kernel: %zu B of shared memory do not fit", w->rvo_smem);
+  w->rvo_grid = std::min(B, per_sm * sms);
+  w->has_rvo = any;
+  NB_CUDA(cudaDeviceSynchronize());
+  return NB_OK;
+}
+
+int nb_world_read_behaviors(nb_world_t* w, int32_t B, double* goals, int32_t* draws, void* stream) {
+  if (int rc = world_ready(w, B, "nb_world_read_behaviors")) return rc;
+  if (!w->d_goal) return fail(NB_ERR_INVALID, "nb_world_read_behaviors: no behaviours set (nb_world_set_behaviors)");
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (goals && w->O) NB_CUDA(cudaMemcpyAsync(goals, w->d_goal, sizeof(double) * 2 * w->O, cudaMemcpyDeviceToDevice, st));
+  if (draws && w->O) NB_CUDA(cudaMemcpyAsync(draws, w->d_draws, sizeof(int32_t) * w->O, cudaMemcpyDeviceToDevice, st));
+  return NB_OK;
+}
 
 int nb_world_scan(nb_world_t* w, int32_t B, float* ranges, float* velocity, int32_t* hit, void* stream) {
   if (int rc = world_ready(w, B, "nb_world_scan")) return rc;
@@ -1573,6 +1733,12 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
   if (int rc = world_ready(w, B, "nb_world_step")) return rc;
   if (!action) return fail(NB_ERR_INVALID, "nb_world_step: null action");
   NB_CUDA(cudaSetDevice(w->cfg.device));
+  if (w->has_rvo) {  // reactive obstacles choose their velocities from the states at the start of the step
+    NB_CUDA(cudaFuncSetAttribute(nb::world_rvo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
+    nb::world_rvo_kernel<<<w->rvo_grid, 32 * nb::kWorldRvoWarps, w->rvo_smem, (cudaStream_t)stream>>>(world_params(w), world_rvo_params(w, action));
+    ++g_launches;
+    NB_CUDA(cudaGetLastError());
+  }
   nb::world_step_kernel<<<(B + nb::kWorldStepWarps - 1) / nb::kWorldStepWarps, 32 * nb::kWorldStepWarps, 0, (cudaStream_t)stream>>>(
       world_params(w), action, collided, arrived, clearance);
   ++g_launches;

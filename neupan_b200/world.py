@@ -10,13 +10,24 @@ A scene (one environment) is a dict with the sections of an ``env.yaml``:
     obstacles       list of dicts: {"center": (x, y), "radius": r} (circle), {"center": (x, y), "vertices": [[dx, dy], ...]}
                     (convex polygon, 3..8 vertices relative to the centre) or {"center": (x, y), "outline": [[dx, dy], ...]} (any
                     simple polygon, convex or not, either orientation, 3..16 vertices relative to the centre), each with an
-                    optional "velocity": (vx, vy) in the world frame (constant; default still; polygons do not rotate).  At most
-                    256 obstacles and 2048 polygon edges (convex and outline together) per environment.
+                    optional "velocity": (vx, vy) in the world frame (constant unless the obstacle has a behaviour; default
+                    still; polygons do not rotate) and an optional "behavior" (below).  At most 256 obstacles and 2048 polygon
+                    edges (convex and outline together) per environment.
     bounds          (xmin, ymin, xmax, ymax): a moving obstacle whose centre leaves this rectangle is mirrored back into it and
                     that velocity component is reversed
     start           (x, y, theta) of the robot
     goal            (x, y); goal_threshold: the robot has arrived when it is closer than this to the goal
     path            optional (n, 4) rows [x, y, theta, gear]: an initial path for the planner (the scene builders add one)
+
+An obstacle's "behavior" is {"name": "constant"} (the default) or {"name": "rvo", "vxmax", "vymax", ...} (keys and defaults in
+``RVO_DEFAULTS``): a reactive obstacle that heads for a goal at ``speed`` and steers around the other obstacles and the robot with a
+reciprocal velocity obstacle over a grid of candidate velocities, before every step moves anything; with ``wander`` it draws a new
+goal uniformly in its rectangle on arrival (``goal_threshold``), without it it parks.  This is this project's reading of IR-SIM's
+``rvo`` behaviour (IR-SIM is not a dependency), stated in full in csrc/world_rvo_kernel.cuh.  Stated differences from IR-SIM: all
+velocities of a step are chosen from the states at its start (IR-SIM updates its objects one after another), obstacles are
+holonomic (IR-SIM turns its diff obstacles), every neighbour is a circle (a polygon's circumradius about its centre, the robot's about
+its state point), and the candidates are lo + k grid (np.arange can differ in the last bit).  Goals are drawn from counter-based
+SplitMix64 streams keyed by (seed, environment, obstacle index within it, draw number), so a run is reproducible from its seed.
 
 There is no CPU implementation here: the CUDA library is the product (oracle/world.py restates it for the tests).
 """
@@ -31,6 +42,10 @@ import torch
 from . import _lib
 
 ENV_COLS = 10  # xmin, ymin, xmax, ymax, start x, y, theta, goal x, y, goal threshold
+BEH_COLS = 13  # kind, vxmax, vymax, acce, factor, speed, wander, goal x, y, goal threshold, neighbor range, grid, min speed
+# the keys of an "rvo" behaviour besides vxmax and vymax (required); speed None: min(vxmax, vymax); goal None: drawn
+RVO_DEFAULTS = dict(acce=1.0, factor=1.0, speed=None, wander=False, goal=None, goal_threshold=0.3, neighbor_range=10.0, grid=0.05,
+                    min_speed=0.3)
 
 
 def make_config(robot, lidar: dict, step_time: float, max_envs: int, device: int = 0) -> _lib.WorldConfig:
@@ -85,6 +100,31 @@ def pack_scenes(scenes):
     return packed[:5]
 
 
+def pack_behaviors(scenes) -> np.ndarray:
+    """Scenes -> the (O, 13) float64 rows of nb_world_set_behaviors, in pack_scenes_ex's obstacle order: [kind (0 constant, 1 rvo),
+    vxmax, vymax, acce, factor, speed, wander, goal x, goal y (NaN: drawn), goal_threshold, neighbor_range, grid, min_speed]."""
+    rows = []
+    for sc in scenes:
+        for ob in sc["obstacles"]:
+            beh = dict(ob.get("behavior") or {"name": "constant"})
+            name = beh.pop("name", None)
+            if name == "constant" and not beh:
+                rows.append(np.zeros(BEH_COLS))
+                continue
+            if name != "rvo":
+                raise ValueError(f"unknown obstacle behaviour {ob.get('behavior')!r} (\"constant\" or \"rvo\")")
+            unknown = set(beh) - set(RVO_DEFAULTS) - {"vxmax", "vymax"}
+            if unknown or "vxmax" not in beh or "vymax" not in beh:
+                raise ValueError(f"an rvo behaviour needs vxmax and vymax and takes {sorted(RVO_DEFAULTS)} (got {sorted(beh)})")
+            p = dict(RVO_DEFAULTS, **beh)
+            vxmax, vymax = float(p["vxmax"]), float(p["vymax"])
+            speed = min(vxmax, vymax) if p["speed"] is None else float(p["speed"])
+            goal = (math.nan, math.nan) if p["goal"] is None else tuple(float(v) for v in p["goal"])
+            rows.append(np.array([1.0, vxmax, vymax, p["acce"], p["factor"], speed, 1.0 if p["wander"] else 0.0, *goal,
+                                  p["goal_threshold"], p["neighbor_range"], p["grid"], p["min_speed"]], np.float64))
+    return np.ascontiguousarray(np.asarray(rows, np.float64).reshape(-1, BEH_COLS))
+
+
 def _host_ptrs(packed):
     return [C.c_void_p(a.ctypes.data) for a in packed]
 
@@ -116,14 +156,27 @@ class WorldBatch:
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
-    def set_scenes(self, scenes):
-        """Uploads B scenes, puts every robot at its start and clears the flags (env.reset)."""
+    def set_scenes(self, scenes, seed: int = 0):
+        """Uploads B scenes, puts every robot at its start and clears the flags (env.reset).  When an obstacle has a behaviour,
+        also sets the behaviours (nb_world_set_behaviors); ``seed`` keys the goal draws of reactive obstacles."""
         if len(scenes) != self.B:
             raise ValueError(f"expected {self.B} scenes, got {len(scenes)}")
         packed = pack_scenes_ex(scenes)
+        beh = pack_behaviors(scenes) if any("behavior" in ob for sc in scenes for ob in sc["obstacles"]) else None
         with torch.cuda.device(self.device):
             _lib.check(_lib.load().nb_world_set_scenes_ex(self._handle, self.B, *_host_ptrs(packed)))
-        self.O = int(packed[0][-1])
+            self.O = int(packed[0][-1])
+            if beh is not None:
+                _lib.check(_lib.load().nb_world_set_behaviors(self._handle, self.B, C.c_void_p(beh.ctypes.data), C.c_uint64(int(seed))))
+
+    def goals(self):
+        """(goals (O,2) float64, draws (O,) int32) on the device: every obstacle's current goal and the number of goals drawn for it
+        so far (zeros for constant-velocity obstacles).  Needs scenes with behaviours."""
+        g = torch.empty((self.O, 2), dtype=torch.float64, device=self.device)
+        d = torch.empty(self.O, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nb_world_read_behaviors(self._handle, self.B, C.c_void_p(g.data_ptr()), C.c_void_p(d.data_ptr()), self._stream()))
+        return g, d
 
     def _read(self, states=None, obstacles=None, collided=None, arrived=None):
         p = lambda t: C.c_void_p(0 if t is None else t.data_ptr())
@@ -238,11 +291,26 @@ def corridor(num_envs: int, seed: int = 0, circles: int = 4):
     return scenes
 
 
-def dyna_obs(num_envs: int, seed: int = 0, count: int = 20):
-    """example/dyna_obs/diff/env.yaml: ``count`` (20) circles of radius 0.4..1.0 m placed at random in the box [10, 40]^2, each
-    moving at a constant speed of at most 0.5 m/s in a random direction and bouncing inside that box (the example's RVO 'wander'
-    behaviour is out of scope), goal threshold 0.4.  The robot crosses the box: it starts at (6, y0) facing the goal (44, y1),
-    y0, y1 in 15..35 m, on a straight path."""
+# the obstacles' behaviour in example/dyna_obs and example/dyna_non_obs: {name: 'rvo', wander: True, vxmax: 0.5, vymax: 0.5}, with
+# goal threshold 0.3 for the examples' arrive_mode: position; the other keys at RVO_DEFAULTS
+EXAMPLE_RVO = dict(name="rvo", vxmax=0.5, vymax=0.5, wander=True, goal_threshold=0.3)
+
+
+def _apply_behavior(obs, behavior: str):
+    """behavior "constant": the obstacles as drawn; "rvo": the same obstacles at rest with EXAMPLE_RVO (goals drawn on the device)."""
+    if behavior == "constant":
+        return obs
+    if behavior != "rvo":
+        raise ValueError(f"behavior must be 'constant' or 'rvo' (got {behavior!r})")
+    return [dict(ob, velocity=(0.0, 0.0), behavior=dict(EXAMPLE_RVO)) for ob in obs]
+
+
+def dyna_obs(num_envs: int, seed: int = 0, count: int = 20, behavior: str = "constant"):
+    """example/dyna_obs/diff/env.yaml: ``count`` (20) circles of radius 0.4..1.0 m placed at random in the box [10, 40]^2, goal
+    threshold 0.4.  ``behavior="constant"``: each moves at a constant speed of at most 0.5 m/s in a random direction and bounces
+    inside that box.  ``behavior="rvo"``: the example's reactive obstacles (EXAMPLE_RVO: vxmax = vymax = 0.5, wander, goal threshold
+    0.3), starting at rest at the same centres.  The robot crosses the box: it starts at (6, y0) facing the goal (44, y1), y0, y1 in
+    15..35 m, on a straight path."""
     scenes = []
     for b in range(num_envs):
         rng = _rng(seed, b)
@@ -254,6 +322,7 @@ def dyna_obs(num_envs: int, seed: int = 0, count: int = 20):
         speed, heading = rng.uniform(0.0, 0.5, count), rng.uniform(-math.pi, math.pi, count)
         obs = [dict(center=(c[i, 0], c[i, 1]), radius=r[i], velocity=(speed[i] * math.cos(heading[i]), speed[i] * math.sin(heading[i])))
                for i in range(count)]
+        obs = _apply_behavior(obs, behavior)
         scenes.append(dict(obstacles=obs, bounds=(10.0, 10.0, 40.0, 40.0), start=start, goal=goal, goal_threshold=0.4,
                            path=line_path(start, goal)))
     return scenes
@@ -287,12 +356,13 @@ def _example_outline(rng, avg_radius: float, irregularity: float) -> np.ndarray:
     return random_outline(rng, avg_radius, irregularity, spikeyness, n)
 
 
-def dyna_non_obs(num_envs: int, seed: int = 0):
+def dyna_non_obs(num_envs: int, seed: int = 0, behavior: str = "constant"):
     """example/dyna_non_obs/diff/{env,planner}.yaml: 11 obstacles, each one of the example's four shapes drawn uniformly -- the
     2 x 2 m square, a circle of r = 1.5, a circle of r = 1.0, or an outline of average radius U(0.5, 1.5) and irregularity 0.9 (how
-    IR-SIM assigns a 4-entry shape list to 11 obstacles is a stated choice here).  Centres uniform in [5, 45] x [15, 35], constant
-    velocities (vx, vy) in U(-1, 1)^2, bouncing in that box (the example's RVO 'wander' behaviour is out of scope).  The robot
-    starts at (-1, 25, 0) on the planner's line path to (50, 25), its goal, with threshold 0.4."""
+    IR-SIM assigns a 4-entry shape list to 11 obstacles is a stated choice here).  Centres uniform in [5, 45] x [15, 35].
+    ``behavior="constant"``: constant velocities (vx, vy) in U(-1, 1)^2, bouncing in that box.  ``behavior="rvo"``: the example's
+    reactive obstacles (EXAMPLE_RVO), circles, squares and outlines alike, starting at rest at the same centres.  The robot starts
+    at (-1, 25, 0) on the planner's line path to (50, 25), its goal, with threshold 0.4."""
     square = [[-1.0, -1.0], [1.0, -1.0], [1.0, 1.0], [-1.0, 1.0]]
     start, goal = (-1.0, 25.0, 0.0), (50.0, 25.0)
     scenes = []
@@ -309,6 +379,7 @@ def dyna_non_obs(num_envs: int, seed: int = 0):
             else:
                 ob["outline"] = _example_outline(rng, rng.uniform(0.5, 1.5), 0.9)
             obs.append(ob)
+        obs = _apply_behavior(obs, behavior)
         scenes.append(dict(obstacles=obs, bounds=(5.0, 15.0, 45.0, 35.0), start=start, goal=goal, goal_threshold=0.4,
                            path=line_path(start, goal)))
     return scenes

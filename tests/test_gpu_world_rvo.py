@@ -1,0 +1,285 @@
+"""Reactive obstacles in the batched world on the GPU: world_rvo_kernel against the float64 oracle (tests/world_rvo_oracle.py),
+teacher-forced and free-running, its edge cases, the absence of any change without reactive obstacles, the absence of host
+synchronisation, and closed-loop runs of PlannerBatch in dyna_obs / dyna_non_obs with the examples' reactive obstacles."""
+import ctypes as C
+import math
+
+import numpy as np
+import pytest
+import torch
+
+from gpu_helpers import record
+from neupan_b200 import WorldBatch, _lib, rollout
+from neupan_b200.robot import robot as Robot
+from neupan_b200.world import dyna_non_obs, dyna_obs, pack_behaviors, pack_scenes_ex, random_outline
+from oracle import world as ow
+from test_gpu_world import EXAMPLE_LIDAR, LIDAR, _mixed_scenes, _oracle_cfg, _polygon
+from test_gpu_world_outline import _StillPlanner, _closed_loop
+from world_rvo_oracle import OracleWorld, axis_count
+
+pytestmark = pytest.mark.gpu
+
+ROBOT_KW = {"diff": dict(kinematics="diff", length=1.6, width=2.0), "acker": dict(kinematics="acker", length=4.6, width=1.6, wheelbase=3),
+            "omni": dict(kinematics="omni", vertices=[[-0.8, -1.0], [-1.8, 1.0], [1.8, 1.0], [0.8, -1.0]])}
+
+
+def _behavior(rng, neighbor_range):
+    goal = None if rng.uniform() < 0.5 else tuple(rng.uniform(-11.0, 11.0, 2))
+    return dict(name="rvo", vxmax=rng.uniform(0.3, 1.0), vymax=rng.uniform(0.3, 1.0), acce=rng.uniform(0.2, 1.0), factor=rng.uniform(0.5, 2.0),
+                speed=rng.uniform(0.3, 1.0), wander=bool(rng.uniform() < 0.7), goal=goal, goal_threshold=rng.uniform(0.3, 1.5),
+                neighbor_range=neighbor_range, grid=0.05, min_speed=rng.uniform(0.0, 0.3))
+
+
+def _rvo_scenes(B, seed, robot_far=False):
+    """Circles, convex polygons and outlines, reactive (about 60 %) and constant-velocity obstacles mixed; environment 0 has 256
+    obstacles.  ``robot_far``: the robot starts 60 m away from every obstacle, beyond any neighbour range."""
+    scenes = []
+    for b in range(B):
+        rng = np.random.default_rng([seed, b])
+        n = 256 if b == 0 else int(rng.integers(2, 30))
+        obs = []
+        for _ in range(n):
+            c, u = tuple(rng.uniform(-11.5, 11.5, 2)), rng.uniform()
+            ob = dict(center=c, velocity=tuple(rng.uniform(-0.5, 0.5, 2)))
+            if u < 0.4:
+                ob["radius"] = rng.uniform(0.2, 1.2)
+            elif u < 0.7:
+                ob["vertices"] = _polygon(rng)
+            else:
+                ob["outline"] = random_outline(rng, rng.uniform(0.3, 1.2), rng.uniform(0.0, 1.0), rng.uniform(0.0, 1.0), int(rng.integers(3, 17)))
+            if rng.uniform() < 0.6:
+                ob["behavior"] = _behavior(rng, rng.uniform(1.5, 3.0) if b == 0 else rng.uniform(2.0, 8.0))
+            obs.append(ob)
+        start = (60.0, 60.0, 0.0) if robot_far else (rng.uniform(-4, 4), rng.uniform(-4, 4), rng.uniform(-np.pi, np.pi))
+        scenes.append(dict(obstacles=obs, bounds=(-12.0, -12.0, 12.0, 12.0), start=start, goal=(rng.uniform(-5, 5), rng.uniform(-5, 5)),
+                           goal_threshold=0.5))
+    return scenes
+
+
+def _device_state(w):
+    g, d = w.goals()
+    c, a = w.flags()
+    return dict(obs=w.obstacles().cpu().numpy(), states=w.states.cpu().numpy(), collided=c.cpu().numpy(), arrived=a.cpu().numpy(),
+                goal=g.cpu().numpy(), draws=d.cpu().numpy())
+
+
+@pytest.mark.parametrize("kin", ["diff", "acker", "omni"])
+def test_teacher_forced_choices_match_the_oracle_bit_for_bit(kin):
+    """50 steps of B = 256 environments; before every step the oracle takes the device's state, then the obstacles' rows (chosen
+    velocities, moved), goals and draw counters must be equal bit for bit in every environment.  The only excuse is a decision that
+    involved the robot with a margin below 1e-12 (CUDA's sincos vs libm in the robot's velocity)."""
+    B, steps = 256, 50
+    rb = Robot(10, 0.1, **ROBOT_KW[kin])
+    lidar = dict(LIDAR, number=16)
+    scenes = _rvo_scenes(B, 31)
+    packed, beh = pack_scenes_ex(scenes), pack_behaviors(scenes)
+    w = WorldBatch(B, rb, lidar, 0.1)
+    w.set_scenes(scenes, seed=77)
+    o = OracleWorld(_oracle_cfg(rb, lidar), packed, beh, seed=77)
+    s0 = _device_state(w)
+    assert np.array_equal(s0["goal"], o.goal) and np.array_equal(s0["draws"], o.draws)  # draw 0 on the host
+    rng = np.random.default_rng(12)
+    paths, checked, excused, robot_nb, wrong = {}, 0, 0, 0, []
+    for k in range(steps):
+        s = _device_state(w)
+        o.obs[:], o.states[:], o.collided[:], o.goal[:], o.draws[:] = s["obs"], s["states"], s["collided"], s["goal"], s["draws"]
+        act = np.column_stack([rng.uniform(-1, 2, B), rng.uniform(-0.5, 0.5, B)]).astype(np.float32)
+        envs = range(B)
+        margins = o.rvo(act, envs)
+        for b in envs:
+            for q in range(o.obs_begin[b], o.obs_begin[b + 1]):
+                o.obs[q, :4] = ow.move_obstacle(o.obs[q], o.env[b, :4], 0.1)
+        w.step(torch.from_numpy(act).cuda())
+        d = _device_state(w)
+        for p in o.paths.values():
+            paths[p] = paths.get(p, 0) + 1
+        robot_nb += int(np.isfinite(margins).sum())
+        for b in envs:
+            sl = slice(o.obs_begin[b], o.obs_begin[b + 1])
+            bad = ~(np.all(d["obs"][sl] == o.obs[sl], 1) & np.all(d["goal"][sl] == o.goal[sl], 1) & (d["draws"][sl] == o.draws[sl]))
+            checked += sl.stop - sl.start
+            for q in np.flatnonzero(bad) + sl.start:
+                if margins[q] < 1e-12:
+                    excused += 1
+                else:
+                    wrong.append((k, b, int(q), o.paths.get(int(q)), d["obs"][q].tolist(), o.obs[q].tolist()))
+    draws = _device_state(w)["draws"]
+    record(f"world_rvo_teacher_forced_{kin}", steps=steps, envs=B, obstacle_steps_checked=checked, paths=paths,
+           robot_neighbour_choices=robot_nb, excused=excused, mismatches=len(wrong), goals_drawn=int(draws.sum()))
+    assert not wrong, wrong[:3]
+    assert paths.get("outside", 0) > 10000 and paths.get("penalty", 0) > 100 and robot_nb > 0
+    assert draws.sum() > s0["draws"].sum()  # goals were reached and drawn again
+    w.close()
+
+
+def test_free_running_matches_the_oracle_without_the_robot():
+    """The robot is never a neighbour: 50 free-running steps equal the oracle's bit for bit."""
+    B, steps = 24, 50
+    rb = Robot(10, 0.1, **ROBOT_KW["omni"])
+    lidar = dict(LIDAR, number=16)
+    scenes = _rvo_scenes(B + 1, 41, robot_far=True)[1:]
+    w = WorldBatch(B, rb, lidar, 0.1)
+    w.set_scenes(scenes, seed=3)
+    o = OracleWorld(_oracle_cfg(rb, lidar), pack_scenes_ex(scenes), pack_behaviors(scenes), seed=3)
+    act = np.zeros((B, 2), np.float32)
+    for k in range(steps):
+        w.step(torch.from_numpy(act).cuda())
+        o.step(act)
+        d = _device_state(w)
+        assert np.array_equal(d["obs"], o.obs), k
+        assert np.array_equal(d["goal"], o.goal) and np.array_equal(d["draws"], o.draws), k
+        assert not np.isfinite(o.margins).any()
+    moved = np.abs(d["obs"][:, :2] - pack_scenes_ex(scenes)[1][:, :2]).max()
+    record("world_rvo_free_running", steps=steps, envs=B, goals_drawn=int(d["draws"].sum()), max_displacement=float(moved))
+    w.close()
+
+
+def _edge_scenes():
+    """One environment per edge case; the robot stays far away."""
+    far = (60.0, 60.0, 0.0)
+    sc = lambda obs: dict(obstacles=obs, bounds=(-12.0, -12.0, 12.0, 12.0), start=far, goal=(70.0, 70.0), goal_threshold=0.5)
+    rvo = lambda **kw: dict(dict(name="rvo", vxmax=0.5, vymax=0.5, goal=(10.0, 3.0)), **kw)
+    boxed = [dict(center=(0.0, 0.0), radius=0.5, behavior=rvo())]
+    for a in range(8):  # eight circles pressing on it, heading inwards
+        d = (math.cos(a * math.pi / 4), math.sin(a * math.pi / 4))
+        boxed.append(dict(center=(1.1 * d[0], 1.1 * d[1]), radius=0.6, velocity=(-0.4 * d[0], -0.4 * d[1])))
+    return [
+        sc([dict(center=(0.0, 0.0), radius=0.5, behavior=rvo(vxmax=0.8, vymax=0.8, acce=0.8, grid=0.025)),     # 64 x 64 candidates
+            dict(center=(2.0, 0.1), radius=0.7, velocity=(-0.3, 0.0))]),
+        sc(boxed),                                                                                              # the penalty pass
+        sc([dict(center=(0.0, 0.0), radius=0.5, velocity=(0.1, 0.05), behavior=rvo(vxmax=0.2, vymax=0.2, min_speed=0.5))]),  # no candidate
+        sc([dict(center=(3.0, 3.0), radius=0.5, velocity=(0.2, 0.0), behavior=rvo(goal=(3.1, 3.0), wander=False)),  # parks
+            dict(center=(4.0, 3.0), radius=0.3)]),
+        sc([dict(center=(-3.0, 0.0), radius=0.5, behavior=rvo()), dict(center=(-3.0, 0.0), vertices=_polygon(np.random.default_rng(1)),
+                                                                      behavior=rvo(goal=(-10.0, -3.0)))]),  # the same centre
+    ]
+
+
+def test_edge_cases_match_the_oracle():
+    scenes = _edge_scenes()
+    B = len(scenes)
+    rb = Robot(10, 0.1, **ROBOT_KW["diff"])
+    lidar = dict(LIDAR, number=16)
+    beh = pack_behaviors(scenes)
+    w = WorldBatch(B, rb, lidar, 0.1)
+    w.set_scenes(scenes, seed=9)
+    o = OracleWorld(_oracle_cfg(rb, lidar), pack_scenes_ex(scenes), beh, seed=9)
+    act = np.zeros((B, 2), np.float32)
+    seen = []
+    for k in range(20):
+        w.step(torch.from_numpy(act).cuda())
+        o.step(act)
+        d = _device_state(w)
+        assert np.array_equal(d["obs"], o.obs) and np.array_equal(d["goal"], o.goal) and np.array_equal(d["draws"], o.draws), k
+        seen.append(dict(o.paths))
+    ob = o.obs_begin
+    assert axis_count(-0.8, 0.8, 0.025) == 64 and seen[0][ob[0]] == "outside"
+    assert seen[0][ob[1]] == "penalty"
+    assert all(s[ob[2]] == "none" for s in seen) and tuple(d["obs"][ob[2], 2:4]) == (0.1, 0.05)
+    assert seen[0][ob[3]] == "parked" and tuple(d["obs"][ob[3], :4]) == (3.0, 3.0, 0.0, 0.0) and d["draws"][ob[3]] == 0
+    assert seen[0][ob[4]] == seen[0][ob[4] + 1] == "outside"
+    record("world_rvo_edge_cases", paths_step0=[seen[0][ob[b]] for b in range(B)])
+    w.close()
+
+
+def test_set_scenes_after_behaviours_clears_them():
+    B = 16
+    rb = Robot(10, 0.1, **ROBOT_KW["diff"])
+    lidar = dict(LIDAR, number=64)
+    plain = _mixed_scenes(B + 2, 5)[2:]
+    fresh, reused = WorldBatch(B, rb, lidar, 0.1), WorldBatch(B, rb, lidar, 0.1)
+    reused.set_scenes(_rvo_scenes(B, 8), seed=1)
+    reused.step(torch.zeros(B, 2, device="cuda"))
+    reused.set_scenes(plain)
+    fresh.set_scenes(plain)
+    with pytest.raises(ValueError, match="no behaviours set"):
+        reused.goals()
+    rng = np.random.default_rng(2)
+    for _ in range(10):
+        act = torch.from_numpy(np.column_stack([rng.uniform(-1, 2, B), rng.uniform(-0.5, 0.5, B)]).astype(np.float32)).cuda()
+        a, b = fresh.scan(hit=True), reused.scan(hit=True)
+        assert all(torch.equal(x, y) for x, y in zip(a, b) if torch.is_tensor(x))
+        assert all(torch.equal(x, y) for x, y in zip(fresh.step(act), reused.step(act)))
+        assert torch.equal(fresh.obstacles(), reused.obstacles())
+    fresh.close(); reused.close()
+
+
+def test_constant_behaviours_change_nothing():
+    """Behaviours that are all kind 0: bitwise the same scans, steps, flags and clearances as a world without behaviours, and the
+    same launches."""
+    B = 64
+    rb = Robot(10, 0.1, **ROBOT_KW["diff"])
+    lidar = dict(LIDAR, number=360)
+    scenes = _rvo_scenes(B, 19)
+    for sc in scenes:
+        for ob in sc["obstacles"]:
+            ob.pop("behavior", None)
+    plain, const = WorldBatch(B, rb, lidar, 0.1), WorldBatch(B, rb, lidar, 0.1)
+    plain.set_scenes(scenes)
+    const.set_scenes(scenes)
+    zeros = np.zeros((len(pack_scenes_ex(scenes)[1]), 13))
+    with torch.cuda.device(const.device):
+        _lib.check(_lib.load().nb_world_set_behaviors(const._handle, B, C.c_void_p(zeros.ctypes.data), C.c_uint64(4)))
+    g, d = const.goals()
+    assert not g.any() and not d.any()
+    rng = np.random.default_rng(3)
+    lib = _lib.load()
+    for _ in range(20):
+        act = torch.from_numpy(np.column_stack([rng.uniform(-1, 2, B), rng.uniform(-0.5, 0.5, B)]).astype(np.float32)).cuda()
+        n0 = lib.nb_launch_count()
+        a = plain.scan(hit=True) + plain.step(act)
+        n1 = lib.nb_launch_count()
+        b = const.scan(hit=True) + const.step(act)
+        n2 = lib.nb_launch_count()
+        assert n1 - n0 == n2 - n1 == 2
+        assert all(torch.equal(x, y) for x, y in zip(a, b) if torch.is_tensor(x))
+        assert torch.equal(plain.states, const.states) and torch.equal(plain.obstacles(), const.obstacles())
+    assert all(torch.equal(x, y) for x, y in zip(plain.flags(), const.flags()))
+    plain.close(); const.close()
+
+
+def test_reactive_world_does_not_synchronise_the_host():
+    B = 64
+    rb = Robot(10, 0.1, **ROBOT_KW["diff"])
+    w = WorldBatch(B, rb, EXAMPLE_LIDAR, 0.1)
+    w.set_scenes(dyna_non_obs(B, seed=1, behavior="rvo"), seed=2)
+    action = torch.zeros(B, 2, device="cuda")
+    lib = _lib.load()
+    torch.cuda.synchronize()
+    torch.cuda.set_sync_debug_mode("error")
+    try:
+        n0 = lib.nb_launch_count()
+        for _ in range(3):
+            w.scan()
+            w.step(action)
+            _ = w.states
+            g, d = w.goals()
+        n1 = lib.nb_launch_count()
+        out = rollout(_StillPlanner(B), w, 5)
+    finally:
+        torch.cuda.set_sync_debug_mode(0)
+    assert n1 - n0 == 9  # scan, rvo, step
+    assert out["min_clearance"].shape == (B,) and g.shape == (w.O, 2)
+    w.close()
+
+
+# (scene builder, config, steps).  What the counts turn out to be is a finding, reported next to the constant-velocity ones.
+CLOSED_LOOP = {"dyna_obs": (dyna_obs, "C4", 150), "dyna_non_obs": (dyna_non_obs, "C4", 200)}
+
+
+@pytest.mark.parametrize("scene", list(CLOSED_LOOP))
+def test_closed_loop_among_reactive_obstacles(scene):
+    builder, cfg_id, steps = CLOSED_LOOP[scene]
+    rvo = builder(128, seed=2024, behavior="rvo")
+    seen = _closed_loop(cfg_id, rvo, steps)
+    again = _closed_loop(cfg_id, rvo, steps)
+    for k in ("states", "obstacles", "collided", "arrived", "steps_to_arrive", "min_clearance"):
+        assert np.array_equal(seen[k], again[k]), k
+    blind = _closed_loop(cfg_id, rvo, steps, blind=True)
+    arrived = seen["steps_to_arrive"][seen["arrived"]]
+    moving = np.abs(seen["obstacles"][:, 2:4]).sum(1) > 0
+    record(f"world_rvo_closed_loop_{scene}", envs=128, steps=steps, config=cfg_id, collided_with_scans=int(seen["collided"].sum()),
+           collided_blind=int(blind["collided"].sum()), arrived_with_scans=int(seen["arrived"].sum()), arrived_blind=int(blind["arrived"].sum()),
+           max_steps_to_arrive=int(arrived.max()) if len(arrived) else -1, min_clearance_median=float(np.median(seen["min_clearance"])),
+           obstacles_moving_at_end=float(moving.mean()))
+    assert moving.mean() > 0.5

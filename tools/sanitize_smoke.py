@@ -5,7 +5,7 @@ sys.path.insert(0, os.getcwd()); sys.path.insert(0, "tests")
 import numpy as np, torch
 from gpu_helpers import make_pan, run_pan, to_cuda
 from helpers import CONFIGS, make_inputs
-SECTIONS = os.environ.get("NB_SMOKE_SECTIONS", "variants,screen,adjoint,train").split(",")
+SECTIONS = os.environ.get("NB_SMOKE_SECTIONS", "variants,screen,adjoint,train,world").split(",")
 # N = 300: two slots, then a pass with one; N = 600: keys in shared memory (n > 512)
 for cname, B, N in (("C4", 6, 70), ("C5", 3, 40), ("C2", 5, 33), ("C4", 3, 300), ("C3", 2, 600)) if "variants" in SECTIONS else ():
     cfg = CONFIGS[cname]
@@ -56,5 +56,25 @@ for cname in ("C1", "C5") if "train" in SECTIONS else ():
     tr.train_one_epoch(data, 256, True)
     assert np.isfinite(losses).all()
     tr.sync_model(); tr.close()
+# the batched world with reactive obstacles: world_scan_kernel, world_rvo_kernel (goal draws, the robot as a neighbour of an obstacle
+# placed on its path) and world_step_kernel
+if "world" in SECTIONS:
+    from neupan_b200 import WorldBatch
+    from neupan_b200.world import dyna_non_obs, dyna_obs
+    rb = CONFIGS["C4"].make_robot()
+    lidar = dict(angle_min=-np.pi / 2, angle_max=np.pi / 2, range_min=0.0, range_max=10.0, number=100)
+    for builder in (dyna_obs, dyna_non_obs):
+        scenes = builder(6, seed=1, behavior="rvo")
+        scenes[0]["obstacles"].append(dict(center=(12.0, scenes[0]["start"][1]), radius=0.3, behavior=dict(name="rvo", vxmax=0.5, vymax=0.5,
+                                                                                                       goal=(20.0, 20.0))))
+        w = WorldBatch(6, rb, lidar, 0.1)
+        w.set_scenes(scenes, seed=3)
+        for _ in range(30):
+            w.scan()
+            w.step(torch.full((6, 2), 0.5, device="cuda"))
+        g, d = w.goals()
+        torch.cuda.synchronize()
+        assert torch.isfinite(w.obstacles()).all() and torch.isfinite(g).all()
+        w.close()
 torch.cuda.synchronize()
 print("sanitize smoke ok")

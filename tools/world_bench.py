@@ -1,15 +1,18 @@
 """Times the batched world (csrc/world_kernel.cuh) against the planner it serves, on the device, and prints one JSON line.
 
-    python tools/world_bench.py [--scene dyna_obs|dyna_non_obs] [--envs 4096] [--beams 1080] [--steps 20] [--warmup 3]
+    python tools/world_bench.py [--scene dyna_obs|dyna_non_obs] [--behavior constant|rvo] [--envs 4096] [--beams 1080] [--steps 20]
+                                [--warmup 3]
 
 Scenes: seeded dyna_obs (20 moving circles per environment, neupan_b200.world.dyna_obs; the default) or dyna_non_obs (11 moving
-obstacles after example/dyna_non_obs: squares, circles and non-convex outlines, neupan_b200.world.dyna_non_obs).  Planner:
+obstacles after example/dyna_non_obs: squares, circles and non-convex outlines, neupan_b200.world.dyna_non_obs), with constant-velocity
+obstacles (the default) or the examples' reactive ones (--behavior rvo, csrc/world_rvo_kernel.cuh).  Planner:
 PlannerBatch with C4's robot, adjust values and K, the scans decimated to C4's N = 500 points.  Legs, each timed with CUDA events over --steps iterations after
 --warmup: the world alone (scan + step), the planner alone (PlannerBatch.forward repeated on the initial states and scans, after a
 reset) and the closed-loop step (scan -> PlannerBatch.forward -> step, from the initial scenes after a reset), whose world and planner
 parts are also timed separately with events around each call.  The planner-alone leg repeats one input; in the closed loop the
 inputs change every step (robots move, some arrive or stop), so the two planner times need not agree.  The card's name and power
-limit are read in the same run.
+limit are read in the same run.  With --behavior rvo, one more closed-loop window of --steps iterations runs under torch.profiler,
+which gives the device time of world_rvo_kernel per step and its share of the closed-loop step timed with events.
 """
 import argparse
 import json
@@ -35,6 +38,7 @@ def _card():
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scene", choices=("dyna_obs", "dyna_non_obs"), default="dyna_obs")
+    ap.add_argument("--behavior", choices=("constant", "rvo"), default="constant")
     ap.add_argument("--envs", type=int, default=4096)
     ap.add_argument("--beams", type=int, default=1080)
     ap.add_argument("--steps", type=int, default=20)
@@ -54,7 +58,7 @@ def main():
     B, R = args.envs, args.beams
     cfg = CONFIGS["C4"]
     lidar = dict(angle_min=-math.pi, angle_max=math.pi, range_min=0.0, range_max=10.0, number=R)
-    scenes = (dyna_obs if args.scene == "dyna_obs" else dyna_non_obs)(B, seed=2024)
+    scenes = (dyna_obs if args.scene == "dyna_obs" else dyna_non_obs)(B, seed=2024, behavior=args.behavior)
     packed = pack_scenes_ex(scenes)
     n_obs, n_edges = int(packed[0][-1]), int(packed[2][-1])
     n_circles = int((packed[2][1:] == packed[2][:-1]).sum())
@@ -110,13 +114,23 @@ def main():
     timed_steps = split[-args.steps:]  # the events of the timed window (all recorded and synchronised by timed())
     ms_loop_world = sum(e[0].elapsed_time(e[1]) + e[2].elapsed_time(e[3]) for e in timed_steps) / args.steps
     ms_loop_planner = sum(e[1].elapsed_time(e[2]) for e in timed_steps) / args.steps
+    rvo = {}
+    if args.behavior == "rvo":  # device time of the reactive obstacles' kernel inside the closed loop
+        from torch.profiler import ProfilerActivity, profile
+
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(args.steps):
+                closed_loop()
+            torch.cuda.synchronize()
+        us = sum(getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) for e in prof.key_averages() if "world_rvo_kernel" in e.key)
+        rvo = dict(ms_rvo_kernel=us * 1e-3 / args.steps, rvo_share_of_closed_loop=us * 1e-3 / args.steps / ms_loop)
     tests = R * (n_circles + n_edges)  # ray-boundary tests of one scan: every beam against every circle and polygon edge
-    print(json.dumps(dict(metric="batched world: scan + step vs PlannerBatch.forward", scene=args.scene, envs=B, beams=R,
+    print(json.dumps(dict(metric="batched world: scan + step vs PlannerBatch.forward", scene=args.scene, behavior=args.behavior, envs=B, beams=R,
                           obstacles_per_env=n_obs / B, circles_per_env=n_circles / B, edges_per_env=n_edges / B,
                           steps=args.steps, warmup=args.warmup, ms_scan=ms_scan, ms_world_scan_step=ms_world, ms_planner_forward=ms_planner,
                           ms_closed_loop_step=ms_loop, ms_closed_loop_world=ms_loop_world, ms_closed_loop_planner=ms_loop_planner,
                           world_share_of_closed_loop=ms_loop_world / ms_loop,
-                          ray_obstacle_tests_per_s=tests / (ms_scan * 1e-3), **_card())))
+                          ray_obstacle_tests_per_s=tests / (ms_scan * 1e-3), **rvo, **_card())))
     world.close()
     pl.close()
 
