@@ -125,10 +125,10 @@ int nb_pan_set_adjust(nb_pan_t* pan, const float q_s[3], float p_u, float eta, f
 int nb_pan_set_iteration(nb_pan_t* pan, int32_t iter_num, float iter_threshold);
 
 /* Implementation switches (no reference counterpart).  NB_OPT_DUNE_KERNEL: 2 (the handle's initial value; the Python mirror selects 4) =
- * warpgroup DUNE kernel (wgmma with a shared-memory operand / output tile, fp16 hi/lo split, fp32 accumulate); 1 = the same arithmetic on
- * warp-level mma.sync;
- * 0 = all-FP32 FFMA kernel, kept as the in-tree numerical reference of the same contract (needs the edge count
- * compiled in).
+ * warpgroup DUNE kernel on every point (wgmma with a shared-memory operand / output tile, fp16 hi/lo split, fp32 accumulate);
+ * 4 = wgmma with screening: a single-pass fp16 interval pass over all points, the exact network only for the <= 32 points
+ * per (environment, step) that can be among the M closest, the exact kernel for the items the screen cannot narrow down -- the same
+ * selection and values as 2, bit for bit (csrc/dune_screen_kernel.cuh).  Other values are refused with NB_ERR_INVALID.
  * NB_OPT_OVERLAP: 1..4 = number of environment sub-batches pipelined on internal streams so that the DUNE kernels
  * of one sub-batch share the SMs with the NRMP kernel of another (results are identical; envs are independent; batches with
  * fewer than 64 environments per part are not split).  The handle starts with 2: the straggler tail of one half's NRMP launch
@@ -137,10 +137,6 @@ int nb_pan_set_iteration(nb_pan_t* pan, int32_t iter_num, float iter_threshold);
  * iteration k-1 of the same environment (fewer interior point iterations on average, same optimum to the solver tolerance;
  * a warm start that is not converging by its 12th iteration is abandoned for a cold one); 0 (default) = every solve starts
  * cold.  The first solve of every call is always cold, so results never depend on earlier calls.
- * NB_OPT_DUNE_KERNEL also takes 3 = wgmma with two threads per point (8 warps per 128-point tile, kept for A/B)
- * and 4 = wgmma with screening: a single-pass fp16 interval pass over all points, the exact network only for the <= 32 points
- * per (environment, step) that can be among the M closest, the exact kernel for the items the screen cannot narrow down -- the same
- * selection and values as 2, bit for bit (csrc/dune_screen_kernel.cuh).
  * NB_OPT_DIFFERENTIABLE: 1 = every NRMP solve of nb_pan_forward also stores what nb_pan_backward needs (one extra factorisation
  * at the optimum + ~5 KB per environment and iteration); 0 (default) = inference only.
  * NB_OPT_DUNE_SCREEN_MMA (with NB_OPT_DUNE_KERNEL = 4): 1 (default) = the screening pass runs on warp-level mma.sync with the

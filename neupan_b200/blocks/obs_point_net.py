@@ -2,7 +2,7 @@
 neupan/blocks/obs_point_net.py:25-49 so the reference's checkpoints load unchanged).
 
 On the hot path the network is evaluated by the fused CUDA DUNE kernel
-(neupan_b200/csrc/dune_kernel.cuh) from these parameters; ``forward`` is the plain torch
+(neupan_b200/csrc/dune_tc_kernel.cuh) from these parameters; ``forward`` is the plain torch
 definition of the same function, kept for API compatibility (e.g. DUNE training).
 """
 import torch

@@ -104,8 +104,8 @@ class PAN(torch.nn.Module):
         # launch and the small kernels between the big ones run under the other half's DUNE pass
         self.overlap = int(kwargs.get("overlap", 2))
         self.nrmp_warm = int(kwargs.get("nrmp_warm", 0))  # 1 = NRMP solves of PAN iterations k > 0 start from iteration k-1's solution (fewer IPM iterations on average, but stragglers: DESIGN.md 3.2)
-        # 4 = screening pipeline (default: interval pass + exact wgmma network on the candidates, bit-identical to 2), 2 = wgmma on every point, 3 = two threads per
-        # point (experiment), 1 = mma.sync, 0 = all-FP32 FFMA
+        # 4 = screening pipeline (default: interval pass + exact wgmma network on the candidates, bit-identical to 2), 2 = the exact wgmma
+        # network on every point; the handle refuses any other value
         self.dune_kernel = int(kwargs.get("dune_kernel", 4))
         # with dune_kernel = 4: the screening pass on mma.sync (1, default; clouds of <= 1024 points) or wgmma (0); PAN iterations k > 0
         # keep the step-0 items of iteration 0 (1, default: nom_s[:, 0] is the fixed initial state) or re-evaluate them (0).  Same results.

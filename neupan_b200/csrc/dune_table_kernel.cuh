@@ -5,7 +5,7 @@
 // side h over [-half, half]^2; the screen then costs one 16-byte load (the cell's four corner values), one 4-byte load (its radius)
 // and a bilinear interpolation per point instead of the single-pass fp16 network.
 //
-// Build: (1) dune_table_sample_kernel evaluates the FP32 network (the helpers of dune_kernel, variant 0) on a grid four times finer
+// Build: (1) dune_table_sample_kernel evaluates the FP32 network (layernorm_tanh / dense32 below) on a grid four times finer
 // than the table, (2) dune_table_cell_kernel takes each cell's corners from it and sets the cell's radius to kTableSafety x (the
 // largest |bilinear - network| over the 5 x 5 fine samples of the cell + their largest second difference along x or y), plus
 // kTableFloor.  The second-difference term covers the ReLU kinks of the network that fall between two fine samples: without it the
@@ -14,13 +14,58 @@
 // every radius positive.  The radius is checked at run time like the network's: the refine
 // kernel compares every candidate's |screened - exact| with half of that candidate's radius.
 #pragma once
-#include "dune_kernel.cuh"
+#include "dune_common.cuh"
 
 namespace nb {
 
 constexpr int kTableSub = 4;            // fine samples per cell side used to measure the interpolation error
 constexpr float kTableSafety = 4.f;     // radius = kTableSafety x (sample error + second difference) + kTableFloor
 constexpr float kTableFloor = 1e-4f;
+
+template <int P>
+__device__ __forceinline__ void layernorm_tanh(float (&v)[P][kHidden], const float* __restrict__ g, const float* __restrict__ be) {
+#pragma unroll
+  for (int p = 0; p < P; ++p) {
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < kHidden; ++j) s += v[p][j];
+    const float mean = s * (1.0f / kHidden);
+    float q = 0.f;
+#pragma unroll
+    for (int j = 0; j < kHidden; ++j) {
+      const float d = v[p][j] - mean;
+      q = fmaf(d, d, q);
+    }
+    const float rstd = 1.0f / sqrtf(q * (1.0f / kHidden) + 1e-5f);  // nn.LayerNorm eps, biased variance
+#pragma unroll
+    for (int j = 0; j < kHidden; ++j) v[p][j] = tanhf(fmaf((v[p][j] - mean) * rstd, g[j], be[j]));
+  }
+}
+
+// out[p][j] = act(b[j] + sum_k W[j][k] * in[p][k]); W row-major (out, in) in shared memory.
+template <int P, bool RELU>
+__device__ __forceinline__ void dense32(const float* __restrict__ W, const float* __restrict__ b,
+                                        const float (&in)[P][kHidden], float (&out)[P][kHidden]) {
+#pragma unroll
+  for (int j = 0; j < kHidden; ++j) {
+    float acc[P];
+#pragma unroll
+    for (int p = 0; p < P; ++p) acc[p] = b[j];
+#pragma unroll
+    for (int k4 = 0; k4 < kHidden / 4; ++k4) {
+      const float4 w = reinterpret_cast<const float4*>(W + j * kHidden)[k4];
+#pragma unroll
+      for (int p = 0; p < P; ++p) {
+        acc[p] = fmaf(w.x, in[p][4 * k4 + 0], acc[p]);
+        acc[p] = fmaf(w.y, in[p][4 * k4 + 1], acc[p]);
+        acc[p] = fmaf(w.z, in[p][4 * k4 + 2], acc[p]);
+        acc[p] = fmaf(w.w, in[p][4 * k4 + 3], acc[p]);
+      }
+    }
+#pragma unroll
+    for (int p = 0; p < P; ++p) out[p][j] = RELU ? fmaxf(acc[p], 0.f) : acc[p];
+  }
+}
 
 // out[v * m + u] = d(-half + u hs, -half + v hs), u, v < m, in FP32 (the checkpoint in the packed layout, E <= kMaxEdges)
 __global__ void __launch_bounds__(128) dune_table_sample_kernel(const float* __restrict__ weights, const Geometry geo, int m, float half, float hs,

@@ -6,7 +6,6 @@
 #include <vector>
 
 #include "dune_tc_kernel.cuh"
-#include "dune_tc8_kernel.cuh"
 #include "dune_screen_kernel.cuh"
 #include "dune_screen_mma_kernel.cuh"
 
@@ -126,10 +125,13 @@ static cudaError_t resident_grid(K kern, int threads, size_t smem, int sm_count,
   return e;
 }
 
-int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const unsigned char* d_screen_image, int image_flags, int variant, int sm_count,
+// screen = false: dune_tcp_kernel on every point (NB_OPT_DUNE_KERNEL = 2); true: the screening pipeline (4).  The shared-reciprocal
+// tanh is taken wherever image_flags allows it, in the refine and the exact kernel alike, so both pipelines compute the same bits.
+int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const unsigned char* d_screen_image, int image_flags, bool screen, int sm_count,
                    int max_smem_optin, cudaStream_t st, char* err, size_t errlen) {
   DuneParams prm = prm_in;
-  if (variant == 4) {
+  const bool fast = (image_flags & 1) != 0;
+  if (screen) {
     // screening: (1) interval pass over all points, (2) exact evaluation of the candidates, (3) the exact kernel for the items the
     // screen could not narrow down to 32 candidates (below, with only_flagged)
     if (!d_screen_image || !prm.cand_idx || !prm.cand_cnt || !prm.cand_dt || !prm.cand_rad || !prm.screen_stats || !prm.flag_list || !prm.flag_count || !prm.refine_list) {
@@ -170,12 +172,11 @@ int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const
         e = cudaGetLastError();
       }
     }
-    const bool fast_r = (image_flags & 1) != 0;
     const int groups = (items_ + 7) / 8;  // the number of work units is only known on the device: a persistent grid sized for the worst case
-    if (e == cudaSuccess) e = fast_r ? resident_grid(dune_refine_kernel<true>, 128, smem_r, sm_count, groups, grid)
-                                      : resident_grid(dune_refine_kernel<false>, 128, smem_r, sm_count, groups, grid);
+    if (e == cudaSuccess) e = fast ? resident_grid(dune_refine_kernel<true>, 128, smem_r, sm_count, groups, grid)
+                                    : resident_grid(dune_refine_kernel<false>, 128, smem_r, sm_count, groups, grid);
     if (e == cudaSuccess) {
-      if (fast_r) dune_refine_kernel<true><<<grid, 128, smem_r, st>>>(prm, d_image);
+      if (fast) dune_refine_kernel<true><<<grid, 128, smem_r, st>>>(prm, d_image);
       else dune_refine_kernel<false><<<grid, 128, smem_r, st>>>(prm, d_image);
       e = cudaGetLastError();
     }
@@ -184,40 +185,21 @@ int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const
       return -2;
     }
     prm.only_flagged = 1;
-    variant = 2;
   }
-  const size_t smem = variant == 3 ? dune_tc8_smem_bytes(prm.N, prm.geo.E, prm.M) : dune_tc_smem_bytes(prm.N, prm.geo.E, prm.M);
+  const size_t smem = dune_tc_smem_bytes(prm.N, prm.geo.E, prm.M);
   if ((long long)smem > max_smem_optin) {
     snprintf(err, errlen, "N=%d needs %zu B of shared memory (limit %d)", prm.N, smem, max_smem_optin);
     return -3;
   }
   const int items = prm.B * (prm.T + 1);
-  static int force = -1;  // NB_DUNE_TC=4 (developer switch): plain reciprocals instead of the shared-reciprocal tanh
-  if (force < 0) {
-    const char* v = getenv("NB_DUNE_TC");
-    force = v ? atoi(v) : 0;
-  }
-  static int blocks8 = -1;  // NB_DUNE_TC8_BLOCKS: minimum CTAs per SM the 8-warp kernel is compiled for (3: <= 85 registers, 4: <= 64 registers)
-  if (blocks8 < 0) {
-    const char* v = getenv("NB_DUNE_TC8_BLOCKS");
-    blocks8 = v ? atoi(v) : 3;
-    if (blocks8 != 4) blocks8 = 3;
-  }
-  const bool fast = (image_flags & 1) != 0 && force != 4;
-  auto run = [&](auto kern, int threads) -> cudaError_t {
+  auto run = [&](auto kern) -> cudaError_t {
     int grid = 0;
-    cudaError_t e = resident_grid(kern, threads, smem, sm_count, items, grid);
+    cudaError_t e = resident_grid(kern, 128, smem, sm_count, items, grid);
     if (e != cudaSuccess) return e;
-    kern<<<grid, threads, smem, st>>>(prm, d_image);
+    kern<<<grid, 128, smem, st>>>(prm, d_image);
     return cudaGetLastError();
   };
-  cudaError_t e;
-  if (variant == 3) {
-    if (blocks8 == 4) e = fast ? run(dune_tc8_kernel<true, 4>, 256) : run(dune_tc8_kernel<false, 4>, 256);
-    else e = fast ? run(dune_tc8_kernel<true, 3>, 256) : run(dune_tc8_kernel<false, 3>, 256);
-  } else {
-    e = fast ? run(dune_tcp_kernel<true>, 128) : run(dune_tcp_kernel<false>, 128);
-  }
+  const cudaError_t e = fast ? run(dune_tcp_kernel<true>) : run(dune_tcp_kernel<false>);
   if (e != cudaSuccess) {
     snprintf(err, errlen, "dune_tc kernel launch failed: %s", cudaGetErrorString(e));
     return -2;

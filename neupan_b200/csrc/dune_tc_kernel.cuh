@@ -1,8 +1,8 @@
 // DUNE kernels, warpgroup versions (Hopper wgmma: B operand from shared memory, accumulators in registers).
 //
-// Same contract as dune_mma_kernel.cuh / dune_kernel.cuh.  Mapping: CTA = 128 threads = one warpgroup; thread r owns point r
-// of a 128-point tile for the whole network, so LayerNorm statistics, tanh, ReLU and the distance are thread-local (no
-// shuffles, no fragment bookkeeping).  Per dense layer:
+// Point flow -> robot frame -> ObsPointNet -> distance -> M closest points (dune_common.cuh).
+// Mapping: CTA = 128 threads = one warpgroup; thread r owns point r of a 128-point tile for the whole network, so LayerNorm
+// statistics, tanh, ReLU and the distance are thread-local (no shuffles, no fragment bookkeeping).  Per dense layer:
 //   registers --split x = hi + lo (fp16)--> shared-memory tile (A operand, canonical K-major layout)   [all threads]
 //   D[128 x 32] = ONES.BIASB + A_lo.B_hi + A_hi.B_lo + A_hi.B_hi                                    [the warpgroup, wgmma
 //                                                      m64n32k16 per 64-row half, B and ONES from shared memory]
@@ -13,7 +13,7 @@
 #include <cuda_fp16.h>
 
 #include "common.cuh"
-#include "dune_kernel.cuh"  // DuneParams, orderable(), flow()
+#include "dune_common.cuh"  // DuneParams, orderable(), flow()
 
 namespace nb {
 

@@ -11,7 +11,6 @@
 #include <new>
 
 #include "common.cuh"
-#include "dune_launch.cuh"
 #include "nrmp_kernel.cuh"
 #include "scan_kernel.cuh"
 #include "ipath_kernel.cuh"
@@ -24,13 +23,9 @@
 #include <vector>
 
 namespace nb {
-// dune_mma.cu
-void build_mma_image(const float* w, int E, std::vector<unsigned char>& out);
-int launch_dune_mma(const DuneParams& prm, const unsigned char* d_image, int sm_count, int max_smem_optin, int cta_per_sm_limit, cudaStream_t st,
-                    char* err, size_t errlen);
 // dune_tc.cu
 int build_tc_image(const float* w, int E, std::vector<unsigned char>& out, bool screen);
-int launch_dune_tc(const DuneParams& prm, const unsigned char* d_image, const unsigned char* d_screen_image, int image_flags, int variant, int sm_count,
+int launch_dune_tc(const DuneParams& prm, const unsigned char* d_image, const unsigned char* d_screen_image, int image_flags, bool screen, int sm_count,
                    int max_smem_optin, cudaStream_t st, char* err, size_t errlen);
 }  // namespace nb
 
@@ -294,7 +289,6 @@ struct nb_pan {
   int max_smem_optin = 0;
   // device buffers
   float* d_weights = nullptr;
-  unsigned char* d_image = nullptr;  // fragment-ordered fp16 hi/lo weight image of the mma.sync DUNE kernel
   unsigned char* d_tc_image = nullptr;  // wgmma operand image of the warpgroup DUNE kernels
   int tc_flags = 0;                     // build_tc_image(): bit 0 = bounded tanh arguments
   unsigned char* d_tc_screen = nullptr; // operand image of the screening network (NB_OPT_DUNE_KERNEL = 4)
@@ -312,7 +306,7 @@ struct nb_pan {
   int tab_n = 0;
   float tab_h = 0.f, tab_half = 0.f, tab_ratio = 0.f, tab_ms = 0.f;
   bool tab_built = false;               // built (and kept, or freed as not accurate enough: tab_cell == nullptr)
-  int dune_variant = 2;              // NB_OPT_DUNE_KERNEL: 0 = FP32 FFMA, 1 = mma.sync tensor-core, 2 = wgmma tensor-core kernel
+  int dune_variant = 2;              // NB_OPT_DUNE_KERNEL: 2 = the exact wgmma kernel on every point, 4 = screening pipeline
   int overlap = 1;                   // NB_OPT_OVERLAP: number of env sub-batches pipelined on internal streams
   cudaStream_t streams[4] = {nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t ev_fork = nullptr, ev_join[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -360,55 +354,12 @@ int check_forward_args(const nb_pan* p, int B, int N) {
   return NB_OK;
 }
 
-// NB_EDGE_MASK: bit E set <=> dune_inst.cu was compiled for that edge count (build script)
-#ifndef NB_EDGE_MASK
-#define NB_EDGE_MASK 0x10
-#endif
-
-int launch_dune(nb_pan* p, const nb::DuneParams& prm, cudaStream_t st, int cta_limit = 0) {
-  int rc = NB_ERR_INVALID;
+int launch_dune(nb_pan* p, const nb::DuneParams& prm, cudaStream_t st) {
   char msg[256] = "";
-  if (p->dune_variant >= 2) {
-    rc = nb::launch_dune_tc(prm, p->d_tc_image, p->d_tc_screen, p->tc_flags, p->dune_variant, p->sm_count, p->max_smem_optin, st, msg, sizeof(msg));
-    if (rc) return fail(rc, "%s", msg);
-    g_launches += p->dune_variant == 4 ? 3 : 1;
-    return NB_OK;
-  }
-  if (p->dune_variant == 1) {
-    rc = nb::launch_dune_mma(prm, p->d_image, p->sm_count, p->max_smem_optin, cta_limit, st, msg, sizeof(msg));
-    if (rc) return fail(rc, "%s", msg);
-    ++g_launches;
-    return NB_OK;
-  }
-  switch (p->cfg.edge_dim) {
-#define NB_CASE(E_)                                                                                        \
-  case E_:                                                                                                 \
-    rc = nb::launch_dune_e<E_>(prm, p->sm_count, p->max_smem_optin, st, msg, sizeof(msg));                 \
-    break;
-#if NB_EDGE_MASK & (1 << 3)
-    NB_CASE(3)
-#endif
-#if NB_EDGE_MASK & (1 << 4)
-    NB_CASE(4)
-#endif
-#if NB_EDGE_MASK & (1 << 5)
-    NB_CASE(5)
-#endif
-#if NB_EDGE_MASK & (1 << 6)
-    NB_CASE(6)
-#endif
-#if NB_EDGE_MASK & (1 << 7)
-    NB_CASE(7)
-#endif
-#if NB_EDGE_MASK & (1 << 8)
-    NB_CASE(8)
-#endif
-#undef NB_CASE
-    default:
-      return fail(NB_ERR_INVALID, "edge_dim %d not built into this library (mask 0x%x)", p->cfg.edge_dim, NB_EDGE_MASK);
-  }
-  if (rc) return fail(rc, "%s", msg);
-  ++g_launches;
+  const bool screen = p->dune_variant == 4;
+  if (int rc = nb::launch_dune_tc(prm, p->d_tc_image, p->d_tc_screen, p->tc_flags, screen, p->sm_count, p->max_smem_optin, st, msg, sizeof(msg)))
+    return fail(rc, "%s", msg);
+  g_launches += screen ? 3 : 1;
   return NB_OK;
 }
 
@@ -669,9 +620,6 @@ int nb_pan_create(const nb_pan_config* cfg, const float* weights, int64_t n_weig
     NB_CUDA(dalloc(&p->d_weights, (size_t)n_weights));
     NB_CUDA(cudaMemcpy(p->d_weights, weights, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
     std::vector<unsigned char> image;
-    nb::build_mma_image(weights, cfg->edge_dim, image);
-    NB_CUDA(dalloc(&p->d_image, image.size()));
-    NB_CUDA(cudaMemcpy(p->d_image, image.data(), image.size(), cudaMemcpyHostToDevice));
     p->tc_flags = nb::build_tc_image(weights, cfg->edge_dim, image, false);
     NB_CUDA(dalloc(&p->d_tc_image, image.size()));
     NB_CUDA(cudaMemcpy(p->d_tc_image, image.data(), image.size(), cudaMemcpyHostToDevice));
@@ -742,7 +690,7 @@ int nb_pan_destroy(nb_pan_t* p) {
   if (p->ev_inputs_free) cudaEventDestroy(p->ev_inputs_free);
   for (cudaEvent_t e : p->ev_chunk)
     if (e) cudaEventDestroy(e);
-  void* bufs[] = {p->d_tc_image, p->d_image, p->d_weights, p->sel_mu, p->sel_lam, p->sel_pts, p->sel_dist, p->sel_count, p->prev_s, p->prev_u, p->prev_mu,
+  void* bufs[] = {p->d_tc_image, p->d_weights, p->sel_mu, p->sel_lam, p->sel_pts, p->sel_dist, p->sel_count, p->prev_s, p->prev_u, p->prev_mu,
                   p->prev_lam, p->prev_count, p->prev_valid, p->active, p->iters, p->status, p->ipm_it, p->min_dist, p->h_in, p->h_out, p->h_np, p->h_io,
                   p->d_tc_screen, p->cand_idx, p->cand_cnt, p->cand_dt, p->cand_rad, p->tab_cell, p->tab_rad, p->screen_stats, p->flag_list, p->flag_count, p->refine_list, p->warm, p->warm_valid, p->work_counters, p->adj_rec, p->adj_gs, p->adj_gu, p->adj_gd, p->adj_gtheta, p->adj_valid};
   for (void* b : bufs)
@@ -767,8 +715,8 @@ int nb_pan_set_iteration(nb_pan_t* p, int32_t iter_num, float iter_threshold) {
 int nb_pan_set_option(nb_pan_t* p, int32_t option, int32_t value) {
   if (!p) return fail(NB_ERR_INVALID, "null handle");
   if (option == NB_OPT_DUNE_KERNEL) {
-    if (value < 0 || value > 4)
-      return fail(NB_ERR_INVALID, "NB_OPT_DUNE_KERNEL takes 0 (fp32 ffma), 1 (mma.sync), 2 (wgmma), 3 (wgmma, two threads per point) or 4 (wgmma with screening)");
+    if (value != 2 && value != 4)
+      return fail(NB_ERR_INVALID, "NB_OPT_DUNE_KERNEL takes 2 (wgmma on every point) or 4 (wgmma with screening), got %d", value);
     p->dune_variant = value;
     if (value == 4 && p->d_tc_screen) {
       NB_CUDA(cudaSetDevice(p->cfg.device));
@@ -919,7 +867,7 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
   NB_CUDA(cudaMemcpyAsync(out_u, nom_u, (size_t)B * 2 * T * sizeof(float), cudaMemcpyDeviceToDevice, st));
   NB_CUDA(cudaMemsetAsync(out_d, 0, (size_t)B * T * sizeof(float), st));
   // K iterations of {DUNE, NRMP} for the environments [lo, hi) on stream s
-  auto run_range = [&](int lo, int hi, cudaStream_t s, int dune_cta_limit, int counter_slot, int k0, int k1) -> int {
+  auto run_range = [&](int lo, int hi, cudaStream_t s, int counter_slot, int k0, int k1) -> int {
     const int nb_ = hi - lo;
     const size_t T1s = (size_t)T1, Ms = (size_t)c.nrmp_max_num, Es = (size_t)(c.edge_dim > 0 ? c.edge_dim : 1);
     for (int k = k0; k < k1; ++k) {
@@ -960,10 +908,10 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
             dc.cand_idx = d.cand_idx + off * T1s * nb::kCandMax; dc.cand_dt = d.cand_dt + off * T1s * nb::kCandMax;
             dc.cand_cnt = d.cand_cnt + off * T1s; dc.cand_rad = d.cand_rad + off * T1s * nb::kCandMax;
             dc.flag_list = d.flag_list + off * T1s; dc.refine_list = d.refine_list + (size_t)2 * off * T1s;
-            if (int rc = launch_dune(p, dc, s, dune_cta_limit)) return rc;
+            if (int rc = launch_dune(p, dc, s)) return rc;
           }
         } else {
-          if (int rc = launch_dune(p, d, s, dune_cta_limit)) return rc;
+          if (int rc = launch_dune(p, d, s)) return rc;
         }
       }
       nb::NrmpParams n{};
@@ -992,7 +940,7 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
   };
   const int parts = (p->overlap > 1 && with_dune && B >= 64 * p->overlap) ? p->overlap : 1;
   if (parts == 1) {
-    if (int rc = run_range(0, B, st, 0, 0, 0, c.iter_num)) return rc;
+    if (int rc = run_range(0, B, st, 0, 0, c.iter_num)) return rc;
   } else {
     // sub-batches on internal streams: the DUNE kernel of one part (issue / tensor / MUFU bound) shares the SMs with the
     // NRMP kernel of another (latency bound, few warps)
@@ -1011,13 +959,13 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
         for (int i = 0; i < parts; ++i) {
           int lo, hi;
           range_of(i, lo, hi);
-          if (int rc = run_range(lo, hi, p->streams[i], 1, 1 + i, k, k + 1)) return rc;
+          if (int rc = run_range(lo, hi, p->streams[i], 1 + i, k, k + 1)) return rc;
         }
     } else {
       for (int i = 0; i < parts; ++i) {
         int lo, hi;
         range_of(i, lo, hi);
-        if (int rc = run_range(lo, hi, p->streams[i], 1, 1 + i, 0, c.iter_num)) return rc;
+        if (int rc = run_range(lo, hi, p->streams[i], 1 + i, 0, c.iter_num)) return rc;
       }
     }
     for (int i = 0; i < parts; ++i) {

@@ -293,17 +293,35 @@ def test_capacity_growth_and_shape_checks():
     assert (pan.status.cpu().numpy() == 0).all()
 
 
-@pytest.mark.parametrize("dune_kernel", [4, 2, 1, 0])
-def test_pentagon_robot_five_edges_random_weights(dune_kernel, tmp_path):
+# build_tc_image (csrc/dune_tc.cu): the warpgroup kernels take the shared-reciprocal tanh only when every LayerNorm output j satisfies
+# |2 log2(e) g_j| sqrt(32) + |2 log2(e) beta_j| <= 30 (products rounded to float32 as in the image)
+def _tanh_bound(state_dict):
+    amax = 0.0
+    for i in (1, 6, 11):
+        g, be = ((state_dict[f"MLP.{i}.{k}"].double().numpy() * 2.8853900817779268).astype(np.float32).astype(np.float64) for k in ("weight", "bias"))
+        amax = max(amax, float((np.abs(g) * np.sqrt(32.0) + np.abs(be)).max()))
+    return amax
+
+
+@pytest.mark.parametrize("dune_kernel,ln_gain", [(4, 1.0), (2, 1.0), (4, 2.5), (2, 2.5)], ids=["4", "2", "4-ln_gain2.5", "2-ln_gain2.5"])
+def test_pentagon_robot_five_edges_random_weights(dune_kernel, ln_gain, tmp_path):
     """E = 5 (no shipped checkpoint has E != 4): a randomly initialised ObsPointNet(2, 5) saved in the
-    reference's checkpoint format, run through both DUNE kernels and the oracle."""
+    reference's checkpoint format, run through the DUNE kernel and the oracle.  With its LayerNorm gains scaled by 2.5 the tanh
+    arguments exceed build_tc_image's bound, so the wgmma kernels take plain reciprocals (dune_tcp_kernel<false>,
+    dune_refine_kernel<false>), as for any such checkpoint.  The screening pipeline must give the exact kernel's bits either way."""
     import types
 
     from neupan_b200 import PAN, ObsPointNet, robot
     from oracle import dune as od, nrmp as onr
+    from test_gpu_screen import _assert_equal
 
     torch.manual_seed(11)
     net = ObsPointNet(2, 5)
+    with torch.no_grad():
+        for i in (1, 6, 11):
+            net.MLP[i].weight.mul_(ln_gain)
+    amax = _tanh_bound(net.state_dict())
+    assert (amax <= 30.0) == (ln_gain == 1.0), amax  # 16.3 for the default gains of 1, 40.8 scaled
     ck = str(tmp_path / "model_pentagon.pth")
     torch.save(net.state_dict(), ck)
     verts = [[1.2, 0.0], [0.4, 1.1], [-0.9, 0.7], [-0.9, -0.7], [0.4, -1.1]]
@@ -312,14 +330,39 @@ def test_pentagon_robot_five_edges_random_weights(dune_kernel, tmp_path):
     cfg = CONFIGS["C4"]
     B, N = 4, 96
     inp = make_inputs(cfg, B=B, N=N, scene="obstacles")
-    pan = PAN(10, 0.1, rb, iter_num=1, dune_max_num=N, nrmp_max_num=10, dune_checkpoint=ck, iter_threshold=0.0,
-              adjust_kwargs=dict(cfg.adjust), max_envs=B, max_points=N, dune_kernel=dune_kernel)
-    got = run_pan(pan, inp)
+    new = lambda dk: PAN(10, 0.1, rb, iter_num=1, dune_max_num=N, nrmp_max_num=10, dune_checkpoint=ck, iter_threshold=0.0,
+                         adjust_kwargs=dict(cfg.adjust), max_envs=B, max_points=N, dune_kernel=dk)
+    run = lambda pan: (*run_pan(pan, inp), {k: v.cpu().numpy() for k, v in pan.read_selection().items()})
+    pan = new(dune_kernel)
+    got = run(pan)
     spec = onr.RobotSpec("diff", rb.G, rb.h, rb.max_speed.reshape(-1), rb.max_acce.reshape(-1), 0.1, None)
     w = od.load_weights(ck)
     mk = lambda: op.OraclePAN(spec, w, T=10, iter_num=1, dune_max_num=N, nrmp_max_num=10, iter_threshold=0.0, adjust=onr.Adjust(**cfg.adjust))
-    assert (_cmp(got, op.run_batch(mk, inp)) < TOL).all()
-    assert pan.read_selection()["mu"].shape == (B, 11, 10, 5)
+    assert (_cmp(got[:4], op.run_batch(mk, inp)) < TOL).all()
+    assert got[4]["mu"].shape == (B, 11, 10, 5)
+    if dune_kernel == 4:
+        _assert_equal(got, run(new(2)))  # selection, mu, lam, distances and the PAN outputs, bit for bit
+
+
+def test_dune_kernel_option_takes_2_or_4():
+    """NB_OPT_DUNE_KERNEL selects the exact kernel on every point (2) or the screening pipeline (4); any other value is refused
+    with NB_ERR_INVALID (ValueError in Python) and leaves the handle as it was."""
+    from neupan_b200 import _lib
+
+    cfg = CONFIGS["C4"]
+    inp = make_inputs(cfg, B=2, scene="obstacles")
+    pan = make_pan(cfg, K=1, max_envs=2)
+    before = run_pan(pan, inp)
+    lib = pan._ensure_handle(2, cfg.N)
+    for v in (-1, 0, 1, 3, 5):
+        assert lib.nb_pan_set_option(pan._handle, _lib.OPT_DUNE_KERNEL, v) == _lib.NB_ERR_INVALID
+        msg = lib.nb_last_error().decode()
+        assert "takes 2 (" in msg and "or 4 (" in msg and msg.endswith(f"got {v}"), msg
+    after = run_pan(pan, inp)
+    for x, y in zip(before, after):
+        assert np.array_equal(x, y)
+    with pytest.raises(ValueError, match="NB_OPT_DUNE_KERNEL takes 2"):
+        run_pan(make_pan(cfg, K=1, max_envs=2, dune_kernel=1), inp)
 
 
 @pytest.mark.parametrize("T,M", [(12, 8), (20, 12), (6, 3), (10, 1)])
@@ -337,26 +380,3 @@ def test_generic_horizon_and_hinge_counts(T, M):
     err = _cmp(got, ref)
     assert (err < TOL).all(), (T, M, err)
     assert (pan.status.cpu().numpy() == 0).all()
-
-
-def test_plain_reciprocal_tanh_in_subprocess():
-    """NB_DUNE_TC=4 (read at process start) makes the warpgroup kernels use plain reciprocals instead of the shared-reciprocal
-    tanh.  The result must agree with the mma.sync kernel."""
-    import os
-    import subprocess
-    import sys
-
-    code = (
-        "import sys, os; sys.path.insert(0, os.getcwd()); sys.path.insert(0, 'tests')\n"
-        "import numpy as np\n"
-        "from gpu_helpers import make_pan, run_pan\n"
-        "from helpers import CONFIGS, make_inputs\n"
-        "cfg = CONFIGS['C3']; inp = make_inputs(cfg, B=3)\n"
-        "a = make_pan(cfg, K=1, max_envs=3, dune_kernel=2); run_pan(a, inp); sa = a.read_selection()\n"
-        "b = make_pan(cfg, K=1, max_envs=3, dune_kernel=1); run_pan(b, inp); sb = b.read_selection()\n"
-        "assert np.allclose(sa['distance'].cpu().numpy(), sb['distance'].cpu().numpy(), atol=2e-5)\n"
-        "assert np.allclose(sa['points'].cpu().numpy(), sb['points'].cpu().numpy(), atol=1e-6)\n"
-        "print('variant ok')\n")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-c", code], cwd=root, env=dict(os.environ, NB_DUNE_TC="4"), capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0 and "variant ok" in r.stdout, r.stdout + r.stderr

@@ -37,10 +37,10 @@ def _oracle_dune(cfg, inp, b):
 
 
 @pytest.mark.parametrize("cname", ["C1", "C2", "C3", "C4", "C5"])
-@pytest.mark.parametrize("dune_kernel", [4, 3, 2, 1, 0])
+@pytest.mark.parametrize("dune_kernel", [4, 2])
 def test_dune_half_matches_oracle(cname, dune_kernel):
-    """DUNE kernel alone (tensor-core and all-FP32 variants): the M closest points per (env, step),
-    their mu, lam, distance."""
+    """DUNE kernel alone (the screening pipeline and the exact kernel on every point): the M closest points per
+    (env, step), their mu, lam, distance."""
     cfg = CONFIGS[cname]
     B = 6
     inp = make_inputs(cfg, B=B)

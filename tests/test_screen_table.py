@@ -1,4 +1,4 @@
-"""CPU check of the screen's distance table (csrc/dune_table_kernel.cuh, table_lookup / table_bilerp in csrc/dune_kernel.cuh),
+"""CPU check of the screen's distance table (csrc/dune_table_kernel.cuh, table_lookup / table_bilerp in csrc/dune_common.cuh),
 transcribed to numpy: cells from a grid sampled kTableSub times finer, the cell's radius from the fine samples, the lookup's bilinear
 interpolation.  With the network of every shipped checkpoint, the radius must bound the interpolation error at points the build never
 sampled, and the table's error ratio must stay below the smallest screening bound a handle uses (c_mu >= 0.008) wherever a scene can

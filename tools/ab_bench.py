@@ -24,16 +24,13 @@ def build(specs):
     nb.build()  # default library + all default objects
     os.makedirs(VARDIR, exist_ok=True)
     nvcc = nb._nvcc()
-    edge_dims = [3, 4, 5, 6, 7, 8]
-    mask = sum(1 << e for e in edge_dims)
     for spec in specs:
         name, tu, *flags = spec.split(":")
+        if tu not in nb.UNITS:
+            raise SystemExit(f"{tu} is not one of the library's translation units {nb.UNITS}")
         obj = os.path.join(VARDIR, f"{name}_{os.path.splitext(tu)[0]}.o")
-        extra = [f"-DNB_EDGE_MASK={mask}"] if tu == "pan_api.cu" else []
-        subprocess.run([nvcc, *nb.ARCH, *nb.COMMON, *extra, *flags, "-c", os.path.join(nb.CSRC, tu), "-o", obj], check=True)
-        default_obj = {"pan_api.cu": "pan_api.o", "dune_tc.cu": "dune_tc.o", "dune_mma.cu": "dune_mma.o"}[tu]
-        objs = [os.path.join(nb.OBJDIR, f"dune_e{e}.o") for e in edge_dims] + [os.path.join(nb.OBJDIR, o) for o in ("dune_mma.o", "dune_tc.o", "pan_api.o")]
-        objs = [obj if os.path.basename(o) == default_obj else o for o in objs]
+        subprocess.run([nvcc, *nb.ARCH, *nb.COMMON, *flags, "-c", os.path.join(nb.CSRC, tu), "-o", obj], check=True)
+        objs = [obj if u == tu else nb.obj_path(u) for u in nb.UNITS]
         subprocess.run([nvcc, *nb.ARCH, "-shared", "-o", os.path.join(VARDIR, f"{name}.so"), *objs], check=True)
         print("built", name)
 

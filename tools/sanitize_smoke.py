@@ -10,11 +10,10 @@ SECTIONS = os.environ.get("NB_SMOKE_SECTIONS", "variants,screen,adjoint,train,wo
 for cname, B, N in (("C4", 6, 70), ("C5", 3, 40), ("C2", 5, 33), ("C4", 3, 300), ("C3", 2, 600)) if "variants" in SECTIONS else ():
     cfg = CONFIGS[cname]
     inp = make_inputs(cfg, B=B, N=N, scene="obstacles")
-    for dk in (3, 2, 1, 0):
-        pan = make_pan(cfg, K=2, N=N, max_envs=B, dune_kernel=dk, nrmp_warm=1 if dk == 2 else 0)
-        S, U, D, md = run_pan(pan, inp)
-        assert np.isfinite(S).all() and (pan.status.cpu().numpy() == 0).all()
-        pan.close()
+    pan = make_pan(cfg, K=2, N=N, max_envs=B, dune_kernel=2, nrmp_warm=1)
+    S, U, D, md = run_pan(pan, inp)
+    assert np.isfinite(S).all() and (pan.status.cpu().numpy() == 0).all()
+    pan.close()
 # round 2: the screening pipeline (both screening kernels, step-0 reuse, paired refine, exact remainder), the stop criterion as its own
 # kernel (B >= 256), sub-batches on internal streams (B >= 128) and the chunked upload (nb_pan_forward_h2d / _host)
 if "screen" in SECTIONS:
