@@ -50,7 +50,7 @@ struct DuneParams {
   int skip_t0;              // screen kernels: step-0 items are skipped (cand_cnt = 0) and keep the outputs of the previous launch -- set by
                             // nb_pan_forward for PAN iterations k > 0: nom_s[:, 0] is the fixed initial state (robot.py:234; the NRMP kernel
                             // copies the column bit for bit), so item (b, 0) has the same inputs and the same result in every iteration
-  int screen_mma;           // launcher hint (NB_OPT_DUNE_SCREEN_MMA): 1 = screening pass on mma.sync (dune_screen_mma_kernel.cuh) where N <= 512
+  int screen_mma;           // launcher hint (NB_OPT_DUNE_SCREEN_MMA): 1 = screening pass on mma.sync (dune_screen_mma_kernel.cuh) where N <= 1024
   int calibrate;            // screen kernel: items with N <= 32 are NOT short-cut: all their points become candidates with their screened
                             // distance, so that the refine kernel's statistics compare the two networks on every point (nb_pan calibration)
 };
@@ -62,12 +62,23 @@ __device__ __forceinline__ float table_bilerp(const float4& c, float a, float b)
   return fmaf(b, d1 - d0, d0);
 }
 
-// screened distance d and error radius r of the robot-frame point (x, y) from the table; false when the point lies outside it
-__device__ __forceinline__ bool table_lookup(const DuneParams& prm, float x, float y, float& d, float& r) {
+// the table cell c of the robot-frame point (x, y) and the point's position (a, b) in it; false when the point lies outside the table
+__device__ __forceinline__ bool table_cell(const DuneParams& prm, float x, float y, int& c, float& a, float& b) {
   const float fx = (x + prm.tab_half) * prm.tab_inv_h, fy = (y + prm.tab_half) * prm.tab_inv_h, nf = (float)prm.tab_n;
   if (!(fx >= 0.f && fx < nf && fy >= 0.f && fy < nf)) return false;  // NaN coordinates are outside as well
-  const int ix = (int)fx, iy = (int)fy, c = iy * prm.tab_n + ix;
-  d = table_bilerp(__ldg(prm.tab_cell + c), fx - (float)ix, fy - (float)iy);
+  const int ix = (int)fx, iy = (int)fy;
+  c = iy * prm.tab_n + ix;
+  a = fx - (float)ix;
+  b = fy - (float)iy;
+  return true;
+}
+
+// screened distance d and error radius r of the robot-frame point (x, y) from the table; false when the point lies outside it
+__device__ __forceinline__ bool table_lookup(const DuneParams& prm, float x, float y, float& d, float& r) {
+  int c;
+  float a, b;
+  if (!table_cell(prm, x, y, c, a, b)) return false;
+  d = table_bilerp(__ldg(prm.tab_cell + c), a, b);
   r = __ldg(prm.tab_rad + c);
   return true;
 }

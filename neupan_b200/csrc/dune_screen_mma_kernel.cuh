@@ -9,7 +9,9 @@
 // freely and the MUFU (tanh), FMA, ALU and tensor phases of the four warps of a scheduler overlap.  The exact path (3 passes)
 // keeps the warpgroup kernels (dune_refine_kernel / dune_tcp_kernel).
 //
-// Mapping (clouds of up to 1024 points; see the kP template parameter): CTA = 4 warps = one (environment, step) item at a time; pass p, warp w: points [128 p + 32 w, +32) as two m16 tiles.
+// Two kernels: dune_screen_warp_kernel (clouds of <= 512 points: one warp per (environment, step) item, see its comment) and
+// dune_screen_mma_kernel (513..1024 points: CTA = 4 warps = one item at a time; pass p, warp w: points [128 p + 32 w, +32)).
+// The network tile is the same in both: 32 points as two m16 tiles.
 // Lane (g = lane >> 2, tq = lane & 3) holds rows g, g+8 (tile 0), g, g+8 (tile 1) -- "row slots" 0..3 = local points g + 8 r --
 // and columns 8 j + 2 tq, +1 (j = 0..3) of every 32-wide activation; it OWNS local point 8 tq + g (coordinates in, key out), so
 // the four row slots of a quad are exactly the points its four lanes own (one shuffle each way, no shared memory).
@@ -151,6 +153,92 @@ __device__ __forceinline__ void dense_frag(const uint4* __restrict__ wl, const f
     }
 }
 
+// operand staging by `nthreads` threads: the screen image of dune_screen_kernel (K-major wgmma layout, hi halves) re-ordered into
+// mma.sync B fragments, the permuted vectors and the bias fragments
+__device__ __forceinline__ void stage_operands(const unsigned char* __restrict__ image, uint4* wfrag, float* vec, float4* biasq, int tid, int nthreads) {
+  using I = TcImage;
+  uint32_t* wf = reinterpret_cast<uint32_t*>(wfrag);
+  for (int x = tid; x < kFragBytes / 4; x += nthreads) {
+    const int c = x & 3, ln = (x >> 2) & 31, jp = (x >> 7) & 1, s = (x >> 8) & 1, l = x >> 9;
+    const int n = 8 * (2 * jp + (c >> 1)) + (ln >> 2), k = 16 * s + 2 * (ln & 3) + 8 * (c & 1);
+    const size_t off = (size_t)l * I::kLayerStride + (size_t)(k / 16) * 1024 + ((k % 16) / 8) * 512 + (n / 8) * 128 + (n % 8) * 16 + (k % 8) * 2;
+    wf[x] = *reinterpret_cast<const uint32_t*>(image + off);
+  }
+  const float* fl = reinterpret_cast<const float*>(image + I::kFloatOff);
+  for (int x = tid; x < kVecs * 32; x += nthreads) {
+    const int v = x >> 5, e = x & 31, q = e >> 3, j = (e >> 1) & 3, h = e & 1;
+    const int src = v == V_W0X ? I::W0X : v == V_W0Y ? I::W0Y : v == V_B0 ? I::B0 : I::G1 + 32 * (v - V_G1);
+    vec[x] = fl[src + 8 * j + 2 * q + h];
+  }
+  for (int x = tid; x < 5 * 4 * 4; x += nthreads) {  // [layer][tq][j]
+    const int l = x >> 4, q = (x >> 2) & 3, j = x & 3;
+    const float bx = fl[I::BH + 32 * l + 8 * j + 2 * q], by = fl[I::BH + 32 * l + 8 * j + 2 * q + 1];
+    biasq[x] = make_float4(bx, by, bx, by);
+  }
+}
+
+// The screening network on one 32-point tile, all six layers in the warp's registers.  (x0, y0) = the robot-frame coordinates of the
+// lane's own point (local point 8 tq + g of the tile; zeros for rows beyond the cloud); returns that point's d~.  wl, vq, bqq: the
+// lane's views of the staged operands.
+__device__ __forceinline__ float tile_network(const Geometry& geo, float x0, float y0, int lane, const uint4* __restrict__ wl,
+                                              const float* __restrict__ vq, const float4* __restrict__ bqq) {
+  float xr[4], yr[4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    xr[r] = __shfl_sync(0xffffffffu, x0, (lane & ~3) | r);
+    yr[r] = __shfl_sync(0xffffffffu, y0, (lane & ~3) | r);
+  }
+  f2 acc[4][4];
+  uint32_t a[2][2][4];
+  {  // layer 0 (2 -> 32) on the FMA pipe, directly in accumulator layout
+    const ulonglong2 wx01 = *reinterpret_cast<const ulonglong2*>(vq + 32 * V_W0X), wx23 = *reinterpret_cast<const ulonglong2*>(vq + 32 * V_W0X + 4);
+    const ulonglong2 wy01 = *reinterpret_cast<const ulonglong2*>(vq + 32 * V_W0Y), wy23 = *reinterpret_cast<const ulonglong2*>(vq + 32 * V_W0Y + 4);
+    const ulonglong2 b01 = *reinterpret_cast<const ulonglong2*>(vq + 32 * V_B0), b23 = *reinterpret_cast<const ulonglong2*>(vq + 32 * V_B0 + 4);
+    const f2 wx[4] = {wx01.x, wx01.y, wx23.x, wx23.y}, wy[4] = {wy01.x, wy01.y, wy23.x, wy23.y}, bb[4] = {b01.x, b01.y, b23.x, b23.y};
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const f2 x2 = tc::pk(xr[r], xr[r]), y2 = tc::pk(yr[r], yr[r]);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) acc[r][j] = tc::fma2(wy[j], y2, tc::fma2(wx[j], x2, bb[j]));
+    }
+  }
+  ln_tanh_frag(acc, vq + 32 * V_G1, vq + 32 * V_BE1, lane, a);
+  dense_frag<4>(wl + 0 * 128, bqq + 16 * 0, a, acc);
+  relu_frag(acc, a);
+  dense_frag<4>(wl + 1 * 128, bqq + 16 * 1, a, acc);
+  ln_tanh_frag(acc, vq + 32 * V_G6, vq + 32 * V_BE6, lane, a);
+  dense_frag<4>(wl + 2 * 128, bqq + 16 * 2, a, acc);
+  relu_frag(acc, a);
+  dense_frag<4>(wl + 3 * 128, bqq + 16 * 3, a, acc);
+  ln_tanh_frag(acc, vq + 32 * V_G11, vq + 32 * V_BE11, lane, a);
+  f2 mu[4][1];
+  dense_frag<1>(wl + 4 * 128, bqq + 16 * 4, a, mu);
+
+  // head: d~ = relu(mu)^T (G p0 - h): partial over the lane's two channels for each row slot, transposing quad reduction
+  // geometry rows of the lane's two head channels (zero beyond E: their partial distance is 0)
+  const int e0 = 2 * (lane & 3), e1 = e0 + 1;
+  const float gx0 = e0 < geo.E ? geo.G[e0][0] : 0.f, gy0 = e0 < geo.E ? geo.G[e0][1] : 0.f, h0 = e0 < geo.E ? geo.h[e0] : 0.f;
+  const float gx1 = e1 < geo.E ? geo.G[e1][0] : 0.f, gy1 = e1 < geo.E ? geo.G[e1][1] : 0.f, h1 = e1 < geo.E ? geo.h[e1] : 0.f;
+  float dp[4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    float m0, m1;
+    tc::upk(mu[r][0], m0, m1);
+    const float ge0 = fmaf(gy0, yr[r], gx0 * xr[r]) - h0, ge1 = fmaf(gy1, yr[r], gx1 * xr[r]) - h1;
+    dp[r] = fmaf(fmaxf(m1, 0.f), ge1, fmaxf(m0, 0.f) * ge0);
+  }
+  return quad_transpose_sum(dp, lane & 3);  // the lane's own point
+}
+
+// the error radius the network screen assumes for the point (x0, y0): c_mu sum_e |G_e p0 - h_e| + 1e-4
+__device__ __forceinline__ float network_radius(const DuneParams& prm, float x0, float y0) {
+  float sa = 0.f;
+#pragma unroll
+  for (int e = 0; e < kMaxEdges; ++e)
+    if (e < prm.geo.E) sa += fabsf(fmaf(prm.geo.G[e][1], y0, prm.geo.G[e][0] * x0) - prm.geo.h[e]);
+  return fmaf(prm.c_mu, sa, 1e-4f);
+}
+
 }  // namespace sm
 
 // shared memory: B fragments | permuted vectors | bias fragments | raw points of the item in flight (x | y | vx | vy, N floats each) |
@@ -159,14 +247,11 @@ __host__ __device__ inline size_t dune_screen_mma_smem_bytes(int N, int M) {
   return (size_t)sm::kFragBytes + sm::kVecBytes + sm::kBiasQBytes + (size_t)N * 16 + (size_t)4 * M * 4 + 64;
 }
 
-#ifndef NB_SMMA_BLOCKS
-#define NB_SMMA_BLOCKS 5  // CTAs per SM the register allocation is made for: 96 registers, 12 B of spills (NB_SMMA_BLOCKS is a tuning knob: time 4, 5 and 6 with bench.py)
-#endif
-// kP = the most 128-point passes an item can need: every thread keeps the bounds of its <= kP points in registers, with the point's
-// index in the low kIdxBits bits of the key.  kP = 4: N <= 512 (96 registers, 5 CTAs per SM); kP = 8: N <= 1024 (4 CTAs per SM).  The
-// launcher sends larger clouds to dune_screen_kernel, whose shared-memory key arrays have no such limit.
-template <int kP>
-__global__ void __launch_bounds__(128, kP <= 4 ? NB_SMMA_BLOCKS : 4) dune_screen_mma_kernel(const DuneParams prm, const unsigned char* __restrict__ image) {
+// Clouds of 513..1024 points (smaller ones take dune_screen_warp_kernel below, larger ones dune_screen_kernel, whose shared-memory key
+// arrays have no size limit).  kP = the most 128-point passes an item can need: every thread keeps the bounds of its <= kP points in
+// registers, with the point's index in the low kIdxBits bits of the key.
+__global__ void __launch_bounds__(128, 4) dune_screen_mma_kernel(const DuneParams prm, const unsigned char* __restrict__ image) {
+  constexpr int kP = 8;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   using I = TcImage;
   uint4* wfrag = reinterpret_cast<uint4*>(smem_dyn);
@@ -213,7 +298,7 @@ __global__ void __launch_bounds__(128, kP <= 4 ? NB_SMMA_BLOCKS : 4) dune_screen
   const float gx0 = e0 < E ? prm.geo.G[e0][0] : 0.f, gy0 = e0 < E ? prm.geo.G[e0][1] : 0.f, h0 = e0 < E ? prm.geo.h[e0] : 0.f;
   const float gx1 = e1 < E ? prm.geo.G[e1][0] : 0.f, gy1 = e1 < E ? prm.geo.G[e1][1] : 0.f, h1 = e1 < E ? prm.geo.h[e1] : 0.f;
   const int own0 = 32 * warp + 8 * tq + g;  // the lane's point in pass 0 (pass p: + 128 p)
-  constexpr int kIdxBits = kP <= 4 ? 9 : 10;
+  constexpr int kIdxBits = 10;
   constexpr uint32_t kIdxMask = (1u << kIdxBits) - 1u;
   // smallest value above k whose low kIdxBits bits carry the point's index: keys become unique (a REDUX round removes exactly one entry);
   // rounding an upper bound UP only widens the candidate set
@@ -430,6 +515,307 @@ __global__ void __launch_bounds__(128, kP <= 4 ? NB_SMMA_BLOCKS : 4) dune_screen
     par ^= 1;
   }
   tc::cp_async_wait_all();
+}
+
+// ---- Clouds of <= 512 points: one warp per (environment, step) item.
+// The T+1 items of an environment share its cloud, so a CTA of kScreenWarps warps is persistent over ENVIRONMENTS (over `parts` CTAs
+// per environment when the batch is smaller than the resident grid, each with every parts-th group of W items): the cloud (x | y |
+// vx | vy) is staged once per environment by cp.async, double-buffered (the next environment's copy is issued right after the barrier
+// that opens the current one: one block barrier per environment).  The warps take the environment's items one at a time; lane l of a
+// warp computes the frame of the warp's l-th item (one sincos per step) and the item loop broadcasts it by shuffle.  Per item, a lane
+// owns point 32 j + 8 tq + g of every 32-point tile j (the row slot layout of the network, see the top of this file): all table
+// gathers of the item are issued before any is consumed; a tile with a point outside the table (every tile when there is no table)
+// then runs the network.  tau = the M-th smallest key of the warp (M REDUX rounds), the candidates are compacted by ballot: no merge
+// stage, no block barrier, no shared-memory atomics per item.  Candidate and item counts, and the refine lists, are collected in
+// shared memory and reach global memory once per environment (refine lists: one atomic per size class) or once per CTA (statistics).
+constexpr int kWarpTiles = 16;  // 32-point tiles of an item: N <= 512, 9 index bits in the key (tc::unique_key)
+// warps per CTA and CTAs per SM the register allocation is made for (128 registers).  Measured on C4 (H100 80GB HBM3, 700 W, bench.py
+// 10 steps, 3 runs each): 4 warps x 4 CTAs 16.27-16.41 ms per step, 5 x 3 16.54-16.59 ms, 8 x 2 16.61-16.64 ms.
+#ifndef NB_SCREEN_WARPS
+#define NB_SCREEN_WARPS 4
+#endif
+#ifndef NB_SCREEN_WARP_BLOCKS
+#define NB_SCREEN_WARP_BLOCKS 4
+#endif
+constexpr int kScreenWarps = NB_SCREEN_WARPS;
+#ifndef NB_SCREEN_GATHER
+#define NB_SCREEN_GATHER 4
+#endif
+constexpr int kGather = NB_SCREEN_GATHER;  // table gathers in flight per lane
+
+// shared memory: B fragments | permuted vectors | bias fragments | two clouds (x | y | vx | vy, N floats each) | per-warp network
+// results (kWarpTiles x 32 float2) | refine lists of two environments ([parity][size class][T+1] items)
+__host__ __device__ inline size_t dune_screen_warp_smem_bytes(int N, int T) {
+  return (size_t)sm::kFragBytes + sm::kVecBytes + sm::kBiasQBytes + (size_t)2 * 4 * N * 4 + (size_t)kScreenWarps * kWarpTiles * 32 * 8 +
+         (size_t)2 * 2 * (T + 1) * 4;
+}
+
+__global__ void __launch_bounds__(32 * kScreenWarps, NB_SCREEN_WARP_BLOCKS)
+    dune_screen_warp_kernel(const DuneParams prm, const unsigned char* __restrict__ image, int parts) {
+  constexpr int W = kScreenWarps, kThreads = 32 * W;
+  extern __shared__ __align__(1024) unsigned char smem_dyn[];
+  uint4* wfrag = reinterpret_cast<uint4*>(smem_dyn);
+  float* vec = reinterpret_cast<float*>(smem_dyn + sm::kFragBytes);
+  float4* biasq = reinterpret_cast<float4*>(smem_dyn + sm::kFragBytes + sm::kVecBytes);
+  float* cloud = reinterpret_cast<float*>(smem_dyn + sm::kFragBytes + sm::kVecBytes + sm::kBiasQBytes);
+  const int T1 = prm.T + 1, N = prm.N, M = prm.M, B = prm.B;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, tq = lane & 3;
+  float2* net = reinterpret_cast<float2*>(cloud + (size_t)8 * N) + (size_t)warp * kWarpTiles * 32;
+  int* rlist = reinterpret_cast<int*>(cloud + (size_t)8 * N + (size_t)W * kWarpTiles * 64);
+  __shared__ int rcnt_s[2][2];   // [parity][size class] lengths of the refine lists in rlist
+  __shared__ unsigned stat_s[2];  // candidates and items screened by this CTA (screen_stats[2], [3])
+  __shared__ float4 frame_s[W][32];  // per warp: {sx, sy, cos, sin} of the steps of its next <= 32 items
+
+  sm::stage_operands(image, wfrag, vec, biasq, tid, kThreads);
+  if (tid < 4) rcnt_s[tid >> 1][tid & 1] = 0;
+  if (tid < 2) stat_s[tid] = 0;
+  const uint4* wl = wfrag + lane;
+  const float* vq = vec + 8 * tq;
+  const float4* bqq = biasq + 4 * tq;
+  const int own = 8 * tq + g;  // the lane's point in every tile
+  const int t_first = prm.skip_t0 ? 1 : 0;
+
+  // the points of environment bb its items screen (0: none -- inactive, or <= 32 points outside calibration: every point is a candidate)
+  auto screened_points = [&](int bb) -> int {
+    if (prm.active && prm.active[bb] == 0) return 0;
+    int nn = prm.num_points ? prm.num_points[bb] : N;
+    nn = nn > N ? N : nn;
+    return nn <= 0 || (nn <= kCandMax && !prm.calibrate) ? 0 : nn;
+  };
+  auto stage_cloud = [&](int bb, float* dst) {
+    const int nn = screened_points(bb);
+    const float* px = prm.points + (size_t)bb * 2 * N;
+    const float* vx = prm.velocities ? prm.velocities + (size_t)bb * 2 * N : nullptr;
+    for (int i = tid; i < nn; i += kThreads) {
+      tc::cp_async4(dst + i, px + i);
+      tc::cp_async4(dst + N + i, px + N + i);
+      if (vx) {
+        tc::cp_async4(dst + 2 * N + i, vx + i);
+        tc::cp_async4(dst + 3 * N + i, vx + N + i);
+      }
+    }
+  };
+  // lane 0: item -> the refine list of its size class, in shared memory (dune_refine_kernel packs two items of <= 16 candidates into one warp)
+  auto refine_push = [&](int par, int item, int nc) {
+    if (nc <= 0) return;
+    const int big = nc > 16 ? 1 : 0;
+    rlist[(par * 2 + big) * T1 + atomicAdd(&rcnt_s[par][big], 1)] = item;
+  };
+  // one warp: the refine lists of parity par to global memory, one atomic per non-empty size class
+  auto refine_flush = [&](int par) {
+#pragma unroll 1
+    for (int big = 0; big < 2; ++big) {
+      const int c = rcnt_s[par][big];
+      if (c == 0) continue;
+      int pos = 0;
+      if (lane == 0) pos = atomicAdd(prm.flag_count + 1 + big, c);
+      pos = __shfl_sync(0xffffffffu, pos, 0);
+      for (int x = lane; x < c; x += 32) prm.refine_list[(size_t)big * B * T1 + pos + x] = rlist[(par * 2 + big) * T1 + x];
+      __syncwarp();
+      if (lane == 0) rcnt_s[par][big] = 0;
+    }
+  };
+
+  // work unit u = part u % parts of environment u / parts: its warp w takes the items t_first + (u % parts) W + w + k parts W
+  const int units = B * parts, stride = parts * W;
+  if ((int)blockIdx.x < units) stage_cloud(blockIdx.x / parts, cloud);
+  int par = 0;  // parity of the CTA's unit: its cloud buffer and refine lists
+  for (int u = blockIdx.x; u < units; u += gridDim.x, par ^= 1) {
+    const int b = u / parts, part = u - b * parts;
+    const float* raw = cloud + (size_t)par * 4 * N;
+    tc::cp_async_wait_all();
+    // environment b's cloud has landed for every thread; every warp is done with the previous unit (the other buffer and lists)
+    __syncthreads();
+    if (u + (int)gridDim.x < units) stage_cloud((u + gridDim.x) / parts, cloud + (size_t)(par ^ 1) * 4 * N);
+    if (warp == W - 1) refine_flush(par ^ 1);
+
+    const int act = prm.active ? prm.active[b] : 1;
+    if (act == 0) {
+      if (part == 0)
+        for (int t = tid; t < T1; t += kThreads) prm.cand_cnt[(size_t)b * T1 + t] = 0;
+      continue;
+    }
+    int n = prm.num_points ? prm.num_points[b] : N;
+    n = n < 0 ? 0 : (n > N ? N : n);
+    if (tid == 0 && part == 0) {
+      if (prm.skip_t0) prm.cand_cnt[(size_t)b * T1] = 0;  // same inputs as in the previous PAN iteration: its outputs stand
+      else {
+        prm.sel_count[b] = n < M ? n : M;
+        if (n == 0 && prm.min_dist) prm.min_dist[b] = __int_as_float(0x7f800000);
+      }
+    }
+    const bool screen = n > kCandMax || prm.calibrate;
+    const float* ns = prm.nom_s + (size_t)b * 3 * T1;
+
+#pragma unroll 1
+    for (int t0 = t_first + part * W + warp; t0 < T1; t0 += 32 * stride) {
+      // lane l: the frame of this warp's item t0 + l stride (the arithmetic of tc::item_frame), read by every lane of the item
+      __syncwarp();
+      if (screen && t0 + lane * stride < T1) {
+        const int tl = t0 + lane * stride;
+        const float th = ns[2 * T1 + tl];
+        frame_s[warp][lane] = make_float4(ns[tl], ns[T1 + tl], cosf(th), sinf(th));
+      }
+      __syncwarp();
+#pragma unroll 1
+      for (int l = 0; l < 32 && t0 + l * stride < T1; ++l) {
+        const int t = t0 + l * stride, item = b * T1 + t;
+        if (!screen) {  // nothing to screen: every point is a candidate
+          if (lane < n) { prm.cand_idx[(size_t)item * kCandMax + lane] = lane; prm.cand_dt[(size_t)item * kCandMax + lane] = __int_as_float(0x7fc00000); }
+          if (lane == 0) { prm.cand_cnt[item] = n; refine_push(par, item, n); }
+          continue;
+        }
+        const float4 fr = frame_s[warp][l];
+        const float sx = fr.x, sy = fr.y, cs = fr.z, sn = fr.w;
+        // point i in the robot frame (tc::ItemFrame::local on the staged cloud); rows beyond n run on zeros (their results are never
+        // looked at)
+        auto local = [&](int i, float& x0, float& y0) {
+          x0 = 0.f; y0 = 0.f;
+          if (i < n) {
+            float gx = raw[i], gy = raw[N + i];
+            if (prm.velocities) {
+              gx = flow(gx, raw[2 * N + i], prm.dt, t);
+              gy = flow(gy, raw[3 * N + i], prm.dt, t);
+            }
+            const float dx = gx - sx, dy = gy - sy;
+            x0 = fmaf(cs, dx, sn * dy);
+            y0 = fmaf(cs, dy, -(sn * dx));
+          }
+        };
+
+        // the bounds of the lane's points, d~ and its error radius, collect in net[32 j + lane] (tile j): from the table where it covers
+        // the point, then from the network for the tiles with a point outside it (netm; every tile when there is no table)
+        const int tiles = (n + 31) >> 5;
+        uint32_t netm = 0u;
+        if (prm.tab_cell) {
+          uint32_t hitm = 0u;  // bit j: the point of tile j lies in the table or beyond n
+#pragma unroll 1
+          for (int h = 0; h < tiles; h += kGather) {  // kGather tiles at a time: all their gathers are issued before any is consumed
+            float4 cell[kGather];
+            float rad[kGather], ca[kGather], cb[kGather];
+#pragma unroll
+            for (int q = 0; q < kGather; ++q) {
+              const int j = h + q;
+              if (j < tiles) {
+                const int i = 32 * j + own;
+                float x0, y0;
+                local(i, x0, y0);
+                int c = 0;  // a point outside the table, or beyond n, reads cell 0
+                ca[q] = 0.f; cb[q] = 0.f;
+                const bool hit = i >= n || table_cell(prm, x0, y0, c, ca[q], cb[q]);
+                hitm |= hit ? 1u << j : 0u;
+                if (!__all_sync(0xffffffffu, hit)) netm |= 1u << j;
+                cell[q] = __ldg(prm.tab_cell + c);
+                rad[q] = __ldg(prm.tab_rad + c);
+              }
+            }
+#pragma unroll
+            for (int q = 0; q < kGather; ++q)
+              if (h + q < tiles) net[32 * (h + q) + lane] = make_float2(table_bilerp(cell[q], ca[q], cb[q]), rad[q]);
+          }
+#pragma unroll 1
+          for (uint32_t m = netm; m != 0u; m &= m - 1u) {
+            const int j = __ffs(m) - 1, i = 32 * j + own;
+            float x0, y0;
+            local(i, x0, y0);
+            const float dn = sm::tile_network(prm.geo, x0, y0, lane, wl, vq, bqq);
+            if (!((hitm >> j) & 1u)) net[32 * j + lane] = make_float2(dn, sm::network_radius(prm, x0, y0));
+          }
+        } else {
+#pragma unroll 1
+          for (int j = 0; j < tiles; ++j) {
+            const int i = 32 * j + own;
+            float x0, y0;
+            local(i, x0, y0);
+            const float dn = sm::tile_network(prm.geo, x0, y0, lane, wl, vq, bqq);
+            net[32 * j + lane] = make_float2(dn, sm::network_radius(prm, x0, y0));
+          }
+        }
+        // upper-bound keys, unique through the point's index in the low 9 bits (the bounds stay in net)
+        uint32_t key[kWarpTiles];
+#pragma unroll
+        for (int j = 0; j < kWarpTiles; ++j) {
+          key[j] = 0xFFFFFFFFu;
+          if (32 * j + own < n) {
+            const float2 v = net[32 * j + lane];
+            key[j] = tc::unique_key(orderable(v.x + v.y), 32 * j + own);
+          }
+        }
+        if (NB_WHATIF & 4) {
+          if (lane == 0) prm.cand_cnt[item] = (key[0] ^ key[kWarpTiles - 1]) == 12345u ? 1 : 0;
+          continue;
+        }
+        int32_t* out_idx = prm.cand_idx + (size_t)item * kCandMax;
+        float* out_dt = prm.cand_dt + (size_t)item * kCandMax;
+        if (n <= kCandMax) {  // calibration mode: all points (tile 0), with their screened distance
+          if (key[0] != 0xFFFFFFFFu) { out_idx[own] = own; out_dt[own] = net[lane].x; }
+          if (lane == 0) { prm.cand_cnt[item] = n; refine_push(par, item, n); }
+          continue;
+        }
+        // tau = the M-th smallest upper bound: each REDUX round finds the smallest key above the previous one (keys are unique and
+        // >= 0x200; n > kCandMax >= M: M finite keys exist)
+        uint32_t tau = 0u;
+#pragma unroll 1
+        for (int m = 0; m < M; ++m) {
+          uint32_t mine = 0xFFFFFFFFu;
+#pragma unroll
+          for (int j = 0; j < kWarpTiles; ++j) mine = min(mine, key[j] > tau ? key[j] : 0xFFFFFFFFu);
+          tau = __reduce_min_sync(0xffffffffu, mine);
+        }
+        // the candidates: lower bound <= tau
+        uint32_t takem = 0u;
+        int nc = 0;
+#pragma unroll
+        for (int j = 0; j < kWarpTiles; ++j) {
+          bool tk = false;
+          if (key[j] != 0xFFFFFFFFu) {
+            const float2 v = net[32 * j + lane];
+            tk = orderable(v.x - v.y) <= tau;
+          }
+          takem |= tk ? 1u << j : 0u;
+          nc += __popc(__ballot_sync(0xffffffffu, tk));
+        }
+        if (nc <= kCandMax) {
+          const uint32_t below = (1u << lane) - 1u;
+          int pos = 0;
+#pragma unroll
+          for (int j = 0; j < kWarpTiles; ++j) {
+            const bool tk = (takem >> j) & 1u;
+            const uint32_t bal = __ballot_sync(0xffffffffu, tk);
+            if (tk) {
+              const int p = pos + __popc(bal & below);
+              const float2 v = net[32 * j + lane];
+              const float lb = v.x - v.y;
+              out_idx[p] = 32 * j + own;
+              out_dt[p] = v.x;
+              prm.cand_rad[(size_t)item * kCandMax + p] = v.x - lb;
+            }
+            pos += __popc(bal);
+          }
+          if (lane == 0) {
+            prm.cand_cnt[item] = nc;
+            refine_push(par, item, nc);
+            atomicAdd(&stat_s[0], (unsigned)nc);
+            atomicAdd(&stat_s[1], 1u);
+          }
+        } else if (lane == 0) {
+          prm.cand_cnt[item] = -1;  // too many candidates: the exact kernel evaluates this item in full
+          atomicAdd(&prm.screen_stats[1], 1u);
+          prm.flag_list[atomicAdd(prm.flag_count, 1)] = item;
+        }
+      }
+    }
+  }
+  tc::cp_async_wait_all();
+  __syncthreads();
+  if (warp == W - 1) {
+    refine_flush(0);
+    refine_flush(1);
+  }
+  if (tid == 0 && stat_s[1]) {
+    atomicAdd(&prm.screen_stats[2], stat_s[0]);
+    atomicAdd(&prm.screen_stats[3], stat_s[1]);
+  }
 }
 
 }  // namespace nb

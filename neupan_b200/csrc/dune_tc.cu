@@ -147,11 +147,12 @@ int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const
     const size_t smem_r = TcImage::kBytes + 2 * (size_t)tc::kTileBytes;
     const int screen_mma = prm.screen_mma;
     cudaError_t e = cudaMemsetAsync(prm.flag_count, 0, 3 * sizeof(int32_t), st);
-    const size_t smem_m = dune_screen_mma_smem_bytes(prm.N, prm.M);
+    const bool warp_items = prm.N <= 32 * kWarpTiles;  // one warp per item, CTAs persistent over environments
+    const size_t smem_m = warp_items ? dune_screen_warp_smem_bytes(prm.N, prm.T) : dune_screen_mma_smem_bytes(prm.N, prm.M);
     int grid = 0;
     if (screen_mma && prm.N <= 1024 && (long long)smem_m <= max_smem_optin) {  // larger clouds: the warpgroup screen kernel (key arrays in shared memory)
-      auto go = [&](auto kern) {
-        if (e == cudaSuccess) e = resident_grid(kern, 128, smem_m, sm_count, items_, grid);
+      auto go = [&](auto kern, int threads, int work, auto... args) {
+        if (e == cudaSuccess) e = resident_grid(kern, threads, smem_m, sm_count, work, grid);
         if (e == cudaSuccess) {
           static int cap = -1;  // NB_SCREEN_CTA_CAP (developer switch): fewer CTAs per SM, to leave room for a kernel of another stream (NB_OPT_OVERLAP)
           if (cap < 0) {
@@ -159,12 +160,21 @@ int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const
             cap = v ? atoi(v) : 0;
           }
           if (cap > 0 && grid > sm_count * cap) grid = sm_count * cap;
-          kern<<<grid, 128, smem_m, st>>>(prm, d_screen_image);
+          kern<<<grid, threads, smem_m, st>>>(prm, d_screen_image, args...);
           e = cudaGetLastError();
         }
       };
-      if (prm.N <= 512) go(dune_screen_mma_kernel<4>);
-      else go(dune_screen_mma_kernel<8>);
+      if (warp_items) {
+        // one CTA per environment leaves SMs idle when the batch is smaller than the resident grid: split the items over more
+        int resident = 0;
+        if (e == cudaSuccess) e = resident_grid(dune_screen_warp_kernel, 32 * kScreenWarps, smem_m, sm_count, 1 << 30, resident);
+        const int groups = (prm.T + 1 + kScreenWarps - 1) / kScreenWarps;
+        int parts = resident / (prm.B > 0 ? prm.B : 1);
+        parts = parts < 1 ? 1 : (parts > groups ? groups : parts);
+        go(dune_screen_warp_kernel, 32 * kScreenWarps, prm.B * parts, parts);
+      } else {
+        go(dune_screen_mma_kernel, 128, items_);
+      }
     } else {
       if (e == cudaSuccess) e = resident_grid(dune_screen_kernel<0>, 128, smem_s, sm_count, items_, grid);
       if (e == cudaSuccess) {
