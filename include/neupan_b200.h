@@ -380,6 +380,29 @@ int nb_world_set_behaviors(nb_world_t* w, int32_t B, const double* behaviors, ui
  * enqueued on `stream` without synchronising.  NB_ERR_INVALID before nb_world_set_behaviors. */
 int nb_world_read_behaviors(nb_world_t* w, int32_t B, double* goals, int32_t* draws, void* stream);
 
+/* Several robots per environment (IR-SIM's robot: section as a list; this project's reading, stated in csrc/world_kernel.cuh):
+ *   robots (B*K,6) float64 HOST rows [start x, y, theta, goal x, y, goal_threshold], robot k of environment b at row n = b*K + k.
+ * Every robot has the handle's polygon, kinematics and lidar; 1 <= K <= 16.  nb_world_set_fleet (after nb_world_set_scenes(_ex))
+ * places the B*K robots at their starts and clears their flags; the env rows' start and goal are then unused; behaviours stay set.
+ * nb_world_set_scenes(_ex) returns the handle to one robot per environment.  With a fleet, nb_world_scan, nb_world_step and
+ * nb_world_read_state take N = B*K as their count and their per-robot arrays have N rows (ranges (N,R), velocity (N,2,R), hit (N,R),
+ * action (N,2), collided / arrived / clearance (N), states (N,3)); obstacle rows and nb_world_read_behaviors are unchanged.
+ *   scan    a beam also tests the bodies of the environment's other K-1 robots (the polygon at their current state), never its own;
+ *           robot j is hit index O_b + j (O_b: the environment's obstacle count), so at equal t an obstacle wins; its velocity is the
+ *           world-frame velocity of the action it integrated in the last step (diff / acker v (cos th, sin th) with the heading before
+ *           that step, omni (vx, vy)): 0 before the first step and once it has collided; translation only (omega x r is left out).
+ *   step    Jacobi: every robot that has not collided integrates its own action from the state at the start of the step, obstacles
+ *           move once per environment; a robot's clearance is the minimum over the obstacles and the other robots (convex-convex,
+ *           symmetric bit for bit, so two robots that touch collide in the same step).  collided (sticky) freezes a robot, which
+ *           stays in the scene with velocity 0; arrived is per robot and sticky.
+ *   rvo     reactive obstacles take every robot of their environment as a neighbour (rows after the obstacles, in robot order).
+ * Checks (NB_ERR_INVALID, naming the environment / robot): K in 1..16, finite rows, goal_threshold >= 0, no two start bodies of an
+ * environment that overlap or touch (SAT on the host).  nb_world_check_fleet performs them without a handle or a device.
+ * nb_world_set_fleet allocates the per-robot arrays once and synchronises the device; scan and step neither allocate nor synchronise.
+ * A fleet of K = 1 whose rows repeat the env rows gives exactly the world without a fleet. */
+int nb_world_check_fleet(const nb_world_config* cfg, int32_t B, int32_t K, const double* robots);
+int nb_world_set_fleet(nb_world_t* w, int32_t B, int32_t K, const double* robots);
+
 /* ---- DUNE training on the device (SURVEY 8f "next" row 4) ------------------------------------------------------------ */
 
 /* DUNETrain.generate_data_set / prob_solve (neupan/blocks/dune_train.py:100-140): labels of n sampled points -- the solution of the

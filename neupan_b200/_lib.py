@@ -108,6 +108,8 @@ SYMBOLS = {
     "nb_world_check_behaviors": (C.c_int, [C.POINTER(WorldConfig), C.c_int32] + [_FP] * 7 + [C.c_uint64]),
     "nb_world_set_behaviors": (C.c_int, [C.c_void_p, C.c_int32, _FP, C.c_uint64]),
     "nb_world_read_behaviors": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, C.c_void_p]),
+    "nb_world_check_fleet": (C.c_int, [C.POINTER(WorldConfig), C.c_int32, C.c_int32, _FP]),
+    "nb_world_set_fleet": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _FP]),
     "nb_dune_labels": (C.c_int, [C.c_int32, _FP, _FP, C.c_int64, _FP, _FP, _FP, _FP, C.c_void_p]),
     "nb_dune_train_create": (C.c_int, [C.c_int32, _FP, _FP, _FP, C.c_int64, C.c_int32, C.POINTER(C.c_void_p)]),
     "nb_dune_train_destroy": (C.c_int, [C.c_void_p]),

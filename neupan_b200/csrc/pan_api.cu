@@ -234,6 +234,58 @@ int world_check_behaviors(const nb_world_config* cfg, int32_t B, const int32_t* 
   return NB_OK;
 }
 
+// Convex polygons (x0, y0, x1, y1, ...) overlap or touch: no edge normal of either separates their projections strictly (the step
+// kernels' SAT, on the host).
+bool world_bodies_meet(const double* a, int na, const double* b, int nb_) {
+  for (int pass = 0; pass < 2; ++pass) {
+    const double* p = pass ? b : a;
+    const double* q = pass ? a : b;
+    const int np = pass ? nb_ : na, nq = pass ? na : nb_;
+    for (int k = 0; k < np; ++k) {
+      const int k1 = (k + 1) % np;
+      const double nx = -(p[2 * k1 + 1] - p[2 * k + 1]), ny = p[2 * k1] - p[2 * k];
+      double pmin = INFINITY, pmax = -INFINITY, qmin = INFINITY, qmax = -INFINITY;
+      for (int i = 0; i < np; ++i) { const double d = nx * p[2 * i] + ny * p[2 * i + 1]; pmin = std::min(pmin, d); pmax = std::max(pmax, d); }
+      for (int i = 0; i < nq; ++i) { const double d = nx * q[2 * i] + ny * q[2 * i + 1]; qmin = std::min(qmin, d); qmax = std::max(qmax, d); }
+      if (pmax < qmin || qmax < pmin) return false;
+    }
+  }
+  return true;
+}
+
+// Every check of nb_world_set_fleet on the host: K in 1..kWorldMaxFleet, finite rows, goal_threshold >= 0, and no two robots of an
+// environment whose bodies at their starts overlap or touch.
+int world_check_fleet(const nb_world_config* cfg, int32_t B, int32_t K, const double* robots) {
+  if (int rc = world_check_config(cfg)) return rc;
+  if (B < 1 || B > cfg->max_envs) return fail(NB_ERR_INVALID, "B = %d outside [1, max_envs = %d]", B, cfg->max_envs);
+  if (K < 1 || K > nb::kWorldMaxFleet) return fail(NB_ERR_INVALID, "K = %d robots per environment (1..%d)", K, nb::kWorldMaxFleet);
+  if (!robots) return fail(NB_ERR_INVALID, "nb_world fleet: null robots");
+  for (int b = 0; b < B; ++b)
+    for (int k = 0; k < K; ++k) {
+      const double* r = robots + 6 * ((size_t)b * K + k);
+      if (!world_finite(r, 6)) return fail(NB_ERR_INVALID, "environment %d, robot %d: non-finite value", b, k);
+      if (!(r[5] >= 0)) return fail(NB_ERR_INVALID, "environment %d, robot %d: goal_threshold must be >= 0", b, k);
+    }
+  const int nr = cfg->robot_num_vertices;
+  std::vector<double> body(2 * (size_t)K * nr);
+  for (int b = 0; b < B; ++b) {
+    for (int k = 0; k < K; ++k) {
+      const double* r = robots + 6 * ((size_t)b * K + k);
+      const double c = std::cos(r[2]), s = std::sin(r[2]);
+      for (int v = 0; v < nr; ++v) {
+        const double px = cfg->robot_vertices[2 * v], py = cfg->robot_vertices[2 * v + 1];
+        body[2 * ((size_t)k * nr + v)] = r[0] + (c * px - s * py);
+        body[2 * ((size_t)k * nr + v) + 1] = r[1] + (s * px + c * py);
+      }
+    }
+    for (int i = 0; i < K; ++i)
+      for (int j = i + 1; j < K; ++j)
+        if (world_bodies_meet(body.data() + 2 * (size_t)i * nr, nr, body.data() + 2 * (size_t)j * nr, nr))
+          return fail(NB_ERR_INVALID, "environment %d: the start bodies of robots %d and %d overlap", b, i, j);
+  }
+  return NB_OK;
+}
+
 }  // namespace
 
 struct nb_ipath {
@@ -270,6 +322,11 @@ struct nb_world {
   double robot_r = 0.0;
   double *d_beh = nullptr, *d_rad = nullptr, *d_goal = nullptr;
   int32_t* d_draws = nullptr;
+  int rvo_max_n = 0;  // the largest environment's obstacle count (rvo_cap = rvo_max_n + K)
+  // robots per environment (nb_world_set_fleet; nb_world_set_scenes makes it 1): the per-robot arrays above (states, collided,
+  // arrived) hold B K rows; a fleet also has every robot's goal and the velocity of its last step
+  int K = 1;
+  double *d_fgoal = nullptr, *d_fvel = nullptr;
 };
 
 struct nb_dune_train {
@@ -1420,6 +1477,42 @@ int nb_ipath_read_state(nb_ipath_t* p, int32_t B, int32_t* curve_index, int32_t*
   return NB_OK;
 }
 
+}  // extern "C"
+
+namespace {
+// scan launch shape: the largest environment's circles and edges (and with K > 1 the K robot bodies) in shared memory, one thread
+// per beam of the environment's K R beams (at most 256)
+int world_scan_shape(nb_world* w, int B) {
+  const int nre = w->K > 1 ? w->K * w->cfg.robot_num_vertices : 0;
+  w->scan_smem = (size_t)w->max_circ * (3 * sizeof(double) + sizeof(int32_t)) + (size_t)w->max_edges * (4 * sizeof(double) + sizeof(int32_t)) +
+                 (size_t)nre * (4 * sizeof(double) + sizeof(int32_t));
+  w->scan_threads = std::min(256, std::max(32, (w->K * w->cfg.num_beams + 31) / 32 * 32));
+  // the occupancy query sees the kernel's current limit; nb_world_scan sets it again before every launch
+  NB_CUDA(cudaFuncSetAttribute(nb::world_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
+  int per_sm = 0, sms = 0;
+  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_scan_kernel, w->scan_threads, w->scan_smem));
+  NB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->cfg.device));
+  if (per_sm < 1) return fail(NB_ERR_CUDA, "world_scan_kernel: %zu B of shared memory do not fit", w->scan_smem);
+  w->scan_grid = std::min(B, per_sm * sms);
+  return NB_OK;
+}
+
+// rvo launch shape: the largest environment's rows (+ the K robots) and one cone list per warp in shared memory
+int world_rvo_shape(nb_world* w, int B) {
+  w->rvo_cap = w->rvo_max_n + w->K;
+  w->rvo_smem = (size_t)w->rvo_cap * (5 * sizeof(double) + nb::kWorldRvoWarps * (6 * sizeof(double) + sizeof(int32_t)));
+  NB_CUDA(cudaFuncSetAttribute(nb::world_rvo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
+  int per_sm = 0, sms = 0;
+  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_rvo_kernel, 32 * nb::kWorldRvoWarps, w->rvo_smem));
+  NB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->cfg.device));
+  if (per_sm < 1) return fail(NB_ERR_CUDA, "world_rvo_kernel: %zu B of shared memory do not fit", w->rvo_smem);
+  w->rvo_grid = std::min(B, per_sm * sms);
+  return NB_OK;
+}
+}  // namespace
+
+extern "C" {
+
 // ---- batched 2-D world ----------------------------------------------------------------------------------------------------
 int nb_world_create(const nb_world_config* cfg, nb_world_t** out) {
   if (!out) return fail(NB_ERR_INVALID, "nb_world_create: null argument");
@@ -1455,7 +1548,7 @@ int nb_world_destroy(nb_world_t* w) {
   if (!w) return NB_OK;
   cudaSetDevice(w->cfg.device);
   void* bufs[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
-                  w->d_states, w->d_beam_cs, w->d_beh, w->d_rad, w->d_goal, w->d_draws};
+                  w->d_states, w->d_beam_cs, w->d_beh, w->d_rad, w->d_goal, w->d_draws, w->d_fgoal, w->d_fvel};
   for (void* b : bufs)
     if (b) cudaFree(b);
   delete w;
@@ -1485,12 +1578,13 @@ int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, c
     for (int k = 0; k < 3; ++k) states[3 * b + k] = envs[(size_t)nb::kWorldEnvCols * b + 4 + k];
   NB_CUDA(cudaSetDevice(w->cfg.device));
   void* old[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
-                 w->d_states, w->d_beh, w->d_rad, w->d_goal, w->d_draws};
+                 w->d_states, w->d_beh, w->d_rad, w->d_goal, w->d_draws, w->d_fgoal, w->d_fvel};
   for (void* b : old)
     if (b) cudaFree(b);
   w->d_obs_begin = w->d_vert_begin = w->d_slot = w->d_counts = w->d_kind = w->d_collided = w->d_arrived = w->d_draws = nullptr;
-  w->d_vertices = w->d_env = w->d_obs = w->d_states = w->d_beh = w->d_rad = w->d_goal = nullptr;
+  w->d_vertices = w->d_env = w->d_obs = w->d_states = w->d_beh = w->d_rad = w->d_goal = w->d_fgoal = w->d_fvel = nullptr;
   w->B = 0;
+  w->K = 1;  // new scenes: one robot per environment until nb_world_set_fleet
   w->has_rvo = false;  // new scenes: every obstacle keeps a constant velocity until nb_world_set_behaviors
   w->h_obs_begin.assign(obs_begin, obs_begin + B + 1);
   w->h_vert_begin.assign(vert_begin, vert_begin + O + 1);
@@ -1519,17 +1613,8 @@ int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, c
   NB_CUDA(cudaMemcpy(w->d_env, envs, sizeof(double) * nb::kWorldEnvCols * B, cudaMemcpyHostToDevice));
   if (O) NB_CUDA(cudaMemcpy(w->d_obs, obstacles, sizeof(double) * nb::kWorldObsCols * O, cudaMemcpyHostToDevice));
   NB_CUDA(cudaMemcpy(w->d_states, states.data(), sizeof(double) * 3 * B, cudaMemcpyHostToDevice));
-  // scan launch shape: the largest environment's circles and edges in shared memory, one thread per beam (at most 256)
   w->max_circ = max_circ; w->max_edges = max_edges;
-  w->scan_smem = (size_t)max_circ * (3 * sizeof(double) + sizeof(int32_t)) + (size_t)max_edges * (4 * sizeof(double) + sizeof(int32_t));
-  w->scan_threads = std::min(256, std::max(32, (w->cfg.num_beams + 31) / 32 * 32));
-  // the occupancy query sees the kernel's current limit; nb_world_scan sets it again before every launch
-  NB_CUDA(cudaFuncSetAttribute(nb::world_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
-  int per_sm = 0, sms = 0;
-  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_scan_kernel, w->scan_threads, w->scan_smem));
-  NB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->cfg.device));
-  if (per_sm < 1) return fail(NB_ERR_CUDA, "world_scan_kernel: %zu B of shared memory do not fit", w->scan_smem);
-  w->scan_grid = std::min(B, per_sm * sms);
+  if (int rc = world_scan_shape(w, B)) return rc;
   w->B = B; w->O = O; w->V = V;
   NB_CUDA(cudaDeviceSynchronize());
   return NB_OK;
@@ -1553,12 +1638,19 @@ nb::WorldParams world_params(const nb_world* w) {
   prm.obs_begin = w->d_obs_begin; prm.vert_begin = w->d_vert_begin; prm.slot = w->d_slot; prm.counts = w->d_counts; prm.kind = w->d_kind;
   prm.vertices = w->d_vertices; prm.env = w->d_env; prm.obs = w->d_obs; prm.states = w->d_states;
   prm.collided = w->d_collided; prm.arrived = w->d_arrived;
+  prm.K = w->K; prm.fgoal = w->d_fgoal; prm.fvel = w->d_fvel;
   return prm;
 }
 
-int world_ready(const nb_world* w, int32_t B, const char* what) {
+// per_robot: the count argument is N = B K with a fleet; otherwise (and for the obstacle-side calls) the environment count B
+int world_ready(const nb_world* w, int32_t B, const char* what, bool per_robot = false) {
   if (!w) return fail(NB_ERR_INVALID, "%s: null handle", what);
   if (!w->B) return fail(NB_ERR_INVALID, "%s: no scenes set (nb_world_set_scenes)", what);
+  if (per_robot && w->d_fgoal) {
+    if (B != w->B * w->K)
+      return fail(NB_ERR_INVALID, "%s: count = %d but the world has %d environments x %d robots (N = %d)", what, B, w->B, w->K, w->B * w->K);
+    return NB_OK;
+  }
   if (B != w->B) return fail(NB_ERR_INVALID, "%s: B = %d but the scenes were set for %d environments", what, B, w->B);
   return NB_OK;
 }
@@ -1638,16 +1730,9 @@ int nb_world_set_behaviors(nb_world_t* w, int32_t B, const double* behaviors, ui
     NB_CUDA(cudaMemcpy(w->d_goal, goal.data(), sizeof(double) * 2 * O, cudaMemcpyHostToDevice));
     NB_CUDA(cudaMemcpy(w->d_draws, draws.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice));
   }
-  // launch shape: the largest environment's rows (+ the robot) and one cone list per warp in shared memory
   w->seed = seed; w->robot_r = robot_r;
-  w->rvo_cap = max_n + 1;
-  w->rvo_smem = (size_t)w->rvo_cap * (5 * sizeof(double) + nb::kWorldRvoWarps * (6 * sizeof(double) + sizeof(int32_t)));
-  NB_CUDA(cudaFuncSetAttribute(nb::world_rvo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
-  int per_sm = 0, sms = 0;
-  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_rvo_kernel, 32 * nb::kWorldRvoWarps, w->rvo_smem));
-  NB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->cfg.device));
-  if (per_sm < 1) return fail(NB_ERR_CUDA, "world_rvo_kernel: %zu B of shared memory do not fit", w->rvo_smem);
-  w->rvo_grid = std::min(B, per_sm * sms);
+  w->rvo_max_n = max_n;
+  if (int rc = world_rvo_shape(w, B)) return rc;
   w->has_rvo = any;
   NB_CUDA(cudaDeviceSynchronize());
   return NB_OK;
@@ -1664,7 +1749,7 @@ int nb_world_read_behaviors(nb_world_t* w, int32_t B, double* goals, int32_t* dr
 }
 
 int nb_world_scan(nb_world_t* w, int32_t B, float* ranges, float* velocity, int32_t* hit, void* stream) {
-  if (int rc = world_ready(w, B, "nb_world_scan")) return rc;
+  if (int rc = world_ready(w, B, "nb_world_scan", true)) return rc;
   if (!ranges) return fail(NB_ERR_INVALID, "nb_world_scan: null ranges");
   NB_CUDA(cudaSetDevice(w->cfg.device));
   // the dynamic shared-memory limit is an attribute of the kernel, shared by every handle of the process: set this handle's
@@ -1678,7 +1763,7 @@ int nb_world_scan(nb_world_t* w, int32_t B, float* ranges, float* velocity, int3
 }
 
 int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collided, int32_t* arrived, float* clearance, void* stream) {
-  if (int rc = world_ready(w, B, "nb_world_step")) return rc;
+  if (int rc = world_ready(w, B, "nb_world_step", true)) return rc;
   if (!action) return fail(NB_ERR_INVALID, "nb_world_step: null action");
   NB_CUDA(cudaSetDevice(w->cfg.device));
   if (w->has_rvo) {  // reactive obstacles choose their velocities from the states at the start of the step
@@ -1687,21 +1772,67 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
     ++g_launches;
     NB_CUDA(cudaGetLastError());
   }
-  nb::world_step_kernel<<<(B + nb::kWorldStepWarps - 1) / nb::kWorldStepWarps, 32 * nb::kWorldStepWarps, 0, (cudaStream_t)stream>>>(
-      world_params(w), action, collided, arrived, clearance);
+  if (w->K > 1)  // several robots: one CTA of up to 8 warps per environment, a warp per robot
+    nb::world_fleet_step_kernel<<<w->B, 32 * std::min(w->K, nb::kWorldFleetWarps), 0, (cudaStream_t)stream>>>(world_params(w), action, collided,
+                                                                                                            arrived, clearance);
+  else
+    nb::world_step_kernel<<<(B + nb::kWorldStepWarps - 1) / nb::kWorldStepWarps, 32 * nb::kWorldStepWarps, 0, (cudaStream_t)stream>>>(
+        world_params(w), action, collided, arrived, clearance);
   ++g_launches;
   NB_CUDA(cudaGetLastError());
   return NB_OK;
 }
 
 int nb_world_read_state(nb_world_t* w, int32_t B, double* states, double* obstacles, int32_t* collided, int32_t* arrived, void* stream) {
-  if (int rc = world_ready(w, B, "nb_world_read_state")) return rc;
+  if (int rc = world_ready(w, B, "nb_world_read_state", true)) return rc;
   NB_CUDA(cudaSetDevice(w->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   if (states) NB_CUDA(cudaMemcpyAsync(states, w->d_states, sizeof(double) * 3 * B, cudaMemcpyDeviceToDevice, st));
   if (obstacles && w->O) NB_CUDA(cudaMemcpyAsync(obstacles, w->d_obs, sizeof(double) * nb::kWorldObsCols * w->O, cudaMemcpyDeviceToDevice, st));
   if (collided) NB_CUDA(cudaMemcpyAsync(collided, w->d_collided, sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
   if (arrived) NB_CUDA(cudaMemcpyAsync(arrived, w->d_arrived, sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
+  return NB_OK;
+}
+
+int nb_world_check_fleet(const nb_world_config* cfg, int32_t B, int32_t K, const double* robots) {
+  return world_check_fleet(cfg, B, K, robots);
+}
+
+int nb_world_set_fleet(nb_world_t* w, int32_t B, int32_t K, const double* robots) {
+  if (int rc = world_ready(w, B, "nb_world_set_fleet")) return rc;
+  if (int rc = world_check_fleet(&w->cfg, B, K, robots)) return rc;
+  const size_t N = (size_t)B * K;
+  std::vector<double> states(3 * N), goal(3 * N);
+  for (size_t n = 0; n < N; ++n)
+    for (int c = 0; c < 3; ++c) { states[3 * n + c] = robots[6 * n + c]; goal[3 * n + c] = robots[6 * n + 3 + c]; }
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  void* old[] = {w->d_states, w->d_collided, w->d_arrived, w->d_fgoal, w->d_fvel};
+  for (void* p : old)
+    if (p) cudaFree(p);
+  w->d_states = w->d_fgoal = w->d_fvel = nullptr;
+  w->d_collided = w->d_arrived = nullptr;
+  w->B = 0;  // unusable until the new arrays are in place
+  NB_CUDA(dalloc(&w->d_states, 3 * N));
+  NB_CUDA(dalloc(&w->d_collided, N));
+  NB_CUDA(dalloc(&w->d_arrived, N));
+  NB_CUDA(dalloc(&w->d_fgoal, 3 * N));
+  NB_CUDA(dalloc(&w->d_fvel, 2 * N));
+  NB_CUDA(cudaMemcpy(w->d_states, states.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_fgoal, goal.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemset(w->d_collided, 0, sizeof(int32_t) * N));
+  NB_CUDA(cudaMemset(w->d_arrived, 0, sizeof(int32_t) * N));
+  NB_CUDA(cudaMemset(w->d_fvel, 0, sizeof(double) * 2 * N));
+  if (K == 1) {  // world_step_kernel reads the goal from the env rows: the robot rows take the place of their start and goal columns
+    for (int b = 0; b < B; ++b)
+      for (int c = 0; c < 6; ++c) w->h_env[(size_t)nb::kWorldEnvCols * b + 4 + c] = robots[6 * (size_t)b + c];
+    NB_CUDA(cudaMemcpy(w->d_env, w->h_env.data(), sizeof(double) * nb::kWorldEnvCols * B, cudaMemcpyHostToDevice));
+  }
+  w->K = K;
+  if (int rc = world_scan_shape(w, B)) return rc;
+  if (w->d_beh)
+    if (int rc = world_rvo_shape(w, B)) return rc;
+  w->B = B;
+  NB_CUDA(cudaDeviceSynchronize());
   return NB_OK;
 }
 

@@ -6,10 +6,11 @@
 //                 the obstacle's counter-based SplitMix64 stream, below); without it the obstacle parks (velocity 0, still a
 //                 neighbour of the others).  The initial goal is the scene's, or draw 0.
 //   2. v_des      speed * (goal - c_i) / |goal - c_i|  (0 when the goal is the centre)
-//   3. neighbours every other obstacle of the environment and the robot whose centre lies within neighbor_range of c_i (distance
-//                 <= neighbor_range; a neighbour at the same centre is skipped), each a circle: a circle's radius, a polygon's or
-//                 outline's circumradius about its centre, the robot's circumradius about its state point.  The robot's velocity is
-//                 0 once collided, else that of this step's action in the world frame (diff / acker v (cos th, sin th), omni (vx, vy)).
+//   3. neighbours every other obstacle of the environment and each of its K robots whose centre lies within neighbor_range of c_i
+//                 (distance <= neighbor_range; a neighbour at the same centre is skipped), each a circle: a circle's radius, a
+//                 polygon's or outline's circumradius about its centre, a robot's circumradius about its state point.  A robot's
+//                 velocity is 0 once collided, else that of this step's action in the world frame (diff / acker v (cos th, sin th),
+//                 omni (vx, vy)).  The robots are the rows after the obstacles, in robot order.
 //   4. cones      apex (v_i + v_j) / 2 (RVO); R = r_i + r_j, D = |c_j - c_i|, D' = max(D, R); edges: the unit direction to j turned by
 //                 +-alpha with sin alpha = R / D', cos alpha = sqrt(D'^2 - R^2) / D' (IR-SIM's atan2 / asin / cos / sin construction
 //                 without trigonometry: equal in exact arithmetic, correctly rounded here).  w = v - apex is inside when
@@ -28,7 +29,7 @@
 // FP64 with explicit rounding (dmul / dadd / dsub of world_kernel.cuh, __ddiv_rn, __dsqrt_rn), so that tests/world_rvo_oracle.py
 // agrees bit for bit; the one difference is CUDA's sincos for the robot's velocity.
 //
-// Kernel: one CTA per environment (grid-stride).  Shared memory holds the environment's centres, velocities and radii (the robot
+// Kernel: one CTA per environment (grid-stride).  Shared memory holds the environment's centres, velocities and radii (the K robots
 // last); one warp per reactive obstacle builds its neighbours' cone list by ballot compaction, then the lanes take the candidates and
 // a warp reduction on (key, index) picks the winner; a ballot decides whether the penalty pass is needed.
 #pragma once
@@ -50,10 +51,10 @@ struct WorldRvoParams {
   const double* radius;  // (O) circle radius, or the polygon's circumradius about its centre
   double* goal;          // (O, 2)
   int32_t* draws;        // (O) goals drawn so far
-  const float* action;   // (B, 2) this step's action
+  const float* action;   // (B K, 2) this step's action
   uint64_t seed;
   double robot_r;        // circumradius of the robot polygon about its state point
-  int cap;               // shared rows per environment: the largest obstacle count + 1 (the robot)
+  int cap;               // shared rows per environment: the largest obstacle count + K (the robots)
 };
 
 // SplitMix64 (Steele, Lea and Flood 2014): output n of the generator seeded with s is mix(s + (n + 1) gamma), so any draw is
@@ -122,11 +123,12 @@ __global__ void __launch_bounds__(32 * kWorldRvoWarps) world_rvo_kernel(const Wo
       const double* row = prm.obs + (size_t)kWorldObsCols * (o0 + j);
       s_cx[j] = row[0]; s_cy[j] = row[1]; s_vx[j] = row[2]; s_vy[j] = row[3]; s_r[j] = rp.radius[o0 + j];
     }
-    if (threadIdx.x == 0) {  // the robot, row n: its state point and the velocity of this step's action (world_step_kernel's sincos)
-      const double th = prm.states[3 * b + 2];
+    for (int k = threadIdx.x; k < prm.K; k += blockDim.x) {  // robot k, row n + k: its state point and the velocity of this step's
+      const size_t r = (size_t)b * prm.K + k;               // action (the step kernels' sincos)
+      const double th = prm.states[3 * r + 2];
       double rvx = 0.0, rvy = 0.0;
-      if (prm.collided[b] == 0) {
-        const double a0 = (double)rp.action[2 * b], a1 = (double)rp.action[2 * b + 1];
+      if (prm.collided[r] == 0) {
+        const double a0 = (double)rp.action[2 * r], a1 = (double)rp.action[2 * r + 1];
         if (prm.kinematics == 2) {
           rvx = a0; rvy = a1;
         } else {
@@ -135,7 +137,7 @@ __global__ void __launch_bounds__(32 * kWorldRvoWarps) world_rvo_kernel(const Wo
           rvx = dmul(a0, cs); rvy = dmul(a0, sn);
         }
       }
-      s_cx[n] = prm.states[3 * b]; s_cy[n] = prm.states[3 * b + 1]; s_vx[n] = rvx; s_vy[n] = rvy; s_r[n] = rp.robot_r;
+      s_cx[n + k] = prm.states[3 * r]; s_cy[n + k] = prm.states[3 * r + 1]; s_vx[n + k] = rvx; s_vy[n + k] = rvy; s_r[n + k] = rp.robot_r;
     }
     __syncthreads();
     for (int i = wid; i < n; i += kWorldRvoWarps) {
@@ -165,11 +167,12 @@ __global__ void __launch_bounds__(32 * kWorldRvoWarps) world_rvo_kernel(const Wo
         if (dist > 0.0) { desx = __ddiv_rn(dmul(beh[5], dx), dist); desy = __ddiv_rn(dmul(beh[5], dy), dist); }
         // the neighbours' cones, compacted by ballot in neighbour order
         int m = 0;
-        for (int base = 0; base <= n; base += 32) {
+        const int rows = n + prm.K;
+        for (int base = 0; base < rows; base += 32) {
           const int j = base + lane;
           bool take = false;
           double px = 0.0, py = 0.0, D = 0.0;
-          if (j <= n && j != i) {
+          if (j < rows && j != i) {
             px = dsub(s_cx[j], cx); py = dsub(s_cy[j], cy);
             D = __dsqrt_rn(ddot(px, py, px, py));
             take = D > 0.0 && D <= beh[10];

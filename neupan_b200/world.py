@@ -18,6 +18,8 @@ A scene (one environment) is a dict with the sections of an ``env.yaml``:
     start           (x, y, theta) of the robot
     goal            (x, y); goal_threshold: the robot has arrived when it is closer than this to the goal
     path            optional (n, 4) rows [x, y, theta, gear]: an initial path for the planner (the scene builders add one)
+    robots          in place of start / goal / goal_threshold / path: a list of K (1..16) dicts with those four keys, the robots of
+                    the environment (every scene of a batch has the same K)
 
 An obstacle's "behavior" is {"name": "constant"} (the default) or {"name": "rvo", "vxmax", "vymax", ...} (keys and defaults in
 ``RVO_DEFAULTS``): a reactive obstacle that heads for a goal at ``speed`` and steers around the other obstacles and the robot with a
@@ -28,6 +30,16 @@ velocities of a step are chosen from the states at its start (IR-SIM updates its
 holonomic (IR-SIM turns its diff obstacles), every neighbour is a circle (a polygon's circumradius about its centre, the robot's about
 its state point), and the candidates are lo + k grid (np.arange can differ in the last bit).  Goals are drawn from counter-based
 SplitMix64 streams keyed by (seed, environment, obstacle index within it, draw number), so a run is reproducible from its seed.
+
+Several robots (``robots``, nb_world_set_fleet; this project's reading of an IR-SIM world whose ``robot:`` section is a list): all
+share the planner's robot polygon, kinematics and lidar.  Robot k of environment b is row n = b K + k of every per-robot tensor, so
+``states``, ``scan``, ``step`` and ``flags`` have N = B K rows and a ``PlannerBatch`` of N planners drives them.  A robot's lidar also
+sees the bodies of the other robots of its environment (never its own); a beam that hits robot j reports index O_b + j (after the
+O_b obstacles, so an obstacle wins a tie) and that robot's world-frame velocity from the action it integrated in the last step
+(translation only; 0 before the first step and once it has collided).  A step is Jacobi: every robot integrates from the state at
+the start of the step, then each robot's clearance is the minimum over the obstacles and the other robots (convex-convex, symmetric
+bit for bit, so two robots that touch collide in the same step).  A collided robot is frozen and stays in the scene with velocity 0;
+an arrived robot stays in the scene.  Reactive obstacles take every robot of their environment as a neighbour.
 
 There is no CPU implementation here: the CUDA library is the product (oracle/world.py restates it for the tests).
 """
@@ -42,6 +54,8 @@ import torch
 from . import _lib
 
 ENV_COLS = 10  # xmin, ymin, xmax, ymax, start x, y, theta, goal x, y, goal threshold
+ROBOT_COLS = 6  # start x, y, theta, goal x, y, goal threshold
+MAX_ROBOTS = 16
 BEH_COLS = 13  # kind, vxmax, vymax, acce, factor, speed, wander, goal x, y, goal threshold, neighbor range, grid, min speed
 # the keys of an "rvo" behaviour besides vxmax and vymax (required); speed None: min(vxmax, vymax); goal None: drawn
 RVO_DEFAULTS = dict(acce=1.0, factor=1.0, speed=None, wander=False, goal=None, goal_threshold=0.3, neighbor_range=10.0, grid=0.05,
@@ -84,7 +98,8 @@ def pack_scenes_ex(scenes):
                 rows.append((*ob["center"], *vel, ob["radius"]))
             kinds.append(1 if shape == "outline" else 0)
         obs_begin.append(len(rows))
-        envs.append((*sc["bounds"], *sc["start"], *sc["goal"], sc["goal_threshold"]))
+        first = sc["robots"][0] if "robots" in sc else sc  # a fleet's env row carries its first robot (unused once the fleet is set)
+        envs.append((*sc["bounds"], *first["start"], *first["goal"], first["goal_threshold"]))
     return (np.asarray(obs_begin, np.int32), np.ascontiguousarray(np.asarray(rows, np.float64).reshape(-1, 5)),
             np.asarray(vert_begin, np.int32), np.ascontiguousarray(np.vstack(verts) if verts else np.zeros((0, 2))),
             np.ascontiguousarray(np.asarray(envs, np.float64).reshape(-1, ENV_COLS)), np.asarray(kinds, np.int32))
@@ -98,6 +113,33 @@ def pack_scenes(scenes):
     if packed[5].any():
         raise ValueError("these scenes have outlines: use pack_scenes_ex (nb_world_set_scenes_ex)")
     return packed[:5]
+
+
+def fleet_size(scenes) -> int:
+    """K: the number of robots of every scene (1 for scenes without ``robots``); raises unless all scenes agree."""
+    ks = {len(sc["robots"]) if "robots" in sc else 1 for sc in scenes}
+    if len(ks) != 1:
+        raise ValueError(f"every scene of a batch needs the same number of robots (got {sorted(ks)})")
+    K = ks.pop()
+    if not 1 <= K <= MAX_ROBOTS:
+        raise ValueError(f"a scene has {K} robots (1..{MAX_ROBOTS})")
+    return K
+
+
+def pack_fleet(scenes) -> np.ndarray:
+    """Scenes -> the (B K, 6) float64 rows of nb_world_set_fleet [start x, y, theta, goal x, y, goal_threshold], robot k of
+    environment b at row b K + k (a scene without ``robots`` is one robot)."""
+    fleet_size(scenes)
+    rows = []
+    for sc in scenes:
+        for rb in (sc["robots"] if "robots" in sc else [sc]):
+            rows.append((*rb["start"], *rb["goal"], rb["goal_threshold"]))
+    return np.ascontiguousarray(np.asarray(rows, np.float64).reshape(-1, ROBOT_COLS))
+
+
+def scene_paths(scenes) -> list:
+    """The initial paths of every robot in row order (N = B K): the argument of PlannerBatch.set_initial_paths."""
+    return [rb["path"] for sc in scenes for rb in (sc["robots"] if "robots" in sc else [sc])]
 
 
 def pack_behaviors(scenes) -> np.ndarray:
@@ -130,8 +172,9 @@ def _host_ptrs(packed):
 
 
 class WorldBatch:
-    """B environments of one robot type and one lidar.  ``lidar``: angle_min, angle_max, range_min, range_max, number (R),
-    optional scan_offset.  ``scan`` / ``step`` enqueue on the current stream and never synchronise the host."""
+    """B environments of one robot type and one lidar, K robots each (``K``, set by the scenes; N = B K).  ``lidar``: angle_min,
+    angle_max, range_min, range_max, number (R), optional scan_offset.  ``scan`` / ``step`` enqueue on the current stream and never
+    synchronise the host."""
 
     def __init__(self, num_envs: int, robot, lidar: dict, step_time: float, device=None):
         if not torch.cuda.is_available():
@@ -145,6 +188,7 @@ class WorldBatch:
         self._handle = C.c_void_p()
         _lib.check(_lib.load().nb_world_create(C.byref(self.config), C.byref(self._handle)))
         self.O = 0
+        self.K, self.N = 1, self.B
 
     def close(self):
         if getattr(self, "_handle", None):
@@ -158,16 +202,25 @@ class WorldBatch:
 
     def set_scenes(self, scenes, seed: int = 0):
         """Uploads B scenes, puts every robot at its start and clears the flags (env.reset).  When an obstacle has a behaviour,
-        also sets the behaviours (nb_world_set_behaviors); ``seed`` keys the goal draws of reactive obstacles."""
+        also sets the behaviours (nb_world_set_behaviors); ``seed`` keys the goal draws of reactive obstacles.  Scenes with K > 1
+        ``robots`` also set the fleet (nb_world_set_fleet); K = 1 runs as the single-robot world."""
         if len(scenes) != self.B:
             raise ValueError(f"expected {self.B} scenes, got {len(scenes)}")
+        K = fleet_size(scenes)
         packed = pack_scenes_ex(scenes)
+        fleet = pack_fleet(scenes) if K > 1 else None
         beh = pack_behaviors(scenes) if any("behavior" in ob for sc in scenes for ob in sc["obstacles"]) else None
         with torch.cuda.device(self.device):
-            _lib.check(_lib.load().nb_world_set_scenes_ex(self._handle, self.B, *_host_ptrs(packed)))
-            self.O = int(packed[0][-1])
+            lib = _lib.load()
+            if fleet is not None:  # refuse before anything is uploaded
+                _lib.check(lib.nb_world_check_fleet(C.byref(self.config), self.B, K, C.c_void_p(fleet.ctypes.data)))
+            _lib.check(lib.nb_world_set_scenes_ex(self._handle, self.B, *_host_ptrs(packed)))
+            self.O, self.K, self.N = int(packed[0][-1]), 1, self.B
             if beh is not None:
-                _lib.check(_lib.load().nb_world_set_behaviors(self._handle, self.B, C.c_void_p(beh.ctypes.data), C.c_uint64(int(seed))))
+                _lib.check(lib.nb_world_set_behaviors(self._handle, self.B, C.c_void_p(beh.ctypes.data), C.c_uint64(int(seed))))
+            if fleet is not None:
+                _lib.check(lib.nb_world_set_fleet(self._handle, self.B, K, C.c_void_p(fleet.ctypes.data)))
+                self.K, self.N = K, self.B * K
 
     def goals(self):
         """(goals (O,2) float64, draws (O,) int32) on the device: every obstacle's current goal and the number of goals drawn for it
@@ -181,12 +234,12 @@ class WorldBatch:
     def _read(self, states=None, obstacles=None, collided=None, arrived=None):
         p = lambda t: C.c_void_p(0 if t is None else t.data_ptr())
         with torch.cuda.device(self.device):
-            _lib.check(_lib.load().nb_world_read_state(self._handle, self.B, p(states), p(obstacles), p(collided), p(arrived), self._stream()))
+            _lib.check(_lib.load().nb_world_read_state(self._handle, self.N, p(states), p(obstacles), p(collided), p(arrived), self._stream()))
 
     @property
     def states(self) -> torch.Tensor:
-        """(B,3) float64 [x, y, theta] on the device (env.get_robot_state for every robot): a copy, enqueued on the current stream."""
-        s = torch.empty((self.B, 3), dtype=torch.float64, device=self.device)
+        """(N,3) float64 [x, y, theta] on the device (env.get_robot_state for every robot): a copy, enqueued on the current stream."""
+        s = torch.empty((self.N, 3), dtype=torch.float64, device=self.device)
         self._read(states=s)
         return s
 
@@ -197,43 +250,45 @@ class WorldBatch:
         return o
 
     def flags(self):
-        """(collided, arrived) (B,) int32, sticky since set_scenes."""
-        c, a = (torch.empty(self.B, dtype=torch.int32, device=self.device) for _ in range(2))
+        """(collided, arrived) (N,) int32, sticky since set_scenes."""
+        c, a = (torch.empty(self.N, dtype=torch.int32, device=self.device) for _ in range(2))
         self._read(collided=c, arrived=a)
         return c, a
 
     def scan(self, hit: bool = False):
-        """env.get_lidar_scan() for every robot: (ranges (B,R) f32, velocity (B,2,R) f32, scan dict) -- the arguments of
+        """env.get_lidar_scan() for every robot: (ranges (N,R) f32, velocity (N,2,R) f32, scan dict) -- the arguments of
         PlannerBatch.forward(states, ranges, scan, scan_offset=world.scan_offset, scan_velocity=velocity).  With ``hit``, also the
-        index of the obstacle each beam hit within its environment, -1 on a miss (B,R) int32.  Passing ``velocity`` selects
+        index of the object each beam hit within its environment (obstacles, then robot j as O_b + j), -1 on a miss (N,R) int32.  Passing ``velocity`` selects
         scan_to_point_velocity, which applies the sensor offset inversely (neupan.py:271-273): with a non-zero ``scan_offset`` its
         points do not land on the obstacles (the reference's behaviour); without velocities, or at a zero offset, they do."""
-        ranges = torch.empty((self.B, self.R), dtype=torch.float32, device=self.device)
-        vel = torch.empty((self.B, 2, self.R), dtype=torch.float32, device=self.device)
-        hits = torch.empty((self.B, self.R), dtype=torch.int32, device=self.device) if hit else None
+        ranges = torch.empty((self.N, self.R), dtype=torch.float32, device=self.device)
+        vel = torch.empty((self.N, 2, self.R), dtype=torch.float32, device=self.device)
+        hits = torch.empty((self.N, self.R), dtype=torch.int32, device=self.device) if hit else None
         p = lambda t: C.c_void_p(0 if t is None else t.data_ptr())
         with torch.cuda.device(self.device):
-            _lib.check(_lib.load().nb_world_scan(self._handle, self.B, p(ranges), p(vel), p(hits), self._stream()))
+            _lib.check(_lib.load().nb_world_scan(self._handle, self.N, p(ranges), p(vel), p(hits), self._stream()))
         return (ranges, vel, dict(self.scan_dict), hits) if hit else (ranges, vel, dict(self.scan_dict))
 
     def step(self, action):
-        """env.step(action) + env.done(): action (B,2) [v, omega] (diff), [v, steering] (acker) or [vx, vy] (omni).
-        Returns (collided (B,) int32, arrived (B,) int32, clearance (B,) f32) on the device."""
-        action = torch.as_tensor(action).reshape(self.B, 2).to(device=self.device, dtype=torch.float32).contiguous()
-        col, arr = (torch.empty(self.B, dtype=torch.int32, device=self.device) for _ in range(2))
-        clear = torch.empty(self.B, dtype=torch.float32, device=self.device)
+        """env.step(action) + env.done(): action (N,2) [v, omega] (diff), [v, steering] (acker) or [vx, vy] (omni).
+        Returns (collided (N,) int32, arrived (N,) int32, clearance (N,) f32) on the device."""
+        action = torch.as_tensor(action).reshape(self.N, 2).to(device=self.device, dtype=torch.float32).contiguous()
+        col, arr = (torch.empty(self.N, dtype=torch.int32, device=self.device) for _ in range(2))
+        clear = torch.empty(self.N, dtype=torch.float32, device=self.device)
         p = lambda t: C.c_void_p(t.data_ptr())
         with torch.cuda.device(self.device):
-            _lib.check(_lib.load().nb_world_step(self._handle, self.B, p(action), p(col), p(arr), p(clear), self._stream()))
+            _lib.check(_lib.load().nb_world_step(self._handle, self.N, p(action), p(col), p(arr), p(clear), self._stream()))
         return col, arr, clear
 
 
-def rollout(planner, world: WorldBatch, steps: int, blind: bool = False):
-    """The loop of example/run_exp.py for B robots: scan -> planner.forward -> step, ``steps`` times, all on the device and without
-    a host synchronisation of its own.  ``blind``: the planner gets all-range_max scans (it sees nothing) -- the baseline that shows
-    what the scans are worth.  Returns per-environment collided, arrived (bool), steps_to_arrive (int32, -1 = not arrived) and
-    min_clearance (float32, the smallest clearance after any step)."""
-    B, dev = world.B, world.device
+def rollout(planner, world: WorldBatch, steps: int, blind: bool = False, velocities: bool = True):
+    """The loop of example/run_exp.py for the world's N robots: scan -> planner.forward -> step, ``steps`` times, all on the device
+    and without a host synchronisation of its own.  ``blind``: the planner gets all-range_max scans (it sees nothing) -- the
+    baseline that shows what the scans are worth.  ``velocities=False``: the planner gets the scans without their per-beam
+    velocities (scan_to_point instead of scan_to_point_velocity) -- what the point velocities are worth.  Returns per-robot
+    collided, arrived (bool), steps_to_arrive (int32, -1 = not arrived) and min_clearance (float32, the smallest clearance after
+    any step)."""
+    B, dev = world.N, world.device
     steps_to_arrive = torch.full((B,), -1, dtype=torch.int32, device=dev)
     min_clear = torch.full((B,), math.inf, dtype=torch.float32, device=dev)
     if blind:
@@ -242,7 +297,7 @@ def rollout(planner, world: WorldBatch, steps: int, blind: bool = False):
         blind_scan = dict(world.scan_dict)
     for k in range(steps):
         ranges, vel, scan = (blind_ranges, blind_vel, blind_scan) if blind else world.scan()
-        action, _ = planner.forward(world.states, ranges, scan, scan_offset=world.scan_offset, scan_velocity=vel)
+        action, _ = planner.forward(world.states, ranges, scan, scan_offset=world.scan_offset, scan_velocity=vel if velocities else None)
         _, arrived, clearance = world.step(action)
         steps_to_arrive = torch.where((arrived != 0) & (steps_to_arrive < 0), k + 1, steps_to_arrive)
         min_clear = torch.minimum(min_clear, clearance)
@@ -401,4 +456,34 @@ def non_obs(num_envs: int, seed: int = 0):
         obs = [dict(center=c, outline=_example_outline(rng, rng.uniform(0.5, 1.0), rng.uniform(0.9, 1.0))) for c in NON_OBS_CENTRES]
         scenes.append(dict(obstacles=obs, bounds=(-2.0, 5.0, 51.0, 47.0), start=start, goal=goal, goal_threshold=0.3,
                            path=line_path(start, goal)))
+    return scenes
+
+
+def circle_swap(num_envs: int, robots: int = 8, radius: float = 10.0, seed: int = 0, circles: int = 0):
+    """The standard multi-robot benchmark: ``robots`` robots evenly spaced on a circle of ``radius`` about (0, 0), each facing its
+    antipode, which is its goal (threshold 0.3), on a line path.  Per environment the circle turns by a random angle and every robot
+    gets a small jitter (0.1 m in position, 0.05 rad in heading) so that the configuration is not exactly symmetric.  ``circles``
+    static circles of radius 0.3..0.6 m stand within radius / 3 of the centre.  Rectangle [-(radius + 3), radius + 3]^2.  At the
+    default radius of 10 m, 16 robots of C4's 1.6 x 2.0 m body start about 1.9 m apart.  Seeded per environment (``_rng``)."""
+    K = int(robots)
+    if not 1 <= K <= MAX_ROBOTS:
+        raise ValueError(f"robots must be in 1..{MAX_ROBOTS} (got {K})")
+    ext = radius + 3.0
+    scenes = []
+    for b in range(num_envs):
+        rng = _rng(seed, b)
+        rot = rng.uniform(0.0, 2.0 * math.pi)
+        jit = rng.uniform(-1.0, 1.0, (K, 3)) * np.array([0.1, 0.1, 0.05])
+        fleet = []
+        for k in range(K):
+            a = rot + 2.0 * math.pi * k / K
+            sx, sy = radius * math.cos(a) + jit[k, 0], radius * math.sin(a) + jit[k, 1]
+            goal = (-radius * math.cos(a), -radius * math.sin(a))
+            start = (sx, sy, math.atan2(goal[1] - sy, goal[0] - sx) + jit[k, 2])
+            fleet.append(dict(start=start, goal=goal, goal_threshold=0.3, path=line_path(start, goal)))
+        obs = []
+        for _ in range(circles):
+            r, a = rng.uniform(0.0, radius / 3.0), rng.uniform(0.0, 2.0 * math.pi)
+            obs.append(dict(center=(r * math.cos(a), r * math.sin(a)), radius=rng.uniform(0.3, 0.6)))
+        scenes.append(dict(obstacles=obs, bounds=(-ext, -ext, ext, ext), robots=fleet))
     return scenes

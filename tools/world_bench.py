@@ -1,11 +1,12 @@
 """Times the batched world (csrc/world_kernel.cuh) against the planner it serves, on the device, and prints one JSON line.
 
-    python tools/world_bench.py [--scene dyna_obs|dyna_non_obs] [--behavior constant|rvo] [--envs 4096] [--beams 1080] [--steps 20]
-                                [--warmup 3]
+    python tools/world_bench.py [--scene dyna_obs|dyna_non_obs|circle_swap] [--behavior constant|rvo] [--envs 4096] [--robots 1]
+                                [--beams 1080] [--steps 20] [--warmup 3]
 
 Scenes: seeded dyna_obs (20 moving circles per environment, neupan_b200.world.dyna_obs; the default) or dyna_non_obs (11 moving
 obstacles after example/dyna_non_obs: squares, circles and non-convex outlines, neupan_b200.world.dyna_non_obs), with constant-velocity
-obstacles (the default) or the examples' reactive ones (--behavior rvo, csrc/world_rvo_kernel.cuh).  Planner:
+obstacles (the default) or the examples' reactive ones (--behavior rvo, csrc/world_rvo_kernel.cuh); or circle_swap, --robots K robots
+per environment swapping places on a circle (neupan_b200.world.circle_swap; --envs environments x K robots = N planners).  Planner:
 PlannerBatch with C4's robot, adjust values and K, the scans decimated to C4's N = 500 points.  Legs, each timed with CUDA events over --steps iterations after
 --warmup: the world alone (scan + step), the planner alone (PlannerBatch.forward repeated on the initial states and scans, after a
 reset) and the closed-loop step (scan -> PlannerBatch.forward -> step, from the initial scenes after a reset), whose world and planner
@@ -37,7 +38,8 @@ def _card():
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--scene", choices=("dyna_obs", "dyna_non_obs"), default="dyna_obs")
+    ap.add_argument("--scene", choices=("dyna_obs", "dyna_non_obs", "circle_swap"), default="dyna_obs")
+    ap.add_argument("--robots", type=int, default=1, help="robots per environment (circle_swap only)")
     ap.add_argument("--behavior", choices=("constant", "rvo"), default="constant")
     ap.add_argument("--envs", type=int, default=4096)
     ap.add_argument("--beams", type=int, default=1080)
@@ -51,24 +53,30 @@ def main():
 
     from helpers import CONFIGS, weights_path
     from neupan_b200 import PlannerBatch, WorldBatch
-    from neupan_b200.world import dyna_non_obs, dyna_obs, pack_scenes_ex
+    from neupan_b200.world import circle_swap, dyna_non_obs, dyna_obs, pack_scenes_ex, scene_paths
 
     if not torch.cuda.is_available():
         raise SystemExit("world_bench.py needs a CUDA device")
     B, R = args.envs, args.beams
     cfg = CONFIGS["C4"]
     lidar = dict(angle_min=-math.pi, angle_max=math.pi, range_min=0.0, range_max=10.0, number=R)
-    scenes = (dyna_obs if args.scene == "dyna_obs" else dyna_non_obs)(B, seed=2024, behavior=args.behavior)
+    if args.scene == "circle_swap":
+        scenes = circle_swap(B, robots=args.robots, seed=2024)
+    elif args.robots != 1:
+        raise SystemExit("--robots needs --scene circle_swap")
+    else:
+        scenes = (dyna_obs if args.scene == "dyna_obs" else dyna_non_obs)(B, seed=2024, behavior=args.behavior)
+    N = B * args.robots
     packed = pack_scenes_ex(scenes)
     n_obs, n_edges = int(packed[0][-1]), int(packed[2][-1])
     n_circles = int((packed[2][1:] == packed[2][:-1]).sum())
-    pl = PlannerBatch(B, cfg.T, cfg.dt, 4.0, robot_kwargs=cfg.robot_kwargs, adjust_kwargs=dict(cfg.adjust),
+    pl = PlannerBatch(N, cfg.T, cfg.dt, 4.0, robot_kwargs=cfg.robot_kwargs, adjust_kwargs=dict(cfg.adjust),
                       pan_kwargs=dict(iter_num=cfg.K, dune_max_num=cfg.N, nrmp_max_num=cfg.M, dune_checkpoint=weights_path(cfg.model),
                                       iter_threshold=0.0, max_points=cfg.N))
-    pl.set_initial_paths([sc["path"] for sc in scenes])
+    pl.set_initial_paths(scene_paths(scenes))
     world = WorldBatch(B, pl.robot, lidar, pl.dt)
     world.set_scenes(scenes)
-    zero = torch.zeros(B, 2, device="cuda")
+    zero = torch.zeros(N, 2, device="cuda")
     ranges0, vel0, scan0 = world.scan()
     states0 = world.states
 
@@ -124,8 +132,9 @@ def main():
             torch.cuda.synchronize()
         us = sum(getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) for e in prof.key_averages() if "world_rvo_kernel" in e.key)
         rvo = dict(ms_rvo_kernel=us * 1e-3 / args.steps, rvo_share_of_closed_loop=us * 1e-3 / args.steps / ms_loop)
-    tests = R * (n_circles + n_edges)  # ray-boundary tests of one scan: every beam against every circle and polygon edge
-    print(json.dumps(dict(metric="batched world: scan + step vs PlannerBatch.forward", scene=args.scene, behavior=args.behavior, envs=B, beams=R,
+    tests = args.robots * R * (n_circles + n_edges)  # ray-obstacle tests of one scan: every beam against every circle and polygon edge
+    print(json.dumps(dict(metric="batched world: scan + step vs PlannerBatch.forward", scene=args.scene, behavior=args.behavior, envs=B,
+                          robots_per_env=args.robots, planners=N, beams=R,
                           obstacles_per_env=n_obs / B, circles_per_env=n_circles / B, edges_per_env=n_edges / B,
                           steps=args.steps, warmup=args.warmup, ms_scan=ms_scan, ms_world_scan_step=ms_world, ms_planner_forward=ms_planner,
                           ms_closed_loop_step=ms_loop, ms_closed_loop_world=ms_loop_world, ms_closed_loop_planner=ms_loop_planner,
