@@ -323,8 +323,8 @@ struct nb_world {
   double *d_beh = nullptr, *d_rad = nullptr, *d_goal = nullptr;
   int32_t* d_draws = nullptr;
   int rvo_max_n = 0;  // the largest environment's obstacle count (rvo_cap = rvo_max_n + K)
-  // robots per environment (nb_world_set_fleet; nb_world_set_scenes makes it 1): the per-robot arrays above (states, collided,
-  // arrived) hold B K rows; a fleet also has every robot's goal and the velocity of its last step
+  // robots per environment (nb_world_set_fleet; nb_world_set_scenes makes it 1, from the env rows): the per-robot arrays
+  // (states, collided, arrived above, every robot's goal and the velocity of its last step) hold B K rows (world_set_robots)
   int K = 1;
   double *d_fgoal = nullptr, *d_fvel = nullptr;
 };
@@ -1509,6 +1509,32 @@ int world_rvo_shape(nb_world* w, int B) {
   w->rvo_grid = std::min(B, per_sm * sms);
   return NB_OK;
 }
+
+// (Re)allocates the per-robot arrays for B K robots and uploads the rows [start x, y, theta, goal x, y, threshold] (robot k of
+// environment b at row b K + k): every robot at its start, flags and velocities cleared.
+int world_set_robots(nb_world* w, int B, int K, const double* robots) {
+  const size_t N = (size_t)B * K;
+  std::vector<double> states(3 * N), goal(3 * N);
+  for (size_t n = 0; n < N; ++n)
+    for (int c = 0; c < 3; ++c) { states[3 * n + c] = robots[6 * n + c]; goal[3 * n + c] = robots[6 * n + 3 + c]; }
+  void* old[] = {w->d_states, w->d_collided, w->d_arrived, w->d_fgoal, w->d_fvel};
+  for (void* p : old)
+    if (p) cudaFree(p);
+  w->d_states = w->d_fgoal = w->d_fvel = nullptr;
+  w->d_collided = w->d_arrived = nullptr;
+  NB_CUDA(dalloc(&w->d_states, 3 * N));
+  NB_CUDA(dalloc(&w->d_collided, N));
+  NB_CUDA(dalloc(&w->d_arrived, N));
+  NB_CUDA(dalloc(&w->d_fgoal, 3 * N));
+  NB_CUDA(dalloc(&w->d_fvel, 2 * N));
+  NB_CUDA(cudaMemcpy(w->d_states, states.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_fgoal, goal.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemset(w->d_collided, 0, sizeof(int32_t) * N));
+  NB_CUDA(cudaMemset(w->d_arrived, 0, sizeof(int32_t) * N));
+  NB_CUDA(cudaMemset(w->d_fvel, 0, sizeof(double) * 2 * N));
+  w->K = K;
+  return NB_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -1573,18 +1599,17 @@ int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, c
   if (int rc = world_check_scenes(&w->cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, obs_kind, &slot, &counts, &max_circ, &max_edges))
     return rc;
   const int O = obs_begin[B], V = vert_begin[O];
-  std::vector<double> states(3 * (size_t)B);
+  std::vector<double> robots(6 * (size_t)B);  // one robot per environment until nb_world_set_fleet: the env rows' start and goal
   for (int b = 0; b < B; ++b)
-    for (int k = 0; k < 3; ++k) states[3 * b + k] = envs[(size_t)nb::kWorldEnvCols * b + 4 + k];
+    for (int c = 0; c < 6; ++c) robots[6 * (size_t)b + c] = envs[(size_t)nb::kWorldEnvCols * b + 4 + c];
   NB_CUDA(cudaSetDevice(w->cfg.device));
-  void* old[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
-                 w->d_states, w->d_beh, w->d_rad, w->d_goal, w->d_draws, w->d_fgoal, w->d_fvel};
+  void* old[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_vertices, w->d_env, w->d_obs,
+                 w->d_beh, w->d_rad, w->d_goal, w->d_draws};
   for (void* b : old)
     if (b) cudaFree(b);
-  w->d_obs_begin = w->d_vert_begin = w->d_slot = w->d_counts = w->d_kind = w->d_collided = w->d_arrived = w->d_draws = nullptr;
-  w->d_vertices = w->d_env = w->d_obs = w->d_states = w->d_beh = w->d_rad = w->d_goal = w->d_fgoal = w->d_fvel = nullptr;
+  w->d_obs_begin = w->d_vert_begin = w->d_slot = w->d_counts = w->d_kind = w->d_draws = nullptr;
+  w->d_vertices = w->d_env = w->d_obs = w->d_beh = w->d_rad = w->d_goal = nullptr;
   w->B = 0;
-  w->K = 1;  // new scenes: one robot per environment until nb_world_set_fleet
   w->has_rvo = false;  // new scenes: every obstacle keeps a constant velocity until nb_world_set_behaviors
   w->h_obs_begin.assign(obs_begin, obs_begin + B + 1);
   w->h_vert_begin.assign(vert_begin, vert_begin + O + 1);
@@ -1597,22 +1622,17 @@ int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, c
   NB_CUDA(dalloc(&w->d_kind, (size_t)O));
   if (O && obs_kind) NB_CUDA(cudaMemcpy(w->d_kind, obs_kind, sizeof(int32_t) * O, cudaMemcpyHostToDevice));
   else if (O) NB_CUDA(cudaMemset(w->d_kind, 0, sizeof(int32_t) * O));
-  NB_CUDA(dalloc(&w->d_collided, (size_t)B));
-  NB_CUDA(dalloc(&w->d_arrived, (size_t)B));
   NB_CUDA(dalloc(&w->d_vertices, 2 * (size_t)V));
   NB_CUDA(dalloc(&w->d_env, (size_t)nb::kWorldEnvCols * B));
   NB_CUDA(dalloc(&w->d_obs, (size_t)nb::kWorldObsCols * O));
-  NB_CUDA(dalloc(&w->d_states, 3 * (size_t)B));
   NB_CUDA(cudaMemcpy(w->d_obs_begin, obs_begin, sizeof(int32_t) * (B + 1), cudaMemcpyHostToDevice));
   NB_CUDA(cudaMemcpy(w->d_vert_begin, vert_begin, sizeof(int32_t) * (O + 1), cudaMemcpyHostToDevice));
   if (O) NB_CUDA(cudaMemcpy(w->d_slot, slot.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice));
   NB_CUDA(cudaMemcpy(w->d_counts, counts.data(), sizeof(int32_t) * 2 * B, cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemset(w->d_collided, 0, sizeof(int32_t) * B));
-  NB_CUDA(cudaMemset(w->d_arrived, 0, sizeof(int32_t) * B));
   if (V) NB_CUDA(cudaMemcpy(w->d_vertices, vertices, sizeof(double) * 2 * V, cudaMemcpyHostToDevice));
   NB_CUDA(cudaMemcpy(w->d_env, envs, sizeof(double) * nb::kWorldEnvCols * B, cudaMemcpyHostToDevice));
   if (O) NB_CUDA(cudaMemcpy(w->d_obs, obstacles, sizeof(double) * nb::kWorldObsCols * O, cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemcpy(w->d_states, states.data(), sizeof(double) * 3 * B, cudaMemcpyHostToDevice));
+  if (int rc = world_set_robots(w, B, 1, robots.data())) return rc;
   w->max_circ = max_circ; w->max_edges = max_edges;
   if (int rc = world_scan_shape(w, B)) return rc;
   w->B = B; w->O = O; w->V = V;
@@ -1642,11 +1662,12 @@ nb::WorldParams world_params(const nb_world* w) {
   return prm;
 }
 
-// per_robot: the count argument is N = B K with a fleet; otherwise (and for the obstacle-side calls) the environment count B
+// per_robot: the count argument is the robot count N = B K (B itself with one robot per environment); otherwise (the obstacle-side
+// calls) the environment count B
 int world_ready(const nb_world* w, int32_t B, const char* what, bool per_robot = false) {
   if (!w) return fail(NB_ERR_INVALID, "%s: null handle", what);
   if (!w->B) return fail(NB_ERR_INVALID, "%s: no scenes set (nb_world_set_scenes)", what);
-  if (per_robot && w->d_fgoal) {
+  if (per_robot && w->K > 1) {
     if (B != w->B * w->K)
       return fail(NB_ERR_INVALID, "%s: count = %d but the world has %d environments x %d robots (N = %d)", what, B, w->B, w->K, w->B * w->K);
     return NB_OK;
@@ -1772,12 +1793,10 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
     ++g_launches;
     NB_CUDA(cudaGetLastError());
   }
-  if (w->K > 1)  // several robots: one CTA of up to 8 warps per environment, a warp per robot
-    nb::world_fleet_step_kernel<<<w->B, 32 * std::min(w->K, nb::kWorldFleetWarps), 0, (cudaStream_t)stream>>>(world_params(w), action, collided,
-                                                                                                            arrived, clearance);
-  else
-    nb::world_step_kernel<<<(B + nb::kWorldStepWarps - 1) / nb::kWorldStepWarps, 32 * nb::kWorldStepWarps, 0, (cudaStream_t)stream>>>(
-        world_params(w), action, collided, arrived, clearance);
+  // a CTA of up to 8 warps per E environments, a warp per robot
+  const int E = nb::world_step_envs(w->K);
+  nb::world_step_kernel<<<(w->B + E - 1) / E, 32 * std::min(E * w->K, nb::kWorldStepMaxWarps), 0, (cudaStream_t)stream>>>(
+      world_params(w), action, collided, arrived, clearance);
   ++g_launches;
   NB_CUDA(cudaGetLastError());
   return NB_OK;
@@ -1801,33 +1820,9 @@ int nb_world_check_fleet(const nb_world_config* cfg, int32_t B, int32_t K, const
 int nb_world_set_fleet(nb_world_t* w, int32_t B, int32_t K, const double* robots) {
   if (int rc = world_ready(w, B, "nb_world_set_fleet")) return rc;
   if (int rc = world_check_fleet(&w->cfg, B, K, robots)) return rc;
-  const size_t N = (size_t)B * K;
-  std::vector<double> states(3 * N), goal(3 * N);
-  for (size_t n = 0; n < N; ++n)
-    for (int c = 0; c < 3; ++c) { states[3 * n + c] = robots[6 * n + c]; goal[3 * n + c] = robots[6 * n + 3 + c]; }
   NB_CUDA(cudaSetDevice(w->cfg.device));
-  void* old[] = {w->d_states, w->d_collided, w->d_arrived, w->d_fgoal, w->d_fvel};
-  for (void* p : old)
-    if (p) cudaFree(p);
-  w->d_states = w->d_fgoal = w->d_fvel = nullptr;
-  w->d_collided = w->d_arrived = nullptr;
   w->B = 0;  // unusable until the new arrays are in place
-  NB_CUDA(dalloc(&w->d_states, 3 * N));
-  NB_CUDA(dalloc(&w->d_collided, N));
-  NB_CUDA(dalloc(&w->d_arrived, N));
-  NB_CUDA(dalloc(&w->d_fgoal, 3 * N));
-  NB_CUDA(dalloc(&w->d_fvel, 2 * N));
-  NB_CUDA(cudaMemcpy(w->d_states, states.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemcpy(w->d_fgoal, goal.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemset(w->d_collided, 0, sizeof(int32_t) * N));
-  NB_CUDA(cudaMemset(w->d_arrived, 0, sizeof(int32_t) * N));
-  NB_CUDA(cudaMemset(w->d_fvel, 0, sizeof(double) * 2 * N));
-  if (K == 1) {  // world_step_kernel reads the goal from the env rows: the robot rows take the place of their start and goal columns
-    for (int b = 0; b < B; ++b)
-      for (int c = 0; c < 6; ++c) w->h_env[(size_t)nb::kWorldEnvCols * b + 4 + c] = robots[6 * (size_t)b + c];
-    NB_CUDA(cudaMemcpy(w->d_env, w->h_env.data(), sizeof(double) * nb::kWorldEnvCols * B, cudaMemcpyHostToDevice));
-  }
-  w->K = K;
+  if (int rc = world_set_robots(w, B, K, robots)) return rc;
   if (int rc = world_scan_shape(w, B)) return rc;
   if (w->d_beh)
     if (int rc = world_rvo_shape(w, B)) return rc;

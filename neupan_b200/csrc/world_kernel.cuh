@@ -4,19 +4,18 @@
 // Scene: per environment a ragged list of obstacles -- circles (centre, radius), convex polygons (3..8 vertices) and outlines (any
 // simple polygon of 3..16 vertices, convex or not; kind 1), vertices stored relative to the centre so that motion only moves the
 // centre -- each with a constant world-frame velocity, an axis-aligned rectangle in which moving obstacles bounce, and K robots
-// (1 <= K <= 16, nb_world_set_fleet; one without a fleet) of the planner's robot polygon, each with its goal.  Robot k of
-// environment b is row n = b K + k of every per-robot array.
+// (1 <= K <= 16: nb_world_set_fleet, or one per environment from the scenes' own start and goal) of the planner's robot polygon,
+// each with its goal.  Robot k of environment b is row n = b K + k of every per-robot array, whatever K is.
 //
-//   world_scan_kernel        one CTA per environment (grid-stride): the environment's circles and polygon edges (convex and outline
-//                            alike) and, with K > 1, the K robot bodies (edges tagged with their owner) are staged in shared memory in
-//                            world coordinates with each robot's sensor pose, then one thread per beam of the K R beams finds the first
-//                            boundary crossing with t > 0; a beam skips its own robot's edges
-//   world_step_kernel        K = 1: one warp per environment: obstacles move (reflecting at the rectangle), the robot integrates its
-//                            action unless it has collided, then the exact clearance robot polygon <-> every obstacle, reduced over the warp
-//   world_fleet_step_kernel  K > 1: one CTA per environment: the robots integrate (Jacobi: from the states at the start of the step),
-//                            their world vertices and velocities go to shared memory and the obstacles move; after a barrier one warp per
-//                            robot takes the clearance to every obstacle (world_step_kernel's branches) and to every other robot
-//                            (convex-convex, symmetric bit for bit), then a warp min
+//   world_scan_kernel  one CTA per environment (grid-stride): the environment's circles and polygon edges (convex and outline
+//                      alike) and, with K > 1, the K robot bodies (edges tagged with their owner) are staged in shared memory in
+//                      world coordinates with each robot's sensor pose, then one thread per beam of the K R beams finds the first
+//                      boundary crossing with t > 0; a beam skips its own robot's edges
+//   world_step_kernel  one CTA per floor(8 / K) environments (K <= 4) or per environment, at most 8 warps: the robots integrate
+//                      (Jacobi: from the states at the start of the step), their world vertices and velocities go to shared memory
+//                      and the obstacles move (reflecting at the rectangle); after a barrier one warp per robot takes the exact
+//                      clearance to every obstacle of its environment and to every other robot of it (convex-convex, symmetric bit
+//                      for bit), then a warp min
 //
 // Several robots (this project's reading of an IR-SIM world whose robot: section lists several robots): a beam also tests the bodies
 // of the other K - 1 robots (the robot polygon at their current state), never its own; a robot hit reports index O_b + j (O_b the
@@ -37,10 +36,13 @@ constexpr int kWorldMaxVertices = 8;     // per convex polygon (obstacles and th
 constexpr int kWorldMaxOutlineVertices = 16;
 constexpr int kWorldMaxEdges = 2048;     // polygon edges (convex and outline) per environment, staged in shared memory by the scan
 constexpr int kWorldObsCols = 5;         // obstacle row: cx, cy, vx, vy, radius (radius unused for polygons)
-constexpr int kWorldEnvCols = 10;        // env row: xmin, ymin, xmax, ymax, start x, y, theta, goal x, y, goal threshold
-constexpr int kWorldStepWarps = 4;
+constexpr int kWorldEnvCols = 10;        // env row: xmin, ymin, xmax, ymax, start x, y, theta, goal x, y, goal threshold (the
+                                         // kernels read the rectangle; the host takes the robot's start and goal from the rest)
 constexpr int kWorldMaxFleet = 16;       // robots per environment
-constexpr int kWorldFleetWarps = 8;      // world_fleet_step_kernel: at most 8 warps per CTA, warp w takes robots w, w + 8
+constexpr int kWorldStepMaxWarps = 8;    // world_step_kernel: at most 8 warps per CTA, warp w takes robots w, w + 8
+
+// world_step_kernel's environments per CTA: floor(8 / K) up to K = 4 (a CTA of at most 8 warps, one per robot), else 1
+__host__ __device__ constexpr int world_step_envs(int K) { return K <= 4 ? kWorldStepMaxWarps / K : 1; }
 
 struct WorldParams {
   int B, R, kinematics, robot_nv;
@@ -56,12 +58,12 @@ struct WorldParams {
   const double* vertices;                 // (V, 2) relative to the obstacle's centre
   const double* env;                      // (B, kWorldEnvCols)
   double* obs;                            // (O, kWorldObsCols) -- centres and velocities change
-  double* states;                         // (B, 3) x, y, theta
-  int32_t* collided;                      // (B) sticky
-  int32_t* arrived;                       // (B) sticky
-  int K;                                  // robots per environment: states (B K, 3), collided and arrived (B K)
-  const double* fgoal;                    // (B K, 3) goal x, y, threshold of every robot (K > 1)
-  double* fvel;                           // (B K, 2) world-frame velocity of each robot's last step (K > 1)
+  int K;                                  // robots per environment
+  double* states;                         // (B K, 3) x, y, theta
+  int32_t* collided;                      // (B K) sticky
+  int32_t* arrived;                       // (B K) sticky
+  const double* fgoal;                    // (B K, 3) goal x, y, threshold of every robot
+  double* fvel;                           // (B K, 2) world-frame velocity of each robot's last step
 };
 
 __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
@@ -321,19 +323,25 @@ __device__ __forceinline__ double world_outline_clearance(const WorldPoly& op, c
 
 // ---- step ----------------------------------------------------------------------------------------------------------------
 
-// One step of the motion models from (x, y, th); (vx, vy) is the world-frame translation rate it used (diff / acker v (cos th, sin th)
-// with the heading before the step, omni (vx, vy)).
-__device__ __forceinline__ void world_integrate(const WorldParams& prm, double a0, double a1, double& x, double& y, double& th, double& vx,
-                                                double& vy) {
-  double dth;
-  if (prm.kinematics == 2) {  // omni: the (vx, vy) PlannerBatch returns
-    vx = a0; vy = a1; dth = 0.0;
+// World-frame translation rate of a robot's action at heading th: diff / acker v (cos th, sin th), omni the (vx, vy) PlannerBatch
+// returns.
+__device__ __forceinline__ void world_robot_velocity(int kinematics, double a0, double a1, double th, double& vx, double& vy) {
+  if (kinematics == 2) {
+    vx = a0; vy = a1;
   } else {
     double sn, cs;
     sincos(th, &sn, &cs);
     vx = dmul(a0, cs); vy = dmul(a0, sn);
-    dth = prm.kinematics == 1 ? dmul(a0, tan(a1)) / prm.L : a1;  // acker: v tan(phi) / L; diff: omega
   }
+}
+
+// One step of the motion models from (x, y, th); (vx, vy) is the world-frame translation rate it used (world_robot_velocity, with
+// the heading before the step).
+__device__ __forceinline__ void world_integrate(const WorldParams& prm, double a0, double a1, double& x, double& y, double& th, double& vx,
+                                                double& vy) {
+  world_robot_velocity(prm.kinematics, a0, a1, th, vx, vy);
+  // omni: no turn; acker: v tan(phi) / L; diff: omega
+  const double dth = prm.kinematics == 2 ? 0.0 : (prm.kinematics == 1 ? dmul(a0, tan(a1)) / prm.L : a1);
   x = dadd(x, dmul(vx, prm.dt)); y = dadd(y, dmul(vy, prm.dt)); th = dadd(th, dmul(dth, prm.dt));
 }
 
@@ -405,123 +413,75 @@ __device__ __forceinline__ double world_robot_clearance(const WorldRobot& a, con
   return d;
 }
 
-__global__ void __launch_bounds__(32 * kWorldStepWarps) world_step_kernel(const WorldParams prm, const float* __restrict__ action,
-                                                                         int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived,
-                                                                         float* __restrict__ clearance) {
-  __shared__ double rob[kWorldStepWarps][2][kWorldMaxVertices];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int b = blockIdx.x * kWorldStepWarps + w;
-  if (b >= prm.B) return;  // whole warps leave together
-  double* rx = rob[w][0];
-  double* ry = rob[w][1];
-  const double* env = prm.env + (size_t)kWorldEnvCols * b;
-  // robot: every lane integrates the same state (no shuffles needed later); a collided robot stays where it is
-  double x = prm.states[3 * b], y = prm.states[3 * b + 1], th = prm.states[3 * b + 2];
-  const bool was_collided = prm.collided[b] != 0;
-  if (!was_collided) {
-    double vx, vy;
-    world_integrate(prm, (double)action[2 * b], (double)action[2 * b + 1], x, y, th, vx, vy);
-  }
-  // everything that needs the robot's state is done before the obstacle loop, which keeps few values live across its divisions
-  const double gx = dsub(x, env[7]), gy = dsub(y, env[8]);
-  const int arr = (prm.arrived[b] != 0 || sqrt(ddot(gx, gy, gx, gy)) < env[9]) ? 1 : 0;
-  {
-    double sn, cs;
-    sincos(th, &sn, &cs);
-    double px = 0.0, py = 0.0;
-#pragma unroll
-    for (int k = 0; k < kWorldMaxVertices; ++k)  // constant indices: a kernel-parameter array indexed by lane would go to local memory
-      if (lane == k) { px = prm.robot_v[2 * k]; py = prm.robot_v[2 * k + 1]; }
-    if (lane < prm.robot_nv) {
-      rx[lane] = dadd(x, dsub(dmul(cs, px), dmul(sn, py)));
-      ry[lane] = dadd(y, dadd(dmul(sn, px), dmul(cs, py)));
-    }
-  }
-  __syncwarp();  // the robot's vertices are published, and every lane has read the old state before lane 0 overwrites it
-  if (lane == 0) { prm.states[3 * b] = x; prm.states[3 * b + 1] = y; prm.states[3 * b + 2] = th; }
-  const int nr = prm.robot_nv;
-  double best = INFINITY;
-  for (int o = prm.obs_begin[b] + lane; o < prm.obs_begin[b + 1]; o += 32) {
-    double cx, cy;
-    world_move_obstacle(prm, env, o, cx, cy);
-    const double c = world_obstacle_clearance(prm, o, cx, cy, rx, ry, nr);
-    best = fmin(best, c > 0.0 ? c : 0.0);
-  }
-#pragma unroll
-  for (int m = 16; m >= 1; m >>= 1) best = fmin(best, __shfl_xor_sync(0xffffffffu, best, m));
-  if (lane == 0) {
-    const int col = (was_collided || best <= 0.0) ? 1 : 0;
-    prm.collided[b] = col; prm.arrived[b] = arr;
-    if (out_collided) out_collided[b] = col;
-    if (out_arrived) out_arrived[b] = arr;
-    if (clearance) clearance[b] = (float)best;
-  }
-}
-
-// K > 1 robots per environment, one CTA of 32 min(K, 8) threads per environment (grid = B).  Phase 1: thread k integrates robot k
-// from the state at the start of the step (unless it has collided), writes its state, arrival flag, world vertices and velocity; every
-// thread moves obstacles.  Phase 2, after the barrier: one warp per robot (warp w takes robots w, w + 8; a 512-thread CTA would cap
-// the registers at 128 and spill) computes its clearance to every obstacle (lanes over the obstacles, the branches of
-// world_step_kernel) and to every other robot (lane j), a warp min, and lane 0 writes the collision flag, the clearance and the
-// velocity the scan reports for the robot (0 once collided).
-__global__ void __launch_bounds__(32 * kWorldFleetWarps) world_fleet_step_kernel(const WorldParams prm, const float* __restrict__ action,
-                                                                              int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived,
-                                                                              float* __restrict__ clearance) {
-  __shared__ double f_x[kWorldMaxFleet][kWorldMaxVertices], f_y[kWorldMaxFleet][kWorldMaxVertices];
+// One CTA per E = world_step_envs(K) environments, 32 min(E K, 8) threads (grid = ceil(B / E)); its robots are the slots
+// s = n - b0 K of the rows n of its environments b0 .. b0 + E - 1.  Phase 1: thread s integrates robot s from the state at the start
+// of the step (unless it has collided), writes its state, arrival flag, world vertices and velocity; every thread moves obstacles.
+// Phase 2, after the barrier: one warp per robot (warp w takes slots w, w + 8; a 512-thread CTA would cap the registers at 128 and
+// spill) computes its clearance to every obstacle of its environment (lanes over the obstacles: the circle, convex and outline
+// branches of world_obstacle_clearance) and to every other robot of it (lane j), a warp min, and lane 0 writes the collision flag,
+// the clearance and the velocity the scan reports for the robot (0 once collided).
+__global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(const WorldParams prm, const float* __restrict__ action,
+                                                                           int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived,
+                                                                           float* __restrict__ clearance) {
+  __shared__ double f_x[kWorldMaxFleet][kWorldMaxVertices], f_y[kWorldMaxFleet][kWorldMaxVertices];  // E K <= 8 or K <= 16 slots
   __shared__ double f_v[kWorldMaxFleet][2];
   const int K = prm.K, nr = prm.robot_nv, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  const int b = blockIdx.x;  // grid = B
+  const int b0 = blockIdx.x * world_step_envs(K);
+  const int nslot = min(world_step_envs(K), prm.B - b0) * K;  // this CTA's robots
+  const size_t n0 = (size_t)b0 * K;
+  for (int s = threadIdx.x; s < nslot; s += blockDim.x) {
+    const size_t n = n0 + s;
+    double x = prm.states[3 * n], y = prm.states[3 * n + 1], th = prm.states[3 * n + 2];
+    double vx = 0.0, vy = 0.0;
+    if (prm.collided[n] == 0) world_integrate(prm, (double)action[2 * n], (double)action[2 * n + 1], x, y, th, vx, vy);
+    prm.states[3 * n] = x; prm.states[3 * n + 1] = y; prm.states[3 * n + 2] = th;
+    const double* g = prm.fgoal + 3 * n;
+    const double gx = dsub(x, g[0]), gy = dsub(y, g[1]);
+    const int arr = (prm.arrived[n] != 0 || sqrt(ddot(gx, gy, gx, gy)) < g[2]) ? 1 : 0;
+    prm.arrived[n] = arr;
+    if (out_arrived) out_arrived[n] = arr;
+    double sn, cs;
+    sincos(th, &sn, &cs);
+#pragma unroll
+    for (int v = 0; v < kWorldMaxVertices; ++v) {  // constant indices into the parameter array
+      const double px = prm.robot_v[2 * v], py = prm.robot_v[2 * v + 1];
+      f_x[s][v] = dadd(x, dsub(dmul(cs, px), dmul(sn, py)));
+      f_y[s][v] = dadd(y, dadd(dmul(sn, px), dmul(cs, py)));
+    }
+    f_v[s][0] = vx; f_v[s][1] = vy;
+  }
   {
-    const double* env = prm.env + (size_t)kWorldEnvCols * b;
-    const int o0 = prm.obs_begin[b], o1 = prm.obs_begin[b + 1];
-    for (int k = threadIdx.x; k < K; k += blockDim.x) {
-      const size_t n = (size_t)b * K + k;
-      double x = prm.states[3 * n], y = prm.states[3 * n + 1], th = prm.states[3 * n + 2];
-      double vx = 0.0, vy = 0.0;
-      if (prm.collided[n] == 0) world_integrate(prm, (double)action[2 * n], (double)action[2 * n + 1], x, y, th, vx, vy);
-      prm.states[3 * n] = x; prm.states[3 * n + 1] = y; prm.states[3 * n + 2] = th;
-      const double* g = prm.fgoal + 3 * n;
-      const double gx = dsub(x, g[0]), gy = dsub(y, g[1]);
-      const int arr = (prm.arrived[n] != 0 || sqrt(ddot(gx, gy, gx, gy)) < g[2]) ? 1 : 0;
-      prm.arrived[n] = arr;
-      if (out_arrived) out_arrived[n] = arr;
-      double sn, cs;
-      sincos(th, &sn, &cs);
-#pragma unroll
-      for (int v = 0; v < kWorldMaxVertices; ++v) {  // constant indices into the parameter array
-        const double px = prm.robot_v[2 * v], py = prm.robot_v[2 * v + 1];
-        f_x[k][v] = dadd(x, dsub(dmul(cs, px), dmul(sn, py)));
-        f_y[k][v] = dadd(y, dadd(dmul(sn, px), dmul(cs, py)));
-      }
-      f_v[k][0] = vx; f_v[k][1] = vy;
-    }
-    for (int o = o0 + (int)threadIdx.x; o < o1; o += blockDim.x) {
+    int b = b0;  // the environment of obstacle o: the CTA's obstacle rows are its environments' back to back
+    for (int o = prm.obs_begin[b0] + (int)threadIdx.x; o < prm.obs_begin[b0 + nslot / K]; o += blockDim.x) {
+      while (o >= prm.obs_begin[b + 1]) ++b;
       double cx, cy;
-      world_move_obstacle(prm, env, o, cx, cy);
+      world_move_obstacle(prm, prm.env + (size_t)kWorldEnvCols * b, o, cx, cy);
     }
-    __syncthreads();  // bodies, velocities and the moved obstacle rows are visible to the whole CTA
-    for (int w = threadIdx.x >> 5; w < K; w += nw) {  // warp-uniform
-      const size_t n = (size_t)b * K + w;
-      double best = INFINITY;
-      for (int o = o0 + lane; o < o1; o += 32) {
-        const double* row = prm.obs + (size_t)kWorldObsCols * o;
-        const double c = world_obstacle_clearance(prm, o, row[0], row[1], f_x[w], f_y[w], nr);
-        best = fmin(best, c > 0.0 ? c : 0.0);
-      }
-      if (lane < K && lane != w) {
-        const double c = world_robot_clearance(WorldRobot{f_x[w], f_y[w], nr}, WorldRobot{f_x[lane], f_y[lane], nr});
-        best = fmin(best, c > 0.0 ? c : 0.0);
-      }
+  }
+  __syncthreads();  // bodies, velocities and the moved obstacle rows are visible to the whole CTA
+  for (int s = threadIdx.x >> 5; s < nslot; s += nw) {  // warp-uniform
+    const int k = s % K, s0 = s - k;  // robot k of the environment whose robots are the slots s0 .. s0 + K - 1
+    const int b = b0 + s / K;
+    const size_t n = n0 + s;
+    double best = INFINITY;
+    for (int o = prm.obs_begin[b] + lane; o < prm.obs_begin[b + 1]; o += 32) {
+      const double* row = prm.obs + (size_t)kWorldObsCols * o;
+      const double c = world_obstacle_clearance(prm, o, row[0], row[1], f_x[s], f_y[s], nr);
+      best = fmin(best, c > 0.0 ? c : 0.0);
+    }
+    if (lane < K && lane != k) {
+      const double c = world_robot_clearance(WorldRobot{f_x[s], f_y[s], nr}, WorldRobot{f_x[s0 + lane], f_y[s0 + lane], nr});
+      best = fmin(best, c > 0.0 ? c : 0.0);
+    }
 #pragma unroll
-      for (int m = 16; m >= 1; m >>= 1) best = fmin(best, __shfl_xor_sync(0xffffffffu, best, m));
-      if (lane == 0) {
-        const int col = (prm.collided[n] != 0 || best <= 0.0) ? 1 : 0;
-        prm.collided[n] = col;
-        prm.fvel[2 * n] = col ? 0.0 : f_v[w][0];
-        prm.fvel[2 * n + 1] = col ? 0.0 : f_v[w][1];
-        if (out_collided) out_collided[n] = col;
-        if (clearance) clearance[n] = (float)best;
-      }
+    for (int m = 16; m >= 1; m >>= 1) best = fmin(best, __shfl_xor_sync(0xffffffffu, best, m));
+    if (lane == 0) {
+      const int col = (prm.collided[n] != 0 || best <= 0.0) ? 1 : 0;
+      prm.collided[n] = col;
+      prm.fvel[2 * n] = col ? 0.0 : f_v[s][0];
+      prm.fvel[2 * n + 1] = col ? 0.0 : f_v[s][1];
+      if (out_collided) out_collided[n] = col;
+      if (clearance) clearance[n] = (float)best;
     }
   }
 }

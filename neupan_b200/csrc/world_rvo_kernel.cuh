@@ -26,8 +26,8 @@
 // objects one after another), obstacles are holonomic (IR-SIM turns its diff obstacles towards the chosen velocity), every neighbour
 // is a circle, and the candidate values are lo + k grid (np.arange can differ in the last bit).
 //
-// FP64 with explicit rounding (dmul / dadd / dsub of world_kernel.cuh, __ddiv_rn, __dsqrt_rn), so that tests/world_rvo_oracle.py
-// agrees bit for bit; the one difference is CUDA's sincos for the robot's velocity.
+// FP64 with explicit rounding (dmul / dadd / dsub of world_kernel.cuh, __ddiv_rn, __dsqrt_rn), so that oracle/world.py agrees bit
+// for bit; the one difference is CUDA's sincos for the robots' velocities.
 //
 // Kernel: one CTA per environment (grid-stride).  Shared memory holds the environment's centres, velocities and radii (the K robots
 // last); one warp per reactive obstacle builds its neighbours' cone list by ballot compaction, then the lanes take the candidates and
@@ -124,19 +124,10 @@ __global__ void __launch_bounds__(32 * kWorldRvoWarps) world_rvo_kernel(const Wo
       s_cx[j] = row[0]; s_cy[j] = row[1]; s_vx[j] = row[2]; s_vy[j] = row[3]; s_r[j] = rp.radius[o0 + j];
     }
     for (int k = threadIdx.x; k < prm.K; k += blockDim.x) {  // robot k, row n + k: its state point and the velocity of this step's
-      const size_t r = (size_t)b * prm.K + k;               // action (the step kernels' sincos)
+      const size_t r = (size_t)b * prm.K + k;               // action, as world_integrate computes it
       const double th = prm.states[3 * r + 2];
       double rvx = 0.0, rvy = 0.0;
-      if (prm.collided[r] == 0) {
-        const double a0 = (double)rp.action[2 * r], a1 = (double)rp.action[2 * r + 1];
-        if (prm.kinematics == 2) {
-          rvx = a0; rvy = a1;
-        } else {
-          double sn, cs;
-          sincos(th, &sn, &cs);
-          rvx = dmul(a0, cs); rvy = dmul(a0, sn);
-        }
-      }
+      if (prm.collided[r] == 0) world_robot_velocity(prm.kinematics, (double)rp.action[2 * r], (double)rp.action[2 * r + 1], th, rvx, rvy);
       s_cx[n + k] = prm.states[3 * r]; s_cy[n + k] = prm.states[3 * r + 1]; s_vx[n + k] = rvx; s_vy[n + k] = rvy; s_r[n + k] = rp.robot_r;
     }
     __syncthreads();

@@ -1,5 +1,5 @@
 """Several robots per environment in the batched world on the GPU: a fleet of one against the single-robot world (bitwise, and the
-same launches), teacher-forced parity of the scan, the fleet step and the reactive obstacles against tests/world_fleet_oracle.py,
+same launches), teacher-forced parity of the scan, the fleet step and the reactive obstacles against oracle/world.py,
 edge cases, and closed-loop circle_swap runs of 1024 planners with and without point velocities."""
 import ctypes as C
 import math
@@ -17,7 +17,7 @@ from oracle import world as ow
 from test_gpu_world import EXAMPLE_LIDAR, LIDAR, _mixed_scenes, _oracle_cfg, _polygon, _ulps
 from test_gpu_world_outline import _StillPlanner
 from test_gpu_world_rvo import ROBOT_KW, _behavior, _rvo_scenes
-from world_fleet_oracle import OracleWorld, clearance_robot_pairs
+from oracle.world import OracleWorld, clearance_robot_pairs
 
 pytestmark = pytest.mark.gpu
 
@@ -137,7 +137,7 @@ def test_teacher_forced_fleet_matches_the_oracle(kin, K):
     w = WorldBatch(B, rb, lidar, 0.1)
     w.set_scenes(scenes, seed=13)
     assert (w.K, w.N) == (K, B * K)
-    o = OracleWorld(_oracle_cfg(rb, lidar), packed, fleet, K, beh, seed=13)
+    o = OracleWorld(_oracle_cfg(rb, lidar), packed, beh, seed=13, fleet=fleet, K=K)
     rng = np.random.default_rng(17)
     robot_hits = robot_collisions = excused_beams = excused_obs = worst_state = ulp1 = 0
     wrong = []
@@ -222,7 +222,7 @@ def test_robot_hits_report_the_index_and_velocity_and_collided_robots_stay():
               robots=[dict(start=s, goal=(50.0, 50.0), goal_threshold=0.1, path=None) for s in ((0.0, 0.0, 0.0), (6.0, 0.0, math.pi), (0.0, -8.0, -math.pi / 2))])
     w = WorldBatch(1, rb, lidar, 0.1)
     w.set_scenes([sc])
-    o = OracleWorld(_oracle_cfg(rb, lidar), pack_scenes_ex([sc]), pack_fleet([sc]), 3)
+    o = OracleWorld(_oracle_cfg(rb, lidar), pack_scenes_ex([sc]), fleet=pack_fleet([sc]), K=3)
     act = np.array([[1.0, 0.0], [1.5, 0.0], [2.0, 0.0]], np.float32)
     collided_at, seen_after = None, 0
     for k in range(40):
@@ -282,7 +282,7 @@ def test_an_obstacle_wins_a_tie_with_a_robot_and_a_sensor_inside_a_robot_sees_th
     sc = _scene([(0.0, 0.0, 0.0), (2.6, 0.0, 0.0)])
     w.set_scenes([sc])
     ranges, _, _, hit = w.scan(hit=True)
-    o = OracleWorld(_oracle_cfg(rb, inside), pack_scenes_ex([sc]), pack_fleet([sc]), 2)
+    o = OracleWorld(_oracle_cfg(rb, inside), pack_scenes_ex([sc]), fleet=pack_fleet([sc]), K=2)
     r64, _, h64, _, _ = o.scan()
     assert hit[0].tolist() == [1, 1] == h64[0].tolist()  # the sensor sits inside robot 1: both beams see its exit crossings
     assert abs(ranges[0, 0].item() - 0.9) < 1e-6 and abs(ranges[0, 1].item() - 0.7) < 1e-6

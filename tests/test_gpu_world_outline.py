@@ -1,4 +1,4 @@
-"""Outline obstacles in the batched world on the GPU: scans and steps against the float64 oracle (tests/world_outline_oracle.py),
+"""Outline obstacles in the batched world on the GPU: scans and steps against the float64 oracle (oracle/world.py),
 the old entry point against nb_world_set_scenes_ex, closed-loop runs of PlannerBatch in seeded non_obs / dyna_non_obs scenes,
 determinism and the absence of host synchronisation."""
 import ctypes as C
@@ -14,7 +14,7 @@ from neupan_b200 import PlannerBatch, WorldBatch, _lib, rollout
 from neupan_b200.robot import robot as Robot
 from neupan_b200.world import dyna_non_obs, non_obs, pack_scenes, pack_scenes_ex, random_outline
 from test_gpu_world import EXAMPLE_LIDAR, LIDAR, _mixed_scenes, _oracle_cfg, _polygon, _ulps
-from world_outline_oracle import OracleWorld
+from oracle.world import OracleWorld
 
 pytestmark = pytest.mark.gpu
 

@@ -1,4 +1,4 @@
-"""Reactive obstacles in the batched world on the GPU: world_rvo_kernel against the float64 oracle (tests/world_rvo_oracle.py),
+"""Reactive obstacles in the batched world on the GPU: world_rvo_kernel against the float64 oracle (oracle/world.py),
 teacher-forced and free-running, its edge cases, the absence of any change without reactive obstacles, the absence of host
 synchronisation, and closed-loop runs of PlannerBatch in dyna_obs / dyna_non_obs with the examples' reactive obstacles."""
 import ctypes as C
@@ -15,7 +15,7 @@ from neupan_b200.world import dyna_non_obs, dyna_obs, pack_behaviors, pack_scene
 from oracle import world as ow
 from test_gpu_world import EXAMPLE_LIDAR, LIDAR, _mixed_scenes, _oracle_cfg, _polygon
 from test_gpu_world_outline import _StillPlanner, _closed_loop
-from world_rvo_oracle import OracleWorld, axis_count
+from oracle.world import OracleWorld, axis_count
 
 pytestmark = pytest.mark.gpu
 

@@ -1,5 +1,5 @@
 """Several robots per environment in the batched world, on the CPU: host validation through nb_world_check_fleet, the packing of
-``robots`` scenes, the circle_swap builder and the sanity of tests/world_fleet_oracle.py (no device needed)."""
+``robots`` scenes, the circle_swap builder and the robot-robot clearance of oracle/world.py (no device needed)."""
 import ctypes as C
 import math
 
@@ -10,7 +10,7 @@ from neupan_b200 import _lib, build as nb_build
 from neupan_b200.robot import robot as Robot
 from neupan_b200.world import circle_swap, fleet_size, make_config, pack_fleet, pack_scenes_ex, rectangle, scene_paths
 from oracle import world as ow
-from world_fleet_oracle import OracleWorld, clearance_robot_pairs, clearance_robots
+from oracle.world import clearance_robot_pairs, clearance_robots
 
 LIDAR = dict(angle_min=-math.pi, angle_max=math.pi, range_min=0.0, range_max=10.0, number=36)
 C4_ROBOT = dict(kinematics="diff", length=1.6, width=2.0)
@@ -127,23 +127,3 @@ def test_oracle_robot_clearance_is_symmetric_and_vectorised_exactly():
     other = [(x + 3.5, y) for x, y in sq]
     assert clearance_robots(sq, other) == clearance_robots(other, sq) == 1.5
 
-
-def test_oracle_fleet_of_one_is_the_single_robot_oracle():
-    """The fleet oracle at K = 1 from the env rows steps and scans exactly like the parent oracles."""
-    from world_rvo_oracle import OracleWorld as RvoOracle
-    rb = Robot(10, 0.1, **C4_ROBOT)
-    cfg = dict(kinematics="diff", step_time=0.1, wheelbase=rb.L, angle_min=LIDAR["angle_min"], angle_max=LIDAR["angle_max"],
-               range_max=LIDAR["range_max"], number=LIDAR["number"], scan_offset=(0.1, 0.0, 0.0), robot_vertices=np.asarray(rb.vertices).T)
-    rng = np.random.default_rng(4)
-    scenes = [dict(obstacles=[dict(center=tuple(rng.uniform(-5, 5, 2)), radius=0.5, velocity=(0.3, -0.2)),
-                              dict(center=tuple(rng.uniform(-5, 5, 2)), vertices=rectangle(1.0, 0.5), velocity=(-0.2, 0.1))],
-                   bounds=(-6.0, -6.0, 6.0, 6.0), start=(0.0, 0.0, 0.3), goal=(4.0, 1.0), goal_threshold=0.3) for _ in range(3)]
-    packed = pack_scenes_ex(scenes)
-    a, b = OracleWorld(cfg, packed), RvoOracle(cfg, packed)
-    for _ in range(20):
-        act = np.column_stack([rng.uniform(0, 1.5, 3), rng.uniform(-0.5, 0.5, 3)]).astype(np.float32)
-        ra, rb_ = a.scan(), b.scan()
-        assert all(np.array_equal(x, y) for x, y in zip(ra, rb_))
-        sa, sb = a.step(act), b.step(act)
-        assert all(np.array_equal(x, y) for x, y in zip(sa, sb))
-        assert np.array_equal(a.states, b.states) and np.array_equal(a.obs, b.obs)

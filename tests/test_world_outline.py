@@ -11,7 +11,7 @@ from neupan_b200 import _lib, build as nb_build
 from neupan_b200.robot import robot as Robot
 from neupan_b200.world import dyna_non_obs, make_config, non_obs, pack_scenes, pack_scenes_ex, random_outline
 from oracle import scan as oscan, world as ow
-from world_outline_oracle import OracleWorld, clearance_outline, inside
+from oracle.world import OracleWorld, clearance_outline, inside_outline
 
 LIDAR = dict(angle_min=-math.pi, angle_max=math.pi, range_min=0.0, range_max=10.0, number=360)
 # a U open upwards: the notch is (-1, 1) x (-1, 3), the arms and the base are 2 m thick
@@ -65,7 +65,7 @@ def test_vertex_to_vertex_diagonal():
 
 
 def test_even_odd_inside_of_a_u():
-    assert not inside(U, 0.0, 1.0) and inside(U, 2.0, 1.0) and inside(U, 0.0, -2.0) and not inside(U, 5.0, 0.0)
+    assert not inside_outline(U, 0.0, 1.0) and inside_outline(U, 2.0, 1.0) and inside_outline(U, 0.0, -2.0) and not inside_outline(U, 5.0, 0.0)
 
 
 def _convex(rng, c):
@@ -278,4 +278,4 @@ def test_random_outline_is_star_shaped_and_simple(lib):
     scenes = [_scene([dict(center=(20.0, 0.0), outline=o) for o in outlines[i:i + 64]]) for i in range(0, 256, 64)]
     assert _check(lib, make_config(rb, LIDAR, 0.1, max_envs=4), pack_scenes_ex(scenes)) == _lib.NB_OK
     for o in outlines:
-        assert inside([tuple(v) for v in o], 0.0, 0.0)  # the centre sees every vertex: it lies inside
+        assert inside_outline([tuple(v) for v in o], 0.0, 0.0)  # the centre sees every vertex: it lies inside

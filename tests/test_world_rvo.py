@@ -1,5 +1,5 @@
 """Reactive obstacles (behaviour kind 1) of the batched world, on the CPU: host validation through nb_world_check_behaviors, the
-SplitMix64 goal draws, the trig-free cones of tests/world_rvo_oracle.py against IR-SIM's atan2 / asin construction, hand-built
+SplitMix64 goal draws, the trig-free cones of oracle/world.py against IR-SIM's atan2 / asin construction, hand-built
 choices of the oracle, pack_behaviors and the scene builders (no device needed)."""
 import ctypes as C
 import hashlib
@@ -11,7 +11,7 @@ import pytest
 from neupan_b200 import _lib, build as nb_build
 from neupan_b200.robot import robot as Robot
 from neupan_b200.world import EXAMPLE_RVO, dyna_non_obs, dyna_obs, make_config, pack_behaviors, pack_scenes_ex
-from world_rvo_oracle import OracleWorld, cone, cone_trig, cross, draw_goal, inside, splitmix64_at, u01
+from oracle.world import OracleWorld, cone, cone_trig, cross, draw_goal, inside_cone, splitmix64_at, u01
 
 LIDAR = dict(angle_min=-math.pi, angle_max=math.pi, range_min=0.0, range_max=10.0, number=36)
 
@@ -150,8 +150,8 @@ def test_trig_free_cones_agree_with_the_atan2_asin_construction():
                 s = rng.uniform(0.1, 2.0)
                 v = np.array([a[0][0] + s * d[0], a[0][1] + s * d[1]])
                 on_edge += 1
-            n_in += inside(a, *v)
-            if inside(a, *v) != inside(t, *v):
+            n_in += inside_cone(a, *v)
+            if inside_cone(a, *v) != inside_cone(t, *v):
                 wx, wy = v[0] - a[0][0], v[1] - a[0][1]
                 edge = min(abs(cross(a[1], wx, wy)), abs(cross(a[2], wx, wy)))
                 assert edge < 1e-9, (ci, cj, vi, vj, ri, rj, v)

@@ -56,7 +56,7 @@ for cname in ("C1", "C5") if "train" in SECTIONS else ():
     assert np.isfinite(losses).all()
     tr.sync_model(); tr.close()
 # the batched world with reactive obstacles: world_scan_kernel, world_rvo_kernel (goal draws, the robot as a neighbour of an obstacle
-# placed on its path) and world_step_kernel
+# placed on its path) and world_step_kernel (every K; here one robot per environment, a one-warp CTA)
 if "world" in SECTIONS:
     from neupan_b200 import WorldBatch
     from neupan_b200.world import dyna_non_obs, dyna_obs
