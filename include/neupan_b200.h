@@ -382,7 +382,7 @@ int nb_world_read_behaviors(nb_world_t* w, int32_t B, double* goals, int32_t* dr
 
 /* Several robots per environment (IR-SIM's robot: section as a list; this project's reading, stated in csrc/world_kernel.cuh):
  *   robots (B*K,6) float64 HOST rows [start x, y, theta, goal x, y, goal_threshold], robot k of environment b at row n = b*K + k.
- * Every robot has the handle's polygon, kinematics and lidar; 1 <= K <= 16.  nb_world_set_fleet (after nb_world_set_scenes(_ex))
+ * Every robot has the handle's polygon, kinematics and lidar (nb_world_set_fleet_ex below: robots of several types); 1 <= K <= 16.  nb_world_set_fleet (after nb_world_set_scenes(_ex))
  * places the B*K robots at their starts and clears their flags; the env rows' start and goal are then unused; behaviours stay set.
  * nb_world_set_scenes(_ex) returns the handle to one robot per environment.  With a fleet, nb_world_scan, nb_world_step and
  * nb_world_read_state take N = B*K as their count and their per-robot arrays have N rows (ranges (N,R), velocity (N,2,R), hit (N,R),
@@ -402,6 +402,30 @@ int nb_world_read_behaviors(nb_world_t* w, int32_t B, double* goals, int32_t* dr
  * A fleet of K = 1 whose rows repeat the env rows gives exactly the world without a fleet. */
 int nb_world_check_fleet(const nb_world_config* cfg, int32_t B, int32_t K, const double* robots);
 int nb_world_set_fleet(nb_world_t* w, int32_t B, int32_t K, const double* robots);
+
+/* Mixed fleets: robots of different shapes and kinematics in one world.  A robot type is a body and a motion model; type 0 is the
+ * robot of nb_world_config, types 1..T are types[0 .. T) (HOST), at most 4 types per handle (T <= 3).  robot_type (B*K) int32 HOST
+ * gives each robot's type (NULL: every robot is type 0).  The lidar (R, angles, range_max, scan_offset) is shared by every type, so
+ * every scan has the shape (N,R).  Each robot integrates with its type's kinematics and wheelbase, its body is its type's polygon
+ * (what the other robots' beams see, and what its clearances are taken from; robot-robot clearances stay symmetric bit for bit
+ * across types), and a reactive obstacle sees it as a circle of its type's circumradius moving with its type's velocity model.  K = 1
+ * is allowed: one robot per environment, of any type.
+ * Checks (NB_ERR_INVALID) besides those of nb_world_check_fleet: T in 0..3 and types not NULL when T > 0; per type (named): the
+ * config polygon's checks (3..8 vertices, finite, convex), a known kinematics, a positive wheelbase for acker; every robot_type in
+ * 0..T (naming the environment and robot); the start bodies' overlap test takes each robot's own polygon.
+ * nb_world_set_fleet / nb_world_check_fleet are these calls with T = 0 and robot_type = NULL (the same checks, messages and uploaded
+ * bytes); nb_world_set_scenes(_ex) returns the handle to one type-0 robot per environment. */
+typedef struct nb_world_robot_type {
+  int32_t kinematics;              /* NB_KIN_* */
+  int32_t num_vertices;            /* 3..8 */
+  double wheelbase;                /* acker only */
+  double vertices[16];             /* x0, y0, x1, y1, ...: the convex polygon in the robot's frame */
+} nb_world_robot_type;
+
+int nb_world_check_fleet_ex(const nb_world_config* cfg, int32_t T, const nb_world_robot_type* types, int32_t B, int32_t K, const double* robots,
+                            const int32_t* robot_type);
+int nb_world_set_fleet_ex(nb_world_t* w, int32_t T, const nb_world_robot_type* types, int32_t B, int32_t K, const double* robots,
+                          const int32_t* robot_type);
 
 /* ---- DUNE training on the device (SURVEY 8f "next" row 4) ------------------------------------------------------------ */
 

@@ -66,6 +66,11 @@ class WorldConfig(C.Structure):
     ]
 
 
+class WorldRobotType(C.Structure):
+    """struct nb_world_robot_type (include/neupan_b200.h)."""
+    _fields_ = [("kinematics", C.c_int32), ("num_vertices", C.c_int32), ("wheelbase", C.c_double), ("vertices", C.c_double * 16)]
+
+
 _FP = C.c_void_p  # device or host float* / int32*: passed as raw addresses
 
 # name -> (restype, argtypes); every symbol include/neupan_b200.h declares
@@ -110,6 +115,8 @@ SYMBOLS = {
     "nb_world_read_behaviors": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, C.c_void_p]),
     "nb_world_check_fleet": (C.c_int, [C.POINTER(WorldConfig), C.c_int32, C.c_int32, _FP]),
     "nb_world_set_fleet": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _FP]),
+    "nb_world_check_fleet_ex": (C.c_int, [C.POINTER(WorldConfig), C.c_int32, _FP, C.c_int32, C.c_int32, _FP, _FP]),
+    "nb_world_set_fleet_ex": (C.c_int, [C.c_void_p, C.c_int32, _FP, C.c_int32, C.c_int32, _FP, _FP]),
     "nb_dune_labels": (C.c_int, [C.c_int32, _FP, _FP, C.c_int64, _FP, _FP, _FP, _FP, C.c_void_p]),
     "nb_dune_train_create": (C.c_int, [C.c_int32, _FP, _FP, _FP, C.c_int64, C.c_int32, C.POINTER(C.c_void_p)]),
     "nb_dune_train_destroy": (C.c_int, [C.c_void_p]),

@@ -253,10 +253,42 @@ bool world_bodies_meet(const double* a, int na, const double* b, int nb_) {
   return true;
 }
 
-// Every check of nb_world_set_fleet on the host: K in 1..kWorldMaxFleet, finite rows, goal_threshold >= 0, and no two robots of an
-// environment whose bodies at their starts overlap or touch.
-int world_check_fleet(const nb_world_config* cfg, int32_t B, int32_t K, const double* robots) {
+// Type 0 (the robot of the config) and types 1..T as rows of the device type table; r is the circumradius about the state point
+// (a reactive obstacle's neighbour circle), computed as the rvo kernel's products are rounded.
+nb::WorldRobotType world_type_row(int32_t kinematics, int32_t nv, double L, const double* vertices) {
+  nb::WorldRobotType t{};
+  t.kinematics = kinematics; t.nv = nv; t.L = L;
+  for (int i = 0; i < 2 * nv; ++i) t.v[i] = vertices[i];
+  for (int k = 0; k < nv; ++k) t.r = std::max(t.r, std::sqrt(host_dmul(t.v[2 * k], t.v[2 * k]) + host_dmul(t.v[2 * k + 1], t.v[2 * k + 1])));
+  return t;
+}
+
+std::vector<nb::WorldRobotType> world_type_table(const nb_world_config* cfg, int32_t T, const nb_world_robot_type* types) {
+  std::vector<nb::WorldRobotType> table{world_type_row(cfg->kinematics, cfg->robot_num_vertices, cfg->wheelbase, cfg->robot_vertices)};
+  for (int t = 0; t < T; ++t) table.push_back(world_type_row(types[t].kinematics, types[t].num_vertices, types[t].wheelbase, types[t].vertices));
+  return table;
+}
+
+// Every check of nb_world_set_fleet_ex on the host: T in 0..kWorldMaxRobotTypes - 1 valid robot types (the checks the config's
+// robot gets), K in 1..kWorldMaxFleet, finite rows, goal_threshold >= 0, every robot's type in 0..T, and no two robots of an
+// environment whose bodies at their starts (each its own type's polygon) overlap or touch.  With T = 0 and no robot_type these are
+// the checks and messages of nb_world_check_fleet.
+int world_check_fleet(const nb_world_config* cfg, int32_t T, const nb_world_robot_type* types, int32_t B, int32_t K, const double* robots,
+                      const int32_t* robot_type) {
   if (int rc = world_check_config(cfg)) return rc;
+  if (T < 0 || T >= nb::kWorldMaxRobotTypes)
+    return fail(NB_ERR_INVALID, "T = %d robot types besides type 0 (0..%d)", T, nb::kWorldMaxRobotTypes - 1);
+  if (T > 0 && !types) return fail(NB_ERR_INVALID, "nb_world fleet: null types");
+  for (int t = 1; t <= T; ++t) {
+    const nb_world_robot_type& ty = types[t - 1];
+    if (ty.kinematics < 0 || ty.kinematics > 2) return fail(NB_ERR_INVALID, "robot type %d: kinematics %d (diff, acker or omni)", t, ty.kinematics);
+    if (ty.kinematics == NB_KIN_ACKER && !(ty.wheelbase > 0 && std::isfinite(ty.wheelbase)))
+      return fail(NB_ERR_INVALID, "robot type %d: acker needs a positive wheelbase", t);
+    const int nr = ty.num_vertices;
+    if (nr < 3 || nr > nb::kWorldMaxVertices)
+      return fail(NB_ERR_INVALID, "robot type %d: the polygon needs 3..%d vertices (got %d)", t, nb::kWorldMaxVertices, nr);
+    if (!world_finite(ty.vertices, 2 * nr) || !world_convex(ty.vertices, nr)) return fail(NB_ERR_INVALID, "robot type %d: the polygon is not convex", t);
+  }
   if (B < 1 || B > cfg->max_envs) return fail(NB_ERR_INVALID, "B = %d outside [1, max_envs = %d]", B, cfg->max_envs);
   if (K < 1 || K > nb::kWorldMaxFleet) return fail(NB_ERR_INVALID, "K = %d robots per environment (1..%d)", K, nb::kWorldMaxFleet);
   if (!robots) return fail(NB_ERR_INVALID, "nb_world fleet: null robots");
@@ -265,22 +297,29 @@ int world_check_fleet(const nb_world_config* cfg, int32_t B, int32_t K, const do
       const double* r = robots + 6 * ((size_t)b * K + k);
       if (!world_finite(r, 6)) return fail(NB_ERR_INVALID, "environment %d, robot %d: non-finite value", b, k);
       if (!(r[5] >= 0)) return fail(NB_ERR_INVALID, "environment %d, robot %d: goal_threshold must be >= 0", b, k);
+      if (robot_type) {
+        const int t = robot_type[(size_t)b * K + k];
+        if (t < 0 || t > T) return fail(NB_ERR_INVALID, "environment %d, robot %d: type %d outside 0..%d", b, k, t, T);
+      }
     }
-  const int nr = cfg->robot_num_vertices;
-  std::vector<double> body(2 * (size_t)K * nr);
+  const std::vector<nb::WorldRobotType> table = world_type_table(cfg, T, types);
+  std::vector<double> body(2 * (size_t)K * nb::kWorldMaxVertices);
+  std::vector<int> nv(K);
   for (int b = 0; b < B; ++b) {
     for (int k = 0; k < K; ++k) {
       const double* r = robots + 6 * ((size_t)b * K + k);
+      const nb::WorldRobotType& ty = table[robot_type ? robot_type[(size_t)b * K + k] : 0];
       const double c = std::cos(r[2]), s = std::sin(r[2]);
-      for (int v = 0; v < nr; ++v) {
-        const double px = cfg->robot_vertices[2 * v], py = cfg->robot_vertices[2 * v + 1];
-        body[2 * ((size_t)k * nr + v)] = r[0] + (c * px - s * py);
-        body[2 * ((size_t)k * nr + v) + 1] = r[1] + (s * px + c * py);
+      nv[k] = ty.nv;
+      for (int v = 0; v < ty.nv; ++v) {
+        const double px = ty.v[2 * v], py = ty.v[2 * v + 1];
+        body[2 * ((size_t)k * nb::kWorldMaxVertices + v)] = r[0] + (c * px - s * py);
+        body[2 * ((size_t)k * nb::kWorldMaxVertices + v) + 1] = r[1] + (s * px + c * py);
       }
     }
     for (int i = 0; i < K; ++i)
       for (int j = i + 1; j < K; ++j)
-        if (world_bodies_meet(body.data() + 2 * (size_t)i * nr, nr, body.data() + 2 * (size_t)j * nr, nr))
+        if (world_bodies_meet(body.data() + 2 * (size_t)i * nb::kWorldMaxVertices, nv[i], body.data() + 2 * (size_t)j * nb::kWorldMaxVertices, nv[j]))
           return fail(NB_ERR_INVALID, "environment %d: the start bodies of robots %d and %d overlap", b, i, j);
   }
   return NB_OK;
@@ -319,7 +358,6 @@ struct nb_world {
   uint64_t seed = 0;
   int rvo_cap = 0, rvo_grid = 0;
   size_t rvo_smem = 0;
-  double robot_r = 0.0;
   double *d_beh = nullptr, *d_rad = nullptr, *d_goal = nullptr;
   int32_t* d_draws = nullptr;
   int rvo_max_n = 0;  // the largest environment's obstacle count (rvo_cap = rvo_max_n + K)
@@ -327,6 +365,11 @@ struct nb_world {
   // (states, collided, arrived above, every robot's goal and the velocity of its last step) hold B K rows (world_set_robots)
   int K = 1;
   double *d_fgoal = nullptr, *d_fvel = nullptr;
+  // robot types (nb_world_set_fleet_ex; type 0 is the config's robot): the table (T + 1 rows), each robot's type (B K, zeros
+  // without a mix) and the largest environment's robot edge count (the scan's staging size; 0 with K = 1)
+  nb::WorldRobotType* d_types = nullptr;
+  int32_t* d_rtype = nullptr;
+  int max_redges = 0;
 };
 
 struct nb_dune_train {
@@ -1483,7 +1526,7 @@ namespace {
 // scan launch shape: the largest environment's circles and edges (and with K > 1 the K robot bodies) in shared memory, one thread
 // per beam of the environment's K R beams (at most 256)
 int world_scan_shape(nb_world* w, int B) {
-  const int nre = w->K > 1 ? w->K * w->cfg.robot_num_vertices : 0;
+  const int nre = w->K > 1 ? w->max_redges : 0;
   w->scan_smem = (size_t)w->max_circ * (3 * sizeof(double) + sizeof(int32_t)) + (size_t)w->max_edges * (4 * sizeof(double) + sizeof(int32_t)) +
                  (size_t)nre * (4 * sizeof(double) + sizeof(int32_t));
   w->scan_threads = std::min(256, std::max(32, (w->K * w->cfg.num_beams + 31) / 32 * 32));
@@ -1511,28 +1554,44 @@ int world_rvo_shape(nb_world* w, int B) {
 }
 
 // (Re)allocates the per-robot arrays for B K robots and uploads the rows [start x, y, theta, goal x, y, threshold] (robot k of
-// environment b at row b K + k): every robot at its start, flags and velocities cleared.
-int world_set_robots(nb_world* w, int B, int K, const double* robots) {
+// environment b at row b K + k): every robot at its start, flags and velocities cleared.  The type table is type 0 and types[0 .. T);
+// robot_type NULL: every robot is type 0.
+int world_set_robots(nb_world* w, int B, int K, const double* robots, int T, const nb_world_robot_type* types, const int32_t* robot_type) {
   const size_t N = (size_t)B * K;
   std::vector<double> states(3 * N), goal(3 * N);
   for (size_t n = 0; n < N; ++n)
     for (int c = 0; c < 3; ++c) { states[3 * n + c] = robots[6 * n + c]; goal[3 * n + c] = robots[6 * n + 3 + c]; }
-  void* old[] = {w->d_states, w->d_collided, w->d_arrived, w->d_fgoal, w->d_fvel};
+  const std::vector<nb::WorldRobotType> table = world_type_table(&w->cfg, T, types);
+  std::vector<int32_t> rtype(N, 0);
+  if (robot_type) rtype.assign(robot_type, robot_type + N);
+  int max_redges = 0;
+  for (int b = 0; K > 1 && b < B; ++b) {
+    int e = 0;
+    for (int k = 0; k < K; ++k) e += table[rtype[(size_t)b * K + k]].nv;
+    max_redges = std::max(max_redges, e);
+  }
+  void* old[] = {w->d_states, w->d_collided, w->d_arrived, w->d_fgoal, w->d_fvel, w->d_types, w->d_rtype};
   for (void* p : old)
     if (p) cudaFree(p);
   w->d_states = w->d_fgoal = w->d_fvel = nullptr;
-  w->d_collided = w->d_arrived = nullptr;
+  w->d_collided = w->d_arrived = w->d_rtype = nullptr;
+  w->d_types = nullptr;
   NB_CUDA(dalloc(&w->d_states, 3 * N));
   NB_CUDA(dalloc(&w->d_collided, N));
   NB_CUDA(dalloc(&w->d_arrived, N));
   NB_CUDA(dalloc(&w->d_fgoal, 3 * N));
   NB_CUDA(dalloc(&w->d_fvel, 2 * N));
+  NB_CUDA(dalloc(&w->d_types, table.size()));
+  NB_CUDA(dalloc(&w->d_rtype, N));
   NB_CUDA(cudaMemcpy(w->d_states, states.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
   NB_CUDA(cudaMemcpy(w->d_fgoal, goal.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_types, table.data(), sizeof(nb::WorldRobotType) * table.size(), cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_rtype, rtype.data(), sizeof(int32_t) * N, cudaMemcpyHostToDevice));
   NB_CUDA(cudaMemset(w->d_collided, 0, sizeof(int32_t) * N));
   NB_CUDA(cudaMemset(w->d_arrived, 0, sizeof(int32_t) * N));
   NB_CUDA(cudaMemset(w->d_fvel, 0, sizeof(double) * 2 * N));
   w->K = K;
+  w->max_redges = max_redges;
   return NB_OK;
 }
 }  // namespace
@@ -1574,7 +1633,7 @@ int nb_world_destroy(nb_world_t* w) {
   if (!w) return NB_OK;
   cudaSetDevice(w->cfg.device);
   void* bufs[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
-                  w->d_states, w->d_beam_cs, w->d_beh, w->d_rad, w->d_goal, w->d_draws, w->d_fgoal, w->d_fvel};
+                  w->d_states, w->d_beam_cs, w->d_beh, w->d_rad, w->d_goal, w->d_draws, w->d_fgoal, w->d_fvel, w->d_types, w->d_rtype};
   for (void* b : bufs)
     if (b) cudaFree(b);
   delete w;
@@ -1632,7 +1691,7 @@ int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, c
   if (V) NB_CUDA(cudaMemcpy(w->d_vertices, vertices, sizeof(double) * 2 * V, cudaMemcpyHostToDevice));
   NB_CUDA(cudaMemcpy(w->d_env, envs, sizeof(double) * nb::kWorldEnvCols * B, cudaMemcpyHostToDevice));
   if (O) NB_CUDA(cudaMemcpy(w->d_obs, obstacles, sizeof(double) * nb::kWorldObsCols * O, cudaMemcpyHostToDevice));
-  if (int rc = world_set_robots(w, B, 1, robots.data())) return rc;
+  if (int rc = world_set_robots(w, B, 1, robots.data(), 0, nullptr, nullptr)) return rc;
   w->max_circ = max_circ; w->max_edges = max_edges;
   if (int rc = world_scan_shape(w, B)) return rc;
   w->B = B; w->O = O; w->V = V;
@@ -1651,10 +1710,10 @@ namespace {
 nb::WorldParams world_params(const nb_world* w) {
   nb::WorldParams prm;
   const nb_world_config& c = w->cfg;
-  prm.B = w->B; prm.R = c.num_beams; prm.kinematics = c.kinematics; prm.robot_nv = c.robot_num_vertices;
-  prm.dt = c.step_time; prm.L = c.wheelbase; prm.range_max = c.range_max; prm.beam_cs = w->d_beam_cs;
+  prm.B = w->B; prm.R = c.num_beams;
+  prm.dt = c.step_time; prm.range_max = c.range_max; prm.beam_cs = w->d_beam_cs;
   prm.off_x = c.scan_offset[0]; prm.off_y = c.scan_offset[1]; prm.off_th = c.scan_offset[2];
-  for (int i = 0; i < 2 * nb::kWorldMaxVertices; ++i) prm.robot_v[i] = c.robot_vertices[i];
+  prm.types = w->d_types; prm.rtype = w->d_rtype;
   prm.obs_begin = w->d_obs_begin; prm.vert_begin = w->d_vert_begin; prm.slot = w->d_slot; prm.counts = w->d_counts; prm.kind = w->d_kind;
   prm.vertices = w->d_vertices; prm.env = w->d_env; prm.obs = w->d_obs; prm.states = w->d_states;
   prm.collided = w->d_collided; prm.arrived = w->d_arrived;
@@ -1679,7 +1738,7 @@ int world_ready(const nb_world* w, int32_t B, const char* what, bool per_robot =
 nb::WorldRvoParams world_rvo_params(const nb_world* w, const float* action) {
   nb::WorldRvoParams rp;
   rp.beh = w->d_beh; rp.radius = w->d_rad; rp.goal = w->d_goal; rp.draws = w->d_draws; rp.action = action;
-  rp.seed = w->seed; rp.robot_r = w->robot_r; rp.cap = w->rvo_cap;
+  rp.seed = w->seed; rp.cap = w->rvo_cap;
   return rp;
 }
 }  // namespace
@@ -1730,11 +1789,6 @@ int nb_world_set_behaviors(nb_world_t* w, int32_t B, const double* behaviors, ui
       }
     }
   }
-  double robot_r = 0.0;
-  for (int k = 0; k < w->cfg.robot_num_vertices; ++k) {
-    const double x = w->cfg.robot_vertices[2 * k], y = w->cfg.robot_vertices[2 * k + 1];
-    robot_r = std::max(robot_r, std::sqrt(host_dmul(x, x) + host_dmul(y, y)));
-  }
   void* old[] = {w->d_beh, w->d_rad, w->d_goal, w->d_draws};
   for (void* p : old)
     if (p) cudaFree(p);
@@ -1751,7 +1805,7 @@ int nb_world_set_behaviors(nb_world_t* w, int32_t B, const double* behaviors, ui
     NB_CUDA(cudaMemcpy(w->d_goal, goal.data(), sizeof(double) * 2 * O, cudaMemcpyHostToDevice));
     NB_CUDA(cudaMemcpy(w->d_draws, draws.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice));
   }
-  w->seed = seed; w->robot_r = robot_r;
+  w->seed = seed;
   w->rvo_max_n = max_n;
   if (int rc = world_rvo_shape(w, B)) return rc;
   w->has_rvo = any;
@@ -1776,8 +1830,8 @@ int nb_world_scan(nb_world_t* w, int32_t B, float* ranges, float* velocity, int3
   // the dynamic shared-memory limit is an attribute of the kernel, shared by every handle of the process: set this handle's
   // size before each launch (another handle's nb_world_set_scenes may have set a smaller one)
   NB_CUDA(cudaFuncSetAttribute(nb::world_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
-  nb::world_scan_kernel<<<w->scan_grid, w->scan_threads, w->scan_smem, (cudaStream_t)stream>>>(world_params(w), w->max_circ, w->max_edges, ranges,
-                                                                                               velocity, hit);
+  nb::world_scan_kernel<<<w->scan_grid, w->scan_threads, w->scan_smem, (cudaStream_t)stream>>>(world_params(w), w->max_circ, w->max_edges,
+                                                                                               w->max_redges, ranges, velocity, hit);
   ++g_launches;
   NB_CUDA(cudaGetLastError());
   return NB_OK;
@@ -1813,22 +1867,32 @@ int nb_world_read_state(nb_world_t* w, int32_t B, double* states, double* obstac
   return NB_OK;
 }
 
-int nb_world_check_fleet(const nb_world_config* cfg, int32_t B, int32_t K, const double* robots) {
-  return world_check_fleet(cfg, B, K, robots);
+int nb_world_check_fleet_ex(const nb_world_config* cfg, int32_t T, const nb_world_robot_type* types, int32_t B, int32_t K, const double* robots,
+                            const int32_t* robot_type) {
+  return world_check_fleet(cfg, T, types, B, K, robots, robot_type);
 }
 
-int nb_world_set_fleet(nb_world_t* w, int32_t B, int32_t K, const double* robots) {
+int nb_world_check_fleet(const nb_world_config* cfg, int32_t B, int32_t K, const double* robots) {
+  return nb_world_check_fleet_ex(cfg, 0, nullptr, B, K, robots, nullptr);
+}
+
+int nb_world_set_fleet_ex(nb_world_t* w, int32_t T, const nb_world_robot_type* types, int32_t B, int32_t K, const double* robots,
+                          const int32_t* robot_type) {
   if (int rc = world_ready(w, B, "nb_world_set_fleet")) return rc;
-  if (int rc = world_check_fleet(&w->cfg, B, K, robots)) return rc;
+  if (int rc = world_check_fleet(&w->cfg, T, types, B, K, robots, robot_type)) return rc;
   NB_CUDA(cudaSetDevice(w->cfg.device));
   w->B = 0;  // unusable until the new arrays are in place
-  if (int rc = world_set_robots(w, B, K, robots)) return rc;
+  if (int rc = world_set_robots(w, B, K, robots, T, types, robot_type)) return rc;
   if (int rc = world_scan_shape(w, B)) return rc;
   if (w->d_beh)
     if (int rc = world_rvo_shape(w, B)) return rc;
   w->B = B;
   NB_CUDA(cudaDeviceSynchronize());
   return NB_OK;
+}
+
+int nb_world_set_fleet(nb_world_t* w, int32_t B, int32_t K, const double* robots) {
+  return nb_world_set_fleet_ex(w, 0, nullptr, B, K, robots, nullptr);
 }
 
 }  // extern "C"

@@ -5,7 +5,10 @@
 // simple polygon of 3..16 vertices, convex or not; kind 1), vertices stored relative to the centre so that motion only moves the
 // centre -- each with a constant world-frame velocity, an axis-aligned rectangle in which moving obstacles bounce, and K robots
 // (1 <= K <= 16: nb_world_set_fleet, or one per environment from the scenes' own start and goal) of the planner's robot polygon,
-// each with its goal.  Robot k of environment b is row n = b K + k of every per-robot array, whatever K is.
+// each with its goal.  Robot k of environment b is row n = b K + k of every per-robot array, whatever K is.  Mixed fleets
+// (nb_world_set_fleet_ex): every robot has a type (rtype, zeros without a mix), a row of the type table (polygon, kinematics,
+// wheelbase, circumradius); the kernels read a robot's body and motion model from its type, indexing global memory (a run-time
+// index into a kernel parameter array would copy it to local memory).
 //
 //   world_scan_kernel  one CTA per environment (grid-stride): the environment's circles and polygon edges (convex and outline
 //                      alike) and, with K > 1, the K robot bodies (edges tagged with their owner) are staged in shared memory in
@@ -39,16 +42,26 @@ constexpr int kWorldObsCols = 5;         // obstacle row: cx, cy, vx, vy, radius
 constexpr int kWorldEnvCols = 10;        // env row: xmin, ymin, xmax, ymax, start x, y, theta, goal x, y, goal threshold (the
                                          // kernels read the rectangle; the host takes the robot's start and goal from the rest)
 constexpr int kWorldMaxFleet = 16;       // robots per environment
+constexpr int kWorldMaxRobotTypes = 4;   // kinds of robot per handle (type 0 and at most 3 more)
 constexpr int kWorldStepMaxWarps = 8;    // world_step_kernel: at most 8 warps per CTA, warp w takes robots w, w + 8
 
 // world_step_kernel's environments per CTA: floor(8 / K) up to K = 4 (a CTA of at most 8 warps, one per robot), else 1
 __host__ __device__ constexpr int world_step_envs(int K) { return K <= 4 ? kWorldStepMaxWarps / K : 1; }
 
+// One kind of robot (nb_world_robot_type; type 0 is the robot of nb_world_config): a row of the handle's device type table.
+struct WorldRobotType {
+  double v[2 * kWorldMaxVertices];  // polygon in its own frame: x0, y0, x1, y1, ... (zero past nv)
+  double L;                         // wheelbase (acker)
+  double r;                         // circumradius about the state point (a reactive obstacle's neighbour circle)
+  int32_t kinematics, nv;           // NB_KIN_*, 3..8 vertices
+};
+
 struct WorldParams {
-  int B, R, kinematics, robot_nv;
-  double dt, L, range_max;
+  int B, R;
+  double dt, range_max;
   double off_x, off_y, off_th;
-  double robot_v[2 * kWorldMaxVertices];  // robot polygon in its own frame: x0, y0, x1, y1, ...
+  const WorldRobotType* types;            // (T + 1) the type table
+  const int32_t* rtype;                   // (B K) each robot's type (all 0 without a mix)
   const double* beam_cs;                  // (R, 2) cos, sin of a_i = linspace(angle_min, angle_max, R)[i] (libm, on the host)
   const int32_t* obs_begin;               // (B + 1) offsets into the obstacle rows
   const int32_t* vert_begin;              // (O + 1) offsets into vertices; an empty range is a circle
@@ -81,17 +94,20 @@ __device__ __forceinline__ double dcross(double ax, double ay, double bx, double
 // obstacle boundary or, with K > 1, the body of another robot of the environment (a sensor inside an obstacle or another robot sees
 // the exit crossing); t >= range_max or no crossing is a miss: range_max, velocity 0, hit -1.  Equal t: the lower index wins
 // (obstacles 0..O_b - 1, then robot j as O_b + j), so the result does not depend on the order of the tests.
-__global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, int max_circ, int max_edges, float* __restrict__ ranges,
-                                                         float* __restrict__ velocity, int32_t* __restrict__ hit) {
+// max_redges: the largest environment's robot edge count (the sum of its robots' vertex counts with K > 1, else 0); robot k's edges
+// follow those of robots 0 .. k - 1, each robot's polygon that of its own type.
+__global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, int max_circ, int max_edges, int max_redges,
+                                                         float* __restrict__ ranges, float* __restrict__ velocity, int32_t* __restrict__ hit) {
   extern __shared__ double wsm[];
   __shared__ double s_sx[kWorldMaxFleet], s_sy[kWorldMaxFleet], s_hc[kWorldMaxFleet], s_hs[kWorldMaxFleet];  // sensor poses
-  const int K = prm.K, nr = prm.robot_nv;
-  const int nre = K > 1 ? K * nr : 0;  // robot edges: a single robot stages none
+  __shared__ int s_nre;  // the environment's robot edges
+  const int K = prm.K;
+  const int mre = K > 1 ? max_redges : 0;  // a single robot stages no robot edges
   double* r_ax = wsm;
-  double* r_ay = r_ax + nre;
-  double* r_bx = r_ay + nre;
-  double* r_by = r_bx + nre;
-  double* c_x = r_by + nre;
+  double* r_ay = r_ax + mre;
+  double* r_bx = r_ay + mre;
+  double* r_by = r_bx + mre;
+  double* c_x = r_by + mre;
   double* c_y = c_x + max_circ;
   double* c_r = c_y + max_circ;
   double* e_ax = c_r + max_circ;
@@ -132,29 +148,25 @@ __global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, 
       double hs, hc;
       sincos(dadd(th, prm.off_th), &hs, &hc);
       s_hc[k] = hc; s_hs[k] = hs;
-      if (nre) {
-        double vx[kWorldMaxVertices], vy[kWorldMaxVertices];
-#pragma unroll
-        for (int v = 0; v < kWorldMaxVertices; ++v) {  // constant indices: the parameter array and vx / vy stay in registers
-          const double px = prm.robot_v[2 * v], py = prm.robot_v[2 * v + 1];
-          vx[v] = dadd(x, dsub(dmul(cs, px), dmul(sn, py)));
-          vy[v] = dadd(y, dadd(dmul(sn, px), dmul(cs, py)));
-        }
-#pragma unroll
-        for (int v = 0; v < kWorldMaxVertices; ++v) {
-          if (v < nr) {
-            const int e = k * nr + v;
-            const bool last = v + 1 == nr;
-            r_ax[e] = vx[v]; r_ay[e] = vy[v];
-            r_bx[e] = last ? vx[0] : vx[v + 1 < kWorldMaxVertices ? v + 1 : 0];
-            r_by[e] = last ? vy[0] : vy[v + 1 < kWorldMaxVertices ? v + 1 : 0];
-            r_id[e] = k;
-          }
+      if (K > 1) {
+        int e0 = 0;  // robot k's first edge: after the edges of robots 0 .. k - 1
+        for (int j = 0; j < k; ++j) e0 += prm.types[prm.rtype[(size_t)b * K + j]].nv;
+        const WorldRobotType* ty = prm.types + prm.rtype[n];
+        const int nr = ty->nv;
+        if (k == K - 1) s_nre = e0 + nr;
+        // world vertex v (the step kernel's arithmetic) starts edge v and ends edge v - 1: one pass, no vertex arrays in registers
+#pragma unroll 1
+        for (int v = 0; v < nr; ++v) {
+          const double px = ty->v[2 * v], py = ty->v[2 * v + 1];
+          const double wx = dadd(x, dsub(dmul(cs, px), dmul(sn, py))), wy = dadd(y, dadd(dmul(sn, px), dmul(cs, py)));
+          const int e = e0 + v, ep = e0 + (v == 0 ? nr - 1 : v - 1);
+          r_ax[e] = wx; r_ay[e] = wy; r_id[e] = k;
+          r_bx[ep] = wx; r_by[ep] = wy;
         }
       }
     }
     __syncthreads();
-    const int nobs = o1 - o0;
+    const int nobs = o1 - o0, nre = K > 1 ? s_nre : 0;
     for (int q = threadIdx.x; q < K * R; q += blockDim.x) {
       const int k = K == 1 ? 0 : q / R, i = q - k * R;
       const double sx = s_sx[k], sy = s_sy[k], hc = s_hc[k], hs = s_hs[k];
@@ -336,13 +348,13 @@ __device__ __forceinline__ void world_robot_velocity(int kinematics, double a0, 
 }
 
 // One step of the motion models from (x, y, th); (vx, vy) is the world-frame translation rate it used (world_robot_velocity, with
-// the heading before the step).
-__device__ __forceinline__ void world_integrate(const WorldParams& prm, double a0, double a1, double& x, double& y, double& th, double& vx,
-                                                double& vy) {
-  world_robot_velocity(prm.kinematics, a0, a1, th, vx, vy);
+// the heading before the step), for a robot of the given kinematics and wheelbase L.
+__device__ __forceinline__ void world_integrate(int kinematics, double L, double dt, double a0, double a1, double& x, double& y, double& th,
+                                                double& vx, double& vy) {
+  world_robot_velocity(kinematics, a0, a1, th, vx, vy);
   // omni: no turn; acker: v tan(phi) / L; diff: omega
-  const double dth = prm.kinematics == 2 ? 0.0 : (prm.kinematics == 1 ? dmul(a0, tan(a1)) / prm.L : a1);
-  x = dadd(x, dmul(vx, prm.dt)); y = dadd(y, dmul(vy, prm.dt)); th = dadd(th, dmul(dth, prm.dt));
+  const double dth = kinematics == 2 ? 0.0 : (kinematics == 1 ? dmul(a0, tan(a1)) / L : a1);
+  x = dadd(x, dmul(vx, dt)); y = dadd(y, dmul(vy, dt)); th = dadd(th, dmul(dth, dt));
 }
 
 // Obstacle o moves by v dt; a moving centre that left the rectangle is mirrored back and its velocity component reversed.  Writes
@@ -425,7 +437,8 @@ __global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(con
                                                                            float* __restrict__ clearance) {
   __shared__ double f_x[kWorldMaxFleet][kWorldMaxVertices], f_y[kWorldMaxFleet][kWorldMaxVertices];  // E K <= 8 or K <= 16 slots
   __shared__ double f_v[kWorldMaxFleet][2];
-  const int K = prm.K, nr = prm.robot_nv, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  __shared__ int f_nv[kWorldMaxFleet];  // each slot's vertex count (its type's)
+  const int K = prm.K, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
   const int b0 = blockIdx.x * world_step_envs(K);
   const int nslot = min(world_step_envs(K), prm.B - b0) * K;  // this CTA's robots
   const size_t n0 = (size_t)b0 * K;
@@ -433,7 +446,8 @@ __global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(con
     const size_t n = n0 + s;
     double x = prm.states[3 * n], y = prm.states[3 * n + 1], th = prm.states[3 * n + 2];
     double vx = 0.0, vy = 0.0;
-    if (prm.collided[n] == 0) world_integrate(prm, (double)action[2 * n], (double)action[2 * n + 1], x, y, th, vx, vy);
+    const WorldRobotType* ty = prm.types + prm.rtype[n];
+    if (prm.collided[n] == 0) world_integrate(ty->kinematics, ty->L, prm.dt, (double)action[2 * n], (double)action[2 * n + 1], x, y, th, vx, vy);
     prm.states[3 * n] = x; prm.states[3 * n + 1] = y; prm.states[3 * n + 2] = th;
     const double* g = prm.fgoal + 3 * n;
     const double gx = dsub(x, g[0]), gy = dsub(y, g[1]);
@@ -443,12 +457,13 @@ __global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(con
     double sn, cs;
     sincos(th, &sn, &cs);
 #pragma unroll
-    for (int v = 0; v < kWorldMaxVertices; ++v) {  // constant indices into the parameter array
-      const double px = prm.robot_v[2 * v], py = prm.robot_v[2 * v + 1];
+    for (int v = 0; v < kWorldMaxVertices; ++v) {  // the type's polygon (zero past nv, unused)
+      const double px = ty->v[2 * v], py = ty->v[2 * v + 1];
       f_x[s][v] = dadd(x, dsub(dmul(cs, px), dmul(sn, py)));
       f_y[s][v] = dadd(y, dadd(dmul(sn, px), dmul(cs, py)));
     }
     f_v[s][0] = vx; f_v[s][1] = vy;
+    f_nv[s] = ty->nv;
   }
   {
     int b = b0;  // the environment of obstacle o: the CTA's obstacle rows are its environments' back to back
@@ -463,14 +478,15 @@ __global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(con
     const int k = s % K, s0 = s - k;  // robot k of the environment whose robots are the slots s0 .. s0 + K - 1
     const int b = b0 + s / K;
     const size_t n = n0 + s;
+    const int nr = f_nv[s];
     double best = INFINITY;
     for (int o = prm.obs_begin[b] + lane; o < prm.obs_begin[b + 1]; o += 32) {
       const double* row = prm.obs + (size_t)kWorldObsCols * o;
       const double c = world_obstacle_clearance(prm, o, row[0], row[1], f_x[s], f_y[s], nr);
       best = fmin(best, c > 0.0 ? c : 0.0);
     }
-    if (lane < K && lane != k) {
-      const double c = world_robot_clearance(WorldRobot{f_x[s], f_y[s], nr}, WorldRobot{f_x[s0 + lane], f_y[s0 + lane], nr});
+    if (lane < K && lane != k) {  // each side with its own vertex count: symmetric bit for bit across types too
+      const double c = world_robot_clearance(WorldRobot{f_x[s], f_y[s], nr}, WorldRobot{f_x[s0 + lane], f_y[s0 + lane], f_nv[s0 + lane]});
       best = fmin(best, c > 0.0 ? c : 0.0);
     }
 #pragma unroll

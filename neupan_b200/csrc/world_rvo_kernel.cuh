@@ -8,9 +8,9 @@
 //   2. v_des      speed * (goal - c_i) / |goal - c_i|  (0 when the goal is the centre)
 //   3. neighbours every other obstacle of the environment and each of its K robots whose centre lies within neighbor_range of c_i
 //                 (distance <= neighbor_range; a neighbour at the same centre is skipped), each a circle: a circle's radius, a
-//                 polygon's or outline's circumradius about its centre, a robot's circumradius about its state point.  A robot's
-//                 velocity is 0 once collided, else that of this step's action in the world frame (diff / acker v (cos th, sin th),
-//                 omni (vx, vy)).  The robots are the rows after the obstacles, in robot order.
+//                 polygon's or outline's circumradius about its centre, a robot's circumradius (its type's) about its state point.
+//                 A robot's velocity is 0 once collided, else that of this step's action in the world frame under its type's
+//                 kinematics (diff / acker v (cos th, sin th), omni (vx, vy)).  The robots are the rows after the obstacles, in robot order.
 //   4. cones      apex (v_i + v_j) / 2 (RVO); R = r_i + r_j, D = |c_j - c_i|, D' = max(D, R); edges: the unit direction to j turned by
 //                 +-alpha with sin alpha = R / D', cos alpha = sqrt(D'^2 - R^2) / D' (IR-SIM's atan2 / asin / cos / sin construction
 //                 without trigonometry: equal in exact arithmetic, correctly rounded here).  w = v - apex is inside when
@@ -53,7 +53,6 @@ struct WorldRvoParams {
   int32_t* draws;        // (O) goals drawn so far
   const float* action;   // (B K, 2) this step's action
   uint64_t seed;
-  double robot_r;        // circumradius of the robot polygon about its state point
   int cap;               // shared rows per environment: the largest obstacle count + K (the robots)
 };
 
@@ -101,7 +100,9 @@ __device__ __forceinline__ void world_rvo_argmin(double& key, int& idx) {
   }
 }
 
-__global__ void __launch_bounds__(32 * kWorldRvoWarps) world_rvo_kernel(const WorldParams prm, const WorldRvoParams rp) {
+// __maxnreg__(128) instead of __launch_bounds__(256): with the launch bound ptxas settles on 80 registers and spills around the
+// sincos slow-path call; with the cap it takes 98 and spills nothing (2 CTAs of 8 warps per SM either way).
+__global__ void __maxnreg__(128) world_rvo_kernel(const WorldParams prm, const WorldRvoParams rp) {
   extern __shared__ double rsm[];
   const int cap = rp.cap, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   double* s_cx = rsm;
@@ -125,10 +126,11 @@ __global__ void __launch_bounds__(32 * kWorldRvoWarps) world_rvo_kernel(const Wo
     }
     for (int k = threadIdx.x; k < prm.K; k += blockDim.x) {  // robot k, row n + k: its state point and the velocity of this step's
       const size_t r = (size_t)b * prm.K + k;               // action, as world_integrate computes it
+      const int t = prm.rtype[r];                           // its own type's velocity model and circumradius
       const double th = prm.states[3 * r + 2];
       double rvx = 0.0, rvy = 0.0;
-      if (prm.collided[r] == 0) world_robot_velocity(prm.kinematics, (double)rp.action[2 * r], (double)rp.action[2 * r + 1], th, rvx, rvy);
-      s_cx[n + k] = prm.states[3 * r]; s_cy[n + k] = prm.states[3 * r + 1]; s_vx[n + k] = rvx; s_vy[n + k] = rvy; s_r[n + k] = rp.robot_r;
+      if (prm.collided[r] == 0) world_robot_velocity(prm.types[t].kinematics, (double)rp.action[2 * r], (double)rp.action[2 * r + 1], th, rvx, rvy);
+      s_cx[n + k] = prm.states[3 * r]; s_cy[n + k] = prm.states[3 * r + 1]; s_vx[n + k] = rvx; s_vy[n + k] = rvy; s_r[n + k] = prm.types[t].r;
     }
     __syncthreads();
     for (int i = wid; i < n; i += kWorldRvoWarps) {

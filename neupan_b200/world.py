@@ -41,6 +41,15 @@ the start of the step, then each robot's clearance is the minimum over the obsta
 bit for bit, so two robots that touch collide in the same step).  A collided robot is frozen and stays in the scene with velocity 0;
 an arrived robot stays in the scene.  Reactive obstacles take every robot of their environment as a neighbour.
 
+Mixed fleets (nb_world_set_fleet_ex): ``WorldBatch`` takes a sequence of robots, entry i being robot type i (type 0 gives the
+config), and a scene robot (or a single-robot scene) may carry ``"type": i`` (default 0), so robots of different shapes and
+kinematics share a world, at most 4 types.  Each robot integrates with its type's motion model, its body (what the other robots see
+and collide with) is its type's polygon, and reactive obstacles see it with its type's circumradius and velocity model; the lidar is
+shared by every type, so scans stay (N, R).  Actions are in each robot's own convention (omni: (vx, vy)).  ``rows_of_type(i)`` gives
+the rows of one kind, ``scene_paths(scenes, type=i)`` their paths, and ``MixedPlanner`` drives every kind with its own
+``PlannerBatch`` behind one ``forward``, so ``rollout`` runs a mixed world unchanged.  K = 1 is allowed: one robot per environment,
+of any type (the same seeded scenes with a diff, an acker and an omni robot side by side).
+
 There is no CPU implementation here: the CUDA library is the product (oracle/world.py restates it for the tests).
 """
 from __future__ import annotations
@@ -56,20 +65,33 @@ from . import _lib
 ENV_COLS = 10  # xmin, ymin, xmax, ymax, start x, y, theta, goal x, y, goal threshold
 ROBOT_COLS = 6  # start x, y, theta, goal x, y, goal threshold
 MAX_ROBOTS = 16
+MAX_ROBOT_TYPES = 4
 BEH_COLS = 13  # kind, vxmax, vymax, acce, factor, speed, wander, goal x, y, goal threshold, neighbor range, grid, min speed
 # the keys of an "rvo" behaviour besides vxmax and vymax (required); speed None: min(vxmax, vymax); goal None: drawn
 RVO_DEFAULTS = dict(acce=1.0, factor=1.0, speed=None, wander=False, goal=None, goal_threshold=0.3, neighbor_range=10.0, grid=0.05,
                     min_speed=0.3)
 
 
-def make_config(robot, lidar: dict, step_time: float, max_envs: int, device: int = 0) -> _lib.WorldConfig:
-    """struct nb_world_config from the planner's robot (its ``vertices`` (2, n), ``kinematics`` and ``L``) and a lidar dict with
-    ``angle_min``, ``angle_max``, ``range_max``, ``number`` (R) and optionally ``scan_offset`` (sensor pose in the robot frame)."""
+def _robot_vertices(robot):
     verts = np.asarray(robot.vertices, dtype=np.float64)
     if verts.ndim != 2 or verts.shape[0] != 2 or verts.shape[1] > 8:
         raise ValueError("robot.vertices must be (2, n) with n <= 8")
     rv = np.zeros(16)
     rv[:2 * verts.shape[1]] = verts.T.reshape(-1)
+    return verts, rv
+
+
+def make_robot_type(robot) -> _lib.WorldRobotType:
+    """struct nb_world_robot_type from a robot (its ``vertices`` (2, n), ``kinematics`` and ``L``)."""
+    verts, rv = _robot_vertices(robot)
+    return _lib.WorldRobotType(kinematics=_lib.NB_KIN[robot.kinematics], num_vertices=verts.shape[1], wheelbase=float(robot.L or 0.0),
+                               vertices=(C.c_double * 16)(*rv))
+
+
+def make_config(robot, lidar: dict, step_time: float, max_envs: int, device: int = 0) -> _lib.WorldConfig:
+    """struct nb_world_config from the planner's robot (its ``vertices`` (2, n), ``kinematics`` and ``L``) and a lidar dict with
+    ``angle_min``, ``angle_max``, ``range_max``, ``number`` (R) and optionally ``scan_offset`` (sensor pose in the robot frame)."""
+    verts, rv = _robot_vertices(robot)
     return _lib.WorldConfig(kinematics=_lib.NB_KIN[robot.kinematics], num_beams=int(lidar["number"]), max_envs=int(max_envs), device=int(device),
                             robot_num_vertices=verts.shape[1], step_time=float(step_time), wheelbase=float(robot.L or 0.0),
                             angle_min=float(lidar["angle_min"]), angle_max=float(lidar["angle_max"]), range_max=float(lidar["range_max"]),
@@ -137,9 +159,16 @@ def pack_fleet(scenes) -> np.ndarray:
     return np.ascontiguousarray(np.asarray(rows, np.float64).reshape(-1, ROBOT_COLS))
 
 
-def scene_paths(scenes) -> list:
-    """The initial paths of every robot in row order (N = B K): the argument of PlannerBatch.set_initial_paths."""
-    return [rb["path"] for sc in scenes for rb in (sc["robots"] if "robots" in sc else [sc])]
+def pack_robot_types(scenes) -> np.ndarray:
+    """Scenes -> the (B K) int32 robot types of nb_world_set_fleet_ex in pack_fleet's row order (a robot's ``type``, default 0)."""
+    fleet_size(scenes)
+    return np.ascontiguousarray([int(rb.get("type", 0)) for sc in scenes for rb in (sc["robots"] if "robots" in sc else [sc])], np.int32)
+
+
+def scene_paths(scenes, type: int = None) -> list:
+    """The initial paths of every robot in row order (N = B K): the argument of PlannerBatch.set_initial_paths.  With ``type``,
+    only the robots of that type, in row order (the rows of WorldBatch.rows_of_type)."""
+    return [rb["path"] for sc in scenes for rb in (sc["robots"] if "robots" in sc else [sc]) if type is None or rb.get("type", 0) == type]
 
 
 def pack_behaviors(scenes) -> np.ndarray:
@@ -172,11 +201,19 @@ def _host_ptrs(packed):
 
 
 class WorldBatch:
-    """B environments of one robot type and one lidar, K robots each (``K``, set by the scenes; N = B K).  ``lidar``: angle_min,
-    angle_max, range_min, range_max, number (R), optional scan_offset.  ``scan`` / ``step`` enqueue on the current stream and never
-    synchronise the host."""
+    """B environments of one lidar, K robots each (``K``, set by the scenes; N = B K).  ``robot``: the robot, or a sequence of
+    robots whose entry i is robot type i (a mixed fleet, at most 4 types; the scenes' robots choose theirs with ``"type"``).
+    ``lidar``: angle_min, angle_max, range_min, range_max, number (R), optional scan_offset.  ``scan`` / ``step`` enqueue on the
+    current stream and never synchronise the host."""
 
     def __init__(self, num_envs: int, robot, lidar: dict, step_time: float, device=None):
+        robots = list(robot) if isinstance(robot, (list, tuple)) else [robot]
+        if not 1 <= len(robots) <= MAX_ROBOT_TYPES:
+            raise ValueError(f"1..{MAX_ROBOT_TYPES} robot types (got {len(robots)})")
+        robot = robots[0]
+        self.robots = robots
+        self.types = (_lib.WorldRobotType * max(1, len(robots) - 1))(*[make_robot_type(r) for r in robots[1:]])
+        self._rows = None
         if not torch.cuda.is_available():
             raise RuntimeError("neupan_b200.WorldBatch needs a CUDA device (no CPU fallback)")
         self.B, self.dt, self.R = int(num_envs), float(step_time), int(lidar["number"])
@@ -203,24 +240,46 @@ class WorldBatch:
     def set_scenes(self, scenes, seed: int = 0):
         """Uploads B scenes, puts every robot at its start and clears the flags (env.reset).  When an obstacle has a behaviour,
         also sets the behaviours (nb_world_set_behaviors); ``seed`` keys the goal draws of reactive obstacles.  Scenes with K > 1
-        ``robots`` also set the fleet (nb_world_set_fleet); K = 1 runs as the single-robot world."""
+        ``robots`` also set the fleet (nb_world_set_fleet); K = 1 runs as the single-robot world.  With several robot types the
+        fleet goes through nb_world_set_fleet_ex with every robot's ``type`` (any K)."""
         if len(scenes) != self.B:
             raise ValueError(f"expected {self.B} scenes, got {len(scenes)}")
         K = fleet_size(scenes)
         packed = pack_scenes_ex(scenes)
-        fleet = pack_fleet(scenes) if K > 1 else None
+        rtype = pack_robot_types(scenes)
+        T = len(self.robots) - 1
+        if T == 0 and rtype.any():
+            raise ValueError(f"a robot has type {int(rtype.max())} but the world has one robot type")
+        fleet = pack_fleet(scenes) if K > 1 or T > 0 else None
         beh = pack_behaviors(scenes) if any("behavior" in ob for sc in scenes for ob in sc["obstacles"]) else None
         with torch.cuda.device(self.device):
             lib = _lib.load()
+            fleet_args = (self.B, K, C.c_void_p(fleet.ctypes.data)) if fleet is not None else None
+            types_args = (T, self.types) if T > 0 else None
             if fleet is not None:  # refuse before anything is uploaded
-                _lib.check(lib.nb_world_check_fleet(C.byref(self.config), self.B, K, C.c_void_p(fleet.ctypes.data)))
+                if types_args:
+                    _lib.check(lib.nb_world_check_fleet_ex(C.byref(self.config), *types_args, *fleet_args, C.c_void_p(rtype.ctypes.data)))
+                else:
+                    _lib.check(lib.nb_world_check_fleet(C.byref(self.config), *fleet_args))
             _lib.check(lib.nb_world_set_scenes_ex(self._handle, self.B, *_host_ptrs(packed)))
             self.O, self.K, self.N = int(packed[0][-1]), 1, self.B
+            self._rows = None
             if beh is not None:
                 _lib.check(lib.nb_world_set_behaviors(self._handle, self.B, C.c_void_p(beh.ctypes.data), C.c_uint64(int(seed))))
             if fleet is not None:
-                _lib.check(lib.nb_world_set_fleet(self._handle, self.B, K, C.c_void_p(fleet.ctypes.data)))
+                if types_args:
+                    _lib.check(lib.nb_world_set_fleet_ex(self._handle, *types_args, *fleet_args, C.c_void_p(rtype.ctypes.data)))
+                else:
+                    _lib.check(lib.nb_world_set_fleet(self._handle, *fleet_args))
                 self.K, self.N = K, self.B * K
+        self.robot_types = rtype
+        self._rows = [torch.from_numpy(np.flatnonzero(rtype == i)).to(self.device) for i in range(len(self.robots))]
+
+    def rows_of_type(self, i: int) -> torch.Tensor:
+        """The rows (int64, on the device, ascending) of the robots of type i, built once by set_scenes."""
+        if self._rows is None:
+            raise ValueError("no scenes set")
+        return self._rows[i]
 
     def goals(self):
         """(goals (O,2) float64, draws (O,) int32) on the device: every obstacle's current goal and the number of goals drawn for it
@@ -303,6 +362,46 @@ def rollout(planner, world: WorldBatch, steps: int, blind: bool = False, velocit
         min_clear = torch.minimum(min_clear, clearance)
     collided, arrived = world.flags()
     return dict(collided=collided.bool(), arrived=arrived.bool(), steps_to_arrive=steps_to_arrive, min_clearance=min_clear)
+
+
+class MixedPlanner:
+    """One PlannerBatch per kind of robot behind a single ``forward``: ``groups`` is [(planner, rows), ...], each planner driving
+    the world rows ``rows`` (WorldBatch.rows_of_type; together every row exactly once).  ``forward`` gathers each kind's states,
+    scans and scan velocities, calls its planner and scatters the actions into one (N, 2) tensor, each kind's in its own convention
+    (omni: (vx, vy)); it enqueues on the current stream without a host synchronisation, so ``rollout(MixedPlanner(...), world, ...)``
+    runs a mixed world.  Returns (action, [info of each planner])."""
+
+    def __init__(self, groups):
+        self.groups = []
+        for pl, rows in groups:
+            rows = torch.as_tensor(rows, dtype=torch.int64).to(pl.device)
+            if len(rows) != pl.B:
+                raise ValueError(f"a planner of {pl.B} robots was given {len(rows)} rows")
+            self.groups.append((pl, rows))
+        self.N = sum(len(r) for _, r in self.groups)
+        self.device = self.groups[0][0].device
+        seen = torch.cat([r.to(self.device) for _, r in self.groups]).sort().values.cpu()  # once, at construction
+        if not torch.equal(seen, torch.arange(self.N)):
+            raise ValueError("the groups' rows must cover 0..N-1 exactly once")
+
+    def forward(self, states, ranges=None, scan: dict = None, scan_offset=(0.0, 0.0, 0.0), scan_velocity=None, **kw):
+        states = torch.as_tensor(states).reshape(self.N, 3)
+        action = torch.empty((self.N, 2), dtype=torch.float32, device=self.device)
+        infos = []
+        for pl, rows in self.groups:
+            pick = lambda t: None if t is None else t.index_select(0, rows)
+            a, info = pl.forward(pick(states), pick(ranges), scan, scan_offset=scan_offset, scan_velocity=pick(scan_velocity), **kw)
+            action.index_copy_(0, rows, a)
+            infos.append(info)
+        return action, infos
+
+    def reset(self):
+        for pl, _ in self.groups:
+            pl.reset()
+
+    def close(self):
+        for pl, _ in self.groups:
+            pl.close()
 
 
 # ---- seeded scenes after the reference's examples -------------------------------------------------------------------------
@@ -486,4 +585,18 @@ def circle_swap(num_envs: int, robots: int = 8, radius: float = 10.0, seed: int 
             r, a = rng.uniform(0.0, radius / 3.0), rng.uniform(0.0, 2.0 * math.pi)
             obs.append(dict(center=(r * math.cos(a), r * math.sin(a)), radius=rng.uniform(0.3, 0.6)))
         scenes.append(dict(obstacles=obs, bounds=(-ext, -ext, ext, ext), robots=fleet))
+    return scenes
+
+
+def mixed_swap(num_envs: int, types=(0, 1, 2), robots: int = 6, radius: float = 10.0, seed: int = 0, circles: int = 0):
+    """circle_swap with robot k of type ``types[k % len(types)]`` (a WorldBatch of several robot types): the same starts, goals,
+    paths and obstacles as circle_swap(num_envs, robots, radius, seed, circles).  With the default types (0, 1, 2) and the shipped
+    bodies (C4's 1.6 x 2.0 m diff robot, C2's 4.6 x 1.6 m car, C5's trapezoid) six robots on the default 10 m circle start 10 m
+    apart, clear of the car's 3.9 m circumradius about its rear axle; nb_world_check_fleet_ex refuses starts whose bodies meet."""
+    types = tuple(int(t) for t in types)
+    if not types or min(types) < 0 or max(types) >= MAX_ROBOT_TYPES:
+        raise ValueError(f"types must be a non-empty sequence of 0..{MAX_ROBOT_TYPES - 1} (got {types})")
+    scenes = circle_swap(num_envs, robots=robots, radius=radius, seed=seed, circles=circles)
+    for sc in scenes:
+        sc["robots"] = [dict(rb, type=types[k % len(types)]) for k, rb in enumerate(sc["robots"])]
     return scenes

@@ -75,5 +75,19 @@ if "world" in SECTIONS:
         torch.cuda.synchronize()
         assert torch.isfinite(w.obstacles()).all() and torch.isfinite(g).all()
         w.close()
+    # a mixed fleet: C4's diff robot, C2's car and C5's trapezoid, six robots per environment, with reactive obstacles among them
+    from neupan_b200.world import mixed_swap
+    kinds = [CONFIGS[c].make_robot() for c in ("C4", "C2", "C5")]
+    scenes = mixed_swap(6, robots=6, seed=1, circles=3)
+    for sc in scenes:
+        sc["obstacles"] = [dict(ob, behavior=dict(name="rvo", vxmax=0.5, vymax=0.5, wander=True)) for ob in sc["obstacles"]]
+    w = WorldBatch(6, kinds, lidar, 0.1)
+    w.set_scenes(scenes, seed=3)
+    for _ in range(30):
+        w.scan()
+        w.step(torch.full((36, 2), 0.5, device="cuda"))
+    torch.cuda.synchronize()
+    assert torch.isfinite(w.states).all() and torch.isfinite(w.obstacles()).all()
+    w.close()
 torch.cuda.synchronize()
 print("sanitize smoke ok")

@@ -2,6 +2,7 @@
 
     python tools/world_bench.py [--scene dyna_obs|dyna_non_obs|circle_swap] [--behavior constant|rvo] [--envs 4096] [--robots 1]
                                 [--beams 1080] [--steps 20] [--warmup 3]
+    python tools/world_bench.py --mixed [--envs 4096] [--robots 6] [--beams 1080] [--steps 20] [--warmup 3]
 
 Scenes: seeded dyna_obs (20 moving circles per environment, neupan_b200.world.dyna_obs; the default) or dyna_non_obs (11 moving
 obstacles after example/dyna_non_obs: squares, circles and non-convex outlines, neupan_b200.world.dyna_non_obs), with constant-velocity
@@ -12,7 +13,9 @@ PlannerBatch with C4's robot, adjust values and K, the scans decimated to C4's N
 reset) and the closed-loop step (scan -> PlannerBatch.forward -> step, from the initial scenes after a reset), whose world and planner
 parts are also timed separately with events around each call.  The planner-alone leg repeats one input; in the closed loop the
 inputs change every step (robots move, some arrive or stop), so the two planner times need not agree.  The card's name and power
-limit are read in the same run.  With --behavior rvo, one more closed-loop window of --steps iterations runs under torch.profiler,
+limit are read in the same run.  --mixed: mixed_swap (diff, acker and omni robots in turn, types 0, 1, 2: C4's, C2's and C5's bodies)
+against circle_swap of C4's robot at the same B and K, world alone and closed loop, each kind driven by its own config's PlannerBatch
+through MixedPlanner (circle_swap: one C4 PlannerBatch of N planners).  With --behavior rvo, one more closed-loop window of --steps iterations runs under torch.profiler,
 which gives the device time of world_rvo_kernel per step and its share of the closed-loop step timed with events.
 """
 import argparse
@@ -45,7 +48,10 @@ def main():
     ap.add_argument("--beams", type=int, default=1080)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--mixed", action="store_true", help="mixed_swap against circle_swap at the same N")
     args = ap.parse_args()
+    if args.mixed:
+        return mixed(args)
 
     import math
 
@@ -142,6 +148,81 @@ def main():
                           ray_obstacle_tests_per_s=tests / (ms_scan * 1e-3), **rvo, **_card())))
     world.close()
     pl.close()
+
+
+def _timed(fn, args):
+    import torch
+
+    for _ in range(args.warmup):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(args.steps):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / args.steps
+
+
+def mixed(args):
+    """scan + step and the closed-loop step of mixed_swap against circle_swap at the same B, K and R."""
+    import math
+
+    import torch
+
+    from helpers import CONFIGS, weights_path
+    from neupan_b200 import MixedPlanner, PlannerBatch, WorldBatch
+    from neupan_b200.world import circle_swap, mixed_swap, scene_paths
+
+    if not torch.cuda.is_available():
+        raise SystemExit("world_bench.py needs a CUDA device")
+    B, K, R = args.envs, 6 if args.robots == 1 else args.robots, args.beams
+    lidar = dict(angle_min=-math.pi, angle_max=math.pi, range_min=0.0, range_max=10.0, number=R)
+
+    def planner(cname, n):
+        cfg = CONFIGS[cname]
+        return PlannerBatch(n, cfg.T, cfg.dt, 4.0, robot_kwargs=cfg.robot_kwargs, adjust_kwargs=dict(cfg.adjust),
+                            pan_kwargs=dict(iter_num=cfg.K, dune_max_num=CONFIGS["C4"].N, nrmp_max_num=cfg.M,
+                                            dune_checkpoint=weights_path(cfg.model), iter_threshold=0.0, max_points=CONFIGS["C4"].N))
+
+    out = {}
+    for name in ("circle_swap", "mixed_swap"):
+        if name == "circle_swap":
+            scenes = circle_swap(B, robots=K, seed=2024)
+            pl = planner("C4", B * K)
+            pl.set_initial_paths(scene_paths(scenes))
+            world = WorldBatch(B, pl.robot, lidar, pl.dt)
+            world.set_scenes(scenes)
+        else:
+            scenes = mixed_swap(B, robots=K, seed=2024)
+            counts = [sum(1 for sc in scenes for rb in sc["robots"] if rb["type"] == t) for t in range(3)]
+            pls = [planner(c, n) for c, n in zip(("C4", "C2", "C5"), counts)]
+            for t, p in enumerate(pls):
+                p.set_initial_paths(scene_paths(scenes, type=t))
+            world = WorldBatch(B, [p.robot for p in pls], lidar, pls[0].dt)
+            world.set_scenes(scenes)
+            pl = MixedPlanner([(p, world.rows_of_type(t)) for t, p in enumerate(pls)])
+        zero = torch.zeros(B * K, 2, device="cuda")
+
+        def world_only():
+            world.scan()
+            world.step(zero)
+
+        def closed_loop():
+            r, v, s = world.scan()
+            a, _ = pl.forward(world.states, r, s, scan_offset=world.scan_offset, scan_velocity=v)
+            world.step(a)
+
+        ms_world = _timed(world_only, args)
+        world.set_scenes(scenes)
+        pl.reset()
+        ms_loop = _timed(closed_loop, args)
+        out[name] = dict(ms_world_scan_step=ms_world, ms_closed_loop_step=ms_loop)
+        world.close()
+        pl.close()
+    print(json.dumps(dict(metric="batched world: mixed_swap vs circle_swap", envs=B, robots_per_env=K, planners=B * K, beams=R,
+                          steps=args.steps, warmup=args.warmup, **out, **_card())))
 
 
 if __name__ == "__main__":
