@@ -19,7 +19,7 @@ OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libneupan_b200.so")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
-UNITS = ["dune_tc.cu", "pan_api.cu"]  # translation units under csrc/, linked in this order
+UNITS = ["nrmp.cu", "dune_tc.cu", "pan_api.cu", "world_api.cu", "aux_api.cu"]  # translation units under csrc/, linked in this order
 
 
 def obj_path(unit: str) -> str:

@@ -9,6 +9,8 @@
 // (nrmp.py:136-138,254-256; pan.py:234-237), so the full argsort of dune.py:100 is replaced by a
 // deterministic top-M selection (ascending distance, ties -> lower point index).
 #pragma once
+#include <vector>
+
 #include "common.cuh"
 
 namespace nb {
@@ -93,5 +95,11 @@ __device__ __forceinline__ uint32_t orderable(float d) {
 __device__ __forceinline__ float flow(float p, float v, float dt, int t) {
   return __fadd_rn(p, __fmul_rn((float)t, __fmul_rn(v, dt)));
 }
+
+// dune_tc.cu: the operand images of the warpgroup kernels (screen = true: of the screening network) from a packed checkpoint, and the
+// launch of the exact DUNE pass (screen = false) or of the screening pipeline (true); errors are reported through nb::fail
+int build_tc_image(const float* w, int E, std::vector<unsigned char>& out, bool screen);
+int launch_dune_tc(const DuneParams& prm, const unsigned char* d_image, const unsigned char* d_screen_image, int image_flags, bool screen, int sm_count,
+                   int max_smem_optin, cudaStream_t st);
 
 }  // namespace nb

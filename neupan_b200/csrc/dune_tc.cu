@@ -1,10 +1,10 @@
 // Translation unit of the warpgroup (wgmma) DUNE kernels: host-side operand image + launchers.
 #include <cmath>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
 
+#include "host_common.h"
 #include "dune_tc_kernel.cuh"
 #include "dune_screen_kernel.cuh"
 #include "dune_screen_mma_kernel.cuh"
@@ -127,23 +127,20 @@ static cudaError_t resident_grid(K kern, int threads, size_t smem, int sm_count,
 
 // screen = false: dune_tcp_kernel on every point (NB_OPT_DUNE_KERNEL = 2); true: the screening pipeline (4).  The shared-reciprocal
 // tanh is taken wherever image_flags allows it, in the refine and the exact kernel alike, so both pipelines compute the same bits.
+// Counts its launches (3 with screening, 1 without) once all of them are enqueued.
 int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const unsigned char* d_screen_image, int image_flags, bool screen, int sm_count,
-                   int max_smem_optin, cudaStream_t st, char* err, size_t errlen) {
+                   int max_smem_optin, cudaStream_t st) {
   DuneParams prm = prm_in;
   const bool fast = (image_flags & 1) != 0;
   if (screen) {
     // screening: (1) interval pass over all points, (2) exact evaluation of the candidates, (3) the exact kernel for the items the
     // screen could not narrow down to 32 candidates (below, with only_flagged)
-    if (!d_screen_image || !prm.cand_idx || !prm.cand_cnt || !prm.cand_dt || !prm.cand_rad || !prm.screen_stats || !prm.flag_list || !prm.flag_count || !prm.refine_list) {
-      snprintf(err, errlen, "screening buffers are not allocated");
-      return -1;
-    }
+    if (!d_screen_image || !prm.cand_idx || !prm.cand_cnt || !prm.cand_dt || !prm.cand_rad || !prm.screen_stats || !prm.flag_list || !prm.flag_count || !prm.refine_list)
+      return fail(NB_ERR_INVALID, "screening buffers are not allocated");
     const int items_ = prm.B * (prm.T + 1);
     const size_t smem_s = dune_screen_smem_bytes(prm.N, prm.M);
-    if ((long long)smem_s > max_smem_optin) {
-      snprintf(err, errlen, "N=%d needs %zu B of shared memory (limit %d)", prm.N, smem_s, max_smem_optin);
-      return -3;
-    }
+    if ((long long)smem_s > max_smem_optin)
+      return fail(NB_ERR_CAPACITY, "N=%d needs %zu B of shared memory (limit %d)", prm.N, smem_s, max_smem_optin);
     const size_t smem_r = TcImage::kBytes + 2 * (size_t)tc::kTileBytes;
     const int screen_mma = prm.screen_mma;
     cudaError_t e = cudaMemsetAsync(prm.flag_count, 0, 3 * sizeof(int32_t), st);
@@ -190,17 +187,11 @@ int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const
       else dune_refine_kernel<false><<<grid, 128, smem_r, st>>>(prm, d_image);
       e = cudaGetLastError();
     }
-    if (e != cudaSuccess) {
-      snprintf(err, errlen, "dune screen / refine launch failed: %s", cudaGetErrorString(e));
-      return -2;
-    }
+    if (e != cudaSuccess) return fail(NB_ERR_CUDA, "dune screen / refine launch failed: %s", cudaGetErrorString(e));
     prm.only_flagged = 1;
   }
   const size_t smem = dune_tc_smem_bytes(prm.N, prm.geo.E, prm.M);
-  if ((long long)smem > max_smem_optin) {
-    snprintf(err, errlen, "N=%d needs %zu B of shared memory (limit %d)", prm.N, smem, max_smem_optin);
-    return -3;
-  }
+  if ((long long)smem > max_smem_optin) return fail(NB_ERR_CAPACITY, "N=%d needs %zu B of shared memory (limit %d)", prm.N, smem, max_smem_optin);
   const int items = prm.B * (prm.T + 1);
   auto run = [&](auto kern) -> cudaError_t {
     int grid = 0;
@@ -210,11 +201,9 @@ int launch_dune_tc(const DuneParams& prm_in, const unsigned char* d_image, const
     return cudaGetLastError();
   };
   const cudaError_t e = fast ? run(dune_tcp_kernel<true>) : run(dune_tcp_kernel<false>);
-  if (e != cudaSuccess) {
-    snprintf(err, errlen, "dune_tc kernel launch failed: %s", cudaGetErrorString(e));
-    return -2;
-  }
-  return 0;
+  if (e != cudaSuccess) return fail(NB_ERR_CUDA, "dune_tc kernel launch failed: %s", cudaGetErrorString(e));
+  launches += screen ? 3 : 1;
+  return NB_OK;
 }
 
 }  // namespace nb

@@ -1,0 +1,687 @@
+// C ABI of the batched 2-D world (nb_world_*, include/neupan_b200.h): the host-side checks of configs, scenes, behaviours and fleets,
+// the world handle, and the launches of the scan, rvo and step kernels.
+#include <algorithm>
+#include <cmath>
+#include <new>
+#include <vector>
+
+#include "host_common.h"
+#include "world_kernel.cuh"
+#include "world_rvo_kernel.cuh"
+
+using nb::dalloc;
+using nb::fail;
+
+struct nb_world {
+  nb_world_config cfg;
+  int B = 0, O = 0, V = 0;
+  int max_circ = 0, max_edges = 0, scan_threads = 0, scan_grid = 0;
+  size_t scan_smem = 0;
+  int32_t *d_obs_begin = nullptr, *d_vert_begin = nullptr, *d_slot = nullptr, *d_counts = nullptr, *d_kind = nullptr;
+  int32_t *d_collided = nullptr, *d_arrived = nullptr;
+  double *d_vertices = nullptr, *d_env = nullptr, *d_obs = nullptr, *d_states = nullptr;
+  double* d_beam_cs = nullptr;  // (R, 2), fixed at creation
+  // host copies of the scene (nb_world_set_behaviors checks against them)
+  std::vector<int32_t> h_obs_begin, h_vert_begin;
+  std::vector<double> h_vertices, h_env;
+  // obstacle behaviours (nb_world_set_behaviors; nb_world_set_scenes clears them): has_rvo false -> nb_world_step launches only
+  // world_step_kernel
+  bool has_rvo = false;
+  uint64_t seed = 0;
+  int rvo_cap = 0, rvo_grid = 0;
+  size_t rvo_smem = 0;
+  double *d_beh = nullptr, *d_rad = nullptr, *d_goal = nullptr;
+  int32_t* d_draws = nullptr;
+  int rvo_max_n = 0;  // the largest environment's obstacle count (rvo_cap = rvo_max_n + K)
+  // robots per environment (nb_world_set_fleet; nb_world_set_scenes makes it 1, from the env rows): the per-robot arrays
+  // (states, collided, arrived above, every robot's goal and the velocity of its last step) hold B K rows (world_set_robots)
+  int K = 1;
+  double *d_fgoal = nullptr, *d_fvel = nullptr;
+  // robot types (nb_world_set_fleet_ex; type 0 is the config's robot): the table (T + 1 rows), each robot's type (B K, zeros
+  // without a mix) and the largest environment's robot edge count (the scan's staging size; 0 with K = 1)
+  nb::WorldRobotType* d_types = nullptr;
+  int32_t* d_rtype = nullptr;
+  int max_redges = 0;
+};
+
+namespace {
+
+// A convex polygon of n vertices (x0, y0, x1, y1, ...): every vertex off an edge lies strictly on the same side of it
+// (rejects repeated and collinear vertices, reflex corners and self-intersecting stars).
+bool world_convex(const double* v, int n) {
+  double sign = 0.0;
+  for (int k = 0; k < n; ++k) {
+    const int k1 = (k + 1) % n;
+    const double ex = v[2 * k1] - v[2 * k], ey = v[2 * k1 + 1] - v[2 * k + 1];
+    for (int i = 0; i < n; ++i) {
+      if (i == k || i == k1) continue;
+      const double c = ex * (v[2 * i + 1] - v[2 * k + 1]) - ey * (v[2 * i] - v[2 * k]);
+      if (!(c != 0.0) || (sign != 0.0 && (c > 0.0) != (sign > 0.0))) return false;
+      sign = c;
+    }
+  }
+  return true;
+}
+
+// Closed segments p-q and a-b intersect or touch (orientation tests; a zero orientation counts inside the other's bounding box).
+bool world_segs_meet(const double* p, const double* q, const double* a, const double* b) {
+  auto orient = [](const double* u, const double* v, const double* w) { return (v[0] - u[0]) * (w[1] - u[1]) - (v[1] - u[1]) * (w[0] - u[0]); };
+  auto in_box = [](const double* u, const double* v, const double* w) {
+    return std::min(u[0], v[0]) <= w[0] && w[0] <= std::max(u[0], v[0]) && std::min(u[1], v[1]) <= w[1] && w[1] <= std::max(u[1], v[1]);
+  };
+  const double d1 = orient(a, b, p), d2 = orient(a, b, q), d3 = orient(p, q, a), d4 = orient(p, q, b);
+  if (((d1 > 0 && d2 < 0) || (d1 < 0 && d2 > 0)) && ((d3 > 0 && d4 < 0) || (d3 < 0 && d4 > 0))) return true;
+  return (d1 == 0 && in_box(a, b, p)) || (d2 == 0 && in_box(a, b, q)) || (d3 == 0 && in_box(p, q, a)) || (d4 == 0 && in_box(p, q, b));
+}
+
+// Why the outline of n vertices (x0, y0, x1, y1, ...) is not a simple polygon, or nullptr when it is one: every edge has a length,
+// the area is not zero, and no two non-adjacent edges intersect or touch.
+const char* world_outline_problem(const double* v, int n) {
+  double area2 = 0.0;
+  for (int k = 0; k < n; ++k) {
+    const int k1 = (k + 1) % n;
+    if (v[2 * k] == v[2 * k1] && v[2 * k + 1] == v[2 * k1 + 1]) return "has a zero-length edge";
+    area2 += v[2 * k] * v[2 * k1 + 1] - v[2 * k1] * v[2 * k + 1];
+  }
+  if (!(area2 != 0.0)) return "has zero area";
+  for (int i = 0; i < n; ++i)
+    for (int j = i + 2; j < n; ++j) {
+      if (i == 0 && j == n - 1) continue;  // adjacent through the closing vertex
+      if (world_segs_meet(v + 2 * i, v + 2 * ((i + 1) % n), v + 2 * j, v + 2 * ((j + 1) % n))) return "is not simple (two edges that do not share a vertex meet)";
+    }
+  return nullptr;
+}
+
+// a * b rounded on its own: the host compiler may not fuse it into a following sum (the device's dmul / dadd order)
+double host_dmul(double a, double b) {
+  volatile double p = a * b;
+  return p;
+}
+
+bool world_finite(const double* a, size_t n) {
+  for (size_t i = 0; i < n; ++i)
+    if (!std::isfinite(a[i])) return false;
+  return true;
+}
+
+int world_check_config(const nb_world_config* cfg) {
+  if (!cfg) return fail(NB_ERR_INVALID, "nb_world: null config");
+  if (cfg->kinematics < 0 || cfg->kinematics > 2) return fail(NB_ERR_INVALID, "kinematics currently only supports diff, acker or omni");
+  if (cfg->num_beams < 1) return fail(NB_ERR_INVALID, "the lidar needs R >= 1 beams (got %d)", cfg->num_beams);
+  if (cfg->max_envs < 1) return fail(NB_ERR_INVALID, "max_envs must be positive");
+  if (!(cfg->step_time > 0) || !std::isfinite(cfg->step_time)) return fail(NB_ERR_INVALID, "step_time must be positive");
+  if (cfg->kinematics == NB_KIN_ACKER && !(cfg->wheelbase > 0)) return fail(NB_ERR_INVALID, "acker needs a positive wheelbase");
+  if (!(cfg->range_max > 0) || !std::isfinite(cfg->range_max)) return fail(NB_ERR_INVALID, "range_max must be positive and finite");
+  if (!std::isfinite(cfg->angle_min) || !std::isfinite(cfg->angle_max) || !world_finite(cfg->scan_offset, 3))
+    return fail(NB_ERR_INVALID, "lidar angles and scan_offset must be finite");
+  const int nr = cfg->robot_num_vertices;
+  if (nr < 3 || nr > nb::kWorldMaxVertices) return fail(NB_ERR_INVALID, "the robot polygon needs 3..%d vertices (got %d)", nb::kWorldMaxVertices, nr);
+  if (!world_finite(cfg->robot_vertices, 2 * nr) || !world_convex(cfg->robot_vertices, nr)) return fail(NB_ERR_INVALID, "the robot polygon is not convex");
+  return NB_OK;
+}
+
+// Every check of nb_world_set_scenes_ex, on the host (kind NULL: every obstacle is a circle or a convex polygon).  Fills the
+// per-obstacle slots (circle rank / first edge index within the environment), the per-environment (circles, edges) counts and the
+// largest counts of any environment when asked to.
+int world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obs, const int32_t* vert_begin,
+                       const double* vertices, const double* envs, const int32_t* kind, std::vector<int32_t>* slot, std::vector<int32_t>* counts,
+                       int* max_circ, int* max_edges) {
+  if (int rc = world_check_config(cfg)) return rc;
+  if (!obs_begin || !vert_begin || !envs) return fail(NB_ERR_INVALID, "nb_world scenes: null argument");
+  if (B < 1 || B > cfg->max_envs) return fail(NB_ERR_INVALID, "B = %d outside [1, max_envs = %d]", B, cfg->max_envs);
+  if (obs_begin[0] != 0) return fail(NB_ERR_INVALID, "obs_begin[0] must be 0");
+  for (int b = 0; b < B; ++b) {
+    const int n = obs_begin[b + 1] - obs_begin[b];
+    if (n < 0) return fail(NB_ERR_INVALID, "obs_begin is not ascending at environment %d", b);
+    if (n > nb::kWorldMaxObstacles) return fail(NB_ERR_INVALID, "environment %d has %d obstacles (at most %d)", b, n, nb::kWorldMaxObstacles);
+  }
+  const int O = obs_begin[B];
+  if (O > 0 && !obs) return fail(NB_ERR_INVALID, "nb_world scenes: null obstacles");
+  if (vert_begin[0] != 0) return fail(NB_ERR_INVALID, "vert_begin[0] must be 0");
+  for (int o = 0; o < O; ++o) {
+    const int nv = vert_begin[o + 1] - vert_begin[o];
+    if (kind && kind[o] != 0) {
+      if (kind[o] != 1) return fail(NB_ERR_INVALID, "obstacle %d has kind %d (0: circle or convex polygon, 1: outline)", o, kind[o]);
+      if (nv < 3 || nv > nb::kWorldMaxOutlineVertices)
+        return fail(NB_ERR_INVALID, "obstacle %d: an outline needs 3..%d vertices (got %d)", o, nb::kWorldMaxOutlineVertices, nv);
+      continue;
+    }
+    if (nv != 0 && (nv < 3 || nv > nb::kWorldMaxVertices))
+      return fail(NB_ERR_INVALID, "obstacle %d has %d vertices (0 for a circle, 3..%d for a polygon)", o, nv, nb::kWorldMaxVertices);
+  }
+  const int V = vert_begin[O];
+  if (V > 0 && !vertices) return fail(NB_ERR_INVALID, "nb_world scenes: null vertices");
+  if (!world_finite(envs, (size_t)B * nb::kWorldEnvCols) || !world_finite(obs, (size_t)O * nb::kWorldObsCols) || !world_finite(vertices, (size_t)V * 2))
+    return fail(NB_ERR_INVALID, "nb_world scenes: non-finite value");
+  if (slot) { slot->assign(O, 0); counts->assign(2 * (size_t)B, 0); *max_circ = 0; *max_edges = 0; }
+  const double dt = cfg->step_time;
+  for (int b = 0; b < B; ++b) {
+    const double* e = envs + (size_t)nb::kWorldEnvCols * b;
+    if (!(e[0] < e[2]) || !(e[1] < e[3])) return fail(NB_ERR_INVALID, "environment %d: the rectangle needs xmin < xmax and ymin < ymax", b);
+    if (!(e[9] >= 0)) return fail(NB_ERR_INVALID, "environment %d: goal_threshold must be >= 0", b);
+    int nc = 0, ne = 0;
+    for (int o = obs_begin[b]; o < obs_begin[b + 1]; ++o) {
+      const double* r = obs + (size_t)nb::kWorldObsCols * o;
+      const int nv = vert_begin[o + 1] - vert_begin[o];
+      if (nv == 0 && !(r[4] > 0)) return fail(NB_ERR_INVALID, "obstacle %d: a circle needs a positive radius", o);
+      if (kind && kind[o] == 1) {
+        if (const char* why = world_outline_problem(vertices + 2 * (size_t)vert_begin[o], nv)) return fail(NB_ERR_INVALID, "obstacle %d: the outline %s", o, why);
+      } else if (nv > 0 && !world_convex(vertices + 2 * (size_t)vert_begin[o], nv)) {
+        return fail(NB_ERR_INVALID, "obstacle %d is not a convex polygon", o);
+      }
+      for (int a = 0; a < 2; ++a) {
+        if (r[2 + a] == 0.0) continue;
+        const double lo = e[a], hi = e[2 + a];
+        if (r[a] < lo || r[a] > hi) return fail(NB_ERR_INVALID, "obstacle %d moves but its centre starts outside the rectangle of environment %d", o, b);
+        if (!(std::fabs(r[2 + a]) * dt < hi - lo)) return fail(NB_ERR_INVALID, "obstacle %d: |v| * step_time exceeds the rectangle of environment %d", o, b);
+      }
+      if (slot) (*slot)[o] = nv == 0 ? nc : ne;
+      if (nv == 0) ++nc; else ne += nv;
+    }
+    // the scan stages an environment's edges in shared memory; 256 convex polygons cannot exceed this, outlines can
+    if (ne > nb::kWorldMaxEdges) return fail(NB_ERR_INVALID, "environment %d has %d polygon edges (at most %d)", b, ne, nb::kWorldMaxEdges);
+    if (slot) {
+      (*counts)[2 * b] = nc; (*counts)[2 * b + 1] = ne;
+      *max_circ = std::max(*max_circ, nc); *max_edges = std::max(*max_edges, ne);
+    }
+  }
+  return NB_OK;
+}
+
+// Every check of nb_world_set_behaviors on the rows (kWorldBehCols) of valid scenes; obs holds the obstacles' current centres.
+int world_check_behaviors(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obs, const double* envs,
+                          const double* beh) {
+  if (!beh) return fail(NB_ERR_INVALID, "nb_world behaviors: null behaviors");
+  const double dt = cfg->step_time;
+  for (int b = 0; b < B; ++b) {
+    const double* e = envs + (size_t)nb::kWorldEnvCols * b;
+    for (int o = obs_begin[b]; o < obs_begin[b + 1]; ++o) {
+      const double* r = beh + (size_t)nb::kWorldBehCols * o;
+      if (r[0] == 0.0) continue;  // constant velocity: the other columns are not read
+      if (r[0] != 1.0) return fail(NB_ERR_INVALID, "obstacle %d has behaviour kind %g (0: constant velocity, 1: rvo)", o, r[0]);
+      for (int c = 1; c < nb::kWorldBehCols; ++c)
+        if (c != 7 && c != 8 && !std::isfinite(r[c])) return fail(NB_ERR_INVALID, "obstacle %d: behaviour column %d is not finite", o, c);
+      const bool draw = std::isnan(r[7]) && std::isnan(r[8]);
+      if (!draw && (!std::isfinite(r[7]) || !std::isfinite(r[8])))
+        return fail(NB_ERR_INVALID, "obstacle %d: the goal must be finite, or NaN in both coordinates (drawn)", o);
+      static const char* const names[] = {nullptr, "vxmax", "vymax", "acce", "factor", "speed", nullptr, nullptr, nullptr, "goal_threshold",
+                                          "neighbor_range", "grid"};
+      for (int c : {1, 2, 3, 4, 5, 9, 10, 11})
+        if (!(r[c] > 0)) return fail(NB_ERR_INVALID, "obstacle %d: %s must be positive", o, names[c]);
+      if (!(r[12] >= 0)) return fail(NB_ERR_INVALID, "obstacle %d: min_speed must be >= 0", o);
+      if (r[6] != 0.0 && r[6] != 1.0) return fail(NB_ERR_INVALID, "obstacle %d: wander must be 0 or 1", o);
+      for (int a = 0; a < 2; ++a) {
+        const double span = 2.0 * std::min(r[3], r[1 + a]), n = std::ceil(span / r[11]);
+        if (n > nb::kWorldRvoMaxAxis)
+          return fail(NB_ERR_INVALID, "obstacle %d: up to %.0f candidate velocities on an axis (at most %d)", o, n, nb::kWorldRvoMaxAxis);
+      }
+      for (int a = 0; a < 2; ++a) {
+        const double lo = e[a], hi = e[2 + a];
+        if (obs[(size_t)nb::kWorldObsCols * o + a] < lo || obs[(size_t)nb::kWorldObsCols * o + a] > hi)
+          return fail(NB_ERR_INVALID, "obstacle %d is reactive but its centre starts outside the rectangle of environment %d", o, b);
+        if (!(r[1 + a] * dt < hi - lo)) return fail(NB_ERR_INVALID, "obstacle %d: %s * step_time exceeds the rectangle of environment %d", o, names[1 + a], b);
+        if (!draw && (r[7 + a] < lo || r[7 + a] > hi)) return fail(NB_ERR_INVALID, "obstacle %d: its goal lies outside the rectangle of environment %d", o, b);
+      }
+    }
+  }
+  return NB_OK;
+}
+
+// Convex polygons (x0, y0, x1, y1, ...) overlap or touch: no edge normal of either separates their projections strictly (the step
+// kernels' SAT, on the host).
+bool world_bodies_meet(const double* a, int na, const double* b, int nb_) {
+  for (int pass = 0; pass < 2; ++pass) {
+    const double* p = pass ? b : a;
+    const double* q = pass ? a : b;
+    const int np = pass ? nb_ : na, nq = pass ? na : nb_;
+    for (int k = 0; k < np; ++k) {
+      const int k1 = (k + 1) % np;
+      const double nx = -(p[2 * k1 + 1] - p[2 * k + 1]), ny = p[2 * k1] - p[2 * k];
+      double pmin = INFINITY, pmax = -INFINITY, qmin = INFINITY, qmax = -INFINITY;
+      for (int i = 0; i < np; ++i) { const double d = nx * p[2 * i] + ny * p[2 * i + 1]; pmin = std::min(pmin, d); pmax = std::max(pmax, d); }
+      for (int i = 0; i < nq; ++i) { const double d = nx * q[2 * i] + ny * q[2 * i + 1]; qmin = std::min(qmin, d); qmax = std::max(qmax, d); }
+      if (pmax < qmin || qmax < pmin) return false;
+    }
+  }
+  return true;
+}
+
+// Type 0 (the robot of the config) and types 1..T as rows of the device type table; r is the circumradius about the state point
+// (a reactive obstacle's neighbour circle), computed as the rvo kernel's products are rounded.
+nb::WorldRobotType world_type_row(int32_t kinematics, int32_t nv, double L, const double* vertices) {
+  nb::WorldRobotType t{};
+  t.kinematics = kinematics; t.nv = nv; t.L = L;
+  for (int i = 0; i < 2 * nv; ++i) t.v[i] = vertices[i];
+  for (int k = 0; k < nv; ++k) t.r = std::max(t.r, std::sqrt(host_dmul(t.v[2 * k], t.v[2 * k]) + host_dmul(t.v[2 * k + 1], t.v[2 * k + 1])));
+  return t;
+}
+
+std::vector<nb::WorldRobotType> world_type_table(const nb_world_config* cfg, int32_t T, const nb_world_robot_type* types) {
+  std::vector<nb::WorldRobotType> table{world_type_row(cfg->kinematics, cfg->robot_num_vertices, cfg->wheelbase, cfg->robot_vertices)};
+  for (int t = 0; t < T; ++t) table.push_back(world_type_row(types[t].kinematics, types[t].num_vertices, types[t].wheelbase, types[t].vertices));
+  return table;
+}
+
+// Every check of nb_world_set_fleet_ex on the host: T in 0..kWorldMaxRobotTypes - 1 valid robot types (the checks the config's
+// robot gets), K in 1..kWorldMaxFleet, finite rows, goal_threshold >= 0, every robot's type in 0..T, and no two robots of an
+// environment whose bodies at their starts (each its own type's polygon) overlap or touch.  With T = 0 and no robot_type these are
+// the checks and messages of nb_world_check_fleet.
+int world_check_fleet(const nb_world_config* cfg, int32_t T, const nb_world_robot_type* types, int32_t B, int32_t K, const double* robots,
+                      const int32_t* robot_type) {
+  if (int rc = world_check_config(cfg)) return rc;
+  if (T < 0 || T >= nb::kWorldMaxRobotTypes)
+    return fail(NB_ERR_INVALID, "T = %d robot types besides type 0 (0..%d)", T, nb::kWorldMaxRobotTypes - 1);
+  if (T > 0 && !types) return fail(NB_ERR_INVALID, "nb_world fleet: null types");
+  for (int t = 1; t <= T; ++t) {
+    const nb_world_robot_type& ty = types[t - 1];
+    if (ty.kinematics < 0 || ty.kinematics > 2) return fail(NB_ERR_INVALID, "robot type %d: kinematics %d (diff, acker or omni)", t, ty.kinematics);
+    if (ty.kinematics == NB_KIN_ACKER && !(ty.wheelbase > 0 && std::isfinite(ty.wheelbase)))
+      return fail(NB_ERR_INVALID, "robot type %d: acker needs a positive wheelbase", t);
+    const int nr = ty.num_vertices;
+    if (nr < 3 || nr > nb::kWorldMaxVertices)
+      return fail(NB_ERR_INVALID, "robot type %d: the polygon needs 3..%d vertices (got %d)", t, nb::kWorldMaxVertices, nr);
+    if (!world_finite(ty.vertices, 2 * nr) || !world_convex(ty.vertices, nr)) return fail(NB_ERR_INVALID, "robot type %d: the polygon is not convex", t);
+  }
+  if (B < 1 || B > cfg->max_envs) return fail(NB_ERR_INVALID, "B = %d outside [1, max_envs = %d]", B, cfg->max_envs);
+  if (K < 1 || K > nb::kWorldMaxFleet) return fail(NB_ERR_INVALID, "K = %d robots per environment (1..%d)", K, nb::kWorldMaxFleet);
+  if (!robots) return fail(NB_ERR_INVALID, "nb_world fleet: null robots");
+  for (int b = 0; b < B; ++b)
+    for (int k = 0; k < K; ++k) {
+      const double* r = robots + 6 * ((size_t)b * K + k);
+      if (!world_finite(r, 6)) return fail(NB_ERR_INVALID, "environment %d, robot %d: non-finite value", b, k);
+      if (!(r[5] >= 0)) return fail(NB_ERR_INVALID, "environment %d, robot %d: goal_threshold must be >= 0", b, k);
+      if (robot_type) {
+        const int t = robot_type[(size_t)b * K + k];
+        if (t < 0 || t > T) return fail(NB_ERR_INVALID, "environment %d, robot %d: type %d outside 0..%d", b, k, t, T);
+      }
+    }
+  const std::vector<nb::WorldRobotType> table = world_type_table(cfg, T, types);
+  std::vector<double> body(2 * (size_t)K * nb::kWorldMaxVertices);
+  std::vector<int> nv(K);
+  for (int b = 0; b < B; ++b) {
+    for (int k = 0; k < K; ++k) {
+      const double* r = robots + 6 * ((size_t)b * K + k);
+      const nb::WorldRobotType& ty = table[robot_type ? robot_type[(size_t)b * K + k] : 0];
+      const double c = std::cos(r[2]), s = std::sin(r[2]);
+      nv[k] = ty.nv;
+      for (int v = 0; v < ty.nv; ++v) {
+        const double px = ty.v[2 * v], py = ty.v[2 * v + 1];
+        body[2 * ((size_t)k * nb::kWorldMaxVertices + v)] = r[0] + (c * px - s * py);
+        body[2 * ((size_t)k * nb::kWorldMaxVertices + v) + 1] = r[1] + (s * px + c * py);
+      }
+    }
+    for (int i = 0; i < K; ++i)
+      for (int j = i + 1; j < K; ++j)
+        if (world_bodies_meet(body.data() + 2 * (size_t)i * nb::kWorldMaxVertices, nv[i], body.data() + 2 * (size_t)j * nb::kWorldMaxVertices, nv[j]))
+          return fail(NB_ERR_INVALID, "environment %d: the start bodies of robots %d and %d overlap", b, i, j);
+  }
+  return NB_OK;
+}
+
+// scan launch shape: the largest environment's circles and edges (and with K > 1 the K robot bodies) in shared memory, one thread
+// per beam of the environment's K R beams (at most 256)
+int world_scan_shape(nb_world* w, int B) {
+  const int nre = w->K > 1 ? w->max_redges : 0;
+  w->scan_smem = (size_t)w->max_circ * (3 * sizeof(double) + sizeof(int32_t)) + (size_t)w->max_edges * (4 * sizeof(double) + sizeof(int32_t)) +
+                 (size_t)nre * (4 * sizeof(double) + sizeof(int32_t));
+  w->scan_threads = std::min(256, std::max(32, (w->K * w->cfg.num_beams + 31) / 32 * 32));
+  // the occupancy query sees the kernel's current limit; nb_world_scan sets it again before every launch
+  NB_CUDA(cudaFuncSetAttribute(nb::world_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
+  int per_sm = 0, sms = 0;
+  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_scan_kernel, w->scan_threads, w->scan_smem));
+  NB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->cfg.device));
+  if (per_sm < 1) return fail(NB_ERR_CUDA, "world_scan_kernel: %zu B of shared memory do not fit", w->scan_smem);
+  w->scan_grid = std::min(B, per_sm * sms);
+  return NB_OK;
+}
+
+// rvo launch shape: the largest environment's rows (+ the K robots) and one cone list per warp in shared memory
+int world_rvo_shape(nb_world* w, int B) {
+  w->rvo_cap = w->rvo_max_n + w->K;
+  w->rvo_smem = (size_t)w->rvo_cap * (5 * sizeof(double) + nb::kWorldRvoWarps * (6 * sizeof(double) + sizeof(int32_t)));
+  NB_CUDA(cudaFuncSetAttribute(nb::world_rvo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
+  int per_sm = 0, sms = 0;
+  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_rvo_kernel, 32 * nb::kWorldRvoWarps, w->rvo_smem));
+  NB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->cfg.device));
+  if (per_sm < 1) return fail(NB_ERR_CUDA, "world_rvo_kernel: %zu B of shared memory do not fit", w->rvo_smem);
+  w->rvo_grid = std::min(B, per_sm * sms);
+  return NB_OK;
+}
+
+// (Re)allocates the per-robot arrays for B K robots and uploads the rows [start x, y, theta, goal x, y, threshold] (robot k of
+// environment b at row b K + k): every robot at its start, flags and velocities cleared.  The type table is type 0 and types[0 .. T);
+// robot_type NULL: every robot is type 0.
+int world_set_robots(nb_world* w, int B, int K, const double* robots, int T, const nb_world_robot_type* types, const int32_t* robot_type) {
+  const size_t N = (size_t)B * K;
+  std::vector<double> states(3 * N), goal(3 * N);
+  for (size_t n = 0; n < N; ++n)
+    for (int c = 0; c < 3; ++c) { states[3 * n + c] = robots[6 * n + c]; goal[3 * n + c] = robots[6 * n + 3 + c]; }
+  const std::vector<nb::WorldRobotType> table = world_type_table(&w->cfg, T, types);
+  std::vector<int32_t> rtype(N, 0);
+  if (robot_type) rtype.assign(robot_type, robot_type + N);
+  int max_redges = 0;
+  for (int b = 0; K > 1 && b < B; ++b) {
+    int e = 0;
+    for (int k = 0; k < K; ++k) e += table[rtype[(size_t)b * K + k]].nv;
+    max_redges = std::max(max_redges, e);
+  }
+  void* old[] = {w->d_states, w->d_collided, w->d_arrived, w->d_fgoal, w->d_fvel, w->d_types, w->d_rtype};
+  for (void* p : old)
+    if (p) cudaFree(p);
+  w->d_states = w->d_fgoal = w->d_fvel = nullptr;
+  w->d_collided = w->d_arrived = w->d_rtype = nullptr;
+  w->d_types = nullptr;
+  NB_CUDA(dalloc(&w->d_states, 3 * N));
+  NB_CUDA(dalloc(&w->d_collided, N));
+  NB_CUDA(dalloc(&w->d_arrived, N));
+  NB_CUDA(dalloc(&w->d_fgoal, 3 * N));
+  NB_CUDA(dalloc(&w->d_fvel, 2 * N));
+  NB_CUDA(dalloc(&w->d_types, table.size()));
+  NB_CUDA(dalloc(&w->d_rtype, N));
+  NB_CUDA(cudaMemcpy(w->d_states, states.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_fgoal, goal.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_types, table.data(), sizeof(nb::WorldRobotType) * table.size(), cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_rtype, rtype.data(), sizeof(int32_t) * N, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemset(w->d_collided, 0, sizeof(int32_t) * N));
+  NB_CUDA(cudaMemset(w->d_arrived, 0, sizeof(int32_t) * N));
+  NB_CUDA(cudaMemset(w->d_fvel, 0, sizeof(double) * 2 * N));
+  w->K = K;
+  w->max_redges = max_redges;
+  return NB_OK;
+}
+
+nb::WorldParams world_params(const nb_world* w) {
+  nb::WorldParams prm;
+  const nb_world_config& c = w->cfg;
+  prm.B = w->B; prm.R = c.num_beams;
+  prm.dt = c.step_time; prm.range_max = c.range_max; prm.beam_cs = w->d_beam_cs;
+  prm.off_x = c.scan_offset[0]; prm.off_y = c.scan_offset[1]; prm.off_th = c.scan_offset[2];
+  prm.types = w->d_types; prm.rtype = w->d_rtype;
+  prm.obs_begin = w->d_obs_begin; prm.vert_begin = w->d_vert_begin; prm.slot = w->d_slot; prm.counts = w->d_counts; prm.kind = w->d_kind;
+  prm.vertices = w->d_vertices; prm.env = w->d_env; prm.obs = w->d_obs; prm.states = w->d_states;
+  prm.collided = w->d_collided; prm.arrived = w->d_arrived;
+  prm.K = w->K; prm.fgoal = w->d_fgoal; prm.fvel = w->d_fvel;
+  return prm;
+}
+
+// per_robot: the count argument is the robot count N = B K (B itself with one robot per environment); otherwise (the obstacle-side
+// calls) the environment count B
+int world_ready(const nb_world* w, int32_t B, const char* what, bool per_robot = false) {
+  if (!w) return fail(NB_ERR_INVALID, "%s: null handle", what);
+  if (!w->B) return fail(NB_ERR_INVALID, "%s: no scenes set (nb_world_set_scenes)", what);
+  if (per_robot && w->K > 1) {
+    if (B != w->B * w->K)
+      return fail(NB_ERR_INVALID, "%s: count = %d but the world has %d environments x %d robots (N = %d)", what, B, w->B, w->K, w->B * w->K);
+    return NB_OK;
+  }
+  if (B != w->B) return fail(NB_ERR_INVALID, "%s: B = %d but the scenes were set for %d environments", what, B, w->B);
+  return NB_OK;
+}
+
+nb::WorldRvoParams world_rvo_params(const nb_world* w, const float* action) {
+  nb::WorldRvoParams rp;
+  rp.beh = w->d_beh; rp.radius = w->d_rad; rp.goal = w->d_goal; rp.draws = w->d_draws; rp.action = action;
+  rp.seed = w->seed; rp.cap = w->rvo_cap;
+  return rp;
+}
+
+}  // namespace
+
+extern "C" {
+
+int nb_world_create(const nb_world_config* cfg, nb_world_t** out) {
+  if (!out) return fail(NB_ERR_INVALID, "nb_world_create: null argument");
+  *out = nullptr;
+  if (int rc = world_check_config(cfg)) return rc;
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cfg->device < 0 || cfg->device >= ndev)
+    return fail(NB_ERR_NO_DEVICE, "no CUDA device available: neupan_b200 has no CPU fallback");
+  NB_CUDA(cudaSetDevice(cfg->device));
+  nb_world* w = new (std::nothrow) nb_world();
+  if (!w) return fail(NB_ERR_INVALID, "out of host memory");
+  w->cfg = *cfg;
+  // cos / sin of the beam angles a_i = numpy.linspace(angle_min, angle_max, R)[i] (i * step + start, the last one = stop)
+  const int R = cfg->num_beams;
+  const double step = R > 1 ? (cfg->angle_max - cfg->angle_min) / (double)(R - 1) : 0.0;
+  std::vector<double> cs(2 * (size_t)R);
+  for (int i = 0; i < R; ++i) {
+    const double a = R == 1 ? cfg->angle_min : (i == R - 1 ? cfg->angle_max : (double)i * step + cfg->angle_min);
+    cs[2 * i] = std::cos(a);
+    cs[2 * i + 1] = std::sin(a);
+  }
+  cudaError_t e = dalloc(&w->d_beam_cs, cs.size());
+  if (e == cudaSuccess) e = cudaMemcpy(w->d_beam_cs, cs.data(), sizeof(double) * cs.size(), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    nb_world_destroy(w);
+    return fail(NB_ERR_CUDA, "nb_world_create: %s", cudaGetErrorString(e));
+  }
+  *out = w;
+  return NB_OK;
+}
+
+int nb_world_destroy(nb_world_t* w) {
+  if (!w) return NB_OK;
+  cudaSetDevice(w->cfg.device);
+  void* bufs[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
+                  w->d_states, w->d_beam_cs, w->d_beh, w->d_rad, w->d_goal, w->d_draws, w->d_fgoal, w->d_fvel, w->d_types, w->d_rtype};
+  for (void* b : bufs)
+    if (b) cudaFree(b);
+  delete w;
+  return NB_OK;
+}
+
+int nb_world_check_scenes_ex(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                             const double* vertices, const double* envs, const int32_t* obs_kind) {
+  return world_check_scenes(cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, obs_kind, nullptr, nullptr, nullptr, nullptr);
+}
+
+int nb_world_check_scenes(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                          const double* vertices, const double* envs) {
+  return nb_world_check_scenes_ex(cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, nullptr);
+}
+
+int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                           const double* vertices, const double* envs, const int32_t* obs_kind) {
+  if (!w) return fail(NB_ERR_INVALID, "nb_world_set_scenes: null handle");
+  std::vector<int32_t> slot, counts;
+  int max_circ = 0, max_edges = 0;
+  if (int rc = world_check_scenes(&w->cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, obs_kind, &slot, &counts, &max_circ, &max_edges))
+    return rc;
+  const int O = obs_begin[B], V = vert_begin[O];
+  std::vector<double> robots(6 * (size_t)B);  // one robot per environment until nb_world_set_fleet: the env rows' start and goal
+  for (int b = 0; b < B; ++b)
+    for (int c = 0; c < 6; ++c) robots[6 * (size_t)b + c] = envs[(size_t)nb::kWorldEnvCols * b + 4 + c];
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  void* old[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_vertices, w->d_env, w->d_obs,
+                 w->d_beh, w->d_rad, w->d_goal, w->d_draws};
+  for (void* b : old)
+    if (b) cudaFree(b);
+  w->d_obs_begin = w->d_vert_begin = w->d_slot = w->d_counts = w->d_kind = w->d_draws = nullptr;
+  w->d_vertices = w->d_env = w->d_obs = w->d_beh = w->d_rad = w->d_goal = nullptr;
+  w->B = 0;
+  w->has_rvo = false;  // new scenes: every obstacle keeps a constant velocity until nb_world_set_behaviors
+  w->h_obs_begin.assign(obs_begin, obs_begin + B + 1);
+  w->h_vert_begin.assign(vert_begin, vert_begin + O + 1);
+  w->h_vertices.assign(vertices, vertices + 2 * (size_t)V);
+  w->h_env.assign(envs, envs + (size_t)nb::kWorldEnvCols * B);
+  NB_CUDA(dalloc(&w->d_obs_begin, (size_t)B + 1));
+  NB_CUDA(dalloc(&w->d_vert_begin, (size_t)O + 1));
+  NB_CUDA(dalloc(&w->d_slot, (size_t)O));
+  NB_CUDA(dalloc(&w->d_counts, 2 * (size_t)B));
+  NB_CUDA(dalloc(&w->d_kind, (size_t)O));
+  if (O && obs_kind) NB_CUDA(cudaMemcpy(w->d_kind, obs_kind, sizeof(int32_t) * O, cudaMemcpyHostToDevice));
+  else if (O) NB_CUDA(cudaMemset(w->d_kind, 0, sizeof(int32_t) * O));
+  NB_CUDA(dalloc(&w->d_vertices, 2 * (size_t)V));
+  NB_CUDA(dalloc(&w->d_env, (size_t)nb::kWorldEnvCols * B));
+  NB_CUDA(dalloc(&w->d_obs, (size_t)nb::kWorldObsCols * O));
+  NB_CUDA(cudaMemcpy(w->d_obs_begin, obs_begin, sizeof(int32_t) * (B + 1), cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_vert_begin, vert_begin, sizeof(int32_t) * (O + 1), cudaMemcpyHostToDevice));
+  if (O) NB_CUDA(cudaMemcpy(w->d_slot, slot.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_counts, counts.data(), sizeof(int32_t) * 2 * B, cudaMemcpyHostToDevice));
+  if (V) NB_CUDA(cudaMemcpy(w->d_vertices, vertices, sizeof(double) * 2 * V, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(w->d_env, envs, sizeof(double) * nb::kWorldEnvCols * B, cudaMemcpyHostToDevice));
+  if (O) NB_CUDA(cudaMemcpy(w->d_obs, obstacles, sizeof(double) * nb::kWorldObsCols * O, cudaMemcpyHostToDevice));
+  if (int rc = world_set_robots(w, B, 1, robots.data(), 0, nullptr, nullptr)) return rc;
+  w->max_circ = max_circ; w->max_edges = max_edges;
+  if (int rc = world_scan_shape(w, B)) return rc;
+  w->B = B; w->O = O; w->V = V;
+  NB_CUDA(cudaDeviceSynchronize());
+  return NB_OK;
+}
+
+int nb_world_set_scenes(nb_world_t* w, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                        const double* vertices, const double* envs) {
+  return nb_world_set_scenes_ex(w, B, obs_begin, obstacles, vert_begin, vertices, envs, nullptr);
+}
+
+int nb_world_check_behaviors(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                             const double* vertices, const double* envs, const int32_t* obs_kind, const double* behaviors, uint64_t seed) {
+  (void)seed;  // every seed is valid: drawn goals lie in the rectangle by construction
+  if (int rc = world_check_scenes(cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, obs_kind, nullptr, nullptr, nullptr, nullptr)) return rc;
+  return world_check_behaviors(cfg, B, obs_begin, obstacles, envs, behaviors);
+}
+
+int nb_world_set_behaviors(nb_world_t* w, int32_t B, const double* behaviors, uint64_t seed) {
+  if (int rc = world_ready(w, B, "nb_world_set_behaviors")) return rc;
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  const int O = w->O;
+  std::vector<double> obs((size_t)nb::kWorldObsCols * O);
+  if (O) NB_CUDA(cudaMemcpy(obs.data(), w->d_obs, sizeof(double) * obs.size(), cudaMemcpyDeviceToHost));  // the current centres
+  if (int rc = world_check_behaviors(&w->cfg, B, w->h_obs_begin.data(), obs.data(), w->h_env.data(), behaviors)) return rc;
+  // radii (circle: its own; polygon: the largest vertex norm), initial goals (NaN: draw 0) and draw counters
+  std::vector<double> rad(O), goal(2 * (size_t)O, 0.0);
+  std::vector<int32_t> draws(O, 0);
+  bool any = false;
+  int max_n = 0;
+  for (int b = 0; b < B; ++b) {
+    const int o0 = w->h_obs_begin[b], o1 = w->h_obs_begin[b + 1];
+    const double* e = w->h_env.data() + (size_t)nb::kWorldEnvCols * b;
+    max_n = std::max(max_n, o1 - o0);
+    for (int o = o0; o < o1; ++o) {
+      const int v0 = w->h_vert_begin[o], v1 = w->h_vert_begin[o + 1];
+      double r = v0 == v1 ? obs[(size_t)nb::kWorldObsCols * o + 4] : 0.0;
+      for (int k = v0; k < v1; ++k) {
+        const double x = w->h_vertices[2 * k], y = w->h_vertices[2 * k + 1];
+        r = std::max(r, std::sqrt(host_dmul(x, x) + host_dmul(y, y)));
+      }
+      rad[o] = r;
+      const double* row = behaviors + (size_t)nb::kWorldBehCols * o;
+      if (row[0] != 1.0) continue;
+      any = true;
+      if (std::isnan(row[7])) {
+        const uint64_t key = nb::world_rvo_key(seed, b, o - o0);
+        goal[2 * o] = e[0] + host_dmul(nb::world_u01(nb::splitmix64_at(key, 0)), e[2] - e[0]);  // draw 0
+        goal[2 * o + 1] = e[1] + host_dmul(nb::world_u01(nb::splitmix64_at(key, 1)), e[3] - e[1]);
+        draws[o] = 1;
+      } else {
+        goal[2 * o] = row[7]; goal[2 * o + 1] = row[8];
+      }
+    }
+  }
+  void* old[] = {w->d_beh, w->d_rad, w->d_goal, w->d_draws};
+  for (void* p : old)
+    if (p) cudaFree(p);
+  w->d_beh = w->d_rad = w->d_goal = nullptr;
+  w->d_draws = nullptr;
+  w->has_rvo = false;
+  NB_CUDA(dalloc(&w->d_beh, (size_t)nb::kWorldBehCols * O));
+  NB_CUDA(dalloc(&w->d_rad, (size_t)O));
+  NB_CUDA(dalloc(&w->d_goal, 2 * (size_t)O));
+  NB_CUDA(dalloc(&w->d_draws, (size_t)O));
+  if (O) {
+    NB_CUDA(cudaMemcpy(w->d_beh, behaviors, sizeof(double) * nb::kWorldBehCols * O, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemcpy(w->d_rad, rad.data(), sizeof(double) * O, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemcpy(w->d_goal, goal.data(), sizeof(double) * 2 * O, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemcpy(w->d_draws, draws.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice));
+  }
+  w->seed = seed;
+  w->rvo_max_n = max_n;
+  if (int rc = world_rvo_shape(w, B)) return rc;
+  w->has_rvo = any;
+  NB_CUDA(cudaDeviceSynchronize());
+  return NB_OK;
+}
+
+int nb_world_read_behaviors(nb_world_t* w, int32_t B, double* goals, int32_t* draws, void* stream) {
+  if (int rc = world_ready(w, B, "nb_world_read_behaviors")) return rc;
+  if (!w->d_goal) return fail(NB_ERR_INVALID, "nb_world_read_behaviors: no behaviours set (nb_world_set_behaviors)");
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (goals && w->O) NB_CUDA(cudaMemcpyAsync(goals, w->d_goal, sizeof(double) * 2 * w->O, cudaMemcpyDeviceToDevice, st));
+  if (draws && w->O) NB_CUDA(cudaMemcpyAsync(draws, w->d_draws, sizeof(int32_t) * w->O, cudaMemcpyDeviceToDevice, st));
+  return NB_OK;
+}
+
+int nb_world_scan(nb_world_t* w, int32_t B, float* ranges, float* velocity, int32_t* hit, void* stream) {
+  if (int rc = world_ready(w, B, "nb_world_scan", true)) return rc;
+  if (!ranges) return fail(NB_ERR_INVALID, "nb_world_scan: null ranges");
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  // the dynamic shared-memory limit is an attribute of the kernel, shared by every handle of the process: set this handle's
+  // size before each launch (another handle's nb_world_set_scenes may have set a smaller one)
+  NB_CUDA(cudaFuncSetAttribute(nb::world_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
+  nb::world_scan_kernel<<<w->scan_grid, w->scan_threads, w->scan_smem, (cudaStream_t)stream>>>(world_params(w), w->max_circ, w->max_edges,
+                                                                                               w->max_redges, ranges, velocity, hit);
+  ++nb::launches;
+  NB_CUDA(cudaGetLastError());
+  return NB_OK;
+}
+
+int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collided, int32_t* arrived, float* clearance, void* stream) {
+  if (int rc = world_ready(w, B, "nb_world_step", true)) return rc;
+  if (!action) return fail(NB_ERR_INVALID, "nb_world_step: null action");
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  if (w->has_rvo) {  // reactive obstacles choose their velocities from the states at the start of the step
+    NB_CUDA(cudaFuncSetAttribute(nb::world_rvo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
+    nb::world_rvo_kernel<<<w->rvo_grid, 32 * nb::kWorldRvoWarps, w->rvo_smem, (cudaStream_t)stream>>>(world_params(w), world_rvo_params(w, action));
+    ++nb::launches;
+    NB_CUDA(cudaGetLastError());
+  }
+  // a CTA of up to 8 warps per E environments, a warp per robot
+  const int E = nb::world_step_envs(w->K);
+  nb::world_step_kernel<<<(w->B + E - 1) / E, 32 * std::min(E * w->K, nb::kWorldStepMaxWarps), 0, (cudaStream_t)stream>>>(
+      world_params(w), action, collided, arrived, clearance);
+  ++nb::launches;
+  NB_CUDA(cudaGetLastError());
+  return NB_OK;
+}
+
+int nb_world_read_state(nb_world_t* w, int32_t B, double* states, double* obstacles, int32_t* collided, int32_t* arrived, void* stream) {
+  if (int rc = world_ready(w, B, "nb_world_read_state", true)) return rc;
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (states) NB_CUDA(cudaMemcpyAsync(states, w->d_states, sizeof(double) * 3 * B, cudaMemcpyDeviceToDevice, st));
+  if (obstacles && w->O) NB_CUDA(cudaMemcpyAsync(obstacles, w->d_obs, sizeof(double) * nb::kWorldObsCols * w->O, cudaMemcpyDeviceToDevice, st));
+  if (collided) NB_CUDA(cudaMemcpyAsync(collided, w->d_collided, sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
+  if (arrived) NB_CUDA(cudaMemcpyAsync(arrived, w->d_arrived, sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
+  return NB_OK;
+}
+
+int nb_world_check_fleet_ex(const nb_world_config* cfg, int32_t T, const nb_world_robot_type* types, int32_t B, int32_t K, const double* robots,
+                            const int32_t* robot_type) {
+  return world_check_fleet(cfg, T, types, B, K, robots, robot_type);
+}
+
+int nb_world_check_fleet(const nb_world_config* cfg, int32_t B, int32_t K, const double* robots) {
+  return nb_world_check_fleet_ex(cfg, 0, nullptr, B, K, robots, nullptr);
+}
+
+int nb_world_set_fleet_ex(nb_world_t* w, int32_t T, const nb_world_robot_type* types, int32_t B, int32_t K, const double* robots,
+                          const int32_t* robot_type) {
+  if (int rc = world_ready(w, B, "nb_world_set_fleet")) return rc;
+  if (int rc = world_check_fleet(&w->cfg, T, types, B, K, robots, robot_type)) return rc;
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  w->B = 0;  // unusable until the new arrays are in place
+  if (int rc = world_set_robots(w, B, K, robots, T, types, robot_type)) return rc;
+  if (int rc = world_scan_shape(w, B)) return rc;
+  if (w->d_beh)
+    if (int rc = world_rvo_shape(w, B)) return rc;
+  w->B = B;
+  NB_CUDA(cudaDeviceSynchronize());
+  return NB_OK;
+}
+
+int nb_world_set_fleet(nb_world_t* w, int32_t B, int32_t K, const double* robots) {
+  return nb_world_set_fleet_ex(w, 0, nullptr, B, K, robots, nullptr);
+}
+
+}  // extern "C"

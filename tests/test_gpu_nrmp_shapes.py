@@ -1,4 +1,4 @@
-"""The NRMP solve at every instantiation of nrmp_kernel that launch_nrmp (csrc/pan_api.cu) can pick, for the diff, acker and omni
+"""The NRMP solve at every instantiation of nrmp_kernel that launch_nrmp (csrc/nrmp.cu) can pick, for the diff, acker and omni
 robots, against the float64 interior point oracle; with tight, mixed-infinite and negative-d_min bounds, fewer points than M, no
 obstacles at all, the status paths of the generic instantiations, and the persistent-warp schedule.  The case tables, the dispatch
 mirror and the problem builder live in tests/test_oracle_nrmp_shapes.py, which checks them on the CPU.

@@ -1,7 +1,7 @@
 """The NRMP solve at every kernel instantiation, for the three kinematics, and under bound regimes the shipped configurations never
 reach: the case tables and the problem builder of tests/test_gpu_nrmp_shapes.py, and their checks on the CPU.
 
-launch_nrmp (csrc/pan_api.cu) sends a handle to one of nine instantiations nrmp_kernel<HPL, SMALL, TT, MM>, chosen from the
+launch_nrmp (csrc/nrmp.cu) sends a handle to one of nine instantiations nrmp_kernel<HPL, SMALL, TT, MM>, chosen from the
 horizon T, nrmp_max_num M and TM = T M; the kinematics is a run-time branch inside every one of them.  `instantiation` mirrors
 that table.  Every shape of SHAPES runs with the diff (C4), acker (C2) and omni (C5) robot, each config with its own robot and
 checkpoint.  Obstacle coefficients fa / fb come from the float64 oracle's DUNE selection, so the NRMP solve is compared on its own,
@@ -54,7 +54,7 @@ REGIMES = {
 
 
 def instantiation(T, M):
-    """(HPL, SMALL, TT, MM) of the nrmp_kernel that launch_nrmp (csrc/pan_api.cu) launches for horizon T and nrmp_max_num M."""
+    """(HPL, SMALL, TT, MM) of the nrmp_kernel that launch_nrmp (csrc/nrmp.cu) launches for horizon T and nrmp_max_num M."""
     if (T, M) == (10, 10):
         return (4, True, 10, 10)
     if (T, M) == (15, 10):

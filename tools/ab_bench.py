@@ -1,7 +1,7 @@
 """A/B timing of build variants in ONE process launch per variant (saves gpurun round trips).
 
     # here (no GPU): build the default library plus variants that differ by -D flags on one translation unit
-    python tools/ab_bench.py build  nrmp7:pan_api.cu:-DNB_SOME_FLAG=1  tcx:dune_tc.cu:-DNB_OTHER=2
+    python tools/ab_bench.py build  nrmp7:nrmp.cu:-DNB_SOME_FLAG=1  tcx:dune_tc.cu:-DNB_OTHER=2
     # on the GPU machine: time the default and every built variant with bench.py
     python tools/ab_bench.py run --steps 6 --warmup 3
 
