@@ -107,3 +107,17 @@ int launch_nrmp_backward(NrmpAdjParams a, int K, int rec_envs, const float* grad
 }
 
 }  // namespace nb
+
+#if NB_NRMP_PHASES
+// timing builds only (NB_NRMP_PHASES, tools/nrmp_bench.py --phases): copies the 8 phase counters of nrmp_kernel.cuh to `out` (host),
+// then zeroes them when `reset` is set.  Not part of the public header.
+extern "C" int nb_nrmp_read_phases(unsigned long long* out, int reset) {
+  if (cudaDeviceSynchronize() != cudaSuccess) return NB_ERR_CUDA;
+  if (out && cudaMemcpyFromSymbol(out, nb::nb_nrmp_phase_cycles, sizeof(nb::nb_nrmp_phase_cycles)) != cudaSuccess) return NB_ERR_CUDA;
+  if (reset) {
+    const unsigned long long zero[8] = {};
+    if (cudaMemcpyToSymbol(nb::nb_nrmp_phase_cycles, zero, sizeof(zero)) != cudaSuccess) return NB_ERR_CUDA;
+  }
+  return NB_OK;
+}
+#endif

@@ -66,7 +66,6 @@ __host__ __device__ inline size_t nrmp_warp_doubles(int T, int M) {
   n += 4 * (size_t)mb;             // s, z, ds, dz of the box / rate / D rows
   n += ((size_t)mb + 1) / 2;       // is (float)
   n += (size_t)TM;                 // fax, fay (float)
-  n += ((size_t)mb + 7) / 8;       // row-enable flags (bytes)
   return n + 1;
 }
 __host__ __device__ inline size_t nrmp_cta_extra_bytes(int T) {  // pair table (uint16) shared by the CTA's warps

@@ -34,6 +34,33 @@
 namespace nb {
 
 #define NB_LL(i, n) _Pragma("unroll 1") for (int i = lane; i < (n); i += 32)
+// the lane loop of the interior point iteration: with compile-time shapes (kFixed, nrmp_solve_env) it has a fixed trip count, is
+// unrolled, and each step is predicated on the lane's row existing; otherwise it is NB_LL
+#define NB_LW(i, n)                                                                 \
+  _Pragma("unroll(kLaneUnroll)") for (int i##_b = kFixed ? 0 : lane; i##_b < (n); i##_b += 32) \
+    if (const int i = i##_b + (kFixed ? lane : 0); i < (n))
+
+// NB_NRMP_PHASES (timing only, off by default): each warp adds the clock64() cycles it spends in the setup (sections 1-5) and in
+// the phases (a)-(e) of the interior point iteration to nb_nrmp_phase_cycles[0..5], [6] counts the iterations that ran (e) and
+// [7] the setups.  Read back through nb_nrmp_read_phases (nrmp.cu); tools/nrmp_bench.py --phases builds and reads that variant.
+// The arithmetic is untouched, so results are the same with the flag on.
+#ifndef NB_NRMP_PHASES
+#define NB_NRMP_PHASES 0
+#endif
+#if NB_NRMP_PHASES
+__device__ unsigned long long nb_nrmp_phase_cycles[8];
+#define NB_PHASE(p)                                                                                    \
+  do {                                                                                                 \
+    const long long now_ = clock64();                                                                  \
+    if (lane == 0) atomicAdd(&nb_nrmp_phase_cycles[p], (unsigned long long)(now_ - phase_t0));         \
+    if (lane == 0 && ((p) == 0 || (p) == 5)) atomicAdd(&nb_nrmp_phase_cycles[(p) == 0 ? 7 : 6], 1ull); \
+    phase_t0 = clock64();                                                                              \
+  } while (0)
+#else
+#define NB_PHASE(p) \
+  do {              \
+  } while (0)
+#endif
 
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
@@ -208,7 +235,7 @@ __device__ __forceinline__ bool nrmp_block_cholesky(double (&w0)[NT * (NT + 1) /
 // workspace offset, loop bound and row stride folds into immediates -- half of the generic kernel's
 // instructions were integer address arithmetic.
 // Residency: the (10, 10) specialisation is built for 5 CTAs of 3 warps (15 warps) per SM (NB_NRMP_WPC) -- 128 registers with
-// ~240 B of spill stores, and ~43 KB of shared memory per CTA, which also caps the SM at 15 warps.  At B = 4096 that is 1980
+// ~220 B of spill stores, and ~43 KB of shared memory per CTA, which also caps the SM at 15 warps.  At B = 4096 that is 1980
 // resident solves on 132 SMs.  (__maxnreg__(144) instead of the min-blocks bound makes ptxas spill more.)
 template <int HPL, bool SMALL, int TT, int MM>
 __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int b, double* wsp, const unsigned short* __restrict__ ptab, const int lane) {
@@ -218,6 +245,9 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
   const int oBU = 0, oBL = nU, oRU = 2 * nU, oRL = oRU + nR, oDU = oRL + nR, oDL = oDU + TD;
   const int mb = oDL + TD;
   auto hrow = [](int i) { return (i * (i + 3)) >> 1; };  // offset of row i of the lower-triangular H / L
+#if NB_NRMP_PHASES
+  long long phase_t0 = clock64();
+#endif
 #ifndef NB_NRMP_DMMA
 #define NB_NRMP_DMMA 1
 #endif
@@ -239,6 +269,11 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
   // compile-time (T, M) with DMMA assembly: the Hessian tiles stay in the accumulators and are factored there (nrmp_block_cholesky)
   constexpr bool kBlockChol = NB_NRMP_BLOCKCHOL != 0 && NB_NRMP_DMMA != 0 && SMALL && TT > 0 && MM > 0;
   constexpr int kNT = TT > 0 ? (2 * TT + 7) / 8 : 1, kTiles = kNT * (kNT + 1) / 2;
+  // compile-time (T, M): the phases of the iteration run as fixed-trip, unrolled code with immediate shared-memory offsets; what
+  // depends on the lane's row is a predicate, not a loop bound.  Every floating-point operation and its order are those of the
+  // lane-bounded loops the generic instantiations run.
+  constexpr bool kFixed = TT > 0;
+  constexpr int kLaneUnroll = kFixed ? 8 : 1;
 
   // ---- carve this warp's workspace -------------------------------------------------------
   const int FT = T * (T + 1);                      // packed size of one component of F / G
@@ -274,7 +309,6 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
   float* cis = reinterpret_cast<float*>(wsp);  wsp += (mb + 1) / 2;  // inverse slacks
   float* fax_s = reinterpret_cast<float*>(wsp);
   float* fay_s = fax_s + TM;
-  unsigned char* cen = reinterpret_cast<unsigned char*>(fay_s + TM);  // 1 for rows whose bound is finite, else 0
   // setup-only linearisation data lives in the scratch region
   double* a02 = scratch;      double* a12 = scratch + T;  double* Bm = scratch + 2 * T;  double* Cm = scratch + 8 * T;
   double* gam_b = scratch + 11 * T;
@@ -290,13 +324,12 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
   const double rho = prm.ro, eta = (double)prm.eta;
   const double dlo = fmax((double)prm.d_min, 0.0), dhi = (double)prm.d_max;
   const bool dfix = TD > 0 && dhi == dlo;  // d_max == d_min: D is a constant, its bound rows and its Newton block drop out
-  NB_LL(k, mb) {  // rows of the shared-memory constraint block that are switched on
-    bool on = !dfix;  // D rows
-    if (k < oRU) on = en_speed[(k % nU) & 1];
-    else if (k < oDU) on = en_acce[((k - oRU) % nR) & 1];
-    cen[k] = on ? 1 : 0;
-  }
-  auto enabled = [&](int k) -> bool { return cen[k] != 0; };
+  // rows of the shared-memory constraint block that are switched on: a row's class (box, rate, D) follows from k, and its control
+  // component is k & 1 (the box and rate blocks start at even offsets and have even lengths nU and nR)
+  auto enabled = [&](int k) -> bool {
+    const bool c1 = (k & 1) != 0;
+    return k < oRU ? (c1 ? en_speed[1] : en_speed[0]) : (k < oDU ? (c1 ? en_acce[1] : en_acce[0]) : !dfix);
+  };
   int m_active = (dfix ? 0 : 2 * TD) + TM;
   for (int c = 0; c < 2; ++c) m_active += (en_speed[c] ? 2 * T : 0) + (en_acce[c] ? 2 * (T - 1) : 0);
   const double inv_m = 1.0 / (double)(m_active > 0 ? m_active : 1);
@@ -516,6 +549,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
     }
   }
   __syncwarp();
+  NB_PHASE(0);
 
   // ---- 6. interior point iterations -------------------------------------------------------------
   converged = false;
@@ -531,7 +565,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
         if (k < TM) tmpk[k] = hz[q_];
       }
       __syncwarp();
-      NB_LL(t, TD) {
+      NB_LW(t, TD) {
         double gx = 0, gy = 0, sz = 0;
         for (int mm = 0; mm < M; ++mm) {
           const int k = t * M + mm;
@@ -543,9 +577,20 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
       }
       __syncwarp();
       double res = 0.0, gsum = 0.0;
-      NB_LL(i, nU) {
+      NB_LW(i, nU) {
         double acc = cv[i];
-        {
+        if constexpr (kFixed) {
+          // row i of the packed lower triangle (Hc[i(i+1)/2 + j], j <= i), then column i below the diagonal (Hc[j(j+1)/2 + i],
+          // j > i): the two parts are independent FMA chains
+          const double* hp = Hc + i * (i + 1) / 2;
+          double accq = 0.0;
+#pragma unroll
+          for (int j = 0; j < nU; ++j) {
+            if (j <= i) acc += hp[j] * x[j];
+            else accq += Hc[j * (j + 1) / 2 + i] * x[j];
+          }
+          acc += accq;
+        } else {
           const double* hp = Hc + i * (i + 1) / 2;  // row i of the packed lower triangle, then column i below the diagonal
           const double* hq = hp + i + i + 1;        // element (i+1, i)
           double accq = 0.0;                        // the two parts are independent FMA chains
@@ -559,18 +604,24 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
         if (i >= 2) acc += cz[oRU + i - 2] - cz[oRL + i - 2];
         if (i < nR) acc -= cz[oRU + i] - cz[oRL + i];
         if (TD > 0) {
-          const double* fxp = F + (i >> 1) * ((i >> 1) + 1) + i;
-          const double* fyp = fxp + FT;
           double accy = 0.0;
+          if constexpr (kFixed) {
+#pragma unroll
+            for (int t = 0; t < T; ++t)  // F_t has columns [0, 2t + 2)
+              if (i < 2 * t + 2) { acc -= F[t * (t + 1) + i] * e0[t]; accy -= F[FT + t * (t + 1) + i] * e1[t]; }
+          } else {
+            const double* fxp = F + (i >> 1) * ((i >> 1) + 1) + i;
+            const double* fyp = fxp + FT;
 #pragma unroll 2
-          for (int t = i >> 1; t < T; ++t) { acc -= fxp[0] * e0[t]; accy -= fyp[0] * e1[t]; fxp += 2 * (t + 1); fyp += 2 * (t + 1); }
+            for (int t = i >> 1; t < T; ++t) { acc -= fxp[0] * e0[t]; accy -= fyp[0] * e1[t]; fxp += 2 * (t + 1); fyp += 2 * (t + 1); }
+          }
           acc += accy;
         }
         rdU[i] = acc;
         res = fmax(res, fabs(acc));
       }
-      if (!dfix) NB_LL(t, TD) res = fmax(res, fabs(rdD[t]));
-      NB_LL(k, mb) if (enabled(k)) gsum += cs[k] * cz[k];
+      if (!dfix) NB_LW(t, TD) res = fmax(res, fabs(rdD[t]));
+      NB_LW(k, mb) if (enabled(k)) gsum += cs[k] * cz[k];
 #pragma unroll
       for (int q_ = 0; q_ < HPL; ++q_)
         if (lane + 32 * q_ < TM) gsum += hs[q_] * hz[q_];
@@ -585,6 +636,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
       // abandoned for a cold start -- rare (<1 % on C4), but one 60-iteration straggler would set the duration of the launch
       if (warm && ((it == 12 && gap > 1e-5) || (it == prm.warm_check_it && gap > prm.warm_check_gap))) { restart = true; break; }
       accept_gap = gap < 1e-9 && res < 10.0 * res_tol;  // good enough to keep if the next factorisation fails in rounding noise
+      NB_PHASE(1);
 
       // (b) barrier weights; hinge rows publish omega for the per-step reductions
       __syncwarp();
@@ -595,7 +647,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
       // acceleration-limited) that grew to 3e-1 with a tighter gap; a pinned direction held by 1e9 instead of infinity moves the
       // result by 1e-7.  A weight that grows with z instead (z^2 / 1e-10) leaves a row held by a small multiplier soft: z = 4e-4
       // gave W = 1.6e3 and a 3.6e-2 error of the chain gradient (C4 `obstacles`, env 141 of 1024).
-      NB_LL(k, mb) {
+      NB_LW(k, mb) {
         if (finishing && enabled(k)) {
           const double sk = cs[k], zk = cz[k];
           cis[k] = (float)(zk > sk ? 1e9 / zk : 1.0 / sk);
@@ -614,7 +666,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
         }
       }
       __syncwarp();
-      NB_LL(t, TD) {
+      NB_LW(t, TD) {
         double a00 = 0, a01 = 0, a11 = 0, b0 = 0, b1 = 0, nn = 0;
         for (int mm = 0; mm < M; ++mm) {
           const int k = t * M + mm;
@@ -639,17 +691,30 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
         }
       }
       __syncwarp();
+      NB_PHASE(2);
       double tl0[kTiles], tl1[kTiles];  // kBlockChol: the Hessian tiles of (c), factored in place by (d)
       if (kDmma) {
         // V (packed like F, in the Gx | Gy scratch): row 2t = r00 Fx_t + r01 Fy_t, row 2t+1 = r11 Fy_t
-        NB_LL(j, nU) {
-          int o = (j >> 1) * ((j >> 1) + 1) + j;
+        NB_LW(j, nU) {
+          if constexpr (kFixed) {
+#pragma unroll
+            for (int t = 0; t < T; ++t) {
+              if (j < 2 * t + 2) {
+                const int o = t * (t + 1) + j;
+                const double fx = F[o], fy = F[FT + o];
+                Gx[o] = N00[t] * fx + N01[t] * fy;
+                Gy[o] = N11[t] * fy;
+              }
+            }
+          } else {
+            int o = (j >> 1) * ((j >> 1) + 1) + j;
 #pragma unroll 2
-          for (int t = j >> 1; t < T; ++t) {
-            const double fx = F[o], fy = F[FT + o];
-            Gx[o] = N00[t] * fx + N01[t] * fy;
-            Gy[o] = N11[t] * fy;
-            o += 2 * (t + 1);
+            for (int t = j >> 1; t < T; ++t) {
+              const double fx = F[o], fy = F[FT + o];
+              Gx[o] = N00[t] * fx + N01[t] * fy;
+              Gy[o] = N11[t] * fy;
+              o += 2 * (t + 1);
+            }
           }
         }
         __syncwarp();
@@ -735,6 +800,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
       }
       }
       __syncwarp();
+      NB_PHASE(3);
       // (d) Cholesky.  kBlockChol: blocked, on the tiles of (c) (nrmp_block_cholesky).  Otherwise left-looking; lane owns rows
       //     lane, lane+32; inverse diagonal in registers.  SMALL: two columns per step (nU = 2T is even) -- row i is read once
       //     for both dot products, which are two independent FMA chains; the second column then takes the rank-1 correction
@@ -826,6 +892,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
 #if NB_NRMP_CHOL_TWICE
       }
 #endif
+      NB_PHASE(4);
       if (bad) {  // H lost definiteness: at barrier weights of 1e13+ that is rounding, and the iterate is already the optimum
         if (accept_gap) converged = true;
         else stat |= 2;
@@ -834,7 +901,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
 
       if (finishing) { converged = true; have_factor = true; break; }
       // (e) predictor (pass 0) and corrector (pass 1) share one Newton body
-      NB_LL(k, mb) cdz[k] = enabled(k) ? -cs[k] * cz[k] : 0.0;
+      NB_LW(k, mb) cdz[k] = enabled(k) ? -cs[k] * cz[k] : 0.0;
 #pragma unroll
       for (int q_ = 0; q_ < HPL; ++q_) hdz[q_] = -hs[q_] * hz[q_];
       double alpha = 1.0;
@@ -853,7 +920,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
           }
         }
         __syncwarp();
-        NB_LL(t, TD) {
+        NB_LW(t, TD) {
           double Y0 = 0, Y1 = 0, Ys = 0;
           for (int mm = 0; mm < M; ++mm) {
             const int k = t * M + mm;
@@ -877,11 +944,17 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
             if (i >= 2) acc -= cdz[oRU + i - 2] * (double)cis[oRU + i - 2] - cdz[oRL + i - 2] * (double)cis[oRL + i - 2];
             if (i < nR) acc += cdz[oRU + i] * (double)cis[oRU + i] - cdz[oRL + i] * (double)cis[oRL + i];
             if (TD > 0) {
-              const double* fxp = F + (i >> 1) * ((i >> 1) + 1) + i;
-              const double* fyp = fxp + FT;
               double accy = 0.0;
+              if constexpr (kFixed) {
+#pragma unroll
+                for (int t = 0; t < T; ++t)  // F_t has columns [0, 2t + 2)
+                  if (i < 2 * t + 2) { acc += F[t * (t + 1) + i] * e0[t]; accy += F[FT + t * (t + 1) + i] * e1[t]; }
+              } else {
+                const double* fxp = F + (i >> 1) * ((i >> 1) + 1) + i;
+                const double* fyp = fxp + FT;
 #pragma unroll 2
-              for (int t = i >> 1; t < T; ++t) { acc += fxp[0] * e0[t]; accy += fyp[0] * e1[t]; fxp += 2 * (t + 1); fyp += 2 * (t + 1); }
+                for (int t = i >> 1; t < T; ++t) { acc += fxp[0] * e0[t]; accy += fyp[0] * e1[t]; fxp += 2 * (t + 1); fyp += 2 * (t + 1); }
+              }
               acc += accy;
             }
             if (sl == 0) r0 = acc; else r1 = acc;
@@ -925,14 +998,20 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
         if (lane < nU) dU[lane] = r0;
         if (!SMALL && lane + 32 < nU) dU[lane + 32] = r1;
         __syncwarp();
-        NB_LL(t, TD) {
+        NB_LW(t, TD) {
           double ax = 0, ay = 0;
           const double* fxp = F + t * (t + 1);
           const double* fyp = fxp + FT;
+          if constexpr (kFixed) {
+#pragma unroll
+            for (int i = 0; i < nU; ++i)
+              if (i < 2 * t + 2) { ax += fxp[i] * dU[i]; ay += fyp[i] * dU[i]; }
+          } else {
 #pragma unroll 2
-          for (int i = 0; i < 2 * (t + 1); ++i) {
-            ax += fxp[i] * dU[i];
-            ay += fyp[i] * dU[i];
+            for (int i = 0; i < 2 * (t + 1); ++i) {
+              ax += fxp[i] * dU[i];
+              ay += fyp[i] * dU[i];
+            }
           }
           qx[t] = ax; qy[t] = ay;
           dD[t] = (bD[t] + n0[t] * ax + n1[t] * ay) * iHDD[t];
@@ -953,7 +1032,7 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
             ratio = fmaxf(ratio, fmaxf(-(float)hds[q_] * his[q_], -(float)hdz[q_] * rcpf(hz[q_])));
           }
         }
-        NB_LL(i, nU) {
+        NB_LW(i, nU) {
           const double d = dU[i];
           cdz[oBU + i] = (cdz[oBU + i] + cz[oBU + i] * d) * (double)cis[oBU + i]; cds[oBU + i] = -d;
           cdz[oBL + i] = (cdz[oBL + i] - cz[oBL + i] * d) * (double)cis[oBL + i]; cds[oBL + i] = d;
@@ -963,13 +1042,13 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
             cdz[oRL + i] = (cdz[oRL + i] - cz[oRL + i] * dd) * (double)cis[oRL + i]; cds[oRL + i] = dd;
           }
         }
-        NB_LL(t, TD) {
+        NB_LW(t, TD) {
           const double d = dD[t];
           cdz[oDU + t] = (cdz[oDU + t] + cz[oDU + t] * d) * (double)cis[oDU + t]; cds[oDU + t] = -d;
           cdz[oDL + t] = (cdz[oDL + t] - cz[oDL + t] * d) * (double)cis[oDL + t]; cds[oDL + t] = d;
         }
         __syncwarp();
-        NB_LL(k, mb) {
+        NB_LW(k, mb) {
           if (!enabled(k)) continue;
           ratio = fmaxf(ratio, fmaxf(-(float)cds[k] * cis[k], -(float)cdz[k] * rcpf(cz[k])));
         }
@@ -977,27 +1056,28 @@ __device__ __forceinline__ void nrmp_solve_env(const NrmpParams& prm, const int 
         if (pass == 0) {
           const double amax = ratio > 1.0f ? 1.0 / (double)ratio : 1.0;  // largest step <= 1 keeping s, z >= 0
           double ga = 0.0;
-          NB_LL(k, mb) if (enabled(k)) ga += (cs[k] + amax * cds[k]) * (cz[k] + amax * cdz[k]);
+          NB_LW(k, mb) if (enabled(k)) ga += (cs[k] + amax * cds[k]) * (cz[k] + amax * cdz[k]);
 #pragma unroll
           for (int q_ = 0; q_ < HPL; ++q_)
             if (lane + 32 * q_ < TM) ga += (hs[q_] + amax * hds[q_]) * (hz[q_] + amax * hdz[q_]);
           const double sr = fmax(warp_sum(ga) * inv_m, 0.0) / gap;
           const double smu = sr * sr * sr * gap;  // sigma * mu
-          NB_LL(k, mb) cdz[k] = enabled(k) ? (-cs[k] * cz[k] + smu - cds[k] * cdz[k]) : 0.0;
+          NB_LW(k, mb) cdz[k] = enabled(k) ? (-cs[k] * cz[k] + smu - cds[k] * cdz[k]) : 0.0;
 #pragma unroll
           for (int q_ = 0; q_ < HPL; ++q_) hdz[q_] = -hs[q_] * hz[q_] + smu - hds[q_] * hdz[q_];
         } else {
           alpha = ratio > 0.995f ? 0.995 / (double)ratio : 1.0;
         }
       }
-      NB_LL(i, nU) x[i] += alpha * dU[i];
-      NB_LL(t, TD) Dv[t] += alpha * dD[t];
-      NB_LL(k, mb) if (enabled(k)) { cs[k] += alpha * cds[k]; cz[k] += alpha * cdz[k]; }
+      NB_LW(i, nU) x[i] += alpha * dU[i];
+      NB_LW(t, TD) Dv[t] += alpha * dD[t];
+      NB_LW(k, mb) if (enabled(k)) { cs[k] += alpha * cds[k]; cz[k] += alpha * cdz[k]; }
 #pragma unroll
       for (int q_ = 0; q_ < HPL; ++q_) {
         if (lane + 32 * q_ < TM) { hs[q_] += alpha * hds[q_]; hz[q_] += alpha * hdz[q_]; }
       }
       __syncwarp();
+      NB_PHASE(5);
     }
     if (!converged && !(stat & 2) && !restart) stat |= 1;
   }
@@ -1243,5 +1323,7 @@ __global__ void __launch_bounds__(128) nrmp_stop_kernel(const NrmpParams prm) {
   nrmp_stop_env<0, 0>(prm, b, lane);
 }
 
+#undef NB_PHASE
+#undef NB_LW
 #undef NB_LL
 }  // namespace nb

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Times the NRMP solve alone (nb_nrmp_forward) at the shapes of a benchmark workload, on obstacle coefficients made once per input set.
 
-    python tools/nrmp_bench.py [--workload C4] [--envs B] [--reps 20] [--warmup 3] [--dump DIR] [--split]
+    python tools/nrmp_bench.py [--workload C4] [--envs B] [--reps 20] [--warmup 3] [--dump DIR] [--split] [--phases]
 
 The inputs are bench.py's (tests/helpers.make_inputs, two sets of distinct environments).  For each set, nb_dune_forward runs once
 and the obstacle coefficients of the NRMP program are formed on the device from its selection (nrmp.py:220-261, as
@@ -11,10 +11,14 @@ launches alternate between the sets with a 256 MiB L2 flush before each, outside
 Prints one JSON line: ms per launch (mean, min, max), mean / max interior point iterations (nb_pan_read_diagnostics), status
 count, the card's name, power limit and SM clock.  --dump DIR writes S, U, D, ipm_iters and status of set 0 as DIR/<name>.npy, so
 two builds can be compared output for output.  --split adds a second JSON line: torch.profiler's per-kernel device time of a
-bench.py-shaped control step (K PAN iterations, two overlapped sub-batches) of the same workload.
+bench.py-shaped control step (K PAN iterations, two overlapped sub-batches) of the same workload.  --phases times a build of the
+library with -DNB_NRMP_PHASES=1 instead (made and cached under neupan_b200/lib/phases/ when its sources changed) and adds the mean
+clock64() cycles per warp of the setup (per solve) and of the phases (a)-(e) of the interior point iteration (per iteration) to the
+line; the timers' atomics lengthen that build's launch a little.
 """
 import argparse
 import ctypes as C
+import hashlib
 import json
 import os
 import subprocess
@@ -36,6 +40,37 @@ def gpu_info():
         return dict(gpu=name, power_limit=plim, sm_clock=sm, sm_max_clock=smmax)
     except Exception as e:  # noqa: BLE001 -- reported, not fatal
         return dict(gpu=torch.cuda.get_device_name(0), power_limit=None, sm_clock=None, sm_max_clock=None, nvidia_smi=str(e))
+
+
+PHASES = ("setup", "a_residual_gap", "b_weights_2x2", "c_V_dmma_assembly", "d_cholesky", "e_newton_passes")
+
+
+def phases_lib():
+    """libneupan_b200.so with nrmp.cu compiled with -DNB_NRMP_PHASES=1, rebuilt when the sources change."""
+    from neupan_b200 import build as nb
+
+    nb.build()
+    out = os.path.join(nb.LIBDIR, "phases")
+    lib, stamp = os.path.join(out, "libneupan_b200.so"), os.path.join(out, "build.stamp")
+    digest = hashlib.sha256(nb._sources_digest().encode() + b"NB_NRMP_PHASES").hexdigest()
+    if os.path.exists(lib) and os.path.exists(stamp) and open(stamp).read().strip() == digest:
+        return lib
+    os.makedirs(out, exist_ok=True)
+    obj = os.path.join(out, "nrmp.o")
+    nvcc = nb._nvcc()
+    subprocess.run([nvcc, *nb.ARCH, *nb.COMMON, "-DNB_NRMP_PHASES=1", "-c", os.path.join(nb.CSRC, "nrmp.cu"), "-o", obj], check=True)
+    subprocess.run([nvcc, *nb.ARCH, "-shared", "-o", lib, *[obj if u == "nrmp.cu" else nb.obj_path(u) for u in nb.UNITS]], check=True)
+    with open(stamp, "w") as f:
+        f.write(digest)
+    return lib
+
+
+def read_phases(lib, reset):
+    from neupan_b200 import _lib
+
+    buf = (C.c_ulonglong * 8)()
+    _lib.check(lib.nb_nrmp_read_phases(buf, int(reset)))
+    return [int(v) for v in buf]
 
 
 def coefficients(sel, h, T, M):
@@ -62,8 +97,13 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--dump", default=None, metavar="DIR")
     ap.add_argument("--split", action="store_true", help="also print torch.profiler's per-kernel split of a bench.py-shaped step")
+    ap.add_argument("--phases", action="store_true", help="time the NB_NRMP_PHASES build and report cycles per phase")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "nrmp_bench.py times the device"
+    if args.phases:
+        from neupan_b200 import _lib
+
+        _lib.LIB_PATH = phases_lib()  # before the first _lib.load()
 
     from gpu_helpers import make_pan
     from helpers import CONFIGS, make_inputs
@@ -98,6 +138,9 @@ def main():
         flush.zero_()
         launch(sets[i % 2])
     torch.cuda.synchronize()
+    if args.phases:
+        lib.nb_nrmp_read_phases.restype, lib.nb_nrmp_read_phases.argtypes = C.c_int, [C.c_void_p, C.c_int]
+        read_phases(lib, True)
     ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.reps)]
     iters = []
     for i in range(args.reps):
@@ -116,6 +159,13 @@ def main():
     line = dict(metric="nb_nrmp_forward ms per launch", workload=f"{args.workload} {cfg.name}", envs=B, T=T, M=M, reps=args.reps, warmup=args.warmup,
                 ms_per_launch=float(ms.mean()), ms_min=float(ms.min()), ms_max=float(ms.max()), ipm_iters_mean=float(it_all.mean()),
                 ipm_iters_max=int(it_all.max()), envs_with_status=bad, lib=os.path.basename(_lib.LIB_PATH), **gpu_info())
+    if args.phases:
+        cyc = read_phases(lib, True)
+        iters_, solves = max(cyc[6], 1), max(cyc[7], 1)
+        line["phase_cycles"] = dict(setup_per_solve=cyc[0] / solves, **{k: cyc[i] / iters_ for i, k in enumerate(PHASES) if i > 0})
+        line["phase_cycles"]["iteration_total"] = sum(cyc[1:6]) / iters_
+        line["phase_counts"] = dict(solves=cyc[7], iterations=cyc[6])
+        line["lib"] = "phases/" + line["lib"]
     print(json.dumps(line), flush=True)
 
     if args.dump:
