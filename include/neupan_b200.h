@@ -427,6 +427,36 @@ int nb_world_check_fleet_ex(const nb_world_config* cfg, int32_t T, const nb_worl
 int nb_world_set_fleet_ex(nb_world_t* w, int32_t T, const nb_world_robot_type* types, int32_t B, int32_t K, const double* robots,
                           const int32_t* robot_type);
 
+/* Occupancy maps (this project's reading of IR-SIM's `world: obstacle_map:`; semantics in csrc/world_kernel.cuh): a static grid of
+ * width x height square cells of side `resolution` (m), origin (x, y) the lower-left corner of cell (0, 0); cells outside the grid
+ * are free.  Each environment uses at most one map and may use none; maps never move and are not obstacles (the obstacle rows of
+ * nb_world_read_state do not change; reactive obstacles do not see maps and moving obstacles pass over them).
+ *   maps (P) HOST; bits uint32 HOST: the maps back to back, each `height` rows of ceil(width/32) words, row j being y index j, bit
+ *   (i mod 32) of word i/32 being cell (i, j) (padding bits 0); env_map (B) int32 HOST: each environment's map, -1 for none;
+ *   window (0, 10] m, for the whole handle.
+ *   scan    a beam also stops where it crosses from a free into an occupied cell or back (the first t > 0, corners count), with
+ *           hit index O_b + K (after the obstacles and the robots, which win a tie) and velocity 0
+ *   step    each robot's clearance is also bounded by m = min(window, its exact clearance to the occupied cells, each a square);
+ *           m <= 0 sets collided
+ * nb_world_set_maps comes after nb_world_set_scenes(_ex) and, if used, nb_world_set_fleet(_ex), which both drop the maps (a new
+ * placement needs a new start check); behaviours are untouched.  It uploads the maps, checks them against the robots the handle
+ * has placed, and synchronises the device.  A world without maps launches the same kernels as before.
+ * Checks (NB_ERR_INVALID, naming the map, environment or robot): P in 1..max_envs; width and height in 1..8192; a finite origin;
+ * a finite resolution >= 0.01; no padding bit set; env_map entries in -1..P-1; window in (0, 10]; no start body that overlaps or
+ * touches an occupied cell of its environment's map (SAT, each robot's own polygon).  nb_world_check_maps performs them on the
+ * host without a handle or a device; its first arguments are those of nb_world_check_fleet_ex (robots NULL: the maps are checked
+ * without the start bodies).  Maps too large for the device fail with NB_ERR_CUDA and leave the handle usable, without maps. */
+typedef struct nb_world_map {
+  int32_t width, height;           /* cells, 1..8192 each */
+  double origin[2];                /* the lower-left corner of cell (0, 0) */
+  double resolution;               /* the side of a cell (m), >= 0.01 */
+} nb_world_map;
+
+int nb_world_check_maps(const nb_world_config* cfg, int32_t T, const nb_world_robot_type* types, int32_t B, int32_t K, const double* robots,
+                        const int32_t* robot_type, int32_t P, const nb_world_map* maps, const uint32_t* bits, const int32_t* env_map,
+                        double window);
+int nb_world_set_maps(nb_world_t* w, int32_t P, const nb_world_map* maps, const uint32_t* bits, const int32_t* env_map, double window);
+
 /* ---- DUNE training on the device (SURVEY 8f "next" row 4) ------------------------------------------------------------ */
 
 /* DUNETrain.generate_data_set / prob_solve (neupan/blocks/dune_train.py:100-140): labels of n sampled points -- the solution of the

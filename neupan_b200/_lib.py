@@ -71,6 +71,11 @@ class WorldRobotType(C.Structure):
     _fields_ = [("kinematics", C.c_int32), ("num_vertices", C.c_int32), ("wheelbase", C.c_double), ("vertices", C.c_double * 16)]
 
 
+class WorldMap(C.Structure):
+    """struct nb_world_map (include/neupan_b200.h)."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("origin", C.c_double * 2), ("resolution", C.c_double)]
+
+
 _FP = C.c_void_p  # device or host float* / int32*: passed as raw addresses
 
 # name -> (restype, argtypes); every symbol include/neupan_b200.h declares
@@ -117,6 +122,9 @@ SYMBOLS = {
     "nb_world_set_fleet": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _FP]),
     "nb_world_check_fleet_ex": (C.c_int, [C.POINTER(WorldConfig), C.c_int32, _FP, C.c_int32, C.c_int32, _FP, _FP]),
     "nb_world_set_fleet_ex": (C.c_int, [C.c_void_p, C.c_int32, _FP, C.c_int32, C.c_int32, _FP, _FP]),
+    "nb_world_check_maps": (C.c_int, [C.POINTER(WorldConfig), C.c_int32, _FP, C.c_int32, C.c_int32, _FP, _FP, C.c_int32, _FP, _FP, _FP,
+                                      C.c_double]),
+    "nb_world_set_maps": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, C.c_double]),
     "nb_dune_labels": (C.c_int, [C.c_int32, _FP, _FP, C.c_int64, _FP, _FP, _FP, _FP, C.c_void_p]),
     "nb_dune_train_create": (C.c_int, [C.c_int32, _FP, _FP, _FP, C.c_int64, C.c_int32, C.POINTER(C.c_void_p)]),
     "nb_dune_train_destroy": (C.c_int, [C.c_void_p]),

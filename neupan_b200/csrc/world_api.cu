@@ -42,6 +42,17 @@ struct nb_world {
   nb::WorldRobotType* d_types = nullptr;
   int32_t* d_rtype = nullptr;
   int max_redges = 0;
+  // host copies of the placed robots (nb_world_set_maps checks the start bodies against them): rows, types 1..T, each robot's type
+  std::vector<double> h_robots;
+  std::vector<nb_world_robot_type> h_types;
+  std::vector<int32_t> h_rtype;
+  // occupancy maps (nb_world_set_maps; nb_world_set_scenes(_ex) and nb_world_set_fleet(_ex) drop them): has_map false -> the
+  // kernels' map-free instantiations
+  bool has_map = false;
+  nb::WorldMap* d_maps = nullptr;
+  uint32_t* d_bits = nullptr;
+  int32_t* d_env_map = nullptr;
+  double window = 0.0;
 };
 
 namespace {
@@ -318,17 +329,107 @@ int world_check_fleet(const nb_world_config* cfg, int32_t T, const nb_world_robo
   return NB_OK;
 }
 
+// Grid line k of a map axis, rounded as the kernels round it (world_map_line), and the clamped floor index of world_map_floor.
+double map_line(double lo, double r, int k) { return lo + host_dmul((double)k, r); }
+int map_floor(double s, double lo, double r, int n) {
+  const double f = std::floor((s - lo) / r);
+  return f < -1.0 ? -1 : (f > (double)n ? n : (int)f);
+}
+
+// Every check of nb_world_set_maps on the host (robots NULL: without the start bodies).  Fills the device table when asked to.
+int world_check_maps(const nb_world_config* cfg, int32_t T, const nb_world_robot_type* types, int32_t B, int32_t K, const double* robots,
+                     const int32_t* robot_type, int32_t P, const nb_world_map* maps, const uint32_t* bits, const int32_t* env_map, double window,
+                     std::vector<nb::WorldMap>* table) {
+  if (robots) {
+    if (int rc = world_check_fleet(cfg, T, types, B, K, robots, robot_type)) return rc;
+  } else {
+    if (int rc = world_check_config(cfg)) return rc;
+    if (B < 1 || B > cfg->max_envs) return fail(NB_ERR_INVALID, "B = %d outside [1, max_envs = %d]", B, cfg->max_envs);
+  }
+  if (!maps || !bits || !env_map) return fail(NB_ERR_INVALID, "nb_world maps: null argument");
+  if (P < 1 || P > cfg->max_envs) return fail(NB_ERR_INVALID, "P = %d maps outside [1, max_envs = %d]", P, cfg->max_envs);
+  std::vector<nb::WorldMap> t(P);
+  int64_t off = 0;
+  for (int p = 0; p < P; ++p) {
+    const nb_world_map& m = maps[p];
+    if (m.width < 1 || m.width > nb::kWorldMaxMapSide || m.height < 1 || m.height > nb::kWorldMaxMapSide)
+      return fail(NB_ERR_INVALID, "map %d: width %d and height %d must be in 1..%d", p, m.width, m.height, nb::kWorldMaxMapSide);
+    if (!world_finite(m.origin, 2)) return fail(NB_ERR_INVALID, "map %d: the origin is not finite", p);
+    if (!(std::isfinite(m.resolution) && m.resolution >= 0.01)) return fail(NB_ERR_INVALID, "map %d: the resolution must be finite and >= 0.01 m (got %g)", p, m.resolution);
+    const int words = (m.width + 31) / 32;
+    if (m.width % 32)
+      for (int j = 0; j < m.height; ++j)
+        if (bits[off + (int64_t)j * words + words - 1] >> (m.width % 32))
+          return fail(NB_ERR_INVALID, "map %d: row %d has padding bits set past width %d", p, j, m.width);
+    t[p] = nb::WorldMap{m.origin[0], m.origin[1], m.resolution, off, m.width, m.height, words, 0};
+    off += (int64_t)m.height * words;
+  }
+  for (int b = 0; b < B; ++b)
+    if (env_map[b] < -1 || env_map[b] >= P) return fail(NB_ERR_INVALID, "environment %d: map %d outside -1..%d", b, env_map[b], P - 1);
+  if (!(window > 0.0 && window <= 10.0)) return fail(NB_ERR_INVALID, "window = %g outside (0, 10] m", window);
+  if (robots) {  // no start body may overlap or touch an occupied cell (the fleet check's SAT and bodies)
+    const std::vector<nb::WorldRobotType> tt = world_type_table(cfg, T, types);
+    double body[2 * nb::kWorldMaxVertices];
+    for (int b = 0; b < B; ++b) {
+      if (env_map[b] < 0) continue;
+      const nb::WorldMap& m = t[env_map[b]];
+      for (int k = 0; k < K; ++k) {
+        const double* r = robots + 6 * ((size_t)b * K + k);
+        const nb::WorldRobotType& ty = tt[robot_type ? robot_type[(size_t)b * K + k] : 0];
+        const double c = std::cos(r[2]), s = std::sin(r[2]);
+        double xmin = INFINITY, xmax = -INFINITY, ymin = INFINITY, ymax = -INFINITY;
+        for (int v = 0; v < ty.nv; ++v) {
+          const double px = ty.v[2 * v], py = ty.v[2 * v + 1];
+          body[2 * v] = r[0] + (c * px - s * py);
+          body[2 * v + 1] = r[1] + (s * px + c * py);
+          xmin = std::min(xmin, body[2 * v]); xmax = std::max(xmax, body[2 * v]);
+          ymin = std::min(ymin, body[2 * v + 1]); ymax = std::max(ymax, body[2 * v + 1]);
+        }
+        const int i0 = std::max(map_floor(xmin, m.x0, m.r, m.W) - 1, 0), i1 = std::min(map_floor(xmax, m.x0, m.r, m.W) + 1, m.W - 1);
+        const int j0 = std::max(map_floor(ymin, m.y0, m.r, m.H) - 1, 0), j1 = std::min(map_floor(ymax, m.y0, m.r, m.H) + 1, m.H - 1);
+        for (int j = j0; j <= j1; ++j)
+          for (int i = i0; i <= i1; ++i) {
+            if (!((bits[m.off + (int64_t)j * m.words + (i >> 5)] >> (i & 31)) & 1u)) continue;
+            const double xa = map_line(m.x0, m.r, i), xb = map_line(m.x0, m.r, i + 1), ya = map_line(m.y0, m.r, j), yb = map_line(m.y0, m.r, j + 1);
+            const double cell[8] = {xa, ya, xb, ya, xb, yb, xa, yb};
+            if (world_bodies_meet(body, ty.nv, cell, 4))
+              return fail(NB_ERR_INVALID, "environment %d, robot %d: the start body overlaps or touches occupied cell (%d, %d) of map %d", b, k, i, j, env_map[b]);
+          }
+      }
+    }
+  }
+  if (table) *table = std::move(t);
+  return NB_OK;
+}
+
+// Frees the maps: the kernels' map-free instantiations from here on.
+void world_drop_maps(nb_world* w) {
+  void* old[] = {w->d_maps, w->d_bits, w->d_env_map};
+  for (void* p : old)
+    if (p) cudaFree(p);
+  w->d_maps = nullptr; w->d_bits = nullptr; w->d_env_map = nullptr;
+  w->has_map = false;
+}
+
+nb::WorldMapParams world_map_params(const nb_world* w) { return nb::WorldMapParams{w->d_maps, w->d_bits, w->d_env_map, w->window}; }
+
+template <bool kMap>
+int world_scan_occupancy(nb_world* w, int* per_sm) {
+  // the occupancy query sees the kernel's current limit; nb_world_scan sets it again before every launch
+  NB_CUDA(cudaFuncSetAttribute(nb::world_scan_kernel<kMap>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
+  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, nb::world_scan_kernel<kMap>, w->scan_threads, w->scan_smem));
+  return NB_OK;
+}
+
 // scan launch shape: the largest environment's circles and edges (and with K > 1 the K robot bodies) in shared memory, one thread
-// per beam of the environment's K R beams (at most 256)
+// per beam of the environment's K R beams (at most 256); the instantiation with maps when the handle has any
 int world_scan_shape(nb_world* w, int B) {
   const int nre = w->K > 1 ? w->max_redges : 0;
   w->scan_smem = (size_t)w->max_circ * (3 * sizeof(double) + sizeof(int32_t)) + (size_t)w->max_edges * (4 * sizeof(double) + sizeof(int32_t)) +
                  (size_t)nre * (4 * sizeof(double) + sizeof(int32_t));
   w->scan_threads = std::min(256, std::max(32, (w->K * w->cfg.num_beams + 31) / 32 * 32));
-  // the occupancy query sees the kernel's current limit; nb_world_scan sets it again before every launch
-  NB_CUDA(cudaFuncSetAttribute(nb::world_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
   int per_sm = 0, sms = 0;
-  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_scan_kernel, w->scan_threads, w->scan_smem));
+  if (int rc = w->has_map ? world_scan_occupancy<true>(w, &per_sm) : world_scan_occupancy<false>(w, &per_sm)) return rc;
   NB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->cfg.device));
   if (per_sm < 1) return fail(NB_ERR_CUDA, "world_scan_kernel: %zu B of shared memory do not fit", w->scan_smem);
   w->scan_grid = std::min(B, per_sm * sms);
@@ -387,6 +488,9 @@ int world_set_robots(nb_world* w, int B, int K, const double* robots, int T, con
   NB_CUDA(cudaMemset(w->d_fvel, 0, sizeof(double) * 2 * N));
   w->K = K;
   w->max_redges = max_redges;
+  w->h_robots.assign(robots, robots + 6 * N);
+  w->h_types.assign(types, types + T);
+  w->h_rtype = rtype;
   return NB_OK;
 }
 
@@ -463,7 +567,8 @@ int nb_world_destroy(nb_world_t* w) {
   if (!w) return NB_OK;
   cudaSetDevice(w->cfg.device);
   void* bufs[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
-                  w->d_states, w->d_beam_cs, w->d_beh, w->d_rad, w->d_goal, w->d_draws, w->d_fgoal, w->d_fvel, w->d_types, w->d_rtype};
+                  w->d_states, w->d_beam_cs, w->d_beh, w->d_rad, w->d_goal, w->d_draws, w->d_fgoal, w->d_fvel, w->d_types, w->d_rtype,
+                  w->d_maps, w->d_bits, w->d_env_map};
   for (void* b : bufs)
     if (b) cudaFree(b);
   delete w;
@@ -500,6 +605,7 @@ int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, c
   w->d_vertices = w->d_env = w->d_obs = w->d_beh = w->d_rad = w->d_goal = nullptr;
   w->B = 0;
   w->has_rvo = false;  // new scenes: every obstacle keeps a constant velocity until nb_world_set_behaviors
+  world_drop_maps(w);  // and has no map until nb_world_set_maps
   w->h_obs_begin.assign(obs_begin, obs_begin + B + 1);
   w->h_vert_begin.assign(vert_begin, vert_begin + O + 1);
   w->h_vertices.assign(vertices, vertices + 2 * (size_t)V);
@@ -618,9 +724,10 @@ int nb_world_scan(nb_world_t* w, int32_t B, float* ranges, float* velocity, int3
   NB_CUDA(cudaSetDevice(w->cfg.device));
   // the dynamic shared-memory limit is an attribute of the kernel, shared by every handle of the process: set this handle's
   // size before each launch (another handle's nb_world_set_scenes may have set a smaller one)
-  NB_CUDA(cudaFuncSetAttribute(nb::world_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
-  nb::world_scan_kernel<<<w->scan_grid, w->scan_threads, w->scan_smem, (cudaStream_t)stream>>>(world_params(w), w->max_circ, w->max_edges,
-                                                                                               w->max_redges, ranges, velocity, hit);
+  auto* kernel = w->has_map ? nb::world_scan_kernel<true> : nb::world_scan_kernel<false>;
+  NB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
+  kernel<<<w->scan_grid, w->scan_threads, w->scan_smem, (cudaStream_t)stream>>>(world_params(w), world_map_params(w), w->max_circ, w->max_edges,
+                                                                                w->max_redges, ranges, velocity, hit);
   ++nb::launches;
   NB_CUDA(cudaGetLastError());
   return NB_OK;
@@ -638,8 +745,9 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
   }
   // a CTA of up to 8 warps per E environments, a warp per robot
   const int E = nb::world_step_envs(w->K);
-  nb::world_step_kernel<<<(w->B + E - 1) / E, 32 * std::min(E * w->K, nb::kWorldStepMaxWarps), 0, (cudaStream_t)stream>>>(
-      world_params(w), action, collided, arrived, clearance);
+  auto* kernel = w->has_map ? nb::world_step_kernel<true> : nb::world_step_kernel<false>;
+  kernel<<<(w->B + E - 1) / E, 32 * std::min(E * w->K, nb::kWorldStepMaxWarps), 0, (cudaStream_t)stream>>>(world_params(w), world_map_params(w),
+                                                                                                          action, collided, arrived, clearance);
   ++nb::launches;
   NB_CUDA(cudaGetLastError());
   return NB_OK;
@@ -671,6 +779,7 @@ int nb_world_set_fleet_ex(nb_world_t* w, int32_t T, const nb_world_robot_type* t
   if (int rc = world_check_fleet(&w->cfg, T, types, B, K, robots, robot_type)) return rc;
   NB_CUDA(cudaSetDevice(w->cfg.device));
   w->B = 0;  // unusable until the new arrays are in place
+  world_drop_maps(w);  // the new starts need a new map check
   if (int rc = world_set_robots(w, B, K, robots, T, types, robot_type)) return rc;
   if (int rc = world_scan_shape(w, B)) return rc;
   if (w->d_beh)
@@ -682,6 +791,41 @@ int nb_world_set_fleet_ex(nb_world_t* w, int32_t T, const nb_world_robot_type* t
 
 int nb_world_set_fleet(nb_world_t* w, int32_t B, int32_t K, const double* robots) {
   return nb_world_set_fleet_ex(w, 0, nullptr, B, K, robots, nullptr);
+}
+
+int nb_world_check_maps(const nb_world_config* cfg, int32_t T, const nb_world_robot_type* types, int32_t B, int32_t K, const double* robots,
+                        const int32_t* robot_type, int32_t P, const nb_world_map* maps, const uint32_t* bits, const int32_t* env_map,
+                        double window) {
+  return world_check_maps(cfg, T, types, B, K, robots, robot_type, P, maps, bits, env_map, window, nullptr);
+}
+
+int nb_world_set_maps(nb_world_t* w, int32_t P, const nb_world_map* maps, const uint32_t* bits, const int32_t* env_map, double window) {
+  if (!w) return fail(NB_ERR_INVALID, "nb_world_set_maps: null handle");
+  if (int rc = world_ready(w, w->B, "nb_world_set_maps")) return rc;
+  std::vector<nb::WorldMap> table;
+  if (int rc = world_check_maps(&w->cfg, (int32_t)w->h_types.size(), w->h_types.data(), w->B, w->K, w->h_robots.data(), w->h_rtype.data(), P, maps,
+                                bits, env_map, window, &table))
+    return rc;
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  world_drop_maps(w);
+  const size_t words = (size_t)(table.back().off + (int64_t)table.back().H * table.back().words);
+  cudaError_t e = nb::dalloc(&w->d_maps, table.size());
+  if (e == cudaSuccess) e = nb::dalloc(&w->d_bits, words);
+  if (e == cudaSuccess) e = nb::dalloc(&w->d_env_map, (size_t)w->B);
+  if (e == cudaSuccess) e = cudaMemcpy(w->d_maps, table.data(), sizeof(nb::WorldMap) * table.size(), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(w->d_bits, bits, sizeof(uint32_t) * words, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(w->d_env_map, env_map, sizeof(int32_t) * w->B, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {  // the handle stays usable, without maps
+    cudaGetLastError();
+    world_drop_maps(w);
+    if (int rc = world_scan_shape(w, w->B)) return rc;
+    return fail(NB_ERR_CUDA, "nb_world_set_maps: %zu words of maps: %s", words, cudaGetErrorString(e));
+  }
+  w->has_map = std::any_of(env_map, env_map + w->B, [](int32_t m) { return m >= 0; });
+  w->window = window;
+  if (int rc = world_scan_shape(w, w->B)) return rc;
+  NB_CUDA(cudaDeviceSynchronize());
+  return NB_OK;
 }
 
 }  // extern "C"

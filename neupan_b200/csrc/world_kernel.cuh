@@ -26,6 +26,25 @@
 // the last step (0 before the first step and once it has collided; translation only, omega x r left out).  collided is sticky and
 // freezes a robot, which stays in the scene; arrived is sticky and an arrived robot stays in the scene.
 //
+// Occupancy maps (nb_world_set_maps; this project's reading of IR-SIM's `world: obstacle_map:`): an environment may carry one static
+// grid of W x H square cells of side r whose origin (x0, y0) is the lower-left corner of cell (0, 0); cell (i, j) is
+// [X(i), X(i+1)] x [Y(j), Y(j+1)] with X(i) = dadd(x0, dmul((double)i, r)), Y(j) likewise -- every corner is computed this way,
+// nothing is accumulated.  Cells outside the grid are free (a border is a wall only if the map draws one).  A map is a kind of
+// scene, not an obstacle: the obstacle rows do not change, and reactive obstacles do not see it and moving obstacles pass over it.
+// Both kernels take the map path as a compile-time variant (kMap), launched only when some environment of the handle has a map:
+//   scan  after the shape and robot tests, the beam walks the grid cell by cell (world_map_cast) and reports the first t > 0 at
+//         which it crosses from a cell of one state into a cell of the other, with index O_b + K (after the obstacles and the
+//         robots, so at equal t they win and the walk stops at the current best) and velocity 0.  Every crossing is
+//         (boundary - s) / d from the cell index.  The sensor's cell is (floor((s_x - x0) / r), ...) corrected by one step so that
+//         X(i) <= s_x < X(i+1): a sensor on a grid line lies in the cell above / to the right of it, and a beam running along that
+//         line sees that row (column) only.  At a corner (t_x == t_y) the beam enters the x-neighbour, the y-neighbour and the
+//         diagonal cell at once: a crossing if any of the three differs, and the walk continues from the diagonal cell.  A sensor
+//         outside the grid enters through its box; a sensor in an occupied cell sees the exit crossing.
+//   step  m = min(window, the clearance to the occupied cells that meet the robot's world bounding box grown by window, each
+//         cell a 4-vertex CCW polygon through world_convex_clearance), which is the exact clearance to the map whenever it is
+//         <= window; the robot's clearance is min(obstacles, robots, m) and m <= 0 sets collided.
+// There is no sub-cell geometry.
+//
 // All arithmetic is FP64 with explicit rounding (__dmul_rn / __dadd_rn / __dsub_rn: no FMA contraction), so that oracle/world.py,
 // which performs the same operations in the same order in numpy, agrees to the last bit wherever the inputs agree (the only
 // differences come from CUDA's sin / cos / tan vs libm).
@@ -79,11 +98,94 @@ struct WorldParams {
   double* fvel;                           // (B K, 2) world-frame velocity of each robot's last step
 };
 
+constexpr int kWorldMaxMapSide = 8192;  // cells per side of an occupancy map
+
+// One occupancy map (nb_world_map) as the kernels read it: rows of `words` = ceil(W / 32) uint32 words from bits + off, row j
+// being y index j, bit (i mod 32) of word i / 32 being cell (i, j).
+struct WorldMap {
+  double x0, y0, r;
+  int64_t off;
+  int32_t W, H, words, pad_;
+};
+
+struct WorldMapParams {
+  const WorldMap* maps;     // (P)
+  const uint32_t* bits;     // every map's words back to back
+  const int32_t* env_map;   // (B) the environment's map, -1 for none
+  double window;            // the step's search distance (0, 10] m
+};
+
 __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
 __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
 __device__ __forceinline__ double ddot(double ax, double ay, double bx, double by) { return dadd(dmul(ax, bx), dmul(ay, by)); }
 __device__ __forceinline__ double dcross(double ax, double ay, double bx, double by) { return dsub(dmul(ax, by), dmul(ay, bx)); }
+
+// ---- occupancy maps ---------------------------------------------------------------------------------------------------------
+
+// grid line k of an axis: lo + k r (X(k) or Y(k))
+__device__ __forceinline__ double world_map_line(double lo, double r, int k) { return dadd(lo, dmul((double)k, r)); }
+
+// floor((s - lo) / r) clamped to -1..n (every index past either end is a free cell alike)
+__device__ __forceinline__ int world_map_floor(double s, double lo, double r, int n) {
+  const double f = floor(dsub(s, lo) / r);
+  return f < -1.0 ? -1 : (f > (double)n ? n : (int)f);
+}
+
+__device__ __forceinline__ bool world_map_occupied(const WorldMap& m, const uint32_t* bits, int i, int j) {
+  if (i < 0 || i >= m.W || j < 0 || j >= m.H) return false;
+  return (__ldg(bits + m.off + (int64_t)j * m.words + (i >> 5)) >> (i & 31)) & 1u;
+}
+
+// The cell of coordinate s on an axis of n cells: world_map_floor, corrected by one step so that line(i) <= s < line(i + 1)
+__device__ __forceinline__ int world_map_cell(double s, double lo, double r, int n) {
+  int i = world_map_floor(s, lo, r, n);
+  if (i > -1 && s < world_map_line(lo, r, i)) --i;
+  else if (i < n && s >= world_map_line(lo, r, i + 1)) ++i;
+  return i;
+}
+
+// The next grid line that a ray from s along d (in cell i of n) crosses on this axis: t = (line(k) - s) / d, and ni the cell past
+// it (an index before the grid jumps to its first line); INFINITY when d == 0
+__device__ __forceinline__ double world_map_next(double s, double d, double lo, double r, int i, int n, int& ni) {
+  int k;
+  if (d > 0.0) { k = i < 0 ? 0 : i + 1; ni = k; }
+  else if (d < 0.0) { k = i >= n ? n : i; ni = k - 1; }
+  else return INFINITY;
+  return dsub(world_map_line(lo, r, k), s) / d;
+}
+
+// The first t in (0, lim) at which the ray s + t d crosses from a cell of one state into a cell of the other (the corner rule of
+// the header), INFINITY when there is none before lim.  Each t comes from the cell index, none is accumulated.
+__device__ __forceinline__ double world_map_cast(const WorldMap& m, const uint32_t* bits, double sx, double sy, double dx, double dy,
+                                                 double lim) {
+  int i = world_map_cell(sx, m.x0, m.r, m.W), j = world_map_cell(sy, m.y0, m.r, m.H), ni = i, nj = j;
+  bool cur = world_map_occupied(m, bits, i, j);
+  double tx = world_map_next(sx, dx, m.x0, m.r, i, m.W, ni), ty = world_map_next(sy, dy, m.y0, m.r, j, m.H, nj);
+  while (true) {
+    // outside the grid on an axis and not heading into it: every cell left is free
+    if ((i < 0 && !(dx > 0.0)) || (i >= m.W && !(dx < 0.0)) || (j < 0 && !(dy > 0.0)) || (j >= m.H && !(dy < 0.0))) break;
+    const double t = fmin(tx, ty);
+    if (!(t < lim)) break;
+    bool changed;
+    if (tx < ty) {
+      const bool s = world_map_occupied(m, bits, ni, j);
+      changed = s != cur; cur = s; i = ni;
+      tx = world_map_next(sx, dx, m.x0, m.r, i, m.W, ni);
+    } else if (ty < tx) {
+      const bool s = world_map_occupied(m, bits, i, nj);
+      changed = s != cur; cur = s; j = nj;
+      ty = world_map_next(sy, dy, m.y0, m.r, j, m.H, nj);
+    } else {  // a corner: the x-neighbour, the y-neighbour and the diagonal cell at once
+      const bool a = world_map_occupied(m, bits, ni, j), c = world_map_occupied(m, bits, i, nj), s = world_map_occupied(m, bits, ni, nj);
+      changed = a != cur || c != cur || s != cur; cur = s; i = ni; j = nj;
+      tx = world_map_next(sx, dx, m.x0, m.r, i, m.W, ni);
+      ty = world_map_next(sy, dy, m.y0, m.r, j, m.H, nj);
+    }
+    if (changed && t > 0.0) return t;
+  }
+  return INFINITY;
+}
 
 // ---- lidar ----------------------------------------------------------------------------------------------------------------
 
@@ -95,8 +197,10 @@ __device__ __forceinline__ double dcross(double ax, double ay, double bx, double
 // the exit crossing); t >= range_max or no crossing is a miss: range_max, velocity 0, hit -1.  Equal t: the lower index wins
 // (obstacles 0..O_b - 1, then robot j as O_b + j), so the result does not depend on the order of the tests.
 // max_redges: the largest environment's robot edge count (the sum of its robots' vertex counts with K > 1, else 0); robot k's edges
-// follow those of robots 0 .. k - 1, each robot's polygon that of its own type.
-__global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, int max_circ, int max_edges, int max_redges,
+// follow those of robots 0 .. k - 1, each robot's polygon that of its own type.  kMap: then the environment's map (world_map_cast,
+// index O_b + K, velocity 0); mp is not read without it.
+template <bool kMap>
+__global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, const WorldMapParams mp, int max_circ, int max_edges, int max_redges,
                                                          float* __restrict__ ranges, float* __restrict__ velocity, int32_t* __restrict__ hit) {
   extern __shared__ double wsm[];
   __shared__ double s_sx[kWorldMaxFleet], s_sy[kWorldMaxFleet], s_hc[kWorldMaxFleet], s_hs[kWorldMaxFleet];  // sensor poses
@@ -206,12 +310,21 @@ __global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, 
           if (u >= 0.0 && u <= 1.0 && t > 0.0 && (t < best || (t == best && id < bid))) { best = t; bid = id; }
         }
       }
+      if constexpr (kMap) {  // the highest index: only a strictly closer crossing counts, so the walk stops at best
+        const int mi = mp.env_map[b];
+        if (mi >= 0) {
+          const double t = world_map_cast(mp.maps[mi], mp.bits, sx, sy, dx, dy, fmin(best, prm.range_max));
+          if (t < best) { best = t; bid = nobs + K; }
+        }
+      }
       if (!(best < prm.range_max)) { best = prm.range_max; bid = -1; }
       const size_t n = (size_t)b * K + k;
       ranges[n * R + i] = (float)best;
       if (velocity) {
         float vx = 0.f, vy = 0.f;
-        if (bid >= nobs) {
+        if (kMap && bid == nobs + K) {
+          // the map does not move
+        } else if (bid >= nobs) {
           const double* fv = prm.fvel + 2 * ((size_t)b * K + (bid - nobs));
           vx = (float)fv[0]; vy = (float)fv[1];
         } else if (bid >= 0) {
@@ -408,19 +521,65 @@ __device__ __forceinline__ double world_obstacle_clearance(const WorldParams& pr
   return d;
 }
 
-// Robot <-> robot (both convex): 0 unless an edge normal of either separates them (both SAT orders), else the smallest vertex-edge
-// distance both ways.  Swapping a and b evaluates the same tests and distances and reduces them with fmin, so the result is
-// symmetric bit for bit: two robots that touch collide in the same step.
-__device__ __forceinline__ double world_robot_clearance(const WorldRobot& a, const WorldRobot& b) {
+// Convex <-> convex: 0 unless an edge normal of either separates them (both SAT orders), else the smallest vertex-edge distance both
+// ways.  Swapping a and b evaluates the same tests and distances and reduces them with fmin, so the result is symmetric bit for
+// bit: two robots that touch collide in the same step.
+template <class PA, class PB>
+__device__ __forceinline__ double world_convex_clearance(const PA& a, const PB& b) {
   if (!(world_sat_separates(a, b) || world_sat_separates(b, a))) return 0.0;
   double d = INFINITY;
   for (int k = 0; k < b.nv; ++k) {
     const int k1 = k + 1 < b.nv ? k + 1 : 0;
-    for (int i = 0; i < a.nv; ++i) d = fmin(d, world_seg_dist(a.x[i], a.y[i], b.x[k], b.y[k], b.x[k1], b.y[k1]));
+    for (int i = 0; i < a.nv; ++i) d = fmin(d, world_seg_dist(a.vx(i), a.vy(i), b.vx(k), b.vy(k), b.vx(k1), b.vy(k1)));
   }
   for (int k = 0; k < a.nv; ++k) {
     const int k1 = k + 1 < a.nv ? k + 1 : 0;
-    for (int i = 0; i < b.nv; ++i) d = fmin(d, world_seg_dist(b.x[i], b.y[i], a.x[k], a.y[k], a.x[k1], a.y[k1]));
+    for (int i = 0; i < b.nv; ++i) d = fmin(d, world_seg_dist(b.vx(i), b.vy(i), a.vx(k), a.vy(k), a.vx(k1), a.vy(k1)));
+  }
+  return d;
+}
+
+// Robot <-> robot
+__device__ __forceinline__ double world_robot_clearance(const WorldRobot& a, const WorldRobot& b) { return world_convex_clearance(a, b); }
+
+// An occupancy cell [xa, xb] x [ya, yb] as a convex polygon: (xa, ya), (xb, ya), (xb, yb), (xa, yb) (CCW)
+struct WorldCell {
+  double xa, ya, xb, yb;
+  static constexpr int nv = 4;
+  __device__ __forceinline__ double vx(int k) const { return (k == 1 || k == 2) ? xb : xa; }
+  __device__ __forceinline__ double vy(int k) const { return k >= 2 ? yb : ya; }
+};
+
+// The robot's (world vertices rx, ry) smallest clearance, clamped at 0, to the occupied cells of map m that meet its bounding box
+// grown by window (widened by one cell on each side, so that rounding cannot drop a cell within window); lane `lane` of the warp
+// takes the (row, word) pairs lane, lane + 32, ... of that range, skips zero words and visits the set bits.  INFINITY for none.
+__device__ __forceinline__ double world_map_clearance(const WorldMap& m, const uint32_t* bits, double window, const double* rx, const double* ry,
+                                                      int nr, int lane) {
+  double xmin = rx[0], xmax = rx[0], ymin = ry[0], ymax = ry[0];
+  for (int k = 1; k < nr; ++k) {
+    xmin = fmin(xmin, rx[k]); xmax = fmax(xmax, rx[k]);
+    ymin = fmin(ymin, ry[k]); ymax = fmax(ymax, ry[k]);
+  }
+  const int i0 = max(world_map_floor(dsub(xmin, window), m.x0, m.r, m.W) - 1, 0);
+  const int i1 = min(world_map_floor(dadd(xmax, window), m.x0, m.r, m.W) + 1, m.W - 1);
+  const int j0 = max(world_map_floor(dsub(ymin, window), m.y0, m.r, m.H) - 1, 0);
+  const int j1 = min(world_map_floor(dadd(ymax, window), m.y0, m.r, m.H) + 1, m.H - 1);
+  double d = INFINITY;
+  if (i0 > i1 || j0 > j1) return d;
+  const int w0 = i0 >> 5, nw = (i1 >> 5) - w0 + 1;
+  for (int p = lane; p < (j1 - j0 + 1) * nw; p += 32) {
+    const int j = j0 + p / nw, wd = w0 + p % nw, lo = i0 - 32 * wd, hi = i1 - 32 * wd;
+    uint32_t word = __ldg(bits + m.off + (int64_t)j * m.words + wd);
+    if (lo > 0) word &= ~0u << lo;
+    if (hi < 31) word &= (2u << hi) - 1u;
+    while (word) {
+      const int i = 32 * wd + __ffs(word) - 1;
+      word &= word - 1u;
+      const WorldCell c{world_map_line(m.x0, m.r, i), world_map_line(m.y0, m.r, j), world_map_line(m.x0, m.r, i + 1),
+                        world_map_line(m.y0, m.r, j + 1)};
+      const double cc = world_convex_clearance(WorldRobot{rx, ry, nr}, c);
+      d = fmin(d, cc > 0.0 ? cc : 0.0);
+    }
   }
   return d;
 }
@@ -431,8 +590,10 @@ __device__ __forceinline__ double world_robot_clearance(const WorldRobot& a, con
 // Phase 2, after the barrier: one warp per robot (warp w takes slots w, w + 8; a 512-thread CTA would cap the registers at 128 and
 // spill) computes its clearance to every obstacle of its environment (lanes over the obstacles: the circle, convex and outline
 // branches of world_obstacle_clearance) and to every other robot of it (lane j), a warp min, and lane 0 writes the collision flag,
-// the clearance and the velocity the scan reports for the robot (0 once collided).
-__global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(const WorldParams prm, const float* __restrict__ action,
+// the clearance and the velocity the scan reports for the robot (0 once collided).  kMap: the warp also takes min(window, the
+// clearance to the environment's map) (world_map_clearance) into the warp min; mp is not read without it.
+template <bool kMap>
+__global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(const WorldParams prm, const WorldMapParams mp, const float* __restrict__ action,
                                                                            int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived,
                                                                            float* __restrict__ clearance) {
   __shared__ double f_x[kWorldMaxFleet][kWorldMaxVertices], f_y[kWorldMaxFleet][kWorldMaxVertices];  // E K <= 8 or K <= 16 slots
@@ -488,6 +649,10 @@ __global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(con
     if (lane < K && lane != k) {  // each side with its own vertex count: symmetric bit for bit across types too
       const double c = world_robot_clearance(WorldRobot{f_x[s], f_y[s], nr}, WorldRobot{f_x[s0 + lane], f_y[s0 + lane], f_nv[s0 + lane]});
       best = fmin(best, c > 0.0 ? c : 0.0);
+    }
+    if constexpr (kMap) {
+      const int mi = mp.env_map[b];
+      if (mi >= 0) best = fmin(best, fmin(mp.window, world_map_clearance(mp.maps[mi], mp.bits, mp.window, f_x[s], f_y[s], nr, lane)));
     }
 #pragma unroll
     for (int m = 16; m >= 1; m >>= 1) best = fmin(best, __shfl_xor_sync(0xffffffffu, best, m));

@@ -20,6 +20,13 @@ A scene (one environment) is a dict with the sections of an ``env.yaml``:
     path            optional (n, 4) rows [x, y, theta, gear]: an initial path for the planner (the scene builders add one)
     robots          in place of start / goal / goal_threshold / path: a list of K (1..16) dicts with those four keys, the robots of
                     the environment (every scene of a batch has the same K)
+    map             optional static occupancy grid {"occupancy": (H, W) bool array, row 0 the lowest y, "origin": (x, y) the
+                    lower-left corner of cell (0, 0), "resolution": r the side of a cell in m} (1..8192 cells per side, r >= 0.01):
+                    this project's reading of IR-SIM's ``world: obstacle_map:``.  Cells outside the grid are free.  The lidar sees
+                    where a beam crosses from a free into an occupied cell (hit index O_b + K, velocity 0), the step takes the exact
+                    clearance to the occupied cells within ``map_window`` of each robot (csrc/world_kernel.cuh states the rules).
+                    Reactive obstacles do not see the map and moving obstacles pass over it.  Scenes that share one occupancy array
+                    (the same object, origin and resolution) share one copy of it on the device.
 
 An obstacle's "behavior" is {"name": "constant"} (the default) or {"name": "rvo", "vxmax", "vymax", ...} (keys and defaults in
 ``RVO_DEFAULTS``): a reactive obstacle that heads for a goal at ``speed`` and steers around the other obstacles and the robot with a
@@ -196,6 +203,35 @@ def pack_behaviors(scenes) -> np.ndarray:
     return np.ascontiguousarray(np.asarray(rows, np.float64).reshape(-1, BEH_COLS))
 
 
+def pack_maps(scenes):
+    """Scenes -> the host arrays of nb_world_set_maps: maps (P) of struct nb_world_map, bits (words,) uint32 (each map ``height``
+    rows of ceil(width / 32) words, bit i mod 32 of word i / 32 being cell (i, j), padding bits 0), env_map (B) int32 (-1: no map).
+    A map shared by several scenes (the same occupancy array object, origin and resolution) is stored once."""
+    index, structs, chunks, env_map = {}, [], [], []
+    for sc in scenes:
+        m = sc.get("map")
+        if m is None:
+            env_map.append(-1)
+            continue
+        origin, res = tuple(float(v) for v in m["origin"]), float(m["resolution"])
+        key = (id(m["occupancy"]), origin, res)
+        if key not in index:
+            occ = np.asarray(m["occupancy"], bool)
+            if occ.ndim != 2:
+                raise ValueError(f"a map's occupancy must be an (H, W) array (got shape {occ.shape})")
+            H, W = occ.shape
+            words = (W + 31) // 32
+            padded = np.zeros((H, 32 * words), bool)
+            padded[:, :W] = occ
+            chunks.append(np.packbits(padded, axis=1, bitorder="little").view("<u4").astype(np.uint32).reshape(-1))
+            index[key] = len(structs)
+            structs.append(_lib.WorldMap(width=W, height=H, origin=(C.c_double * 2)(*origin), resolution=res))
+        env_map.append(index[key])
+    maps = (_lib.WorldMap * max(1, len(structs)))(*structs)
+    bits = np.ascontiguousarray(np.concatenate(chunks) if chunks else np.zeros(1, np.uint32))
+    return maps, bits, np.ascontiguousarray(env_map, np.int32)
+
+
 def _host_ptrs(packed):
     return [C.c_void_p(a.ctypes.data) for a in packed]
 
@@ -237,11 +273,13 @@ class WorldBatch:
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
-    def set_scenes(self, scenes, seed: int = 0):
+    def set_scenes(self, scenes, seed: int = 0, map_window: float = 1.0):
         """Uploads B scenes, puts every robot at its start and clears the flags (env.reset).  When an obstacle has a behaviour,
         also sets the behaviours (nb_world_set_behaviors); ``seed`` keys the goal draws of reactive obstacles.  Scenes with K > 1
         ``robots`` also set the fleet (nb_world_set_fleet); K = 1 runs as the single-robot world.  With several robot types the
-        fleet goes through nb_world_set_fleet_ex with every robot's ``type`` (any K)."""
+        fleet goes through nb_world_set_fleet_ex with every robot's ``type`` (any K).  When a scene has a ``map``, also sets the
+        maps (nb_world_set_maps, pack_maps) with ``map_window`` (m, in (0, 10]): a robot's map clearance is exact up to it and
+        reported as ``map_window`` beyond."""
         if len(scenes) != self.B:
             raise ValueError(f"expected {self.B} scenes, got {len(scenes)}")
         K = fleet_size(scenes)
@@ -252,6 +290,7 @@ class WorldBatch:
             raise ValueError(f"a robot has type {int(rtype.max())} but the world has one robot type")
         fleet = pack_fleet(scenes) if K > 1 or T > 0 else None
         beh = pack_behaviors(scenes) if any("behavior" in ob for sc in scenes for ob in sc["obstacles"]) else None
+        maps = pack_maps(scenes) if any("map" in sc for sc in scenes) else None
         with torch.cuda.device(self.device):
             lib = _lib.load()
             fleet_args = (self.B, K, C.c_void_p(fleet.ctypes.data)) if fleet is not None else None
@@ -261,6 +300,12 @@ class WorldBatch:
                     _lib.check(lib.nb_world_check_fleet_ex(C.byref(self.config), *types_args, *fleet_args, C.c_void_p(rtype.ctypes.data)))
                 else:
                     _lib.check(lib.nb_world_check_fleet(C.byref(self.config), *fleet_args))
+            if maps is not None:
+                rows = pack_fleet(scenes)
+                map_args = (len(maps[0]), maps[0], C.c_void_p(maps[1].ctypes.data),
+                            C.c_void_p(maps[2].ctypes.data), C.c_double(float(map_window)))
+                _lib.check(lib.nb_world_check_maps(C.byref(self.config), T, self.types, self.B, K, C.c_void_p(rows.ctypes.data),
+                                                   C.c_void_p(rtype.ctypes.data), *map_args))
             _lib.check(lib.nb_world_set_scenes_ex(self._handle, self.B, *_host_ptrs(packed)))
             self.O, self.K, self.N = int(packed[0][-1]), 1, self.B
             self._rows = None
@@ -272,6 +317,8 @@ class WorldBatch:
                 else:
                     _lib.check(lib.nb_world_set_fleet(self._handle, *fleet_args))
                 self.K, self.N = K, self.B * K
+            if maps is not None:
+                _lib.check(lib.nb_world_set_maps(self._handle, *map_args))
         self.robot_types = rtype
         self._rows = [torch.from_numpy(np.flatnonzero(rtype == i)).to(self.device) for i in range(len(self.robots))]
 
@@ -317,7 +364,8 @@ class WorldBatch:
     def scan(self, hit: bool = False):
         """env.get_lidar_scan() for every robot: (ranges (N,R) f32, velocity (N,2,R) f32, scan dict) -- the arguments of
         PlannerBatch.forward(states, ranges, scan, scan_offset=world.scan_offset, scan_velocity=velocity).  With ``hit``, also the
-        index of the object each beam hit within its environment (obstacles, then robot j as O_b + j), -1 on a miss (N,R) int32.  Passing ``velocity`` selects
+        index of the object each beam hit within its environment (obstacles, then robot j as O_b + j, then the environment's map as
+        O_b + K, which reports velocity 0), -1 on a miss (N,R) int32.  Passing ``velocity`` selects
         scan_to_point_velocity, which applies the sensor offset inversely (neupan.py:271-273): with a non-zero ``scan_offset`` its
         points do not land on the obstacles (the reference's behaviour); without velocities, or at a zero offset, they do."""
         ranges = torch.empty((self.N, self.R), dtype=torch.float32, device=self.device)
@@ -599,4 +647,194 @@ def mixed_swap(num_envs: int, types=(0, 1, 2), robots: int = 6, radius: float = 
     scenes = circle_swap(num_envs, robots=robots, radius=radius, seed=seed, circles=circles)
     for sc in scenes:
         sc["robots"] = [dict(rb, type=types[k % len(types)]) for k, rb in enumerate(sc["robots"])]
+    return scenes
+
+
+# ---- occupancy-map scenes ----------------------------------------------------------------------------------------------------
+
+def _layouts(num_envs: int, layouts):
+    L = int(num_envs) if layouts is None else int(layouts)
+    if L < 1:
+        raise ValueError(f"layouts must be positive (got {L})")
+    return L
+
+
+def _polyline_path(points, spacing: float = 0.1) -> np.ndarray:
+    """(n,4) rows [x, y, theta, gear = 1] along the polyline through ``points``, each segment at ``spacing`` with its own heading."""
+    segs = [line_path(a, b, spacing) for a, b in zip(points[:-1], points[1:])]
+    return np.concatenate([segs[0]] + [s[1:] for s in segs[1:]])
+
+
+def _fill_rect(occ, x0, x1, y0, y1, origin, res):
+    """Marks the cells of occ whose centres lie in [x0, x1] x [y0, y1]."""
+    H, W = occ.shape
+    i0, i1 = max(0, math.ceil((x0 - origin[0]) / res - 0.5)), min(W - 1, math.floor((x1 - origin[0]) / res - 0.5))
+    j0, j1 = max(0, math.ceil((y0 - origin[1]) / res - 0.5)), min(H - 1, math.floor((y1 - origin[1]) / res - 0.5))
+    if i0 <= i1 and j0 <= j1:
+        occ[j0:j1 + 1, i0:i1 + 1] = True
+
+
+def _maze_layout(rng, nx: int, ny: int):
+    """A perfect maze on nx x ny cells by randomised depth-first search from cell (0, 0): the set of open passages
+    {((a, c), (a', c'))} and the solution from (0, 0) to (nx - 1, ny - 1) as a list of cells."""
+    seen, stack, parent, open_ = {(0, 0)}, [(0, 0)], {(0, 0): None}, set()
+    while stack:
+        a, c = stack[-1]
+        nbrs = [(a + da, c + dc) for da, dc in ((1, 0), (-1, 0), (0, 1), (0, -1)) if 0 <= a + da < nx and 0 <= c + dc < ny
+                and (a + da, c + dc) not in seen]
+        if not nbrs:
+            stack.pop()
+            continue
+        nxt = nbrs[int(rng.integers(len(nbrs)))]
+        seen.add(nxt)
+        parent[nxt] = (a, c)
+        open_.add(frozenset(((a, c), nxt)))
+        stack.append(nxt)
+    sol, cell = [], (nx - 1, ny - 1)
+    while cell is not None:  # the tree path back to the root
+        sol.append(cell)
+        cell = parent[cell]
+    return open_, sol[::-1]
+
+
+def maze(num_envs: int, cells=(6, 6), cell_size: float = 5.0, wall: float = 0.3, resolution: float = 0.1, seed: int = 0, layouts=None):
+    """Perfect mazes on an occupancy map: ``cells`` (nx, ny) maze cells of ``cell_size`` m, carved by a randomised depth-first search
+    (every cell reachable by exactly one route), rasterised at ``resolution`` with walls ``wall`` m thick centred on the closed cell
+    boundaries, the outer border included.  Maze cell (a, c) is [a s, (a + 1) s] x [c s, (c + 1) s]; the map covers that area plus
+    ``wall`` on every side.  The robot starts at the centre of cell (0, 0) facing along the solution; its goal is the centre of cell
+    (nx - 1, ny - 1) with threshold 0.3; ``path`` is the solution through the cell centres at 0.1 m spacing (each segment's heading,
+    gear 1).  ``layouts`` distinct mazes (default: one per environment), environment b taking layout b mod layouts, each seeded by
+    its own child stream (``_rng(seed, layout)``); environments of one layout share its occupancy array (one copy on the device)."""
+    nx, ny = (int(v) for v in cells)
+    if nx < 1 or ny < 1 or not (0.0 < wall < cell_size):
+        raise ValueError("maze needs cells >= 1 and 0 < wall < cell_size")
+    L = _layouts(num_envs, layouts)
+    origin = (-wall, -wall)
+    W, H = int(round((nx * cell_size + 2 * wall) / resolution)), int(round((ny * cell_size + 2 * wall) / resolution))
+    built = []
+    for lay in range(min(L, num_envs)):
+        open_, sol = _maze_layout(_rng(seed, lay), nx, ny)
+        occ = np.zeros((H, W), bool)
+        h = wall / 2.0
+        for a in range(nx + 1):  # vertical walls x = a s between (a - 1, c) and (a, c)
+            for c in range(ny):
+                if 0 < a < nx and frozenset(((a - 1, c), (a, c))) in open_:
+                    continue
+                _fill_rect(occ, a * cell_size - h, a * cell_size + h, c * cell_size - h, (c + 1) * cell_size + h, origin, resolution)
+        for c in range(ny + 1):  # horizontal walls y = c s between (a, c - 1) and (a, c)
+            for a in range(nx):
+                if 0 < c < ny and frozenset(((a, c - 1), (a, c))) in open_:
+                    continue
+                _fill_rect(occ, a * cell_size - h, (a + 1) * cell_size + h, c * cell_size - h, c * cell_size + h, origin, resolution)
+        pts = [((a + 0.5) * cell_size, (c + 0.5) * cell_size) for a, c in sol]
+        built.append((occ, pts))
+    scenes = []
+    for b in range(num_envs):
+        occ, pts = built[b % L]
+        th = math.atan2(pts[1][1] - pts[0][1], pts[1][0] - pts[0][0]) if len(pts) > 1 else 0.0
+        path = _polyline_path(pts) if len(pts) > 1 else np.array([[pts[0][0], pts[0][1], th, 1.0]])
+        scenes.append(dict(obstacles=[], bounds=(0.0, 0.0, nx * cell_size, ny * cell_size), start=(pts[0][0], pts[0][1], th), goal=pts[-1],
+                           goal_threshold=0.3, path=path, map=dict(occupancy=occ, origin=origin, resolution=resolution)))
+    return scenes
+
+
+def _components(free):
+    """Labels of the 4-connected components of the True cells of ``free`` (-1 elsewhere) and their sizes."""
+    H, W = free.shape
+    lab = np.full((H, W), -1, np.int64)
+    sizes = []
+    for j0, i0 in zip(*np.nonzero(free)):
+        if lab[j0, i0] >= 0:
+            continue
+        lab[j0, i0] = len(sizes)
+        queue, n = [(j0, i0)], 0
+        while queue:
+            j, i = queue.pop()
+            n += 1
+            for jj, ii in ((j + 1, i), (j - 1, i), (j, i + 1), (j, i - 1)):
+                if 0 <= jj < H and 0 <= ii < W and free[jj, ii] and lab[jj, ii] < 0:
+                    lab[jj, ii] = len(sizes)
+                    queue.append((jj, ii))
+        sizes.append(n)
+    return lab, sizes
+
+
+def _bfs(free, start):
+    """Breadth-first search over the 4-connected True cells of ``free`` from ``start`` (j, i): (distance (-1 unreached), parent)."""
+    H, W = free.shape
+    dist = np.full((H, W), -1, np.int64)
+    parent = {start: None}
+    dist[start] = 0
+    queue, q = [start], 0
+    while q < len(queue):
+        j, i = queue[q]
+        q += 1
+        for jj, ii in ((j + 1, i), (j - 1, i), (j, i + 1), (j, i - 1)):
+            if 0 <= jj < H and 0 <= ii < W and free[jj, ii] and dist[jj, ii] < 0:
+                dist[jj, ii] = dist[j, i] + 1
+                parent[(jj, ii)] = (j, i)
+                queue.append((jj, ii))
+    return dist, parent
+
+
+def cave(num_envs: int, size=(40.0, 40.0), resolution: float = 0.1, fill: float = 0.45, seed: int = 0, layouts=None,
+         coarse: float = 1.0, clearance: float = 2.0):
+    """Caves on an occupancy map: a cellular automaton on a coarse grid of ``coarse`` m cells over ``size`` (m) -- each cell a wall
+    with probability ``fill``, the border always a wall, then 5 rounds of the 4-5 rule (a cell becomes a wall when at least 5 of
+    its 8 neighbours are walls, free when at most 3 are, cells past the border counting as walls) -- of which only the largest
+    4-connected free region is kept free; upsampled to ``resolution``, origin (0, 0).  Start and goal are the centres of coarse
+    cells whose distance to every wall cell's centre exceeds ``clearance`` + ``coarse`` (``clearance``: the robot's circumradius
+    plus a margin; the default 2.0 m covers C4's 1.28 m body): the start a random such cell of the largest 4-connected group of
+    them, the goal the cell of that group farthest from it by breadth-first search; ``path`` is that breadth-first path through the
+    cell centres at 0.1 m spacing, the start facing along it, goal threshold 0.3.  ``layouts`` as in ``maze``."""
+    sx, sy = float(size[0]), float(size[1])
+    nx, ny = int(round(sx / coarse)), int(round(sy / coarse))
+    up = int(round(coarse / resolution))
+    if nx < 3 or ny < 3 or up < 1 or abs(up * resolution - coarse) > 1e-9 * coarse:
+        raise ValueError("cave needs at least 3 x 3 coarse cells and a coarse side that is a multiple of the resolution")
+    L = _layouts(num_envs, layouts)
+    built = []
+    for lay in range(min(L, num_envs)):
+        rng = _rng(seed, lay)
+        for _ in range(64):  # a draw without a cell far enough from the walls is drawn again
+            wall = rng.uniform(size=(ny, nx)) < fill
+            wall[0], wall[-1], wall[:, 0], wall[:, -1] = True, True, True, True
+            for _ in range(5):
+                pad = np.pad(wall, 1, constant_values=True).astype(np.int64)
+                n = sum(np.roll(np.roll(pad, dj, 0), di, 1) for dj in (-1, 0, 1) for di in (-1, 0, 1) if dj or di)[1:-1, 1:-1]
+                wall = np.where(n >= 5, True, np.where(n <= 3, False, wall))
+                wall[0], wall[-1], wall[:, 0], wall[:, -1] = True, True, True, True
+            lab, sizes = _components(~wall)
+            if not sizes:
+                continue
+            wall = lab != int(np.argmax(sizes))
+            jw, iw = np.nonzero(wall)
+            jf, if_ = np.nonzero(~wall)
+            d = np.sqrt((jf[:, None] - jw[None]) ** 2 + (if_[:, None] - iw[None]) ** 2).min(1) * coarse
+            safe = np.zeros_like(wall)
+            safe[jf[d > clearance + coarse], if_[d > clearance + coarse]] = True
+            slab, ssizes = _components(safe)
+            if not ssizes or max(ssizes) < 2:
+                continue
+            group = slab == int(np.argmax(ssizes))
+            cand = np.argwhere(group)
+            start = tuple(int(v) for v in cand[int(rng.integers(len(cand)))])
+            dist, parent = _bfs(group, start)
+            goal = tuple(int(v) for v in np.unravel_index(int(np.argmax(dist)), dist.shape))
+            route, cell = [], goal
+            while cell is not None:
+                route.append(cell)
+                cell = parent[cell]
+            pts = [((i + 0.5) * coarse, (j + 0.5) * coarse) for j, i in route[::-1]]
+            break
+        else:
+            raise ValueError("cave: no layout with a start far enough from the walls (lower fill or clearance)")
+        occ = np.kron(wall, np.ones((up, up), bool))
+        built.append((occ, pts))
+    scenes = []
+    for b in range(num_envs):
+        occ, pts = built[b % L]
+        th = math.atan2(pts[1][1] - pts[0][1], pts[1][0] - pts[0][0])
+        scenes.append(dict(obstacles=[], bounds=(0.0, 0.0, sx, sy), start=(pts[0][0], pts[0][1], th), goal=pts[-1], goal_threshold=0.3,
+                           path=_polyline_path(pts), map=dict(occupancy=occ, origin=(0.0, 0.0), resolution=resolution)))
     return scenes

@@ -89,5 +89,17 @@ if "world" in SECTIONS:
     torch.cuda.synchronize()
     assert torch.isfinite(w.states).all() and torch.isfinite(w.obstacles()).all()
     w.close()
+    # occupancy maps: the map instantiations of world_scan_kernel and world_step_kernel, a maze in four environments and a map-free
+    # environment beside them
+    from neupan_b200.world import maze
+    scenes = maze(5, cells=(3, 3), seed=1, layouts=2) + dyna_obs(1, seed=1)
+    w = WorldBatch(6, rb, lidar, 0.1)
+    w.set_scenes(scenes)
+    for _ in range(30):
+        r, _, _, hit = w.scan(hit=True)
+        w.step(torch.full((6, 2), 0.5, device="cuda"))
+    torch.cuda.synchronize()
+    assert torch.isfinite(w.states).all() and (hit[:5] == 1).any()  # no obstacles, K = 1: the map is index 1
+    w.close()
 torch.cuda.synchronize()
 print("sanitize smoke ok")

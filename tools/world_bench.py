@@ -1,13 +1,15 @@
 """Times the batched world (csrc/world_kernel.cuh) against the planner it serves, on the device, and prints one JSON line.
 
-    python tools/world_bench.py [--scene dyna_obs|dyna_non_obs|circle_swap] [--behavior constant|rvo] [--envs 4096] [--robots 1]
+    python tools/world_bench.py [--scene dyna_obs|dyna_non_obs|circle_swap|maze|cave] [--behavior constant|rvo] [--envs 4096] [--robots 1]
                                 [--beams 1080] [--steps 20] [--warmup 3]
     python tools/world_bench.py --mixed [--envs 4096] [--robots 6] [--beams 1080] [--steps 20] [--warmup 3]
 
 Scenes: seeded dyna_obs (20 moving circles per environment, neupan_b200.world.dyna_obs; the default) or dyna_non_obs (11 moving
 obstacles after example/dyna_non_obs: squares, circles and non-convex outlines, neupan_b200.world.dyna_non_obs), with constant-velocity
 obstacles (the default) or the examples' reactive ones (--behavior rvo, csrc/world_rvo_kernel.cuh); or circle_swap, --robots K robots
-per environment swapping places on a circle (neupan_b200.world.circle_swap; --envs environments x K robots = N planners).  Planner:
+per environment swapping places on a circle (neupan_b200.world.circle_swap; --envs environments x K robots = N planners); or the
+occupancy-map scenes maze (a 6 x 6 perfect maze of 5 m cells at 0.1 m, neupan_b200.world.maze) and cave (40 x 40 m at 0.1 m,
+neupan_b200.world.cave), 64 layouts shared by the environments, map window 1 m.  Planner:
 PlannerBatch with C4's robot, adjust values and K, the scans decimated to C4's N = 500 points.  Legs, each timed with CUDA events over --steps iterations after
 --warmup: the world alone (scan + step), the planner alone (PlannerBatch.forward repeated on the initial states and scans, after a
 reset) and the closed-loop step (scan -> PlannerBatch.forward -> step, from the initial scenes after a reset), whose world and planner
@@ -41,7 +43,7 @@ def _card():
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--scene", choices=("dyna_obs", "dyna_non_obs", "circle_swap"), default="dyna_obs")
+    ap.add_argument("--scene", choices=("dyna_obs", "dyna_non_obs", "circle_swap", "maze", "cave"), default="dyna_obs")
     ap.add_argument("--robots", type=int, default=1, help="robots per environment (circle_swap only)")
     ap.add_argument("--behavior", choices=("constant", "rvo"), default="constant")
     ap.add_argument("--envs", type=int, default=4096)
@@ -59,7 +61,7 @@ def main():
 
     from helpers import CONFIGS, weights_path
     from neupan_b200 import PlannerBatch, WorldBatch
-    from neupan_b200.world import circle_swap, dyna_non_obs, dyna_obs, pack_scenes_ex, scene_paths
+    from neupan_b200.world import cave, circle_swap, dyna_non_obs, dyna_obs, maze, pack_scenes_ex, scene_paths
 
     if not torch.cuda.is_available():
         raise SystemExit("world_bench.py needs a CUDA device")
@@ -70,6 +72,8 @@ def main():
         scenes = circle_swap(B, robots=args.robots, seed=2024)
     elif args.robots != 1:
         raise SystemExit("--robots needs --scene circle_swap")
+    elif args.scene in ("maze", "cave"):
+        scenes = (maze if args.scene == "maze" else cave)(B, seed=2024, layouts=min(B, 64))
     else:
         scenes = (dyna_obs if args.scene == "dyna_obs" else dyna_non_obs)(B, seed=2024, behavior=args.behavior)
     N = B * args.robots
@@ -139,13 +143,17 @@ def main():
         us = sum(getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) for e in prof.key_averages() if "world_rvo_kernel" in e.key)
         rvo = dict(ms_rvo_kernel=us * 1e-3 / args.steps, rvo_share_of_closed_loop=us * 1e-3 / args.steps / ms_loop)
     tests = args.robots * R * (n_circles + n_edges)  # ray-obstacle tests of one scan: every beam against every circle and polygon edge
+    maps = {}
+    if args.scene in ("maze", "cave"):
+        occ = scenes[0]["map"]["occupancy"]
+        maps = dict(map_cells=int(occ.size), map_occupied=float(occ.mean()), map_resolution=scenes[0]["map"]["resolution"], map_layouts=min(B, 64))
     print(json.dumps(dict(metric="batched world: scan + step vs PlannerBatch.forward", scene=args.scene, behavior=args.behavior, envs=B,
                           robots_per_env=args.robots, planners=N, beams=R,
                           obstacles_per_env=n_obs / B, circles_per_env=n_circles / B, edges_per_env=n_edges / B,
                           steps=args.steps, warmup=args.warmup, ms_scan=ms_scan, ms_world_scan_step=ms_world, ms_planner_forward=ms_planner,
                           ms_closed_loop_step=ms_loop, ms_closed_loop_world=ms_loop_world, ms_closed_loop_planner=ms_loop_planner,
                           world_share_of_closed_loop=ms_loop_world / ms_loop,
-                          ray_obstacle_tests_per_s=tests / (ms_scan * 1e-3), **rvo, **_card())))
+                          ray_obstacle_tests_per_s=tests / (ms_scan * 1e-3), **maps, **rvo, **_card())))
     world.close()
     pl.close()
 
