@@ -170,6 +170,10 @@ int nb_pan_backward(nb_pan_t* pan, int32_t B, const float* ref_s, const float* r
  * re-using a handle on a new batch.) */
 int nb_pan_reset_state(nb_pan_t* pan);                      /* legacy default stream, returns after completion */
 int nb_pan_reset_state_async(nb_pan_t* pan, void* stream);   /* ordered with the forwards enqueued on `stream` */
+/* The same for the environments b < B whose mask[b] (DEVICE int32, B <= max_envs) is non-zero; the others keep their state.  One
+ * small kernel on `stream`, no synchronisation (what a batched closed loop calls when some environments start a new episode).  With
+ * every mask entry 1 and B = max_envs it clears exactly what nb_pan_reset_state_async clears. */
+int nb_pan_reset_envs_async(nb_pan_t* pan, int32_t B, const int32_t* mask, void* stream);
 
 /* The sorted selections of the last executed iteration, what DUNE.forward returns restricted to
  * the first M columns (dune.py:100-104): mu (B,T+1,M,E) lam (B,T+1,M,2) points (B,T+1,M,2)
@@ -268,6 +272,12 @@ int nb_ipath_set_paths(nb_ipath_t* ip, int32_t B, const double* points, int64_t 
  * arrived (B) int32.  Environments that have arrived get zero trajectories (the reference returns before generating). */
 int nb_ipath_step(nb_ipath_t* ip, int32_t B, const double* states, const float* cur_vel, double ref_speed,
                   float* nom_s, float* nom_u, float* ref_s, float* ref_us, int32_t* arrived, void* stream);
+/* The same with env_index (B) int32 DEVICE: row b (states, cur_vel and every output) steps the path and the persistent indices of
+ * environment env_index[b] of a handle that holds paths for S environments (nb_ipath_set_paths with S); B is any positive count,
+ * and rows must name distinct environments.  An index outside 0..S-1 gives its row arrived = 1 and zero trajectories.  NULL is
+ * the identity: exactly nb_ipath_step (B must equal S). */
+int nb_ipath_step_ex(nb_ipath_t* ip, int32_t B, const int32_t* env_index, const double* states, const float* cur_vel, double ref_speed,
+                     float* nom_s, float* nom_u, float* ref_s, float* ref_us, int32_t* arrived, void* stream);
 
 /* neupan.reset (neupan/neupan.py:287-294): point_index = curve_index = 0, arrive_flag = False for every environment.
  * The path headings rewritten so far stay as they are (as in the reference). */
@@ -456,6 +466,42 @@ int nb_world_check_maps(const nb_world_config* cfg, int32_t T, const nb_world_ro
                         const int32_t* robot_type, int32_t P, const nb_world_map* maps, const uint32_t* bits, const int32_t* env_map,
                         double window);
 int nb_world_set_maps(nb_world_t* w, int32_t P, const nb_world_map* maps, const uint32_t* bits, const int32_t* env_map, double window);
+
+/* Continuous episodes (semantics in csrc/world_episode_kernel.cuh): a bank of S scenes runs through `slots` slots, and a slot starts
+ * the next unstarted scene on the device when its episode ends.  The bank is uploaded as a world of B = S environments
+ * (nb_world_set_scenes(_ex), then optionally nb_world_set_behaviors, nb_world_set_fleet(_ex), nb_world_set_maps; S <= max_envs, one
+ * K for every scene, and robot k of the same type in every scene).  nb_world_set_episodes(w, slots, max_steps) then switches the
+ * handle to episode mode: slot b starts on scene b; every per-scene array stays where the set calls put it, a slot only names the
+ * scene it runs (scene_of), and every scene runs once.  It allocates the slot and result arrays and synchronises the device.
+ *   nb_world_scan, nb_world_step, nb_world_read_state take N = slots*K; their per-robot arrays are slot rows (robot k of slot b at
+ *           row b*K + k): ranges, velocity, hit, action, collided / arrived / clearance, states.  Reactive obstacles draw their goals
+ *           keyed by the scene index, as environment s of a plain world does.  nb_world_read_state with N = S*K reads the scenes' own
+ *           rows instead (a scene's final state once its episode has ended: nothing touches its rows again); obstacles are the S
+ *           scenes' rows either way.  nb_world_read_behaviors takes B = S.
+ *   end     after step t of a scene (t = 1 at its first step in its slot) its episode ends when every robot of the scene has collided
+ *           or arrived (reason 1, "flags") or when t == max_steps (reason 2, "timeout"; flags win a tie at the same step).
+ *   next    after every nb_world_step a kernel records the ended episodes' results and hands out the next unstarted scenes: the slots
+ *           whose episode ended in this step, in ascending slot order, take the next scenes in ascending scene order.  When the bank
+ *           is exhausted a slot goes idle: its scene is frozen (no integration, no obstacle motion, no flag or result changes; its
+ *           scan is that scene's scan, its step outputs are the frozen flags and clearance +inf).  reset[b] = 1 for a slot that has
+ *           just taken a new scene (every slot after nb_world_set_episodes), else 0.  In episode mode nb_world_step launches one
+ *           more kernel than a plain world (the advance kernel), and nb_world_read_state of slot rows launches one gather kernel where
+ *           a plain world copies.  Nothing synchronises the host.
+ * nb_world_read_episodes (B = S) reads, DEVICE outputs, any may be NULL, enqueued on `stream`: per robot of a scene (S*K rows)
+ * collided, arrived (the flags at the episode's end), arrive_step (the step of arrival, -1 if none: rollout's steps_to_arrive) and
+ * min_clearance (the smallest clearance over the episode's steps), all 0 / -1 / +inf until it has ended; per scene (S) end_step
+ * (0 until it has ended), reason (0 until then, 1 flags, 2 timeout) and slot (the slot that ran it, -1 until it has started); per
+ * slot scene_of and reset (slots); finished (1): the episodes ended so far.
+ * nb_world_set_scenes(_ex), nb_world_set_fleet(_ex), nb_world_set_behaviors and nb_world_set_maps leave episode mode.
+ * Checks (NB_ERR_INVALID, naming the scene and robot): S in 1..max_envs, K in 1..16, slots in 1..S, max_steps >= 1, robot_type (S*K,
+ * HOST, or NULL: every robot type 0) giving robot k the type of robot k of scene 0 in every scene.  nb_world_check_episodes performs
+ * them on the host without a handle or a device.
+ * Limits: one max_steps per handle; no multi-GPU episode runs; the bank must fit max_envs and device memory. */
+int nb_world_check_episodes(const nb_world_config* cfg, int32_t S, int32_t K, const int32_t* robot_type, int32_t slots, int32_t max_steps);
+int nb_world_set_episodes(nb_world_t* w, int32_t slots, int32_t max_steps);
+int nb_world_read_episodes(nb_world_t* w, int32_t S, int32_t* collided, int32_t* arrived, int32_t* arrive_step, float* min_clearance,
+                           int32_t* end_step, int32_t* reason, int32_t* slot, int32_t* scene_of, int32_t* reset, int32_t* finished,
+                           void* stream);
 
 /* ---- DUNE training on the device (SURVEY 8f "next" row 4) ------------------------------------------------------------ */
 

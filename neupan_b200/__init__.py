@@ -12,8 +12,8 @@ from .neupan import neupan
 from .scan import scan_to_points
 from .ipath import InitialPathBatch
 from .planner_batch import PlannerBatch
-from .world import MixedPlanner, WorldBatch, pack_maps, rollout
+from .world import MixedPlanner, WorldBatch, pack_maps, rollout, run_episodes
 
 __all__ = ["configuration", "util", "robot", "neupan", "PAN", "DUNE", "NRMP", "ObsPointNet", "InitialPath", "scan_to_points", "InitialPathBatch", "PlannerBatch", "WorldBatch", "MixedPlanner",
-           "rollout", "pack_maps"]
+           "rollout", "pack_maps", "run_episodes"]
 __version__ = "0.1.0"

@@ -91,6 +91,7 @@ SYMBOLS = {
     "nb_pan_set_option": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "nb_pan_reset_state": (C.c_int, [C.c_void_p]),
     "nb_pan_reset_state_async": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "nb_pan_reset_envs_async": (C.c_int, [C.c_void_p, C.c_int32, _FP, C.c_void_p]),
     "nb_pan_backward": (C.c_int, [C.c_void_p, C.c_int32] + [_FP] * 6 + [C.c_void_p]),
     "nb_pan_read_selection": (C.c_int, [C.c_void_p, C.c_int32] + [_FP] * 5 + [C.c_void_p]),
     "nb_pan_read_screen_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_float * 3), C.POINTER(C.c_int32 * 3), C.c_int32]),
@@ -103,6 +104,7 @@ SYMBOLS = {
     "nb_ipath_destroy": (C.c_int, [C.c_void_p]),
     "nb_ipath_set_paths": (C.c_int, [C.c_void_p, C.c_int32, _FP, C.c_int64, _FP, C.c_int32, _FP, _FP]),
     "nb_ipath_step": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, C.c_double, _FP, _FP, _FP, _FP, _FP, C.c_void_p]),
+    "nb_ipath_step_ex": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, C.c_double, _FP, _FP, _FP, _FP, _FP, C.c_void_p]),
     "nb_ipath_reset": (C.c_int, [C.c_void_p]),
     "nb_ipath_reset_async": (C.c_int, [C.c_void_p, C.c_void_p]),
     "nb_ipath_read_state": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, _FP, C.c_void_p]),
@@ -125,6 +127,9 @@ SYMBOLS = {
     "nb_world_check_maps": (C.c_int, [C.POINTER(WorldConfig), C.c_int32, _FP, C.c_int32, C.c_int32, _FP, _FP, C.c_int32, _FP, _FP, _FP,
                                       C.c_double]),
     "nb_world_set_maps": (C.c_int, [C.c_void_p, C.c_int32, _FP, _FP, _FP, C.c_double]),
+    "nb_world_check_episodes": (C.c_int, [C.POINTER(WorldConfig), C.c_int32, C.c_int32, _FP, C.c_int32, C.c_int32]),
+    "nb_world_set_episodes": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
+    "nb_world_read_episodes": (C.c_int, [C.c_void_p, C.c_int32] + [_FP] * 10 + [C.c_void_p]),
     "nb_dune_labels": (C.c_int, [C.c_int32, _FP, _FP, C.c_int64, _FP, _FP, _FP, _FP, C.c_void_p]),
     "nb_dune_train_create": (C.c_int, [C.c_int32, _FP, _FP, _FP, C.c_int64, C.c_int32, C.POINTER(C.c_void_p)]),
     "nb_dune_train_destroy": (C.c_int, [C.c_void_p]),

@@ -210,6 +210,15 @@ class PAN(torch.nn.Module):
                 stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
                 _lib.check(_lib.load().nb_pan_reset_state_async(self._handle, stream))
 
+    def reset_envs(self, mask):
+        """Forget the stop criterion's memory of the environments where ``mask`` ((B,) int32 on the device) is non-zero
+        (nb_pan_reset_envs_async on the current stream, no host synchronisation); before the native handle exists there is none."""
+        if self._handle is not None:
+            mask = mask.to(device=self.device, dtype=torch.int32).contiguous()
+            with torch.cuda.device(self.device):
+                stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+                _lib.check(_lib.load().nb_pan_reset_envs_async(self._handle, int(mask.numel()), C.c_void_p(mask.data_ptr()), stream))
+
     # ------------------------------------------------------------------ forward
     def forward(self, nom_s: torch.Tensor, nom_u: torch.Tensor, ref_s: torch.Tensor, ref_us: torch.Tensor,
                 obs_points: torch.Tensor = None, point_velocities: torch.Tensor = None, num_points: torch.Tensor = None, device_out: bool = False):

@@ -239,11 +239,14 @@ int nb_ipath_set_paths(nb_ipath_t* p, int32_t B, const double* points, int64_t P
   return nb_ipath_reset(p);
 }
 
-int nb_ipath_step(nb_ipath_t* p, int32_t B, const double* states, const float* cur_vel, double ref_speed,
-                  float* nom_s, float* nom_u, float* ref_s, float* ref_us, int32_t* arrived, void* stream) {
+int nb_ipath_step_ex(nb_ipath_t* p, int32_t B, const int32_t* env_index, const double* states, const float* cur_vel, double ref_speed,
+                     float* nom_s, float* nom_u, float* ref_s, float* ref_us, int32_t* arrived, void* stream) {
   if (!p || !states || !cur_vel || !nom_s || !nom_u || !ref_s || !ref_us || !arrived) return fail(NB_ERR_INVALID, "nb_ipath_step: null argument");
   if (!p->d_pts) return fail(NB_ERR_INVALID, "initial path is not set (nb_ipath_set_paths)");
-  if (B != p->B) return fail(NB_ERR_INVALID, "B = %d but the paths were set for %d environments", B, p->B);
+  if (env_index ? B < 1 : B != p->B) {
+    if (env_index) return fail(NB_ERR_INVALID, "nb_ipath_step_ex: B = %d rows must be positive", B);
+    return fail(NB_ERR_INVALID, "B = %d but the paths were set for %d environments", B, p->B);
+  }
   NB_CUDA(cudaSetDevice(p->cfg.device));
   nb::IpathParams prm;
   prm.B = B; prm.T = p->cfg.receding; prm.kinematics = p->cfg.kinematics; prm.loop = p->cfg.loop;
@@ -253,10 +256,17 @@ int nb_ipath_step(nb_ipath_t* p, int32_t B, const double* states, const float* c
   prm.pts = p->d_pts; prm.curve_begin = p->d_curve_begin; prm.env_curve_begin = p->d_env_curve_begin; prm.interval = p->d_interval;
   prm.curve_index = p->d_curve_index; prm.point_index = p->d_point_index; prm.arrive_flag = p->d_arrive_flag;
   prm.states = states; prm.cur_vel = cur_vel; prm.nom_s = nom_s; prm.nom_u = nom_u; prm.ref_s = ref_s; prm.ref_us = ref_us; prm.arrived = arrived;
-  nb::ipath_step_kernel<<<(B + 63) / 64, 64, 0, (cudaStream_t)stream>>>(prm);
+  prm.env_index = env_index; prm.n_env = p->B;
+  auto* kernel = env_index ? nb::ipath_step_kernel<true> : nb::ipath_step_kernel<false>;
+  kernel<<<(B + 63) / 64, 64, 0, (cudaStream_t)stream>>>(prm);
   ++nb::launches;
   NB_CUDA(cudaGetLastError());
   return NB_OK;
+}
+
+int nb_ipath_step(nb_ipath_t* p, int32_t B, const double* states, const float* cur_vel, double ref_speed,
+                  float* nom_s, float* nom_u, float* ref_s, float* ref_us, int32_t* arrived, void* stream) {
+  return nb_ipath_step_ex(p, B, nullptr, states, cur_vel, ref_speed, nom_s, nom_u, ref_s, ref_us, arrived, stream);
 }
 
 int nb_ipath_read_state(nb_ipath_t* p, int32_t B, int32_t* curve_index, int32_t* point_index, int32_t* arrive_flag,

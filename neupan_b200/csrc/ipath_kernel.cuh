@@ -31,6 +31,8 @@ struct IpathParams {
   float* ref_s;                  // (B, 3, T+1)
   float* ref_us;                 // (B, T)
   int32_t* arrived;              // (B): return value of check_arrive
+  const int32_t* env_index;      // (B) kIndex: row b steps the path and persistent state env_index[b] (0 .. n_env - 1)
+  int n_env;                     // kIndex: the environments the handle holds paths for
 };
 
 constexpr int kIpathMaxT = 64;
@@ -48,13 +50,25 @@ __device__ __forceinline__ double wrap_to_pi(double rad) {  // util.WrapToPi (ne
   return rad;
 }
 
+// kIndex (nb_ipath_step_ex with an env_index): row b (states, cur_vel and the outputs) steps environment e = env_index[b] (its path,
+// interval and persistent indices); an index outside 0 .. n_env - 1 gives row b an arrived flag and zero trajectories.  Without it,
+// e = b.
+template <bool kIndex>
 __global__ void __launch_bounds__(64) ipath_step_kernel(const IpathParams prm) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= prm.B) return;
   const int T = prm.T, T1 = T + 1;
+  const int e = kIndex ? prm.env_index[b] : b;
+  if (kIndex && (e < 0 || e >= prm.n_env)) {
+    prm.arrived[b] = 1;
+    for (int i = 0; i < 3 * T1; ++i) { prm.nom_s[(size_t)b * 3 * T1 + i] = 0.f; prm.ref_s[(size_t)b * 3 * T1 + i] = 0.f; }
+    for (int i = 0; i < 2 * T; ++i) prm.nom_u[(size_t)b * 2 * T + i] = 0.f;
+    for (int t = 0; t < T; ++t) prm.ref_us[(size_t)b * T + t] = 0.f;
+    return;
+  }
   const double sx = prm.states[3 * b], sy = prm.states[3 * b + 1], sth = prm.states[3 * b + 2];
-  const int c0 = prm.env_curve_begin[b], ncurves = prm.env_curve_begin[b + 1] - c0;
-  int ci = prm.curve_index[b], pi = prm.point_index[b];
+  const int c0 = prm.env_curve_begin[e], ncurves = prm.env_curve_begin[e + 1] - c0;
+  int ci = prm.curve_index[e], pi = prm.point_index[e];
   int p0 = prm.curve_begin[c0 + ci], len = prm.curve_begin[c0 + ci + 1] - p0;
   double* P = prm.pts;
 #define PX(i) P[4 * (size_t)(p0 + (i))]
@@ -84,7 +98,7 @@ __global__ void __launch_bounds__(64) ipath_step_kernel(const IpathParams prm) {
     if (arrive) {
       if (ci + 1 >= ncurves) {
         if (prm.loop) { ci = 0; pi = 0; }
-        else { prm.arrive_flag[b] = 1; ret = true; }
+        else { prm.arrive_flag[e] = 1; ret = true; }
       } else {
         ci += 1; pi = 0;
       }
@@ -92,8 +106,8 @@ __global__ void __launch_bounds__(64) ipath_step_kernel(const IpathParams prm) {
       len = prm.curve_begin[c0 + ci + 1] - p0;
     }
   }
-  prm.curve_index[b] = ci;
-  prm.point_index[b] = pi;
+  prm.curve_index[e] = ci;
+  prm.point_index[e] = pi;
   prm.arrived[b] = ret ? 1 : 0;
   float* ns = prm.nom_s + (size_t)b * 3 * T1;
   float* rs = prm.ref_s + (size_t)b * 3 * T1;
@@ -114,7 +128,7 @@ __global__ void __launch_bounds__(64) ipath_step_kernel(const IpathParams prm) {
   double px_ = sx, py_ = sy, pth = sth;            // pre_state
   const double gear0 = PG(pi);
   const double fwd = prm.ref_speed * prm.dt;
-  const double interval = prm.interval[b];
+  const double interval = prm.interval[e];
   int alias_of[kIpathMaxT];
   ns[0] = (float)px_; ns[T1] = (float)py_; ns[2 * T1] = (float)pth;
   rs[0] = (float)rx; rs[T1] = (float)ry; rs[2 * T1] = (float)rth;

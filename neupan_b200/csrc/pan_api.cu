@@ -262,6 +262,12 @@ __global__ void init_run_kernel(int B, int32_t* active, int32_t* iters, int32_t*
   }
 }
 
+// nb_pan_reset_envs_async: the state nb_pan_reset_state_async clears, for the environments whose mask is non-zero
+__global__ void reset_envs_kernel(int B, const int32_t* mask, int32_t* prev_valid, int32_t* prev_count) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < B && mask[i] != 0) { prev_valid[i] = 0; prev_count[i] = 0; }
+}
+
 __global__ void finish_run_kernel(int B, const int32_t* iters, const int32_t* status, const float* min_dist,
                                   int32_t* out_iters, int32_t* out_status, float* out_min_dist) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -485,6 +491,16 @@ int nb_pan_reset_state_async(nb_pan_t* p, void* stream) {
   NB_CUDA(cudaSetDevice(p->cfg.device));
   NB_CUDA(cudaMemsetAsync(p->prev_valid, 0, (size_t)p->cfg.max_envs * sizeof(int32_t), (cudaStream_t)stream));
   NB_CUDA(cudaMemsetAsync(p->prev_count, 0, (size_t)p->cfg.max_envs * sizeof(int32_t), (cudaStream_t)stream));
+  return NB_OK;
+}
+
+int nb_pan_reset_envs_async(nb_pan_t* p, int32_t B, const int32_t* mask, void* stream) {
+  if (!p || !mask) return fail(NB_ERR_INVALID, "nb_pan_reset_envs_async: null argument");
+  if (B < 1 || B > p->cfg.max_envs) return fail(NB_ERR_CAPACITY, "B = %d outside [1, max_envs = %d]", B, p->cfg.max_envs);
+  NB_CUDA(cudaSetDevice(p->cfg.device));
+  reset_envs_kernel<<<(B + 255) / 256, 256, 0, (cudaStream_t)stream>>>(B, mask, p->prev_valid, p->prev_count);
+  ++nb::launches;
+  NB_CUDA(cudaGetLastError());
   return NB_OK;
 }
 

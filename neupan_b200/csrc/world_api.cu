@@ -8,6 +8,7 @@
 #include "host_common.h"
 #include "world_kernel.cuh"
 #include "world_rvo_kernel.cuh"
+#include "world_episode_kernel.cuh"
 
 using nb::dalloc;
 using nb::fail;
@@ -53,6 +54,12 @@ struct nb_world {
   uint32_t* d_bits = nullptr;
   int32_t* d_env_map = nullptr;
   double window = 0.0;
+  // episode mode (nb_world_set_episodes; every other set call leaves it): ep_slots > 0 slots run the B = S scenes of the bank
+  int ep_slots = 0, ep_max_steps = 0;
+  int32_t *d_scene_of = nullptr, *d_live = nullptr, *d_reset = nullptr, *d_ep_t = nullptr, *d_ep_count = nullptr;  // count: next, finished
+  float* d_ep_clear = nullptr;
+  int32_t *d_r_col = nullptr, *d_r_arr = nullptr, *d_r_astep = nullptr, *d_r_end = nullptr, *d_r_reason = nullptr, *d_r_slot = nullptr;
+  float* d_r_minclr = nullptr;
 };
 
 namespace {
@@ -411,13 +418,42 @@ void world_drop_maps(nb_world* w) {
   w->has_map = false;
 }
 
+// Leaves episode mode: frees the slot and result arrays (the scenes' own rows stay as they are).
+void world_drop_episodes(nb_world* w) {
+  void* old[] = {w->d_scene_of, w->d_live, w->d_reset, w->d_ep_t, w->d_ep_count, w->d_ep_clear, w->d_r_col, w->d_r_arr, w->d_r_astep,
+                 w->d_r_end, w->d_r_reason, w->d_r_slot, w->d_r_minclr};
+  for (void* p : old)
+    if (p) cudaFree(p);
+  w->d_scene_of = w->d_live = w->d_reset = w->d_ep_t = w->d_ep_count = nullptr;
+  w->d_r_col = w->d_r_arr = w->d_r_astep = w->d_r_end = w->d_r_reason = w->d_r_slot = nullptr;
+  w->d_ep_clear = w->d_r_minclr = nullptr;
+  w->ep_slots = 0; w->ep_max_steps = 0;
+}
+
+// Every check of nb_world_set_episodes on the host: S in 1..max_envs, slots in 1..S, max_steps >= 1, and (robot_type not NULL)
+// robot k of every scene of the type of robot k of scene 0.
+int world_check_episodes(const nb_world_config* cfg, int32_t S, int32_t K, const int32_t* robot_type, int32_t slots, int32_t max_steps) {
+  if (int rc = world_check_config(cfg)) return rc;
+  if (S < 1 || S > cfg->max_envs) return fail(NB_ERR_INVALID, "a bank of S = %d scenes outside [1, max_envs = %d]", S, cfg->max_envs);
+  if (K < 1 || K > nb::kWorldMaxFleet) return fail(NB_ERR_INVALID, "K = %d robots per scene (1..%d)", K, nb::kWorldMaxFleet);
+  if (slots < 1 || slots > S) return fail(NB_ERR_INVALID, "slots = %d outside [1, S = %d]", slots, S);
+  if (max_steps < 1) return fail(NB_ERR_INVALID, "max_steps = %d must be >= 1", max_steps);
+  if (robot_type)
+    for (int s = 1; s < S; ++s)
+      for (int k = 0; k < K; ++k)
+        if (robot_type[(size_t)s * K + k] != robot_type[k])
+          return fail(NB_ERR_INVALID, "scene %d, robot %d: type %d but robot %d of scene 0 has type %d (a robot keeps its type in every scene of a bank)",
+                      s, k, robot_type[(size_t)s * K + k], k, robot_type[k]);
+  return NB_OK;
+}
+
 nb::WorldMapParams world_map_params(const nb_world* w) { return nb::WorldMapParams{w->d_maps, w->d_bits, w->d_env_map, w->window}; }
 
 template <bool kMap>
 int world_scan_occupancy(nb_world* w, int* per_sm) {
   // the occupancy query sees the kernel's current limit; nb_world_scan sets it again before every launch
-  NB_CUDA(cudaFuncSetAttribute(nb::world_scan_kernel<kMap>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
-  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, nb::world_scan_kernel<kMap>, w->scan_threads, w->scan_smem));
+  NB_CUDA(cudaFuncSetAttribute(nb::world_scan_kernel<kMap, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
+  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, nb::world_scan_kernel<kMap, false>, w->scan_threads, w->scan_smem));
   return NB_OK;
 }
 
@@ -440,9 +476,9 @@ int world_scan_shape(nb_world* w, int B) {
 int world_rvo_shape(nb_world* w, int B) {
   w->rvo_cap = w->rvo_max_n + w->K;
   w->rvo_smem = (size_t)w->rvo_cap * (5 * sizeof(double) + nb::kWorldRvoWarps * (6 * sizeof(double) + sizeof(int32_t)));
-  NB_CUDA(cudaFuncSetAttribute(nb::world_rvo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
+  NB_CUDA(cudaFuncSetAttribute(nb::world_rvo_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
   int per_sm = 0, sms = 0;
-  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_rvo_kernel, 32 * nb::kWorldRvoWarps, w->rvo_smem));
+  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_rvo_kernel<false>, 32 * nb::kWorldRvoWarps, w->rvo_smem));
   NB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->cfg.device));
   if (per_sm < 1) return fail(NB_ERR_CUDA, "world_rvo_kernel: %zu B of shared memory do not fit", w->rvo_smem);
   w->rvo_grid = std::min(B, per_sm * sms);
@@ -497,7 +533,7 @@ int world_set_robots(nb_world* w, int B, int K, const double* robots, int T, con
 nb::WorldParams world_params(const nb_world* w) {
   nb::WorldParams prm;
   const nb_world_config& c = w->cfg;
-  prm.B = w->B; prm.R = c.num_beams;
+  prm.B = w->ep_slots ? w->ep_slots : w->B; prm.R = c.num_beams;
   prm.dt = c.step_time; prm.range_max = c.range_max; prm.beam_cs = w->d_beam_cs;
   prm.off_x = c.scan_offset[0]; prm.off_y = c.scan_offset[1]; prm.off_th = c.scan_offset[2];
   prm.types = w->d_types; prm.rtype = w->d_rtype;
@@ -505,14 +541,21 @@ nb::WorldParams world_params(const nb_world* w) {
   prm.vertices = w->d_vertices; prm.env = w->d_env; prm.obs = w->d_obs; prm.states = w->d_states;
   prm.collided = w->d_collided; prm.arrived = w->d_arrived;
   prm.K = w->K; prm.fgoal = w->d_fgoal; prm.fvel = w->d_fvel;
+  prm.scene_of = w->d_scene_of; prm.live = w->d_live; prm.ep_clear = w->d_ep_clear;
   return prm;
 }
 
-// per_robot: the count argument is the robot count N = B K (B itself with one robot per environment); otherwise (the obstacle-side
-// calls) the environment count B
+// per_robot: the count argument is the robot count N = B K (B itself with one robot per environment), in episode mode the slot
+// robots slots K; otherwise (the obstacle-side calls) the environment count B (S in episode mode)
 int world_ready(const nb_world* w, int32_t B, const char* what, bool per_robot = false) {
   if (!w) return fail(NB_ERR_INVALID, "%s: null handle", what);
   if (!w->B) return fail(NB_ERR_INVALID, "%s: no scenes set (nb_world_set_scenes)", what);
+  if (per_robot && w->ep_slots) {
+    if (B != w->ep_slots * w->K)
+      return fail(NB_ERR_INVALID, "%s: count = %d but the world runs episodes in %d slots x %d robots (N = %d)", what, B, w->ep_slots, w->K,
+                  w->ep_slots * w->K);
+    return NB_OK;
+  }
   if (per_robot && w->K > 1) {
     if (B != w->B * w->K)
       return fail(NB_ERR_INVALID, "%s: count = %d but the world has %d environments x %d robots (N = %d)", what, B, w->B, w->K, w->B * w->K);
@@ -566,6 +609,7 @@ int nb_world_create(const nb_world_config* cfg, nb_world_t** out) {
 int nb_world_destroy(nb_world_t* w) {
   if (!w) return NB_OK;
   cudaSetDevice(w->cfg.device);
+  world_drop_episodes(w);
   void* bufs[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
                   w->d_states, w->d_beam_cs, w->d_beh, w->d_rad, w->d_goal, w->d_draws, w->d_fgoal, w->d_fvel, w->d_types, w->d_rtype,
                   w->d_maps, w->d_bits, w->d_env_map};
@@ -606,6 +650,7 @@ int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, c
   w->B = 0;
   w->has_rvo = false;  // new scenes: every obstacle keeps a constant velocity until nb_world_set_behaviors
   world_drop_maps(w);  // and has no map until nb_world_set_maps
+  world_drop_episodes(w);  // and runs as a plain world until nb_world_set_episodes
   w->h_obs_begin.assign(obs_begin, obs_begin + B + 1);
   w->h_vert_begin.assign(vert_begin, vert_begin + O + 1);
   w->h_vertices.assign(vertices, vertices + 2 * (size_t)V);
@@ -654,6 +699,7 @@ int nb_world_set_behaviors(nb_world_t* w, int32_t B, const double* behaviors, ui
   std::vector<double> obs((size_t)nb::kWorldObsCols * O);
   if (O) NB_CUDA(cudaMemcpy(obs.data(), w->d_obs, sizeof(double) * obs.size(), cudaMemcpyDeviceToHost));  // the current centres
   if (int rc = world_check_behaviors(&w->cfg, B, w->h_obs_begin.data(), obs.data(), w->h_env.data(), behaviors)) return rc;
+  world_drop_episodes(w);
   // radii (circle: its own; polygon: the largest vertex norm), initial goals (NaN: draw 0) and draw counters
   std::vector<double> rad(O), goal(2 * (size_t)O, 0.0);
   std::vector<int32_t> draws(O, 0);
@@ -724,7 +770,8 @@ int nb_world_scan(nb_world_t* w, int32_t B, float* ranges, float* velocity, int3
   NB_CUDA(cudaSetDevice(w->cfg.device));
   // the dynamic shared-memory limit is an attribute of the kernel, shared by every handle of the process: set this handle's
   // size before each launch (another handle's nb_world_set_scenes may have set a smaller one)
-  auto* kernel = w->has_map ? nb::world_scan_kernel<true> : nb::world_scan_kernel<false>;
+  auto* kernel = w->ep_slots ? (w->has_map ? nb::world_scan_kernel<true, true> : nb::world_scan_kernel<false, true>)
+                             : (w->has_map ? nb::world_scan_kernel<true, false> : nb::world_scan_kernel<false, false>);
   NB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
   kernel<<<w->scan_grid, w->scan_threads, w->scan_smem, (cudaStream_t)stream>>>(world_params(w), world_map_params(w), w->max_circ, w->max_edges,
                                                                                 w->max_redges, ranges, velocity, hit);
@@ -737,26 +784,53 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
   if (int rc = world_ready(w, B, "nb_world_step", true)) return rc;
   if (!action) return fail(NB_ERR_INVALID, "nb_world_step: null action");
   NB_CUDA(cudaSetDevice(w->cfg.device));
+  const nb::WorldParams prm = world_params(w);  // prm.B: the environments, or the slots in episode mode
   if (w->has_rvo) {  // reactive obstacles choose their velocities from the states at the start of the step
-    NB_CUDA(cudaFuncSetAttribute(nb::world_rvo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
-    nb::world_rvo_kernel<<<w->rvo_grid, 32 * nb::kWorldRvoWarps, w->rvo_smem, (cudaStream_t)stream>>>(world_params(w), world_rvo_params(w, action));
+    auto* rvo = w->ep_slots ? nb::world_rvo_kernel<true> : nb::world_rvo_kernel<false>;
+    NB_CUDA(cudaFuncSetAttribute(rvo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
+    rvo<<<std::min(w->rvo_grid, prm.B), 32 * nb::kWorldRvoWarps, w->rvo_smem, (cudaStream_t)stream>>>(prm, world_rvo_params(w, action));
     ++nb::launches;
     NB_CUDA(cudaGetLastError());
   }
   // a CTA of up to 8 warps per E environments, a warp per robot
   const int E = nb::world_step_envs(w->K);
-  auto* kernel = w->has_map ? nb::world_step_kernel<true> : nb::world_step_kernel<false>;
-  kernel<<<(w->B + E - 1) / E, 32 * std::min(E * w->K, nb::kWorldStepMaxWarps), 0, (cudaStream_t)stream>>>(world_params(w), world_map_params(w),
-                                                                                                          action, collided, arrived, clearance);
+  auto* kernel = w->ep_slots ? (w->has_map ? nb::world_step_ep_kernel<true> : nb::world_step_ep_kernel<false>)
+                             : (w->has_map ? nb::world_step_kernel<true> : nb::world_step_kernel<false>);
+  kernel<<<(prm.B + E - 1) / E, 32 * std::min(E * w->K, nb::kWorldStepMaxWarps), 0, (cudaStream_t)stream>>>(prm, world_map_params(w),
+                                                                                                           action, collided, arrived, clearance);
   ++nb::launches;
   NB_CUDA(cudaGetLastError());
+  if (w->ep_slots) {  // end the episodes of this step and hand out the next scenes
+    nb::WorldEpisodeParams ep;
+    ep.S = w->B; ep.slots = w->ep_slots; ep.K = w->K; ep.max_steps = w->ep_max_steps;
+    ep.scene_of = w->d_scene_of; ep.live = w->d_live; ep.reset = w->d_reset; ep.t = w->d_ep_t;
+    ep.next = w->d_ep_count; ep.finished = w->d_ep_count + 1;
+    ep.collided = w->d_collided; ep.arrived = w->d_arrived; ep.clear = w->d_ep_clear;
+    ep.r_col = w->d_r_col; ep.r_arr = w->d_r_arr; ep.r_astep = w->d_r_astep; ep.r_minclr = w->d_r_minclr;
+    ep.r_end = w->d_r_end; ep.r_reason = w->d_r_reason; ep.r_slot = w->d_r_slot;
+    nb::world_advance_kernel<<<1, nb::kWorldAdvanceThreads, 0, (cudaStream_t)stream>>>(ep);
+    ++nb::launches;
+    NB_CUDA(cudaGetLastError());
+  }
   return NB_OK;
 }
 
 int nb_world_read_state(nb_world_t* w, int32_t B, double* states, double* obstacles, int32_t* collided, int32_t* arrived, void* stream) {
-  if (int rc = world_ready(w, B, "nb_world_read_state", true)) return rc;
+  // episode mode: B = slots K reads the slot rows (a gather), B = S K the scenes' own rows (copies, like a plain world)
+  const bool scenes = w && w->ep_slots && B == w->B * w->K;
+  if (!scenes)
+    if (int rc = world_ready(w, B, "nb_world_read_state", true)) return rc;
   NB_CUDA(cudaSetDevice(w->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
+  if (w->ep_slots && !scenes) {
+    if (obstacles && w->O) NB_CUDA(cudaMemcpyAsync(obstacles, w->d_obs, sizeof(double) * nb::kWorldObsCols * w->O, cudaMemcpyDeviceToDevice, st));
+    if (!states && !collided && !arrived) return NB_OK;
+    nb::world_gather_kernel<<<(B + 255) / 256, 256, 0, st>>>(w->ep_slots, w->K, w->d_scene_of, w->d_states, w->d_collided, w->d_arrived, states,
+                                                             collided, arrived);
+    ++nb::launches;
+    NB_CUDA(cudaGetLastError());
+    return NB_OK;
+  }
   if (states) NB_CUDA(cudaMemcpyAsync(states, w->d_states, sizeof(double) * 3 * B, cudaMemcpyDeviceToDevice, st));
   if (obstacles && w->O) NB_CUDA(cudaMemcpyAsync(obstacles, w->d_obs, sizeof(double) * nb::kWorldObsCols * w->O, cudaMemcpyDeviceToDevice, st));
   if (collided) NB_CUDA(cudaMemcpyAsync(collided, w->d_collided, sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
@@ -780,6 +854,7 @@ int nb_world_set_fleet_ex(nb_world_t* w, int32_t T, const nb_world_robot_type* t
   NB_CUDA(cudaSetDevice(w->cfg.device));
   w->B = 0;  // unusable until the new arrays are in place
   world_drop_maps(w);  // the new starts need a new map check
+  world_drop_episodes(w);
   if (int rc = world_set_robots(w, B, K, robots, T, types, robot_type)) return rc;
   if (int rc = world_scan_shape(w, B)) return rc;
   if (w->d_beh)
@@ -808,6 +883,7 @@ int nb_world_set_maps(nb_world_t* w, int32_t P, const nb_world_map* maps, const 
     return rc;
   NB_CUDA(cudaSetDevice(w->cfg.device));
   world_drop_maps(w);
+  world_drop_episodes(w);
   const size_t words = (size_t)(table.back().off + (int64_t)table.back().H * table.back().words);
   cudaError_t e = nb::dalloc(&w->d_maps, table.size());
   if (e == cudaSuccess) e = nb::dalloc(&w->d_bits, words);
@@ -825,6 +901,76 @@ int nb_world_set_maps(nb_world_t* w, int32_t P, const nb_world_map* maps, const 
   w->window = window;
   if (int rc = world_scan_shape(w, w->B)) return rc;
   NB_CUDA(cudaDeviceSynchronize());
+  return NB_OK;
+}
+
+int nb_world_check_episodes(const nb_world_config* cfg, int32_t S, int32_t K, const int32_t* robot_type, int32_t slots, int32_t max_steps) {
+  return world_check_episodes(cfg, S, K, robot_type, slots, max_steps);
+}
+
+int nb_world_set_episodes(nb_world_t* w, int32_t slots, int32_t max_steps) {
+  if (!w) return fail(NB_ERR_INVALID, "nb_world_set_episodes: null handle");
+  if (int rc = world_ready(w, w->B, "nb_world_set_episodes")) return rc;
+  const int S = w->B, K = w->K;
+  if (int rc = world_check_episodes(&w->cfg, S, K, w->h_rtype.data(), slots, max_steps)) return rc;
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  world_drop_episodes(w);
+  const size_t SK = (size_t)S * K, BK = (size_t)slots * K;
+  std::vector<int32_t> scene_of(slots), slot(S, -1), minus(SK, -1);
+  for (int b = 0; b < slots; ++b) scene_of[b] = slot[b] = b;
+  const int32_t count[2] = {slots, 0};  // the next scene, episodes finished
+  std::vector<float> inf(SK, INFINITY);
+  cudaError_t e = cudaSuccess;
+  auto alloc = [&](auto** p, size_t n) { if (e == cudaSuccess) e = dalloc(p, std::max<size_t>(n, 1)); };
+  alloc(&w->d_scene_of, slots); alloc(&w->d_live, slots); alloc(&w->d_reset, slots); alloc(&w->d_ep_t, slots); alloc(&w->d_ep_count, 2);
+  alloc(&w->d_ep_clear, BK);
+  alloc(&w->d_r_col, SK); alloc(&w->d_r_arr, SK); alloc(&w->d_r_astep, SK); alloc(&w->d_r_minclr, SK);
+  alloc(&w->d_r_end, S); alloc(&w->d_r_reason, S); alloc(&w->d_r_slot, S);
+  auto up = [&](void* d, const void* h, size_t bytes) { if (e == cudaSuccess) e = cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice); };
+  auto one = [&](void* d, size_t n) {  // int32 ones
+    std::vector<int32_t> v(n, 1);
+    up(d, v.data(), n * sizeof(int32_t));
+  };
+  up(w->d_scene_of, scene_of.data(), slots * sizeof(int32_t));
+  one(w->d_live, slots);
+  one(w->d_reset, slots);  // every slot has just taken its first scene
+  if (e == cudaSuccess) e = cudaMemset(w->d_ep_t, 0, slots * sizeof(int32_t));
+  up(w->d_ep_count, count, sizeof(count));
+  if (e == cudaSuccess) e = cudaMemset(w->d_r_col, 0, SK * sizeof(int32_t));
+  if (e == cudaSuccess) e = cudaMemset(w->d_r_arr, 0, SK * sizeof(int32_t));
+  up(w->d_r_astep, minus.data(), SK * sizeof(int32_t));
+  up(w->d_r_minclr, inf.data(), SK * sizeof(float));
+  if (e == cudaSuccess) e = cudaMemset(w->d_r_end, 0, S * sizeof(int32_t));
+  if (e == cudaSuccess) e = cudaMemset(w->d_r_reason, 0, S * sizeof(int32_t));
+  up(w->d_r_slot, slot.data(), S * sizeof(int32_t));
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {  // the handle stays usable as a plain world
+    cudaGetLastError();
+    world_drop_episodes(w);
+    return fail(NB_ERR_CUDA, "nb_world_set_episodes: %s", cudaGetErrorString(e));
+  }
+  w->ep_slots = slots; w->ep_max_steps = max_steps;
+  return NB_OK;
+}
+
+int nb_world_read_episodes(nb_world_t* w, int32_t S, int32_t* collided, int32_t* arrived, int32_t* arrive_step, float* min_clearance, int32_t* end_step,
+                           int32_t* reason, int32_t* slot, int32_t* scene_of, int32_t* reset, int32_t* finished, void* stream) {
+  if (int rc = world_ready(w, S, "nb_world_read_episodes")) return rc;
+  if (!w->ep_slots) return fail(NB_ERR_INVALID, "nb_world_read_episodes: not in episode mode (nb_world_set_episodes)");
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t SK = (size_t)S * w->K;
+  auto cp = [&](void* dst, const void* src, size_t bytes) { return dst ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) : cudaSuccess; };
+  NB_CUDA(cp(collided, w->d_r_col, SK * sizeof(int32_t)));
+  NB_CUDA(cp(arrived, w->d_r_arr, SK * sizeof(int32_t)));
+  NB_CUDA(cp(arrive_step, w->d_r_astep, SK * sizeof(int32_t)));
+  NB_CUDA(cp(min_clearance, w->d_r_minclr, SK * sizeof(float)));
+  NB_CUDA(cp(end_step, w->d_r_end, S * sizeof(int32_t)));
+  NB_CUDA(cp(reason, w->d_r_reason, S * sizeof(int32_t)));
+  NB_CUDA(cp(slot, w->d_r_slot, S * sizeof(int32_t)));
+  NB_CUDA(cp(scene_of, w->d_scene_of, w->ep_slots * sizeof(int32_t)));
+  NB_CUDA(cp(reset, w->d_reset, w->ep_slots * sizeof(int32_t)));
+  NB_CUDA(cp(finished, w->d_ep_count + 1, sizeof(int32_t)));
   return NB_OK;
 }
 

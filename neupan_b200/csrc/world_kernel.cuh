@@ -96,6 +96,11 @@ struct WorldParams {
   int32_t* arrived;                       // (B K) sticky
   const double* fgoal;                    // (B K, 3) goal x, y, threshold of every robot
   double* fvel;                           // (B K, 2) world-frame velocity of each robot's last step
+  // episode mode (nb_world_set_episodes; read by the kEp instantiations only): B is then the slot count, slot b runs scene
+  // scene_of[b] while live[b] != 0; every per-scene array above is indexed by the scene, every per-call input and output by the slot
+  const int32_t* scene_of;                // (slots)
+  const int32_t* live;                    // (slots) 0: idle, its scene frozen
+  float* ep_clear;                        // (slots K) this step's clearance of each slot robot, for world_advance_kernel
 };
 
 constexpr int kWorldMaxMapSide = 8192;  // cells per side of an occupancy map
@@ -198,8 +203,9 @@ __device__ __forceinline__ double world_map_cast(const WorldMap& m, const uint32
 // (obstacles 0..O_b - 1, then robot j as O_b + j), so the result does not depend on the order of the tests.
 // max_redges: the largest environment's robot edge count (the sum of its robots' vertex counts with K > 1, else 0); robot k's edges
 // follow those of robots 0 .. k - 1, each robot's polygon that of its own type.  kMap: then the environment's map (world_map_cast,
-// index O_b + K, velocity 0); mp is not read without it.
-template <bool kMap>
+// index O_b + K, velocity 0); mp is not read without it.  kEp (episode mode): the CTA's unit b is a slot, which scans the robots of
+// scene scene_of[b] (an idle slot its frozen scene) into slot rows b K + k.
+template <bool kMap, bool kEp>
 __global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, const WorldMapParams mp, int max_circ, int max_edges, int max_redges,
                                                          float* __restrict__ ranges, float* __restrict__ velocity, int32_t* __restrict__ hit) {
   extern __shared__ double wsm[];
@@ -223,8 +229,9 @@ __global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, 
   int32_t* r_id = e_id + max_edges;  // owner of each robot edge
   const int R = prm.R;
   for (int b = blockIdx.x; b < prm.B; b += gridDim.x) {
-    const int o0 = prm.obs_begin[b], o1 = prm.obs_begin[b + 1];
-    const int nc = prm.counts[2 * b], ne = prm.counts[2 * b + 1];
+    const int e = kEp ? prm.scene_of[b] : b;  // the scene: obstacle and robot rows; b: the output rows
+    const int o0 = prm.obs_begin[e], o1 = prm.obs_begin[e + 1];
+    const int nc = prm.counts[2 * e], ne = prm.counts[2 * e + 1];
     __syncthreads();  // the previous environment's beams are done with the shared lists
     for (int o = o0 + (int)threadIdx.x; o < o1; o += blockDim.x) {
       const double cx = prm.obs[kWorldObsCols * o], cy = prm.obs[kWorldObsCols * o + 1];
@@ -243,7 +250,7 @@ __global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, 
       }
     }
     for (int k = threadIdx.x; k < K; k += blockDim.x) {  // robot k: sensor pose, and with K > 1 its body (the step kernel's vertices)
-      const size_t n = (size_t)b * K + k;
+      const size_t n = (size_t)e * K + k;
       const double x = prm.states[3 * n], y = prm.states[3 * n + 1], th = prm.states[3 * n + 2];
       double sn, cs;
       sincos(th, &sn, &cs);
@@ -254,7 +261,7 @@ __global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, 
       s_hc[k] = hc; s_hs[k] = hs;
       if (K > 1) {
         int e0 = 0;  // robot k's first edge: after the edges of robots 0 .. k - 1
-        for (int j = 0; j < k; ++j) e0 += prm.types[prm.rtype[(size_t)b * K + j]].nv;
+        for (int j = 0; j < k; ++j) e0 += prm.types[prm.rtype[(size_t)e * K + j]].nv;
         const WorldRobotType* ty = prm.types + prm.rtype[n];
         const int nr = ty->nv;
         if (k == K - 1) s_nre = e0 + nr;
@@ -311,7 +318,7 @@ __global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, 
         }
       }
       if constexpr (kMap) {  // the highest index: only a strictly closer crossing counts, so the walk stops at best
-        const int mi = mp.env_map[b];
+        const int mi = mp.env_map[e];
         if (mi >= 0) {
           const double t = world_map_cast(mp.maps[mi], mp.bits, sx, sy, dx, dy, fmin(best, prm.range_max));
           if (t < best) { best = t; bid = nobs + K; }
@@ -325,7 +332,7 @@ __global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, 
         if (kMap && bid == nobs + K) {
           // the map does not move
         } else if (bid >= nobs) {
-          const double* fv = prm.fvel + 2 * ((size_t)b * K + (bid - nobs));
+          const double* fv = prm.fvel + 2 * ((size_t)e * K + (bid - nobs));
           vx = (float)fv[0]; vy = (float)fv[1];
         } else if (bid >= 0) {
           const double* row = prm.obs + (size_t)kWorldObsCols * (o0 + bid);
@@ -592,10 +599,12 @@ __device__ __forceinline__ double world_map_clearance(const WorldMap& m, const u
 // branches of world_obstacle_clearance) and to every other robot of it (lane j), a warp min, and lane 0 writes the collision flag,
 // the clearance and the velocity the scan reports for the robot (0 once collided).  kMap: the warp also takes min(window, the
 // clearance to the environment's map) (world_map_clearance) into the warp min; mp is not read without it.
-template <bool kMap>
-__global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(const WorldParams prm, const WorldMapParams mp, const float* __restrict__ action,
-                                                                           int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived,
-                                                                           float* __restrict__ clearance) {
+// kEp (episode mode): the CTA's units are slots b0 .. b0 + E - 1; a live slot steps the robots and obstacles of scene scene_of[b]
+// (the scene's rows) and writes its outputs to slot rows q = b K + k, its clearances also to ep_clear; an idle slot's scene is not
+// touched, and its outputs are the frozen flags and clearance +inf.
+template <bool kMap, bool kEp>
+__device__ __forceinline__ void world_step_body(const WorldParams& prm, const WorldMapParams& mp, const float* __restrict__ action,
+                                                int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived, float* __restrict__ clearance) {
   __shared__ double f_x[kWorldMaxFleet][kWorldMaxVertices], f_y[kWorldMaxFleet][kWorldMaxVertices];  // E K <= 8 or K <= 16 slots
   __shared__ double f_v[kWorldMaxFleet][2];
   __shared__ int f_nv[kWorldMaxFleet];  // each slot's vertex count (its type's)
@@ -604,17 +613,22 @@ __global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(con
   const int nslot = min(world_step_envs(K), prm.B - b0) * K;  // this CTA's robots
   const size_t n0 = (size_t)b0 * K;
   for (int s = threadIdx.x; s < nslot; s += blockDim.x) {
-    const size_t n = n0 + s;
+    const size_t q = n0 + s;  // the output row
+    const size_t n = kEp ? (size_t)prm.scene_of[b0 + s / K] * K + s % K : q;  // the robot's row
+    if (kEp && prm.live[b0 + s / K] == 0) {
+      if (out_arrived) out_arrived[q] = prm.arrived[n];
+      continue;
+    }
     double x = prm.states[3 * n], y = prm.states[3 * n + 1], th = prm.states[3 * n + 2];
     double vx = 0.0, vy = 0.0;
     const WorldRobotType* ty = prm.types + prm.rtype[n];
-    if (prm.collided[n] == 0) world_integrate(ty->kinematics, ty->L, prm.dt, (double)action[2 * n], (double)action[2 * n + 1], x, y, th, vx, vy);
+    if (prm.collided[n] == 0) world_integrate(ty->kinematics, ty->L, prm.dt, (double)action[2 * q], (double)action[2 * q + 1], x, y, th, vx, vy);
     prm.states[3 * n] = x; prm.states[3 * n + 1] = y; prm.states[3 * n + 2] = th;
     const double* g = prm.fgoal + 3 * n;
     const double gx = dsub(x, g[0]), gy = dsub(y, g[1]);
     const int arr = (prm.arrived[n] != 0 || sqrt(ddot(gx, gy, gx, gy)) < g[2]) ? 1 : 0;
     prm.arrived[n] = arr;
-    if (out_arrived) out_arrived[n] = arr;
+    if (out_arrived) out_arrived[q] = arr;
     double sn, cs;
     sincos(th, &sn, &cs);
 #pragma unroll
@@ -626,7 +640,16 @@ __global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(con
     f_v[s][0] = vx; f_v[s][1] = vy;
     f_nv[s] = ty->nv;
   }
-  {
+  if constexpr (kEp) {  // the slots' scenes are anywhere in the obstacle rows: one live scene after the other
+    for (int j = 0; j < nslot / K; ++j) {
+      if (prm.live[b0 + j] == 0) continue;
+      const int e = prm.scene_of[b0 + j];
+      for (int o = prm.obs_begin[e] + (int)threadIdx.x; o < prm.obs_begin[e + 1]; o += blockDim.x) {
+        double cx, cy;
+        world_move_obstacle(prm, prm.env + (size_t)kWorldEnvCols * e, o, cx, cy);
+      }
+    }
+  } else {
     int b = b0;  // the environment of obstacle o: the CTA's obstacle rows are its environments' back to back
     for (int o = prm.obs_begin[b0] + (int)threadIdx.x; o < prm.obs_begin[b0 + nslot / K]; o += blockDim.x) {
       while (o >= prm.obs_begin[b + 1]) ++b;
@@ -637,8 +660,16 @@ __global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(con
   __syncthreads();  // bodies, velocities and the moved obstacle rows are visible to the whole CTA
   for (int s = threadIdx.x >> 5; s < nslot; s += nw) {  // warp-uniform
     const int k = s % K, s0 = s - k;  // robot k of the environment whose robots are the slots s0 .. s0 + K - 1
-    const int b = b0 + s / K;
-    const size_t n = n0 + s;
+    const size_t q = n0 + s;          // the output row
+    const int b = kEp ? prm.scene_of[b0 + s / K] : b0 + s / K;  // the scene
+    const size_t n = kEp ? (size_t)b * K + k : q;                // the robot's row
+    if (kEp && prm.live[b0 + s / K] == 0) {
+      if (lane == 0) {
+        if (out_collided) out_collided[q] = prm.collided[n];
+        if (clearance) clearance[q] = INFINITY;
+      }
+      continue;
+    }
     const int nr = f_nv[s];
     double best = INFINITY;
     for (int o = prm.obs_begin[b] + lane; o < prm.obs_begin[b + 1]; o += 32) {
@@ -661,10 +692,27 @@ __global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(con
       prm.collided[n] = col;
       prm.fvel[2 * n] = col ? 0.0 : f_v[s][0];
       prm.fvel[2 * n + 1] = col ? 0.0 : f_v[s][1];
-      if (out_collided) out_collided[n] = col;
-      if (clearance) clearance[n] = (float)best;
+      if (out_collided) out_collided[q] = col;
+      if (clearance) clearance[q] = (float)best;
+      if constexpr (kEp) prm.ep_clear[q] = (float)best;
     }
   }
+}
+
+template <bool kMap>
+__global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(const WorldParams prm, const WorldMapParams mp, const float* __restrict__ action,
+                                                                           int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived,
+                                                                           float* __restrict__ clearance) {
+  world_step_body<kMap, false>(prm, mp, action, out_collided, out_arrived, clearance);
+}
+
+// episode mode: __maxnreg__(128) instead of __launch_bounds__(256), under which ptxas settles on 64 registers and spills (at most 8
+// warps per CTA either way)
+template <bool kMap>
+__global__ void __maxnreg__(128) world_step_ep_kernel(const WorldParams prm, const WorldMapParams mp, const float* __restrict__ action,
+                                                      int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived,
+                                                      float* __restrict__ clearance) {
+  world_step_body<kMap, true>(prm, mp, action, out_collided, out_arrived, clearance);
 }
 
 }  // namespace nb

@@ -102,6 +102,9 @@ __device__ __forceinline__ void world_rvo_argmin(double& key, int& idx) {
 
 // __maxnreg__(128) instead of __launch_bounds__(256): with the launch bound ptxas settles on 80 registers and spills around the
 // sincos slow-path call; with the cap it takes 98 and spills nothing (2 CTAs of 8 warps per SM either way).
+// kEp (episode mode): unit b is a slot; a live slot moves the obstacles of scene e = scene_of[b] (goal draws keyed by e, so they do
+// not depend on the slot) with the robots' states of e and the actions of slot rows b K + k; an idle slot is skipped.
+template <bool kEp>
 __global__ void __maxnreg__(128) world_rvo_kernel(const WorldParams prm, const WorldRvoParams rp) {
   extern __shared__ double rsm[];
   const int cap = rp.cap, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -117,7 +120,9 @@ __global__ void __maxnreg__(128) world_rvo_kernel(const WorldParams prm, const W
   double* c_rx = c_ly + cap;
   double* c_ry = c_rx + cap;
   int32_t* nbr = reinterpret_cast<int32_t*>(s_r + cap + (size_t)kWorldRvoWarps * 6 * cap) + (size_t)wid * cap;
-  for (int b = blockIdx.x; b < prm.B; b += gridDim.x) {
+  for (int u = blockIdx.x; u < prm.B; u += gridDim.x) {
+    if (kEp && prm.live[u] == 0) continue;  // block-uniform
+    const int b = kEp ? prm.scene_of[u] : u;  // the scene
     const int o0 = prm.obs_begin[b], n = prm.obs_begin[b + 1] - o0;
     __syncthreads();  // the previous environment's warps are done with the shared rows
     for (int j = threadIdx.x; j < n; j += blockDim.x) {
@@ -126,10 +131,11 @@ __global__ void __maxnreg__(128) world_rvo_kernel(const WorldParams prm, const W
     }
     for (int k = threadIdx.x; k < prm.K; k += blockDim.x) {  // robot k, row n + k: its state point and the velocity of this step's
       const size_t r = (size_t)b * prm.K + k;               // action, as world_integrate computes it
+      const size_t a = (size_t)u * prm.K + k;               // its action's row
       const int t = prm.rtype[r];                           // its own type's velocity model and circumradius
       const double th = prm.states[3 * r + 2];
       double rvx = 0.0, rvy = 0.0;
-      if (prm.collided[r] == 0) world_robot_velocity(prm.types[t].kinematics, (double)rp.action[2 * r], (double)rp.action[2 * r + 1], th, rvx, rvy);
+      if (prm.collided[r] == 0) world_robot_velocity(prm.types[t].kinematics, (double)rp.action[2 * a], (double)rp.action[2 * a + 1], th, rvx, rvy);
       s_cx[n + k] = prm.states[3 * r]; s_cy[n + k] = prm.states[3 * r + 1]; s_vx[n + k] = rvx; s_vy[n + k] = rvy; s_r[n + k] = prm.types[t].r;
     }
     __syncthreads();

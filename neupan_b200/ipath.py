@@ -41,7 +41,7 @@ class InitialPathBatch:
                                close_threshold=float(close_threshold))
         self._handle = C.c_void_p()
         _lib.check(_lib.load().nb_ipath_create(C.byref(cfg), C.byref(self._handle)))
-        self.B, self.P = 0, 0
+        self.B, self.P, self.max_envs = 0, 0, int(max_envs)
 
     def close(self):
         if getattr(self, "_handle", None):
@@ -75,10 +75,14 @@ class InitialPathBatch:
         self.interval = iv
 
     # ---- one control step (neupan.py:114-121) ---------------------------------------------------------------------
-    def step(self, states, cur_vel, ref_speed: float):
+    def step(self, states, cur_vel, ref_speed: float, env_index=None):
         """states (B,3) [x, y, theta]; cur_vel (B,2,T).  Returns (nom_s (B,3,T+1), nom_u (B,2,T), ref_s (B,3,T+1),
-        ref_us (B,T), arrived (B,) int32) on the GPU: the arguments of PAN.forward plus the arrive flags."""
-        dev, B, T = self.device, self.B, self.T
+        ref_us (B,T), arrived (B,) int32) on the GPU: the arguments of PAN.forward plus the arrive flags.  ``env_index`` (B,) int32
+        on the device (nb_ipath_step_ex): row b steps path and state env_index[b] of the paths set, B = len(env_index)."""
+        dev, T = self.device, self.T
+        B = self.B if env_index is None else int(env_index.numel())
+        if env_index is not None:
+            env_index = env_index.to(device=dev, dtype=torch.int32).contiguous()
         states = torch.as_tensor(states).reshape(B, 3).to(device=dev, dtype=torch.float64).contiguous()
         cur_vel = torch.as_tensor(cur_vel).reshape(B, 2, T).to(device=dev, dtype=torch.float32).contiguous()
         mk = lambda *s, dtype=torch.float32: torch.empty(s, dtype=dtype, device=dev)
@@ -86,8 +90,12 @@ class InitialPathBatch:
         ptr = lambda t: C.c_void_p(t.data_ptr())
         with torch.cuda.device(dev):
             stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(_lib.load().nb_ipath_step(self._handle, B, ptr(states), ptr(cur_vel), float(ref_speed), ptr(nom_s), ptr(nom_u), ptr(ref_s),
-                                                 ptr(ref_us), ptr(arrived), stream))
+            if env_index is None:
+                _lib.check(_lib.load().nb_ipath_step(self._handle, B, ptr(states), ptr(cur_vel), float(ref_speed), ptr(nom_s), ptr(nom_u),
+                                                     ptr(ref_s), ptr(ref_us), ptr(arrived), stream))
+            else:
+                _lib.check(_lib.load().nb_ipath_step_ex(self._handle, B, ptr(env_index), ptr(states), ptr(cur_vel), float(ref_speed), ptr(nom_s),
+                                                        ptr(nom_u), ptr(ref_s), ptr(ref_us), ptr(arrived), stream))
         return nom_s, nom_u, ref_s, ref_us, arrived
 
     def reset(self):

@@ -34,13 +34,26 @@ class PlannerBatch:
             pk.setdefault("device", torch.device(device))
         self.pan = PAN(receding, step_time, self.robot, **pk)
         self.device = self.pan.device
-        ik = dict(ipath_kwargs or {})
-        self.ipath = InitialPathBatch(receding, step_time, self.robot.kinematics, self.robot.L, loop=ik.get("loop", False),
-                                      arrive_threshold=ik.get("arrive_threshold", 0.1), close_threshold=ik.get("close_threshold", 0.1),
-                                      ind_range=ik.get("ind_range", 10), arrive_index_threshold=ik.get("arrive_index_threshold", 1),
-                                      max_envs=self.B, device=self.device)
+        self._ipath_kwargs = dict(ipath_kwargs or {})
+        self.ipath = self._make_ipath(self.B)
         self.cur_vel = torch.zeros(self.B, 2, receding, dtype=torch.float32, device=self.device)  # neupan.py:73
         self.info = {}
+
+    def _make_ipath(self, max_envs: int) -> InitialPathBatch:
+        ik = self._ipath_kwargs
+        return InitialPathBatch(self.T, self.dt, self.robot.kinematics, self.robot.L, loop=ik.get("loop", False),
+                                arrive_threshold=ik.get("arrive_threshold", 0.1), close_threshold=ik.get("close_threshold", 0.1),
+                                ind_range=ik.get("ind_range", 10), arrive_index_threshold=ik.get("arrive_index_threshold", 1),
+                                max_envs=max_envs, device=self.device)
+
+    def load_bank(self, paths):
+        """The initial paths of a bank of scenes for continuous episodes (WorldBatch.set_episodes, run_episodes): one per robot of
+        the bank in row order (scene_paths; S K' paths when this planner drives K' robots of each of the slots), any count.  forward
+        with ``scene_of`` then steps row b K' + m on path scene_of[b] K' + m."""
+        if len(paths) > self.ipath.max_envs:
+            self.ipath.close()
+            self.ipath = self._make_ipath(len(paths))
+        self.ipath.set_initial_paths(paths)
 
     def set_initial_paths(self, paths):
         """neupan.set_initial_path (neupan.py:296-303) for every robot."""
@@ -54,12 +67,26 @@ class PlannerBatch:
         self.cur_vel.zero_()
 
     def forward(self, states, ranges=None, scan: dict = None, scan_offset=(0.0, 0.0, 0.0), angle_range=(-np.pi, np.pi), down_sample: int = 1,
-                scan_velocity=None, points=None, point_velocities=None, num_points=None):
+                scan_velocity=None, points=None, point_velocities=None, num_points=None, scene_of=None, reset=None):
         """states (B,3).  Obstacles either as lidar scans (``ranges`` (B,R) + the ``scan`` dict, optional ``scan_velocity``
         (B,2,R)) or as ready point clouds (``points`` (B,2,N), ``point_velocities``, ``num_points``).
+        Continuous episodes (after load_bank): ``scene_of`` (slots,) int32 on the device, the scene each slot runs, with B = slots K';
+        row b K' + m steps path scene_of[b] K' + m.  ``reset`` (slots,) int32: where it is 1 the slot's K' rows start afresh -- cur_vel
+        zeroed and PAN's stop-criterion memory forgotten (nb_pan_reset_envs_async) -- with device ops only.
         Returns (action (B,2) float32 on the device, info)."""
         states = torch.as_tensor(states).reshape(self.B, 3).to(self.device, torch.float64)
-        nom_s, nom_u, ref_s, ref_us, arrived = self.ipath.step(states, self.cur_vel, self.ref_speed)
+        env_index = None
+        if scene_of is not None:
+            scene_of = torch.as_tensor(scene_of, device=self.device)
+            if self.B % scene_of.numel():
+                raise ValueError(f"{self.B} planners do not split into {scene_of.numel()} slots")
+            k = self.B // scene_of.numel()
+            env_index = (scene_of.to(torch.int32)[:, None] * k + torch.arange(k, dtype=torch.int32, device=self.device)).reshape(-1)
+        if reset is not None:
+            rows = torch.as_tensor(reset, device=self.device).to(torch.int32).repeat_interleave(self.B // reset.numel())
+            self.cur_vel = torch.where(rows[:, None, None] != 0, 0.0, self.cur_vel)
+            self.pan.reset_envs(rows)
+        nom_s, nom_u, ref_s, ref_us, arrived = self.ipath.step(states, self.cur_vel, self.ref_speed, env_index=env_index)
         if ranges is not None:
             points, point_velocities, num_points = scan_to_points(states, ranges, scan, scan_offset, angle_range, down_sample,
                                                                   max_points=self.pan.dune_max_num, velocity=scan_velocity, device=self.device)

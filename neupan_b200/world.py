@@ -57,6 +57,13 @@ the rows of one kind, ``scene_paths(scenes, type=i)`` their paths, and ``MixedPl
 ``PlannerBatch`` behind one ``forward``, so ``rollout`` runs a mixed world unchanged.  K = 1 is allowed: one robot per environment,
 of any type (the same seeded scenes with a diff, an acker and an omni robot side by side).
 
+Continuous episodes (nb_world_set_episodes, ``WorldBatch.set_episodes``, ``run_episodes``): a bank of S scenes runs through B
+slots.  When a slot's episode ends (every robot of its scene collided or arrived, or ``max_steps`` steps), the slot takes the next
+unstarted scene on the device: the slots that ended, in ascending order, take the next scenes in ascending order.  Once the bank is
+exhausted a slot goes idle and its scene is frozen.  Each scene runs once in its own rows, so an episode is bitwise the plain run of
+its scene truncated at its end.  The per-scene results are read with ``episodes()``.  Limits: one ``max_steps`` per world, no
+differentiable mode, a single GPU, the bank within ``num_envs`` and device memory, a fixed type per robot index.
+
 There is no CPU implementation here: the CUDA library is the product (oracle/world.py restates it for the tests).
 """
 from __future__ import annotations
@@ -262,6 +269,7 @@ class WorldBatch:
         _lib.check(_lib.load().nb_world_create(C.byref(self.config), C.byref(self._handle)))
         self.O = 0
         self.K, self.N = 1, self.B
+        self._envs, self.S, self.slots = self.B, None, None  # environments on the device; the bank and slots in episode mode
 
     def close(self):
         if getattr(self, "_handle", None):
@@ -282,6 +290,11 @@ class WorldBatch:
         reported as ``map_window`` beyond."""
         if len(scenes) != self.B:
             raise ValueError(f"expected {self.B} scenes, got {len(scenes)}")
+        self._upload(scenes, seed, map_window)
+
+    def _upload(self, scenes, seed: int, map_window: float):
+        """set_scenes for B = len(scenes) <= num_envs environments (the world leaves episode mode)."""
+        B = len(scenes)
         K = fleet_size(scenes)
         packed = pack_scenes_ex(scenes)
         rtype = pack_robot_types(scenes)
@@ -293,7 +306,7 @@ class WorldBatch:
         maps = pack_maps(scenes) if any("map" in sc for sc in scenes) else None
         with torch.cuda.device(self.device):
             lib = _lib.load()
-            fleet_args = (self.B, K, C.c_void_p(fleet.ctypes.data)) if fleet is not None else None
+            fleet_args = (B, K, C.c_void_p(fleet.ctypes.data)) if fleet is not None else None
             types_args = (T, self.types) if T > 0 else None
             if fleet is not None:  # refuse before anything is uploaded
                 if types_args:
@@ -304,19 +317,20 @@ class WorldBatch:
                 rows = pack_fleet(scenes)
                 map_args = (len(maps[0]), maps[0], C.c_void_p(maps[1].ctypes.data),
                             C.c_void_p(maps[2].ctypes.data), C.c_double(float(map_window)))
-                _lib.check(lib.nb_world_check_maps(C.byref(self.config), T, self.types, self.B, K, C.c_void_p(rows.ctypes.data),
+                _lib.check(lib.nb_world_check_maps(C.byref(self.config), T, self.types, B, K, C.c_void_p(rows.ctypes.data),
                                                    C.c_void_p(rtype.ctypes.data), *map_args))
-            _lib.check(lib.nb_world_set_scenes_ex(self._handle, self.B, *_host_ptrs(packed)))
-            self.O, self.K, self.N = int(packed[0][-1]), 1, self.B
+            _lib.check(lib.nb_world_set_scenes_ex(self._handle, B, *_host_ptrs(packed)))
+            self.O, self.K, self.N = int(packed[0][-1]), 1, B
+            self._envs, self.S, self.slots = B, None, None
             self._rows = None
             if beh is not None:
-                _lib.check(lib.nb_world_set_behaviors(self._handle, self.B, C.c_void_p(beh.ctypes.data), C.c_uint64(int(seed))))
+                _lib.check(lib.nb_world_set_behaviors(self._handle, B, C.c_void_p(beh.ctypes.data), C.c_uint64(int(seed))))
             if fleet is not None:
                 if types_args:
                     _lib.check(lib.nb_world_set_fleet_ex(self._handle, *types_args, *fleet_args, C.c_void_p(rtype.ctypes.data)))
                 else:
                     _lib.check(lib.nb_world_set_fleet(self._handle, *fleet_args))
-                self.K, self.N = K, self.B * K
+                self.K, self.N = K, B * K
             if maps is not None:
                 _lib.check(lib.nb_world_set_maps(self._handle, *map_args))
         self.robot_types = rtype
@@ -334,13 +348,78 @@ class WorldBatch:
         g = torch.empty((self.O, 2), dtype=torch.float64, device=self.device)
         d = torch.empty(self.O, dtype=torch.int32, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.load().nb_world_read_behaviors(self._handle, self.B, C.c_void_p(g.data_ptr()), C.c_void_p(d.data_ptr()), self._stream()))
+            _lib.check(_lib.load().nb_world_read_behaviors(self._handle, self._envs, C.c_void_p(g.data_ptr()), C.c_void_p(d.data_ptr()), self._stream()))
         return g, d
 
-    def _read(self, states=None, obstacles=None, collided=None, arrived=None):
+    def _read(self, states=None, obstacles=None, collided=None, arrived=None, rows=None):
         p = lambda t: C.c_void_p(0 if t is None else t.data_ptr())
         with torch.cuda.device(self.device):
-            _lib.check(_lib.load().nb_world_read_state(self._handle, self.N, p(states), p(obstacles), p(collided), p(arrived), self._stream()))
+            _lib.check(_lib.load().nb_world_read_state(self._handle, rows or self.N, p(states), p(obstacles), p(collided), p(arrived),
+                                                       self._stream()))
+
+    # ---- continuous episodes ------------------------------------------------------------------------------------------------
+    def set_episodes(self, scenes, slots: int, max_steps: int, seed: int = 0, map_window: float = 1.0):
+        """Uploads a bank of S = len(scenes) <= num_envs scenes (exactly as set_scenes would for S environments: behaviours keyed by
+        ``seed``, fleets, maps with ``map_window``) and runs it through ``slots`` slots (nb_world_set_episodes): slot b starts on scene
+        b, and when a slot's episode ends (every robot collided or arrived, or ``max_steps`` steps) it takes the next unstarted scene on
+        the device, in ascending slot and scene order; once the bank is exhausted it goes idle.  Afterwards ``N`` is slots K: scan,
+        step, ``states`` and ``flags`` are slot rows (robot k of slot b at row b K + k), ``rows_of_type`` gives slot rows too, and
+        ``episodes()`` the per-scene results.  Every scene of the bank needs the same K, and robot k the same type in every scene.
+        set_scenes leaves episode mode."""
+        check_bank(scenes, slots, max_steps, self.config.max_envs)
+        rtype = pack_robot_types(scenes)
+        S, K = len(scenes), fleet_size(scenes)
+        _lib.check(_lib.load().nb_world_check_episodes(C.byref(self.config), S, K, C.c_void_p(rtype.ctypes.data), int(slots), int(max_steps)))
+        self._upload(scenes, seed, map_window)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nb_world_set_episodes(self._handle, int(slots), int(max_steps)))
+        self.S, self.slots, self.N, self.max_steps = S, int(slots), int(slots) * K, int(max_steps)
+        slot_types = np.tile(rtype[:K], int(slots))  # robot k keeps its type in every scene
+        self._rows = [torch.from_numpy(np.flatnonzero(slot_types == i)).to(self.device) for i in range(len(self.robots))]
+
+    def _read_episodes(self, **out):
+        names = ("collided", "arrived", "arrive_step", "min_clearance", "end_step", "reason", "slot", "scene_of", "reset", "finished")
+        if self.S is None:
+            raise ValueError("not in episode mode (set_episodes)")
+        p = lambda t: C.c_void_p(0 if t is None else t.data_ptr())
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nb_world_read_episodes(self._handle, self.S, *[p(out.get(n)) for n in names], self._stream()))
+
+    def slot_scenes(self):
+        """(scene_of, reset) (slots,) int32 on the device: the scene each slot runs and 1 where a slot has just taken a new scene (every
+        slot right after set_episodes) -- PlannerBatch.forward's ``scene_of`` / ``reset``.  Copies enqueued on the current stream."""
+        sc, rs = (torch.empty(self.slots, dtype=torch.int32, device=self.device) for _ in range(2))
+        self._read_episodes(scene_of=sc, reset=rs)
+        return sc, rs
+
+    def finished(self) -> torch.Tensor:
+        """(1,) int32 on the device: the episodes ended so far."""
+        f = torch.empty(1, dtype=torch.int32, device=self.device)
+        self._read_episodes(finished=f)
+        return f
+
+    def episodes(self) -> dict:
+        """The per-scene results, on the device: per robot of a scene (S K rows, scene s's robot k at s K + k) collided, arrived (bool,
+        the flags at the episode's end), steps_to_arrive (int32, -1 = not arrived: rollout's definition) and min_clearance (float32, the
+        smallest clearance over the episode's steps); per scene (S) end_step (int32, 0 while running), reason (int32: 0 while running,
+        1 every robot collided or arrived, 2 max_steps reached) and slot (int32, the slot that ran it)."""
+        SK, S, dev = self.S * self.K, self.S, self.device
+        out = dict(collided=torch.empty(SK, dtype=torch.int32, device=dev), arrived=torch.empty(SK, dtype=torch.int32, device=dev),
+                   arrive_step=torch.empty(SK, dtype=torch.int32, device=dev), min_clearance=torch.empty(SK, dtype=torch.float32, device=dev),
+                   end_step=torch.empty(S, dtype=torch.int32, device=dev), reason=torch.empty(S, dtype=torch.int32, device=dev),
+                   slot=torch.empty(S, dtype=torch.int32, device=dev))
+        self._read_episodes(**out)
+        return dict(collided=out["collided"].bool(), arrived=out["arrived"].bool(), steps_to_arrive=out["arrive_step"], min_clearance=out["min_clearance"],
+                    end_step=out["end_step"], reason=out["reason"], slot=out["slot"])
+
+    def scene_states(self):
+        """(states (S K,3) float64, collided, arrived (S K,) int32) of the bank's own rows: a scene's final state once its episode has
+        ended (nb_world_read_state with N = S K)."""
+        SK = self.S * self.K
+        s = torch.empty((SK, 3), dtype=torch.float64, device=self.device)
+        c, a = (torch.empty(SK, dtype=torch.int32, device=self.device) for _ in range(2))
+        self._read(states=s, collided=c, arrived=a, rows=SK)
+        return s, c, a
 
     @property
     def states(self) -> torch.Tensor:
@@ -388,6 +467,28 @@ class WorldBatch:
         return col, arr, clear
 
 
+def check_bank(scenes, slots: int, max_steps: int, max_envs: int):
+    """The refusals of WorldBatch.set_episodes on the Python side (ValueError naming the scene and robot): 1 <= S = len(scenes) <=
+    max_envs, 1 <= slots <= S, max_steps >= 1, every scene with the K of scene 0 and robot k of every scene with the type of robot k
+    of scene 0 (nb_world_check_episodes repeats the last on the packed types)."""
+    S = len(scenes)
+    if not 1 <= S <= max_envs:
+        raise ValueError(f"a bank of S = {S} scenes outside [1, max_envs = {max_envs}]")
+    if not 1 <= int(slots) <= S:
+        raise ValueError(f"slots = {slots} outside [1, S = {S}]")
+    if int(max_steps) < 1:
+        raise ValueError(f"max_steps = {max_steps} must be >= 1")
+    robots = [sc["robots"] if "robots" in sc else [sc] for sc in scenes]
+    for s, rb in enumerate(robots):
+        if len(rb) != len(robots[0]):
+            raise ValueError(f"scene {s} has {len(rb)} robots but scene 0 has {len(robots[0])} (every scene of a bank needs the same K)")
+        for k, r in enumerate(rb):
+            t, t0 = int(r.get("type", 0)), int(robots[0][k].get("type", 0))
+            if t != t0:
+                raise ValueError(f"scene {s}, robot {k}: type {t} but robot {k} of scene 0 has type {t0} (a robot keeps its type in every "
+                                 "scene of a bank)")
+
+
 def rollout(planner, world: WorldBatch, steps: int, blind: bool = False, velocities: bool = True):
     """The loop of example/run_exp.py for the world's N robots: scan -> planner.forward -> step, ``steps`` times, all on the device
     and without a host synchronisation of its own.  ``blind``: the planner gets all-range_max scans (it sees nothing) -- the
@@ -410,6 +511,42 @@ def rollout(planner, world: WorldBatch, steps: int, blind: bool = False, velocit
         min_clear = torch.minimum(min_clear, clearance)
     collided, arrived = world.flags()
     return dict(collided=collided.bool(), arrived=arrived.bool(), steps_to_arrive=steps_to_arrive, min_clearance=min_clear)
+
+
+def run_episodes(planner, world: WorldBatch, blind: bool = False, velocities: bool = True, check_every: int = 16):
+    """The loop of ``rollout`` over a bank in episode mode (WorldBatch.set_episodes): scan -> planner.forward (with the world's
+    ``scene_of`` / ``reset``, so that a slot's planner state starts afresh with each scene and steps that scene's path) -> step (whose
+    advance kernel ends episodes and hands out the next scenes), until every scene has finished.  ``planner`` holds the bank's paths
+    (PlannerBatch.load_bank / MixedPlanner.load_bank).  ``blind`` and ``velocities`` as in rollout.  Every ``check_every`` steps
+    the finished count is read to the host: the loop's only host synchronisation, so idle slots cost a planner call for at most
+    ``check_every`` steps after the last episode ends.  Returns WorldBatch.episodes() plus ``steps`` (the loop's step count)."""
+    if world.S is None:
+        raise ValueError("run_episodes needs a world in episode mode (WorldBatch.set_episodes)")
+    check_every = max(1, int(check_every))
+    k = 0
+    while True:
+        episode_steps(planner, world, check_every, blind=blind, velocities=velocities)
+        k += check_every
+        if int(world.finished().item()) >= world.S:  # the host synchronisation
+            break
+    out = world.episodes()
+    out["steps"] = k
+    return out
+
+
+def episode_steps(planner, world: WorldBatch, steps: int, blind: bool = False, velocities: bool = True):
+    """``steps`` steps of run_episodes' loop (scan -> forward with scene_of / reset -> step), without a host synchronisation."""
+    N, dev = world.N, world.device
+    if blind:
+        blind_ranges = torch.full((N, world.R), world.scan_dict["range_max"], dtype=torch.float32, device=dev)
+        blind_vel = torch.zeros((N, 2, world.R), dtype=torch.float32, device=dev)
+        blind_scan = dict(world.scan_dict)
+    for _ in range(steps):
+        scene_of, reset = world.slot_scenes()
+        ranges, vel, scan = (blind_ranges, blind_vel, blind_scan) if blind else world.scan()
+        action, _ = planner.forward(world.states, ranges, scan, scan_offset=world.scan_offset, scan_velocity=vel if velocities else None,
+                                    scene_of=scene_of, reset=reset)
+        world.step(action)
 
 
 class MixedPlanner:
@@ -442,6 +579,12 @@ class MixedPlanner:
             action.index_copy_(0, rows, a)
             infos.append(info)
         return action, infos
+
+    def load_bank(self, scenes):
+        """Each kind's PlannerBatch.load_bank with its robots' paths of the bank (scene_paths(scenes, type=i), i the kind's place in
+        ``groups``): kind i's slot rows b K_i + m then step path row scene_of[b] K_i + m, its m-th robot of scene scene_of[b]."""
+        for i, (pl, _) in enumerate(self.groups):
+            pl.load_bank(scene_paths(scenes, type=i))
 
     def reset(self):
         for pl, _ in self.groups:

@@ -101,5 +101,32 @@ if "world" in SECTIONS:
     torch.cuda.synchronize()
     assert torch.isfinite(w.states).all() and (hit[:5] == 1).any()  # no obstacles, K = 1: the map is index 1
     w.close()
+    # continuous episodes: the episode instantiations of the scan, rvo and step kernels, the advance and slot gather kernels, and the
+    # per-slot ipath and PAN calls, through run_episodes over a bank of 7 scenes in 3 slots (some slots go idle); then a maze bank
+    # with its map through 2 slots, stepped until every slot is idle
+    from helpers import weights_path
+    from neupan_b200 import PlannerBatch, run_episodes
+    from neupan_b200.world import scene_paths
+    c4 = CONFIGS["C4"]
+    pl = PlannerBatch(3, c4.T, c4.dt, 4.0, robot_kwargs=c4.robot_kwargs, adjust_kwargs=dict(c4.adjust),
+                      pan_kwargs=dict(iter_num=2, dune_max_num=100, nrmp_max_num=c4.M, dune_checkpoint=weights_path(c4.model), iter_threshold=0.1,
+                                      max_points=100))
+    scenes = dyna_obs(7, seed=1, behavior="rvo")
+    w = WorldBatch(7, rb, lidar, 0.1)
+    w.set_episodes(scenes, 3, 6, seed=3)
+    pl.load_bank(scene_paths(scenes))
+    out = run_episodes(pl, w, check_every=4)
+    assert (out["reason"] > 0).all()
+    pl.close()
+    w.close()
+    scenes = maze(5, cells=(3, 3), seed=1, layouts=2)
+    w = WorldBatch(5, rb, lidar, 0.1)
+    w.set_episodes(scenes, 2, 3)
+    for _ in range(10):
+        w.scan(hit=True)
+        w.step(torch.full((2, 2), 0.5, device="cuda"))
+    torch.cuda.synchronize()
+    assert int(w.finished().item()) == 5 and torch.isfinite(w.states).all()
+    w.close()
 torch.cuda.synchronize()
 print("sanitize smoke ok")
