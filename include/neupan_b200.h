@@ -440,7 +440,8 @@ int nb_world_set_fleet_ex(nb_world_t* w, int32_t T, const nb_world_robot_type* t
 /* Occupancy maps (this project's reading of IR-SIM's `world: obstacle_map:`; semantics in csrc/world_kernel.cuh): a static grid of
  * width x height square cells of side `resolution` (m), origin (x, y) the lower-left corner of cell (0, 0); cells outside the grid
  * are free.  Each environment uses at most one map and may use none; maps never move and are not obstacles (the obstacle rows of
- * nb_world_read_state do not change; reactive obstacles do not see maps and moving obstacles pass over them).
+ * nb_world_read_state do not change; by default reactive obstacles do not see maps and moving obstacles pass over them, unless
+ * nb_world_set_map_contact below makes an environment's map block its obstacles).
  *   maps (P) HOST; bits uint32 HOST: the maps back to back, each `height` rows of ceil(width/32) words, row j being y index j, bit
  *   (i mod 32) of word i/32 being cell (i, j) (padding bits 0); env_map (B) int32 HOST: each environment's map, -1 for none;
  *   window (0, 10] m, for the whole handle.
@@ -466,6 +467,40 @@ int nb_world_check_maps(const nb_world_config* cfg, int32_t T, const nb_world_ro
                         const int32_t* robot_type, int32_t P, const nb_world_map* maps, const uint32_t* bits, const int32_t* env_map,
                         double window);
 int nb_world_set_maps(nb_world_t* w, int32_t P, const nb_world_map* maps, const uint32_t* bits, const int32_t* env_map, double window);
+
+/* Obstacles in occupancy maps (semantics in csrc/world_kernel.cuh and csrc/world_rvo_kernel.cuh): flags (B) int32 HOST, 1 where an
+ * environment's map blocks its obstacles, 0 (the default, and every environment without this call) where obstacles pass over it.
+ * Where it is 1:
+ *   contact   an obstacle touches the map when its footprint has clearance <= 0 to an occupied cell (a circle: its centre's distance
+ *             to the cell minus r; a convex polygon or an outline: its exact clearance to the cell as a square)
+ *   move      every moving obstacle (constant or reactive) takes, after its move and rectangle mirror (c', v') from (c, v), the first
+ *             of A (c'x, c'y) with (v'x, v'y), B (c'x, cy) with (v'x, -v'y), C (cx, c'y) with (-v'x, v'y), D (cx, cy) with
+ *             (-v'x, -v'y) whose footprint does not touch the map; D always (the start is clear), so no moving obstacle ever touches
+ *             the map.  A step in which A is rejected is a bounce (nb_world_read_map_contact counts them per obstacle).
+ *   reactive  the choice of the velocity is unchanged (the map is not a neighbour and has no cone).  A wander goal is accepted when the
+ *             footprint at the goal does not touch the map and the segment from the centre to the goal keeps a distance > the
+ *             obstacle's circumradius from every occupied cell; a rejected draw uses up its number; at most 16 draws per obstacle and
+ *             step, and when all fail the obstacle parks for the step (goal = its centre) and draws the following numbers at the next
+ *             step.  An obstacle whose move bounced treats its goal as reached at its next step.  A wandering obstacle without an
+ *             explicit goal is set back to goal = its centre and draw 0 by this call, so that its first goal is drawn on the device
+ *             through the test; explicit goals and goals without wander are not tested.
+ * nb_world_set_map_contact comes after nb_world_set_maps (and nb_world_set_behaviors); nb_world_set_scenes(_ex),
+ * nb_world_set_fleet(_ex), nb_world_set_behaviors and nb_world_set_maps drop it, and it leaves episode mode (nb_world_set_episodes
+ * comes after it: then scene s's flag holds for its obstacles in whatever slot runs it).  It zeroes the bounce counts and
+ * synchronises the device.  Without a flag set the kernels launched are those of a world without this call.
+ * Checks (NB_ERR_INVALID, naming the environment and obstacle): every flag is 0 or 1, and 1 only where the environment has a map;
+ * every moving obstacle (v != 0, or reactive) of a blocking environment starts with clearance > 0 to the map, and its top speed times
+ * step_time (|v| for a constant obstacle, sqrt(vxmax^2 + vymax^2) for a reactive one) is below the map's resolution, so that it cannot
+ * jump through a wall at least one cell thick.  Static obstacles may overlap walls.  Occupied cells that meet only at a corner can
+ * still be crossed by a footprint smaller than one step.  nb_world_check_map_contact performs them on the host without a handle or a
+ * device (behaviors NULL: every obstacle keeps its constant velocity).
+ * nb_world_read_map_contact enqueues a device-to-device copy of the O per-obstacle bounce counts on `stream` and does not synchronise.
+ * Not modelled: walls as RVO neighbours (ORCA lines), obstacle-obstacle collisions, moving maps, swept or continuous collision. */
+int nb_world_check_map_contact(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                               const double* vertices, const double* envs, const int32_t* obs_kind, const double* behaviors, int32_t P,
+                               const nb_world_map* maps, const uint32_t* bits, const int32_t* env_map, const int32_t* flags);
+int nb_world_set_map_contact(nb_world_t* w, int32_t B, const int32_t* flags);
+int nb_world_read_map_contact(nb_world_t* w, int32_t O, int32_t* bounces, void* stream);
 
 /* Continuous episodes (semantics in csrc/world_episode_kernel.cuh): a bank of S scenes runs through `slots` slots, and a slot starts
  * the next unstarted scene on the device when its episode ends.  The bank is uploaded as a world of B = S environments

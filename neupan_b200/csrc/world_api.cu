@@ -23,7 +23,7 @@ struct nb_world {
   double *d_vertices = nullptr, *d_env = nullptr, *d_obs = nullptr, *d_states = nullptr;
   double* d_beam_cs = nullptr;  // (R, 2), fixed at creation
   // host copies of the scene (nb_world_set_behaviors checks against them)
-  std::vector<int32_t> h_obs_begin, h_vert_begin;
+  std::vector<int32_t> h_obs_begin, h_vert_begin, h_kind;
   std::vector<double> h_vertices, h_env;
   // obstacle behaviours (nb_world_set_behaviors; nb_world_set_scenes clears them): has_rvo false -> nb_world_step launches only
   // world_step_kernel
@@ -54,6 +54,14 @@ struct nb_world {
   uint32_t* d_bits = nullptr;
   int32_t* d_env_map = nullptr;
   double window = 0.0;
+  // host copies of the maps (nb_world_set_map_contact checks the obstacles' starts against them)
+  std::vector<nb::WorldMap> h_maps;
+  std::vector<uint32_t> h_bits;
+  std::vector<int32_t> h_env_map;
+  // maps that block obstacles (nb_world_set_map_contact; dropped with the maps and by nb_world_set_behaviors): has_block false -> the
+  // kernels' instantiations without it
+  bool has_block = false;
+  int32_t *d_block = nullptr, *d_bounces = nullptr, *d_bounced = nullptr;
   // episode mode (nb_world_set_episodes; every other set call leaves it): ep_slots > 0 slots run the B = S scenes of the bank
   int ep_slots = 0, ep_max_steps = 0;
   int32_t *d_scene_of = nullptr, *d_live = nullptr, *d_reset = nullptr, *d_ep_t = nullptr, *d_ep_count = nullptr;  // count: next, finished
@@ -409,13 +417,93 @@ int world_check_maps(const nb_world_config* cfg, int32_t T, const nb_world_robot
   return NB_OK;
 }
 
-// Frees the maps: the kernels' map-free instantiations from here on.
+// Frees the map-contact arrays: obstacles pass over the maps from here on.
+void world_drop_contact(nb_world* w) {
+  void* old[] = {w->d_block, w->d_bounces, w->d_bounced};
+  for (void* p : old)
+    if (p) cudaFree(p);
+  w->d_block = w->d_bounces = w->d_bounced = nullptr;
+  w->has_block = false;
+}
+
+// Frees the maps (and their contact flags): the kernels' map-free instantiations from here on.
 void world_drop_maps(nb_world* w) {
   void* old[] = {w->d_maps, w->d_bits, w->d_env_map};
   for (void* p : old)
     if (p) cudaFree(p);
   w->d_maps = nullptr; w->d_bits = nullptr; w->d_env_map = nullptr;
   w->has_map = false;
+  w->h_maps.clear(); w->h_bits.clear(); w->h_env_map.clear();
+  world_drop_contact(w);
+}
+
+// Does the footprint of obstacle o at its centre (row) overlap or touch cell [xa, xb] x [ya, yb]?  The host's reading of the
+// kernels' contact test: a circle by its centre's distance to the closed cell, a convex polygon by SAT, an outline by its edges,
+// its vertex 0 in the cell or the cell's corner in it.
+bool world_footprint_meets_cell(const double* row, const double* rel, int nv, int kind, double xa, double ya, double xb, double yb) {
+  const double cell[8] = {xa, ya, xb, ya, xb, yb, xa, yb};
+  if (nv == 0) {
+    const double dx = std::max({xa - row[0], 0.0, row[0] - xb}), dy = std::max({ya - row[1], 0.0, row[1] - yb});
+    return std::sqrt(dx * dx + dy * dy) <= row[4];
+  }
+  double v[2 * nb::kWorldMaxOutlineVertices];
+  for (int k = 0; k < nv; ++k) { v[2 * k] = row[0] + rel[2 * k]; v[2 * k + 1] = row[1] + rel[2 * k + 1]; }
+  if (kind == 0) return world_bodies_meet(v, nv, cell, 4);
+  bool in = false;  // even-odd test of the cell's corner (xa, ya) against the outline
+  for (int k = 0; k < nv; ++k) {
+    const int k1 = (k + 1) % nv;
+    for (int e = 0; e < 4; ++e)
+      if (world_segs_meet(v + 2 * k, v + 2 * k1, cell + 2 * e, cell + 2 * ((e + 1) % 4))) return true;
+    const double ax = v[2 * k], ay = v[2 * k + 1], bx = v[2 * k1], by = v[2 * k1 + 1];
+    if ((ay > ya) != (by > ya) && xa < ax + (ya - ay) * (bx - ax) / (by - ay)) in = !in;
+  }
+  return in || (xa <= v[0] && v[0] <= xb && ya <= v[1] && v[1] <= yb);
+}
+
+// Every check of nb_world_set_map_contact on valid scenes, behaviours (NULL: every obstacle constant) and maps (the device table
+// and its bits); obs holds the obstacles' current centres and velocities.
+int world_check_contact(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obs, const int32_t* vert_begin,
+                        const double* vertices, const int32_t* kind, const double* beh, const std::vector<nb::WorldMap>& maps, const uint32_t* bits,
+                        const int32_t* env_map, const int32_t* flags) {
+  if (!flags) return fail(NB_ERR_INVALID, "nb_world map contact: null flags");
+  const double dt = cfg->step_time;
+  for (int b = 0; b < B; ++b) {
+    if (flags[b] != 0 && flags[b] != 1) return fail(NB_ERR_INVALID, "environment %d: map contact flag %d (0 or 1)", b, flags[b]);
+    if (flags[b] == 0) continue;
+    if (env_map[b] < 0) return fail(NB_ERR_INVALID, "environment %d: its map blocks obstacles but it has no map", b);
+    const nb::WorldMap& m = maps[env_map[b]];
+    for (int o = obs_begin[b]; o < obs_begin[b + 1]; ++o) {
+      const double* row = obs + (size_t)nb::kWorldObsCols * o;
+      const double* br = beh ? beh + (size_t)nb::kWorldBehCols * o : nullptr;
+      const bool reactive = br && br[0] == 1.0;
+      if (!reactive && row[2] == 0.0 && row[3] == 0.0) continue;  // static obstacles may overlap walls
+      const double top = reactive ? std::sqrt(br[1] * br[1] + br[2] * br[2]) : std::sqrt(row[2] * row[2] + row[3] * row[3]);
+      if (!(top * dt < m.r))
+        return fail(NB_ERR_INVALID, "environment %d, obstacle %d: top speed %g m/s * step_time = %g m is not below the map's resolution %g m", b, o,
+                    top, top * dt, m.r);
+      const int v0 = vert_begin[o], nv = vert_begin[o + 1] - v0;
+      const double* rel = vertices + 2 * (size_t)v0;
+      double xmin = row[0] - row[4], xmax = row[0] + row[4], ymin = row[1] - row[4], ymax = row[1] + row[4];
+      if (nv > 0) {
+        xmin = ymin = INFINITY; xmax = ymax = -INFINITY;
+        for (int k = 0; k < nv; ++k) {
+          xmin = std::min(xmin, row[0] + rel[2 * k]); xmax = std::max(xmax, row[0] + rel[2 * k]);
+          ymin = std::min(ymin, row[1] + rel[2 * k + 1]); ymax = std::max(ymax, row[1] + rel[2 * k + 1]);
+        }
+      }
+      const int i0 = std::max(map_floor(xmin, m.x0, m.r, m.W) - 1, 0), i1 = std::min(map_floor(xmax, m.x0, m.r, m.W) + 1, m.W - 1);
+      const int j0 = std::max(map_floor(ymin, m.y0, m.r, m.H) - 1, 0), j1 = std::min(map_floor(ymax, m.y0, m.r, m.H) + 1, m.H - 1);
+      for (int j = j0; j <= j1; ++j)
+        for (int i = i0; i <= i1; ++i) {
+          if (!((bits[m.off + (int64_t)j * m.words + (i >> 5)] >> (i & 31)) & 1u)) continue;
+          if (world_footprint_meets_cell(row, rel, nv, kind ? kind[o] : 0, map_line(m.x0, m.r, i), map_line(m.y0, m.r, j), map_line(m.x0, m.r, i + 1),
+                                         map_line(m.y0, m.r, j + 1)))
+            return fail(NB_ERR_INVALID, "environment %d, obstacle %d: moves but its start footprint overlaps or touches occupied cell (%d, %d) of map %d",
+                        b, o, i, j, env_map[b]);
+        }
+    }
+  }
+  return NB_OK;
 }
 
 // Leaves episode mode: frees the slot and result arrays (the scenes' own rows stay as they are).
@@ -448,6 +536,7 @@ int world_check_episodes(const nb_world_config* cfg, int32_t S, int32_t K, const
 }
 
 nb::WorldMapParams world_map_params(const nb_world* w) { return nb::WorldMapParams{w->d_maps, w->d_bits, w->d_env_map, w->window}; }
+nb::WorldBlockParams world_block_params(const nb_world* w) { return nb::WorldBlockParams{w->d_block, w->d_bounces, w->d_bounced}; }
 
 template <bool kMap>
 int world_scan_occupancy(nb_world* w, int* per_sm) {
@@ -612,7 +701,7 @@ int nb_world_destroy(nb_world_t* w) {
   world_drop_episodes(w);
   void* bufs[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
                   w->d_states, w->d_beam_cs, w->d_beh, w->d_rad, w->d_goal, w->d_draws, w->d_fgoal, w->d_fvel, w->d_types, w->d_rtype,
-                  w->d_maps, w->d_bits, w->d_env_map};
+                  w->d_maps, w->d_bits, w->d_env_map, w->d_block, w->d_bounces, w->d_bounced};
   for (void* b : bufs)
     if (b) cudaFree(b);
   delete w;
@@ -654,6 +743,8 @@ int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, c
   w->h_obs_begin.assign(obs_begin, obs_begin + B + 1);
   w->h_vert_begin.assign(vert_begin, vert_begin + O + 1);
   w->h_vertices.assign(vertices, vertices + 2 * (size_t)V);
+  if (obs_kind) w->h_kind.assign(obs_kind, obs_kind + O);
+  else w->h_kind.assign(O, 0);
   w->h_env.assign(envs, envs + (size_t)nb::kWorldEnvCols * B);
   NB_CUDA(dalloc(&w->d_obs_begin, (size_t)B + 1));
   NB_CUDA(dalloc(&w->d_vert_begin, (size_t)O + 1));
@@ -700,6 +791,7 @@ int nb_world_set_behaviors(nb_world_t* w, int32_t B, const double* behaviors, ui
   if (O) NB_CUDA(cudaMemcpy(obs.data(), w->d_obs, sizeof(double) * obs.size(), cudaMemcpyDeviceToHost));  // the current centres
   if (int rc = world_check_behaviors(&w->cfg, B, w->h_obs_begin.data(), obs.data(), w->h_env.data(), behaviors)) return rc;
   world_drop_episodes(w);
+  world_drop_contact(w);  // which obstacles move has changed: the contact flags need their checks again
   // radii (circle: its own; polygon: the largest vertex norm), initial goals (NaN: draw 0) and draw counters
   std::vector<double> rad(O), goal(2 * (size_t)O, 0.0);
   std::vector<int32_t> draws(O, 0);
@@ -786,18 +878,30 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
   NB_CUDA(cudaSetDevice(w->cfg.device));
   const nb::WorldParams prm = world_params(w);  // prm.B: the environments, or the slots in episode mode
   if (w->has_rvo) {  // reactive obstacles choose their velocities from the states at the start of the step
-    auto* rvo = w->ep_slots ? nb::world_rvo_kernel<true> : nb::world_rvo_kernel<false>;
-    NB_CUDA(cudaFuncSetAttribute(rvo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
-    rvo<<<std::min(w->rvo_grid, prm.B), 32 * nb::kWorldRvoWarps, w->rvo_smem, (cudaStream_t)stream>>>(prm, world_rvo_params(w, action));
+    const int grid = std::min(w->rvo_grid, prm.B);
+    if (w->has_block) {
+      auto* rvo = w->ep_slots ? nb::world_rvo_block_kernel<true> : nb::world_rvo_block_kernel<false>;
+      NB_CUDA(cudaFuncSetAttribute(rvo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
+      rvo<<<grid, 32 * nb::kWorldRvoWarps, w->rvo_smem, (cudaStream_t)stream>>>(prm, world_rvo_params(w, action), world_map_params(w), world_block_params(w));
+    } else {
+      auto* rvo = w->ep_slots ? nb::world_rvo_kernel<true> : nb::world_rvo_kernel<false>;
+      NB_CUDA(cudaFuncSetAttribute(rvo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
+      rvo<<<grid, 32 * nb::kWorldRvoWarps, w->rvo_smem, (cudaStream_t)stream>>>(prm, world_rvo_params(w, action));
+    }
     ++nb::launches;
     NB_CUDA(cudaGetLastError());
   }
   // a CTA of up to 8 warps per E environments, a warp per robot
   const int E = nb::world_step_envs(w->K);
-  auto* kernel = w->ep_slots ? (w->has_map ? nb::world_step_ep_kernel<true> : nb::world_step_ep_kernel<false>)
-                             : (w->has_map ? nb::world_step_kernel<true> : nb::world_step_kernel<false>);
-  kernel<<<(prm.B + E - 1) / E, 32 * std::min(E * w->K, nb::kWorldStepMaxWarps), 0, (cudaStream_t)stream>>>(prm, world_map_params(w),
-                                                                                                           action, collided, arrived, clearance);
+  const dim3 grid((prm.B + E - 1) / E), block(32 * std::min(E * w->K, nb::kWorldStepMaxWarps));
+  if (w->has_block) {
+    auto* kernel = w->ep_slots ? nb::world_step_block_kernel<true> : nb::world_step_block_kernel<false>;
+    kernel<<<grid, block, 0, (cudaStream_t)stream>>>(prm, world_map_params(w), world_block_params(w), action, collided, arrived, clearance);
+  } else {
+    auto* kernel = w->ep_slots ? (w->has_map ? nb::world_step_ep_kernel<true> : nb::world_step_ep_kernel<false>)
+                               : (w->has_map ? nb::world_step_kernel<true> : nb::world_step_kernel<false>);
+    kernel<<<grid, block, 0, (cudaStream_t)stream>>>(prm, world_map_params(w), action, collided, arrived, clearance);
+  }
   ++nb::launches;
   NB_CUDA(cudaGetLastError());
   if (w->ep_slots) {  // end the episodes of this step and hand out the next scenes
@@ -899,6 +1003,9 @@ int nb_world_set_maps(nb_world_t* w, int32_t P, const nb_world_map* maps, const 
   }
   w->has_map = std::any_of(env_map, env_map + w->B, [](int32_t m) { return m >= 0; });
   w->window = window;
+  w->h_maps = table;
+  w->h_bits.assign(bits, bits + words);
+  w->h_env_map.assign(env_map, env_map + w->B);
   if (int rc = world_scan_shape(w, w->B)) return rc;
   NB_CUDA(cudaDeviceSynchronize());
   return NB_OK;
@@ -971,6 +1078,81 @@ int nb_world_read_episodes(nb_world_t* w, int32_t S, int32_t* collided, int32_t*
   NB_CUDA(cp(scene_of, w->d_scene_of, w->ep_slots * sizeof(int32_t)));
   NB_CUDA(cp(reset, w->d_reset, w->ep_slots * sizeof(int32_t)));
   NB_CUDA(cp(finished, w->d_ep_count + 1, sizeof(int32_t)));
+  return NB_OK;
+}
+
+int nb_world_check_map_contact(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                               const double* vertices, const double* envs, const int32_t* obs_kind, const double* behaviors, int32_t P,
+                               const nb_world_map* maps, const uint32_t* bits, const int32_t* env_map, const int32_t* flags) {
+  if (int rc = world_check_scenes(cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, obs_kind, nullptr, nullptr, nullptr, nullptr)) return rc;
+  if (behaviors)
+    if (int rc = world_check_behaviors(cfg, B, obs_begin, obstacles, envs, behaviors)) return rc;
+  std::vector<nb::WorldMap> table;
+  if (int rc = world_check_maps(cfg, 0, nullptr, B, 1, nullptr, nullptr, P, maps, bits, env_map, 1.0, &table)) return rc;
+  return world_check_contact(cfg, B, obs_begin, obstacles, vert_begin, vertices, obs_kind, behaviors, table, bits, env_map, flags);
+}
+
+int nb_world_set_map_contact(nb_world_t* w, int32_t B, const int32_t* flags) {
+  if (int rc = world_ready(w, B, "nb_world_set_map_contact")) return rc;
+  if (!w->d_maps) return fail(NB_ERR_INVALID, "nb_world_set_map_contact: no maps set (nb_world_set_maps)");
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  const int O = w->O;
+  std::vector<double> obs((size_t)nb::kWorldObsCols * O), beh;
+  if (O) NB_CUDA(cudaMemcpy(obs.data(), w->d_obs, sizeof(double) * obs.size(), cudaMemcpyDeviceToHost));  // the current centres
+  if (w->d_beh && O) {
+    beh.resize((size_t)nb::kWorldBehCols * O);
+    NB_CUDA(cudaMemcpy(beh.data(), w->d_beh, sizeof(double) * beh.size(), cudaMemcpyDeviceToHost));
+  }
+  if (int rc = world_check_contact(&w->cfg, B, w->h_obs_begin.data(), obs.data(), w->h_vert_begin.data(), w->h_vertices.data(), w->h_kind.data(),
+                                   beh.empty() ? nullptr : beh.data(), w->h_maps, w->h_bits.data(), w->h_env_map.data(), flags))
+    return rc;
+  world_drop_contact(w);
+  world_drop_episodes(w);
+  // a wandering obstacle without an explicit goal in a blocking environment starts from goal = its centre and draw 0, so that its
+  // first goal is drawn on the device through the map test
+  std::vector<double> goal;
+  std::vector<int32_t> draws;
+  bool reset = false;
+  if (!beh.empty()) {
+    goal.resize(2 * (size_t)O); draws.resize(O);
+    NB_CUDA(cudaMemcpy(goal.data(), w->d_goal, sizeof(double) * goal.size(), cudaMemcpyDeviceToHost));
+    NB_CUDA(cudaMemcpy(draws.data(), w->d_draws, sizeof(int32_t) * O, cudaMemcpyDeviceToHost));
+    for (int b = 0; b < B; ++b) {
+      if (!flags[b]) continue;
+      for (int o = w->h_obs_begin[b]; o < w->h_obs_begin[b + 1]; ++o) {
+        const double* r = beh.data() + (size_t)nb::kWorldBehCols * o;
+        if (r[0] != 1.0 || r[6] == 0.0 || !std::isnan(r[7])) continue;
+        goal[2 * o] = obs[(size_t)nb::kWorldObsCols * o]; goal[2 * o + 1] = obs[(size_t)nb::kWorldObsCols * o + 1];
+        draws[o] = 0;
+        reset = true;
+      }
+    }
+  }
+  cudaError_t e = nb::dalloc(&w->d_block, (size_t)B);
+  if (e == cudaSuccess) e = nb::dalloc(&w->d_bounces, std::max<size_t>(O, 1));
+  if (e == cudaSuccess) e = nb::dalloc(&w->d_bounced, std::max<size_t>(O, 1));
+  if (e == cudaSuccess) e = cudaMemcpy(w->d_block, flags, sizeof(int32_t) * B, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemset(w->d_bounces, 0, sizeof(int32_t) * std::max(O, 1));
+  if (e == cudaSuccess) e = cudaMemset(w->d_bounced, 0, sizeof(int32_t) * std::max(O, 1));
+  if (e == cudaSuccess && reset) e = cudaMemcpy(w->d_goal, goal.data(), sizeof(double) * goal.size(), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && reset) e = cudaMemcpy(w->d_draws, draws.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    world_drop_contact(w);
+    return fail(NB_ERR_CUDA, "nb_world_set_map_contact: %s", cudaGetErrorString(e));
+  }
+  w->has_block = std::any_of(flags, flags + B, [](int32_t f) { return f != 0; });
+  return NB_OK;
+}
+
+int nb_world_read_map_contact(nb_world_t* w, int32_t O, int32_t* bounces, void* stream) {
+  if (!w) return fail(NB_ERR_INVALID, "nb_world_read_map_contact: null handle");
+  if (!w->d_bounces) return fail(NB_ERR_INVALID, "nb_world_read_map_contact: no map contact set (nb_world_set_map_contact)");
+  if (O != w->O) return fail(NB_ERR_INVALID, "nb_world_read_map_contact: O = %d but the scenes have %d obstacles", O, w->O);
+  if (!bounces) return fail(NB_ERR_INVALID, "nb_world_read_map_contact: null bounces");
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  if (O) NB_CUDA(cudaMemcpyAsync(bounces, w->d_bounces, sizeof(int32_t) * O, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return NB_OK;
 }
 

@@ -30,7 +30,8 @@
 // grid of W x H square cells of side r whose origin (x0, y0) is the lower-left corner of cell (0, 0); cell (i, j) is
 // [X(i), X(i+1)] x [Y(j), Y(j+1)] with X(i) = dadd(x0, dmul((double)i, r)), Y(j) likewise -- every corner is computed this way,
 // nothing is accumulated.  Cells outside the grid are free (a border is a wall only if the map draws one).  A map is a kind of
-// scene, not an obstacle: the obstacle rows do not change, and reactive obstacles do not see it and moving obstacles pass over it.
+// scene, not an obstacle: the obstacle rows do not change, and unless the map blocks obstacles (nb_world_set_map_contact, "obstacles
+// in occupancy maps" below) reactive obstacles do not see it and moving obstacles pass over it.
 // Both kernels take the map path as a compile-time variant (kMap), launched only when some environment of the handle has a map:
 //   scan  after the shape and robot tests, the beam walks the grid cell by cell (world_map_cast) and reports the first t > 0 at
 //         which it crosses from a cell of one state into a cell of the other, with index O_b + K (after the obstacles and the
@@ -415,18 +416,22 @@ __device__ __forceinline__ bool world_segs_meet(double px, double py, double qx,
 // The even-odd test of robot vertex 0 shares the edge loop of the segment tests (separate loops spill): an outline edge that
 // straddles the horizontal line through the vertex toggles it when it crosses that line to the vertex's right, which is the sign
 // of the cross product edge x (vertex - edge start) -- no division.
-__device__ __forceinline__ double world_outline_clearance(const WorldPoly& op, const double* rx, const double* ry, int nr) {
+// The convex side is any vertex accessor (vx, vy, nv): the robot's world vertices, or an occupancy cell (WorldCell) when an outline
+// obstacle meets a map.
+template <class PC>
+__device__ __forceinline__ double world_outline_clearance(const WorldPoly& op, const PC& c) {
+  const int nr = c.nv;
   bool in = false;
   for (int k = 0; k < op.nv; ++k) {
     const int k1 = k + 1 < op.nv ? k + 1 : 0;
     const double ax = op.vx(k), ay = op.vy(k), bx = op.vx(k1), by = op.vy(k1);
     for (int i = 0; i < nr; ++i) {
       const int i1 = i + 1 < nr ? i + 1 : 0;
-      if (world_segs_meet(rx[i], ry[i], rx[i1], ry[i1], ax, ay, bx, by)) return 0.0;
+      if (world_segs_meet(c.vx(i), c.vy(i), c.vx(i1), c.vy(i1), ax, ay, bx, by)) return 0.0;
     }
-    if ((ay > ry[0]) != (by > ry[0])) {
-      const double c = dcross(dsub(bx, ax), dsub(by, ay), dsub(rx[0], ax), dsub(ry[0], ay));
-      if (by > ay ? c > 0.0 : c < 0.0) in = !in;
+    if ((ay > c.vy(0)) != (by > c.vy(0))) {
+      const double cr = dcross(dsub(bx, ax), dsub(by, ay), dsub(c.vx(0), ax), dsub(c.vy(0), ay));
+      if (by > ay ? cr > 0.0 : cr < 0.0) in = !in;
     }
   }
   if (in) return 0.0;
@@ -435,7 +440,7 @@ __device__ __forceinline__ double world_outline_clearance(const WorldPoly& op, c
     bool pos = false, neg = false;
     for (int k = 0; k < nr; ++k) {
       const int k1 = k + 1 < nr ? k + 1 : 0;
-      const double cr = dcross(dsub(rx[k1], rx[k]), dsub(ry[k1], ry[k]), dsub(px, rx[k]), dsub(py, ry[k]));
+      const double cr = dcross(dsub(c.vx(k1), c.vx(k)), dsub(c.vy(k1), c.vy(k)), dsub(px, c.vx(k)), dsub(py, c.vy(k)));
       pos |= cr > 0.0; neg |= cr < 0.0;
     }
     if (!(pos && neg)) return 0.0;
@@ -444,11 +449,11 @@ __device__ __forceinline__ double world_outline_clearance(const WorldPoly& op, c
   for (int k = 0; k < op.nv; ++k) {
     const int k1 = k + 1 < op.nv ? k + 1 : 0;
     const double ax = op.vx(k), ay = op.vy(k), bx = op.vx(k1), by = op.vy(k1);
-    for (int i = 0; i < nr; ++i) d = fmin(d, world_seg_dist(rx[i], ry[i], ax, ay, bx, by));
+    for (int i = 0; i < nr; ++i) d = fmin(d, world_seg_dist(c.vx(i), c.vy(i), ax, ay, bx, by));
   }
   for (int k = 0; k < nr; ++k) {
     const int k1 = k + 1 < nr ? k + 1 : 0;
-    for (int i = 0; i < op.nv; ++i) d = fmin(d, world_seg_dist(op.vx(i), op.vy(i), rx[k], ry[k], rx[k1], ry[k1]));
+    for (int i = 0; i < op.nv; ++i) d = fmin(d, world_seg_dist(op.vx(i), op.vy(i), c.vx(k), c.vy(k), c.vx(k1), c.vy(k1)));
   }
   return d;
 }
@@ -510,7 +515,7 @@ __device__ __forceinline__ double world_obstacle_clearance(const WorldParams& pr
     }
     return (pos && neg) ? dsub(d, prm.obs[(size_t)kWorldObsCols * o + 4]) : 0.0;  // centre inside the robot: overlap
   }
-  if (prm.kind[o] != 0) return world_outline_clearance(WorldPoly{prm.vertices + 2 * (size_t)v0, cx, cy, nv}, rx, ry, nr);
+  if (prm.kind[o] != 0) return world_outline_clearance(WorldPoly{prm.vertices + 2 * (size_t)v0, cx, cy, nv}, WorldRobot{rx, ry, nr});
   // convex polygon: 0 unless an edge normal separates them, then the smallest vertex-edge distance
   const WorldPoly op{prm.vertices + 2 * (size_t)v0, cx, cy, nv};
   const WorldRobot rp{rx, ry, nr};
@@ -591,6 +596,131 @@ __device__ __forceinline__ double world_map_clearance(const WorldMap& m, const u
   return d;
 }
 
+// ---- obstacles in occupancy maps (nb_world_set_map_contact) -----------------------------------------------------------------
+//
+// In an environment whose map blocks obstacles, an obstacle touches the map when its footprint has clearance <= 0 to an occupied
+// cell (touch counts, as for the robots): a circle when its centre's distance to the closed cell is <= r, a convex polygon by
+// world_convex_clearance against the cell, an outline by world_outline_clearance with the cell as the convex side.  Every moving
+// obstacle takes the first of these that does not touch the map, (c', v') being the move and mirror of world_move_obstacle from
+// (c, v): A (c'x, c'y) with (v'x, v'y); B (c'x, cy) with (v'x, -v'y); C (cx, c'y) with (-v'x, v'y); D (cx, cy) with (-v'x, -v'y).
+// D is always taken when A..C touch (the start is clear: checked on the host, then kept by induction).  A step that rejects A is
+// a bounce.  Only the occupied cells that meet a bounding box widened by one cell are visited (world_map_any).
+
+// Segment p-q as a two-vertex convex polygon (its two edges are p-q and q-p, whose normals are the segment's normal): SAT and the
+// vertex-edge distances of world_convex_clearance then give the segment's distance to a convex polygon (0 when they meet).
+struct WorldSeg {
+  double px, py, qx, qy;
+  static constexpr int nv = 2;
+  __device__ __forceinline__ double vx(int k) const { return k ? qx : px; }
+  __device__ __forceinline__ double vy(int k) const { return k ? qy : py; }
+};
+
+// An obstacle's footprint centred at (cx, cy): a circle of radius r (nv == 0), a convex polygon or an outline (kind 1).
+struct WorldFootprint {
+  const double* rel;
+  double cx, cy, r;
+  int nv, kind;
+  __device__ __forceinline__ WorldPoly poly() const { return WorldPoly{rel, cx, cy, nv}; }
+  // its bounding box (xmin, ymin, xmax, ymax)
+  __device__ __forceinline__ void box(double& x0, double& y0, double& x1, double& y1) const {
+    if (nv == 0) { x0 = dsub(cx, r); y0 = dsub(cy, r); x1 = dadd(cx, r); y1 = dadd(cy, r); return; }
+    x0 = x1 = dadd(cx, rel[0]); y0 = y1 = dadd(cy, rel[1]);
+    for (int k = 1; k < nv; ++k) {
+      const double x = dadd(cx, rel[2 * k]), y = dadd(cy, rel[2 * k + 1]);
+      x0 = fmin(x0, x); x1 = fmax(x1, x); y0 = fmin(y0, y); y1 = fmax(y1, y);
+    }
+  }
+  __device__ __forceinline__ bool touches(const WorldCell& c) const {
+    if (nv == 0) {
+      if (c.xa <= cx && cx <= c.xb && c.ya <= cy && cy <= c.yb) return true;
+      double d = INFINITY;
+      for (int k = 0; k < 4; ++k) {
+        const int k1 = (k + 1) & 3;
+        d = fmin(d, world_seg_dist(cx, cy, c.vx(k), c.vy(k), c.vx(k1), c.vy(k1)));
+      }
+      return dsub(d, r) <= 0.0;
+    }
+    return (kind != 0 ? world_outline_clearance(poly(), c) : world_convex_clearance(poly(), c)) <= 0.0;
+  }
+};
+
+__device__ __forceinline__ WorldFootprint world_footprint(const WorldParams& prm, int o, double cx, double cy) {
+  const int v0 = prm.vert_begin[o];
+  return WorldFootprint{prm.vertices + 2 * (size_t)v0, cx, cy, prm.obs[(size_t)kWorldObsCols * o + 4], prm.vert_begin[o + 1] - v0, prm.kind[o]};
+}
+
+// Is hit(cell) true for an occupied cell of map m that meets [x0, x1] x [y0, y1] widened by one cell on each side?  This thread
+// takes the (row, word) pairs first, first + stride, ... of that range (a warp: lane, 32; a thread alone: 0, 1) and stops at its
+// first hit; a warp ORs its lanes' answers.
+template <class F>
+__device__ __forceinline__ bool world_map_any(const WorldMap& m, const uint32_t* bits, double x0, double y0, double x1, double y1, int first,
+                                              int stride, const F& hit) {
+  const int i0 = max(world_map_floor(x0, m.x0, m.r, m.W) - 1, 0), i1 = min(world_map_floor(x1, m.x0, m.r, m.W) + 1, m.W - 1);
+  const int j0 = max(world_map_floor(y0, m.y0, m.r, m.H) - 1, 0), j1 = min(world_map_floor(y1, m.y0, m.r, m.H) + 1, m.H - 1);
+  if (i0 > i1 || j0 > j1) return false;
+  const int w0 = i0 >> 5, nw = (i1 >> 5) - w0 + 1;
+  for (int p = first; p < (j1 - j0 + 1) * nw; p += stride) {
+    const int j = j0 + p / nw, wd = w0 + p % nw, lo = i0 - 32 * wd, hi = i1 - 32 * wd;
+    uint32_t word = __ldg(bits + m.off + (int64_t)j * m.words + wd);
+    if (lo > 0) word &= ~0u << lo;
+    if (hi < 31) word &= (2u << hi) - 1u;
+    while (word) {
+      const int i = 32 * wd + __ffs(word) - 1;
+      word &= word - 1u;
+      if (hit(WorldCell{world_map_line(m.x0, m.r, i), world_map_line(m.y0, m.r, j), world_map_line(m.x0, m.r, i + 1),
+                        world_map_line(m.y0, m.r, j + 1)}))
+        return true;
+    }
+  }
+  return false;
+}
+
+// Does the footprint touch map m?  One thread (first, stride = 0, 1) or a warp (lane, 32, then __any_sync by the caller).
+__device__ __forceinline__ bool world_footprint_touches(const WorldMap& m, const uint32_t* bits, const WorldFootprint& f, int first, int stride) {
+  double x0, y0, x1, y1;
+  f.box(x0, y0, x1, y1);
+  return world_map_any(m, bits, x0, y0, x1, y1, first, stride, [&](const WorldCell& c) { return f.touches(c); });
+}
+
+// The map-contact arrays of a handle whose maps block obstacles somewhere (read by the kBlock instantiations only)
+struct WorldBlockParams {
+  const int32_t* block;  // (B) 1: the environment's map blocks its obstacles
+  int32_t* bounces;      // (O) steps in which the obstacle's move A was rejected
+  int32_t* bounced;      // (O) 1: rejected in the last step (a reactive obstacle then treats its goal as reached)
+};
+
+// world_move_obstacle, then in an environment e whose map blocks obstacles the move rule above for an obstacle that moves (v != 0).
+__device__ __forceinline__ void world_move_obstacle_blocked(const WorldParams& prm, const WorldMapParams& mp, const WorldBlockParams& bp, int e, int o) {
+  double* row = prm.obs + (size_t)kWorldObsCols * o;
+  const double x = row[0], y = row[1];
+  const bool moves = row[2] != 0.0 || row[3] != 0.0;
+  double cx, cy;
+  world_move_obstacle(prm, prm.env + (size_t)kWorldEnvCols * e, o, cx, cy);
+  if (bp.block[e] == 0) return;
+  int bounced = 0;
+  if (moves) {
+    const WorldMap& m = mp.maps[mp.env_map[e]];
+    WorldFootprint f = world_footprint(prm, o, cx, cy);
+    if (world_footprint_touches(m, mp.bits, f, 0, 1)) {
+      bounced = 1;
+      const double vx = row[2], vy = row[3];
+      f.cy = y;
+      if (!world_footprint_touches(m, mp.bits, f, 0, 1)) {
+        row[1] = y; row[3] = -vy;  // B
+      } else {
+        f.cx = x; f.cy = cy;
+        if (!world_footprint_touches(m, mp.bits, f, 0, 1)) {
+          row[0] = x; row[2] = -vx;  // C
+        } else {
+          row[0] = x; row[1] = y; row[2] = -vx; row[3] = -vy;  // D
+        }
+      }
+      bp.bounces[o] += 1;
+    }
+  }
+  bp.bounced[o] = bounced;
+}
+
 // One CTA per E = world_step_envs(K) environments, 32 min(E K, 8) threads (grid = ceil(B / E)); its robots are the slots
 // s = n - b0 K of the rows n of its environments b0 .. b0 + E - 1.  Phase 1: thread s integrates robot s from the state at the start
 // of the step (unless it has collided), writes its state, arrival flag, world vertices and velocity; every thread moves obstacles.
@@ -602,8 +732,8 @@ __device__ __forceinline__ double world_map_clearance(const WorldMap& m, const u
 // kEp (episode mode): the CTA's units are slots b0 .. b0 + E - 1; a live slot steps the robots and obstacles of scene scene_of[b]
 // (the scene's rows) and writes its outputs to slot rows q = b K + k, its clearances also to ep_clear; an idle slot's scene is not
 // touched, and its outputs are the frozen flags and clearance +inf.
-template <bool kMap, bool kEp>
-__device__ __forceinline__ void world_step_body(const WorldParams& prm, const WorldMapParams& mp, const float* __restrict__ action,
+template <bool kMap, bool kEp, bool kBlock>
+__device__ __forceinline__ void world_step_body(const WorldParams& prm, const WorldMapParams& mp, const WorldBlockParams& bp, const float* __restrict__ action,
                                                 int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived, float* __restrict__ clearance) {
   __shared__ double f_x[kWorldMaxFleet][kWorldMaxVertices], f_y[kWorldMaxFleet][kWorldMaxVertices];  // E K <= 8 or K <= 16 slots
   __shared__ double f_v[kWorldMaxFleet][2];
@@ -645,16 +775,24 @@ __device__ __forceinline__ void world_step_body(const WorldParams& prm, const Wo
       if (prm.live[b0 + j] == 0) continue;
       const int e = prm.scene_of[b0 + j];
       for (int o = prm.obs_begin[e] + (int)threadIdx.x; o < prm.obs_begin[e + 1]; o += blockDim.x) {
-        double cx, cy;
-        world_move_obstacle(prm, prm.env + (size_t)kWorldEnvCols * e, o, cx, cy);
+        if constexpr (kBlock) {
+          world_move_obstacle_blocked(prm, mp, bp, e, o);
+        } else {
+          double cx, cy;
+          world_move_obstacle(prm, prm.env + (size_t)kWorldEnvCols * e, o, cx, cy);
+        }
       }
     }
   } else {
     int b = b0;  // the environment of obstacle o: the CTA's obstacle rows are its environments' back to back
     for (int o = prm.obs_begin[b0] + (int)threadIdx.x; o < prm.obs_begin[b0 + nslot / K]; o += blockDim.x) {
       while (o >= prm.obs_begin[b + 1]) ++b;
-      double cx, cy;
-      world_move_obstacle(prm, prm.env + (size_t)kWorldEnvCols * b, o, cx, cy);
+      if constexpr (kBlock) {
+        world_move_obstacle_blocked(prm, mp, bp, b, o);
+      } else {
+        double cx, cy;
+        world_move_obstacle(prm, prm.env + (size_t)kWorldEnvCols * b, o, cx, cy);
+      }
     }
   }
   __syncthreads();  // bodies, velocities and the moved obstacle rows are visible to the whole CTA
@@ -703,7 +841,7 @@ template <bool kMap>
 __global__ void __launch_bounds__(32 * kWorldStepMaxWarps) world_step_kernel(const WorldParams prm, const WorldMapParams mp, const float* __restrict__ action,
                                                                            int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived,
                                                                            float* __restrict__ clearance) {
-  world_step_body<kMap, false>(prm, mp, action, out_collided, out_arrived, clearance);
+  world_step_body<kMap, false, false>(prm, mp, WorldBlockParams{}, action, out_collided, out_arrived, clearance);
 }
 
 // episode mode: __maxnreg__(128) instead of __launch_bounds__(256), under which ptxas settles on 64 registers and spills (at most 8
@@ -712,7 +850,16 @@ template <bool kMap>
 __global__ void __maxnreg__(128) world_step_ep_kernel(const WorldParams prm, const WorldMapParams mp, const float* __restrict__ action,
                                                       int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived,
                                                       float* __restrict__ clearance) {
-  world_step_body<kMap, true>(prm, mp, action, out_collided, out_arrived, clearance);
+  world_step_body<kMap, true, false>(prm, mp, WorldBlockParams{}, action, out_collided, out_arrived, clearance);
+}
+
+// Maps that block obstacles (nb_world_set_map_contact; always with maps): the obstacles move by world_move_obstacle_blocked.  kEp:
+// episode mode.  __maxnreg__(128) as in world_step_ep_kernel: under __launch_bounds__(256) ptxas settles on 80 registers and spills.
+template <bool kEp>
+__global__ void __maxnreg__(128) world_step_block_kernel(const WorldParams prm, const WorldMapParams mp, const WorldBlockParams bp,
+                                                                                 const float* __restrict__ action, int32_t* __restrict__ out_collided,
+                                                                                 int32_t* __restrict__ out_arrived, float* __restrict__ clearance) {
+  world_step_body<true, kEp, true>(prm, mp, bp, action, out_collided, out_arrived, clearance);
 }
 
 }  // namespace nb

@@ -44,6 +44,7 @@ constexpr int kWorldBehCols = 13;  // kind, vxmax, vymax, acce, factor, speed, w
                                    // grid, min_speed
 constexpr int kWorldRvoWarps = 8;
 constexpr int kWorldRvoMaxAxis = 64;  // candidates per axis
+constexpr int kWorldRvoMaxDraws = 16;  // wander goal draws per obstacle and step in an environment whose map blocks obstacles
 constexpr uint64_t kSplitMixGamma = 0x9E3779B97F4A7C15ull;
 
 struct WorldRvoParams {
@@ -90,6 +91,21 @@ __device__ __forceinline__ double world_rvo_tc(double px, double py, double wx, 
   return t > 0.0 ? t : INFINITY;
 }
 
+// A wander goal g of obstacle o (centre c, circumradius rho) in an environment whose map blocks obstacles is accepted when the
+// footprint at g does not touch the map and the segment c-g keeps a distance > rho from every occupied cell (world_convex_clearance
+// of the segment as a two-vertex polygon; a zero-length segment skips this test).  The warp's lanes share the cells; the answer is
+// warp-uniform.
+__device__ __forceinline__ bool world_rvo_goal_clear(const WorldParams& prm, const WorldMap& m, const uint32_t* bits, int o, double cx, double cy,
+                                                     double gx, double gy, double rho, int lane) {
+  const WorldFootprint f = world_footprint(prm, o, gx, gy);
+  if (__any_sync(0xffffffffu, world_footprint_touches(m, bits, f, lane, 32))) return false;
+  if (gx == cx && gy == cy) return true;
+  const WorldSeg sg{cx, cy, gx, gy};
+  const bool near = world_map_any(m, bits, dsub(fmin(cx, gx), rho), dsub(fmin(cy, gy), rho), dadd(fmax(cx, gx), rho), dadd(fmax(cy, gy), rho), lane, 32,
+                                  [&](const WorldCell& c) { return world_convex_clearance(sg, c) <= rho; });
+  return !__any_sync(0xffffffffu, near);
+}
+
 // warp argmin of (key, index): every lane ends with the smallest key, the lower index on ties
 __device__ __forceinline__ void world_rvo_argmin(double& key, int& idx) {
 #pragma unroll
@@ -104,8 +120,12 @@ __device__ __forceinline__ void world_rvo_argmin(double& key, int& idx) {
 // sincos slow-path call; with the cap it takes 98 and spills nothing (2 CTAs of 8 warps per SM either way).
 // kEp (episode mode): unit b is a slot; a live slot moves the obstacles of scene e = scene_of[b] (goal draws keyed by e, so they do
 // not depend on the slot) with the robots' states of e and the actions of slot rows b K + k; an idle slot is skipped.
-template <bool kEp>
-__global__ void __maxnreg__(128) world_rvo_kernel(const WorldParams prm, const WorldRvoParams rp) {
+// kBlock (maps that block obstacles, nb_world_set_map_contact): in an environment whose map blocks obstacles a wander goal is
+// drawn through world_rvo_goal_clear (at most kWorldRvoMaxDraws draws per step; when all fail the goal becomes the centre and the
+// obstacle parks for this step, so the next step draws again from the following numbers), and an obstacle whose move bounced in
+// the last step treats its goal as reached.  The map is not a neighbour: the choice of the velocity is unchanged.
+template <bool kEp, bool kBlock>
+__device__ __forceinline__ void world_rvo_body(const WorldParams& prm, const WorldRvoParams& rp, const WorldMapParams& mp, const WorldBlockParams& bp) {
   extern __shared__ double rsm[];
   const int cap = rp.cap, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   double* s_cx = rsm;
@@ -149,13 +169,31 @@ __global__ void __maxnreg__(128) world_rvo_kernel(const WorldParams prm, const W
       int draws = rp.draws[o];
       double dx = dsub(gx, cx), dy = dsub(gy, cy), dist = __dsqrt_rn(ddot(dx, dy, dx, dy));
       bool parked = false;
-      if (dist < beh[9]) {
+      bool blocks = false;
+      if constexpr (kBlock) blocks = bp.block[b] != 0;
+      if (dist < beh[9] || (kBlock && blocks && bp.bounced[o] != 0)) {
         if (beh[6] != 0.0) {  // wander: draw n takes the stream's values 2n and 2n + 1
           const uint64_t key = world_rvo_key(rp.seed, b, i);
-          gx = dadd(env[0], dmul(world_u01(splitmix64_at(key, 2 * (uint64_t)draws)), dsub(env[2], env[0])));
-          gy = dadd(env[1], dmul(world_u01(splitmix64_at(key, 2 * (uint64_t)draws + 1)), dsub(env[3], env[1])));
-          ++draws;
-          dx = dsub(gx, cx); dy = dsub(gy, cy); dist = __dsqrt_rn(ddot(dx, dy, dx, dy));
+          if constexpr (kBlock) {
+            if (blocks) {
+              const WorldMap& m = mp.maps[mp.env_map[b]];
+              bool ok = false;
+              for (int t = 0; t < kWorldRvoMaxDraws && !ok; ++t) {  // warp-uniform
+                gx = dadd(env[0], dmul(world_u01(splitmix64_at(key, 2 * (uint64_t)draws)), dsub(env[2], env[0])));
+                gy = dadd(env[1], dmul(world_u01(splitmix64_at(key, 2 * (uint64_t)draws + 1)), dsub(env[3], env[1])));
+                ++draws;
+                ok = world_rvo_goal_clear(prm, m, mp.bits, o, cx, cy, gx, gy, ri, lane);
+              }
+              if (!ok) { gx = cx; gy = cy; parked = true; }
+              dx = dsub(gx, cx); dy = dsub(gy, cy); dist = __dsqrt_rn(ddot(dx, dy, dx, dy));
+            }
+          }
+          if (!blocks) {
+            gx = dadd(env[0], dmul(world_u01(splitmix64_at(key, 2 * (uint64_t)draws)), dsub(env[2], env[0])));
+            gy = dadd(env[1], dmul(world_u01(splitmix64_at(key, 2 * (uint64_t)draws + 1)), dsub(env[3], env[1])));
+            ++draws;
+            dx = dsub(gx, cx); dy = dsub(gy, cy); dist = __dsqrt_rn(ddot(dx, dy, dx, dy));
+          }
         } else {
           parked = true;
         }
@@ -250,6 +288,16 @@ __global__ void __maxnreg__(128) world_rvo_kernel(const WorldParams prm, const W
       }
     }
   }
+}
+
+template <bool kEp>
+__global__ void __maxnreg__(128) world_rvo_kernel(const WorldParams prm, const WorldRvoParams rp) {
+  world_rvo_body<kEp, false>(prm, rp, WorldMapParams{}, WorldBlockParams{});
+}
+
+template <bool kEp>
+__global__ void __maxnreg__(128) world_rvo_block_kernel(const WorldParams prm, const WorldRvoParams rp, const WorldMapParams mp, const WorldBlockParams bp) {
+  world_rvo_body<kEp, true>(prm, rp, mp, bp);
 }
 
 }  // namespace nb

@@ -25,8 +25,17 @@ A scene (one environment) is a dict with the sections of an ``env.yaml``:
                     this project's reading of IR-SIM's ``world: obstacle_map:``.  Cells outside the grid are free.  The lidar sees
                     where a beam crosses from a free into an occupied cell (hit index O_b + K, velocity 0), the step takes the exact
                     clearance to the occupied cells within ``map_window`` of each robot (csrc/world_kernel.cuh states the rules).
-                    Reactive obstacles do not see the map and moving obstacles pass over it.  Scenes that share one occupancy array
-                    (the same object, origin and resolution) share one copy of it on the device.
+                    Scenes that share one occupancy array (the same object, origin and resolution) share one copy of it on the
+                    device.  By default reactive obstacles do not see the map and moving obstacles pass over it; with
+                    ``"blocks_obstacles": True`` the map blocks the scene's obstacles (below).
+
+Obstacles in occupancy maps (``"map": {..., "blocks_obstacles": True}``, nb_world_set_map_contact): a moving obstacle whose move
+would make its footprint touch an occupied cell takes instead the x move alone (y velocity reversed), else the y move alone (x
+velocity reversed), else stays in place with both reversed -- a bounce, counted per obstacle by ``map_bounces()``.  A reactive
+obstacle's wander goal must have a clear footprint and a straight segment to it that keeps more than the obstacle's circumradius from
+every occupied cell (at most 16 draws per step, else it waits a step); after a bounce it draws a new goal.  Every moving obstacle of
+such a scene must start clear of the map, and its top speed times step_time must be below the map's resolution.  Walls are not RVO
+neighbours, obstacles do not collide with each other, and motion is not swept (csrc/world_kernel.cuh states the rules).
 
 An obstacle's "behavior" is {"name": "constant"} (the default) or {"name": "rvo", "vxmax", "vymax", ...} (keys and defaults in
 ``RVO_DEFAULTS``): a reactive obstacle that heads for a goal at ``speed`` and steers around the other obstacles and the robot with a
@@ -239,6 +248,11 @@ def pack_maps(scenes):
     return maps, bits, np.ascontiguousarray(env_map, np.int32)
 
 
+def pack_map_contact(scenes) -> np.ndarray:
+    """Scenes -> the (B) int32 flags of nb_world_set_map_contact: 1 where the scene's map has ``"blocks_obstacles": True``."""
+    return np.ascontiguousarray([1 if (sc.get("map") or {}).get("blocks_obstacles", False) else 0 for sc in scenes], np.int32)
+
+
 def _host_ptrs(packed):
     return [C.c_void_p(a.ctypes.data) for a in packed]
 
@@ -304,6 +318,9 @@ class WorldBatch:
         fleet = pack_fleet(scenes) if K > 1 or T > 0 else None
         beh = pack_behaviors(scenes) if any("behavior" in ob for sc in scenes for ob in sc["obstacles"]) else None
         maps = pack_maps(scenes) if any("map" in sc for sc in scenes) else None
+        contact = pack_map_contact(scenes) if maps is not None else None
+        if contact is not None and not contact.any():
+            contact = None
         with torch.cuda.device(self.device):
             lib = _lib.load()
             fleet_args = (B, K, C.c_void_p(fleet.ctypes.data)) if fleet is not None else None
@@ -319,6 +336,10 @@ class WorldBatch:
                             C.c_void_p(maps[2].ctypes.data), C.c_double(float(map_window)))
                 _lib.check(lib.nb_world_check_maps(C.byref(self.config), T, self.types, B, K, C.c_void_p(rows.ctypes.data),
                                                    C.c_void_p(rtype.ctypes.data), *map_args))
+            if contact is not None:
+                bptr = C.c_void_p(beh.ctypes.data) if beh is not None else C.c_void_p(0)
+                _lib.check(lib.nb_world_check_map_contact(C.byref(self.config), B, *_host_ptrs(packed), bptr, *map_args[:4],
+                                                          C.c_void_p(contact.ctypes.data)))
             _lib.check(lib.nb_world_set_scenes_ex(self._handle, B, *_host_ptrs(packed)))
             self.O, self.K, self.N = int(packed[0][-1]), 1, B
             self._envs, self.S, self.slots = B, None, None
@@ -333,6 +354,9 @@ class WorldBatch:
                 self.K, self.N = K, B * K
             if maps is not None:
                 _lib.check(lib.nb_world_set_maps(self._handle, *map_args))
+            if contact is not None:
+                _lib.check(lib.nb_world_set_map_contact(self._handle, B, C.c_void_p(contact.ctypes.data)))
+        self.map_contact = contact is not None
         self.robot_types = rtype
         self._rows = [torch.from_numpy(np.flatnonzero(rtype == i)).to(self.device) for i in range(len(self.robots))]
 
@@ -350,6 +374,17 @@ class WorldBatch:
         with torch.cuda.device(self.device):
             _lib.check(_lib.load().nb_world_read_behaviors(self._handle, self._envs, C.c_void_p(g.data_ptr()), C.c_void_p(d.data_ptr()), self._stream()))
         return g, d
+
+    def map_bounces(self) -> torch.Tensor:
+        """(O,) int32 on the device: per obstacle, the steps in which a map that blocks obstacles turned its move back (0 for
+        obstacles of scenes whose map does not block them).  Needs scenes with ``"blocks_obstacles": True``; a copy enqueued on the
+        current stream."""
+        if not getattr(self, "map_contact", False):
+            raise ValueError("no scene's map blocks obstacles (\"blocks_obstacles\": True)")
+        out = torch.empty(self.O, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nb_world_read_map_contact(self._handle, self.O, C.c_void_p(out.data_ptr()), self._stream()))
+        return out
 
     def _read(self, states=None, obstacles=None, collided=None, arrived=None, rows=None):
         p = lambda t: C.c_void_p(0 if t is None else t.data_ptr())
@@ -840,14 +875,34 @@ def _maze_layout(rng, nx: int, ny: int):
     return open_, sol[::-1]
 
 
-def maze(num_envs: int, cells=(6, 6), cell_size: float = 5.0, wall: float = 0.3, resolution: float = 0.1, seed: int = 0, layouts=None):
+def _movers(b: int, seed: int, centres, count: int, behavior: str):
+    """``count`` circles of radius U(0.3, 0.6) at centres drawn from ``centres`` (distinct while there are enough), from
+    environment b's own movers stream (apart from the layout streams, so the maps do not change): behavior "constant" moves each at
+    a speed U(0, 0.5) m/s in a random direction, "rvo" starts it at rest with EXAMPLE_RVO."""
+    rng = np.random.Generator(np.random.PCG64(np.random.SeedSequence(seed, spawn_key=(b, 1))))
+    if not len(centres):
+        raise ValueError("no free place for a moving obstacle")
+    pick = rng.choice(len(centres), count, replace=count > len(centres))
+    r = rng.uniform(0.3, 0.6, count)
+    speed, heading = rng.uniform(0.0, 0.5, count), rng.uniform(-math.pi, math.pi, count)
+    obs = [dict(center=tuple(float(v) for v in centres[pick[i]]), radius=float(r[i]),
+                velocity=(speed[i] * math.cos(heading[i]), speed[i] * math.sin(heading[i]))) for i in range(count)]
+    return _apply_behavior(obs, behavior)
+
+
+def maze(num_envs: int, cells=(6, 6), cell_size: float = 5.0, wall: float = 0.3, resolution: float = 0.1, seed: int = 0, layouts=None,
+         movers: int = 0, behavior: str = "constant"):
     """Perfect mazes on an occupancy map: ``cells`` (nx, ny) maze cells of ``cell_size`` m, carved by a randomised depth-first search
     (every cell reachable by exactly one route), rasterised at ``resolution`` with walls ``wall`` m thick centred on the closed cell
     boundaries, the outer border included.  Maze cell (a, c) is [a s, (a + 1) s] x [c s, (c + 1) s]; the map covers that area plus
     ``wall`` on every side.  The robot starts at the centre of cell (0, 0) facing along the solution; its goal is the centre of cell
     (nx - 1, ny - 1) with threshold 0.3; ``path`` is the solution through the cell centres at 0.1 m spacing (each segment's heading,
     gear 1).  ``layouts`` distinct mazes (default: one per environment), environment b taking layout b mod layouts, each seeded by
-    its own child stream (``_rng(seed, layout)``); environments of one layout share its occupancy array (one copy on the device)."""
+    its own child stream (``_rng(seed, layout)``); environments of one layout share its occupancy array (one copy on the device).
+    ``movers`` > 0: that many circles of radius U(0.3, 0.6) m at the centres of maze cells other than the start cell and its eight
+    neighbours, moving at U(0, 0.5) m/s in a random direction (``behavior="constant"``) or starting at rest as the examples' reactive
+    obstacles (``"rvo"``, EXAMPLE_RVO: wander in the maze's rectangle), drawn per environment; the map then blocks obstacles
+    (``"blocks_obstacles": True``).  The speeds need step_time * 0.5 m/s (constant) or * 0.71 m/s (rvo) below ``resolution``."""
     nx, ny = (int(v) for v in cells)
     if nx < 1 or ny < 1 or not (0.0 < wall < cell_size):
         raise ValueError("maze needs cells >= 1 and 0 < wall < cell_size")
@@ -878,6 +933,10 @@ def maze(num_envs: int, cells=(6, 6), cell_size: float = 5.0, wall: float = 0.3,
         path = _polyline_path(pts) if len(pts) > 1 else np.array([[pts[0][0], pts[0][1], th, 1.0]])
         scenes.append(dict(obstacles=[], bounds=(0.0, 0.0, nx * cell_size, ny * cell_size), start=(pts[0][0], pts[0][1], th), goal=pts[-1],
                            goal_threshold=0.3, path=path, map=dict(occupancy=occ, origin=origin, resolution=resolution)))
+        if movers > 0:
+            free = [((a + 0.5) * cell_size, (c + 0.5) * cell_size) for c in range(ny) for a in range(nx) if max(a, c) > 1]
+            scenes[-1]["obstacles"] = _movers(b, seed, free, int(movers), behavior)
+            scenes[-1]["map"]["blocks_obstacles"] = True
     return scenes
 
 
@@ -921,7 +980,7 @@ def _bfs(free, start):
 
 
 def cave(num_envs: int, size=(40.0, 40.0), resolution: float = 0.1, fill: float = 0.45, seed: int = 0, layouts=None,
-         coarse: float = 1.0, clearance: float = 2.0):
+         coarse: float = 1.0, clearance: float = 2.0, movers: int = 0, behavior: str = "constant"):
     """Caves on an occupancy map: a cellular automaton on a coarse grid of ``coarse`` m cells over ``size`` (m) -- each cell a wall
     with probability ``fill``, the border always a wall, then 5 rounds of the 4-5 rule (a cell becomes a wall when at least 5 of
     its 8 neighbours are walls, free when at most 3 are, cells past the border counting as walls) -- of which only the largest
@@ -929,7 +988,9 @@ def cave(num_envs: int, size=(40.0, 40.0), resolution: float = 0.1, fill: float 
     cells whose distance to every wall cell's centre exceeds ``clearance`` + ``coarse`` (``clearance``: the robot's circumradius
     plus a margin; the default 2.0 m covers C4's 1.28 m body): the start a random such cell of the largest 4-connected group of
     them, the goal the cell of that group farthest from it by breadth-first search; ``path`` is that breadth-first path through the
-    cell centres at 0.1 m spacing, the start facing along it, goal threshold 0.3.  ``layouts`` as in ``maze``."""
+    cell centres at 0.1 m spacing, the start facing along it, goal threshold 0.3.  ``layouts`` as in ``maze``.  ``movers`` and
+    ``behavior`` as in ``maze``, the circles at the centres of free coarse cells whose eight neighbours are free too and that lie at
+    least 4 m from the start (wander in the cave's rectangle)."""
     sx, sy = float(size[0]), float(size[1])
     nx, ny = int(round(sx / coarse)), int(round(sy / coarse))
     up = int(round(coarse / resolution))
@@ -973,11 +1034,18 @@ def cave(num_envs: int, size=(40.0, 40.0), resolution: float = 0.1, fill: float 
         else:
             raise ValueError("cave: no layout with a start far enough from the walls (lower fill or clearance)")
         occ = np.kron(wall, np.ones((up, up), bool))
-        built.append((occ, pts))
+        open9 = ~np.pad(wall, 1, constant_values=True)
+        open9 = np.logical_and.reduce([open9[1 + dj:1 + dj + ny, 1 + di:1 + di + nx] for dj in (-1, 0, 1) for di in (-1, 0, 1)])
+        free = [((i + 0.5) * coarse, (j + 0.5) * coarse) for j, i in zip(*np.nonzero(open9))
+                if math.hypot((i + 0.5) * coarse - pts[0][0], (j + 0.5) * coarse - pts[0][1]) >= 4.0]
+        built.append((occ, pts, free))
     scenes = []
     for b in range(num_envs):
-        occ, pts = built[b % L]
+        occ, pts, free = built[b % L]
         th = math.atan2(pts[1][1] - pts[0][1], pts[1][0] - pts[0][0])
         scenes.append(dict(obstacles=[], bounds=(0.0, 0.0, sx, sy), start=(pts[0][0], pts[0][1], th), goal=pts[-1], goal_threshold=0.3,
                            path=_polyline_path(pts), map=dict(occupancy=occ, origin=(0.0, 0.0), resolution=resolution)))
+        if movers > 0:
+            scenes[-1]["obstacles"] = _movers(b, seed, free, int(movers), behavior)
+            scenes[-1]["map"]["blocks_obstacles"] = True
     return scenes

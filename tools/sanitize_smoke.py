@@ -101,6 +101,16 @@ if "world" in SECTIONS:
     torch.cuda.synchronize()
     assert torch.isfinite(w.states).all() and (hit[:5] == 1).any()  # no obstacles, K = 1: the map is index 1
     w.close()
+    # maps that block obstacles: the blocking step and rvo instantiations, constant and reactive movers in mazes
+    for behavior in ("constant", "rvo"):
+        w = WorldBatch(4, rb, lidar, 0.1)
+        w.set_scenes(maze(4, cells=(4, 4), seed=1, layouts=2, movers=6, behavior=behavior))
+        for _ in range(30):
+            w.scan()
+            w.step(torch.full((4, 2), 0.5, device="cuda"))
+        torch.cuda.synchronize()
+        assert torch.isfinite(w.obstacles()).all() and (w.map_bounces() >= 0).all()
+        w.close()
     # continuous episodes: the episode instantiations of the scan, rvo and step kernels, the advance and slot gather kernels, and the
     # per-slot ipath and PAN calls, through run_episodes over a bank of 7 scenes in 3 slots (some slots go idle); then a maze bank
     # with its map through 2 slots, stepped until every slot is idle

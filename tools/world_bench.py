@@ -1,6 +1,6 @@
 """Times the batched world (csrc/world_kernel.cuh) against the planner it serves, on the device, and prints one JSON line.
 
-    python tools/world_bench.py [--scene dyna_obs|dyna_non_obs|circle_swap|maze|cave] [--behavior constant|rvo] [--envs 4096] [--robots 1]
+    python tools/world_bench.py [--scene dyna_obs|dyna_non_obs|circle_swap|maze|cave] [--behavior constant|rvo] [--movers 0] [--envs 4096] [--robots 1]
                                 [--beams 1080] [--steps 20] [--warmup 3]
     python tools/world_bench.py --mixed [--envs 4096] [--robots 6] [--beams 1080] [--steps 20] [--warmup 3]
 
@@ -46,6 +46,7 @@ def main():
     ap.add_argument("--scene", choices=("dyna_obs", "dyna_non_obs", "circle_swap", "maze", "cave"), default="dyna_obs")
     ap.add_argument("--robots", type=int, default=1, help="robots per environment (circle_swap only)")
     ap.add_argument("--behavior", choices=("constant", "rvo"), default="constant")
+    ap.add_argument("--movers", type=int, default=0, help="moving obstacles that the map blocks (maze and cave only)")
     ap.add_argument("--envs", type=int, default=4096)
     ap.add_argument("--beams", type=int, default=1080)
     ap.add_argument("--steps", type=int, default=20)
@@ -73,7 +74,7 @@ def main():
     elif args.robots != 1:
         raise SystemExit("--robots needs --scene circle_swap")
     elif args.scene in ("maze", "cave"):
-        scenes = (maze if args.scene == "maze" else cave)(B, seed=2024, layouts=min(B, 64))
+        scenes = (maze if args.scene == "maze" else cave)(B, seed=2024, layouts=min(B, 64), movers=args.movers, behavior=args.behavior)
     else:
         scenes = (dyna_obs if args.scene == "dyna_obs" else dyna_non_obs)(B, seed=2024, behavior=args.behavior)
     N = B * args.robots
