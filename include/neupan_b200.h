@@ -566,6 +566,9 @@ int nb_dune_train_get_weights(nb_dune_train_t* t, float* weights);
 
 /* Number of kernel launches issued by this library since load (bench.py's gpu_launches). */
 int64_t nb_launch_count(void);
+/* Number of device allocations the library holds right now, over every handle of the process (a handle that is destroyed gives
+ * back all of its own). */
+int64_t nb_buffer_count(void);
 const char* nb_last_error(void);
 int nb_version(void);
 

@@ -139,6 +139,7 @@ SYMBOLS = {
     "nb_dune_train_epoch": (C.c_int, [C.c_void_p, _FP, _FP, _FP, C.c_int64, C.c_int32, _FP, C.c_float, C.c_int32, _FP, C.c_void_p]),
     "nb_dune_train_get_weights": (C.c_int, [C.c_void_p, _FP]),
     "nb_launch_count": (C.c_int64, []),
+    "nb_buffer_count": (C.c_int64, []),
     "nb_last_error": (C.c_char_p, []),
     "nb_version": (C.c_int, []),
 }

@@ -1,6 +1,7 @@
 // C ABI of the single-kernel entry points (include/neupan_b200.h): lidar scans to points, the initial path handle, and the labels and
 // training of DUNE.
 #include <cstdlib>
+#include <memory>
 #include <new>
 
 #include "host_common.h"
@@ -8,28 +9,27 @@
 #include "ipath_kernel.cuh"
 #include "dune_train_kernel.cuh"
 
-using nb::dalloc;
 using nb::fail;
 
 struct nb_ipath {
   nb_ipath_config cfg;
   int B = 0;
   int64_t P = 0;
-  double* d_pts = nullptr;
-  int32_t* d_curve_begin = nullptr;
-  int32_t* d_env_curve_begin = nullptr;
-  double* d_interval = nullptr;
-  int32_t* d_curve_index = nullptr;
-  int32_t* d_point_index = nullptr;
-  int32_t* d_arrive_flag = nullptr;
+  nb::DeviceArray<double> d_pts;
+  nb::DeviceArray<int32_t> d_curve_begin;
+  nb::DeviceArray<int32_t> d_env_curve_begin;
+  nb::DeviceArray<double> d_interval;
+  nb::DeviceArray<int32_t> d_curve_index;
+  nb::DeviceArray<int32_t> d_point_index;
+  nb::DeviceArray<int32_t> d_arrive_flag;
 };
 
 struct nb_dune_train {
   int E = 0, device = 0, n_weights = 0;
   float G[nb::kMaxEdges][2];
   float h[nb::kMaxEdges];
-  float *d_weights = nullptr, *d_m = nullptr, *d_v = nullptr, *d_thetas = nullptr;
-  double* d_losses = nullptr;
+  nb::DeviceArray<float> d_weights, d_m, d_v, d_thetas;
+  nb::DeviceArray<double> d_losses;
   size_t thetas_cap = 0;
   long long steps = 0;  // optimiser steps taken so far (Adam bias correction)
 };
@@ -92,31 +92,24 @@ int nb_dune_train_create(int32_t E, const float* G, const float* h, const float*
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || device < 0 || device >= ndev)
     return fail(NB_ERR_NO_DEVICE, "no CUDA device available: neupan_b200 has no CPU fallback");
   NB_CUDA(cudaSetDevice(device));
-  nb_dune_train* t = new (std::nothrow) nb_dune_train();
+  std::unique_ptr<nb_dune_train> t(new (std::nothrow) nb_dune_train());
   if (!t) return fail(NB_ERR_INVALID, "out of host memory");
   t->E = E; t->device = device; t->n_weights = (int)n_weights;
   for (int e = 0; e < E; ++e) { t->G[e][0] = G[2 * e]; t->G[e][1] = G[2 * e + 1]; t->h[e] = h[e]; }
-  cudaError_t e = dalloc(&t->d_weights, (size_t)n_weights);
-  if (e == cudaSuccess) e = dalloc(&t->d_m, (size_t)n_weights);
-  if (e == cudaSuccess) e = dalloc(&t->d_v, (size_t)n_weights);
-  if (e == cudaSuccess) e = dalloc(&t->d_losses, (size_t)4);
-  if (e == cudaSuccess) e = cudaMemcpy(t->d_weights, weights, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemset(t->d_m, 0, (size_t)n_weights * sizeof(float));
-  if (e == cudaSuccess) e = cudaMemset(t->d_v, 0, (size_t)n_weights * sizeof(float));
-  if (e != cudaSuccess) {
-    nb_dune_train_destroy(t);
-    return fail(NB_ERR_CUDA, "nb_dune_train_create: %s", cudaGetErrorString(e));
-  }
-  *out = t;
+  NB_CUDA(nb::alloc(t->d_weights, (size_t)n_weights));
+  NB_CUDA(nb::alloc(t->d_m, (size_t)n_weights));
+  NB_CUDA(nb::alloc(t->d_v, (size_t)n_weights));
+  NB_CUDA(nb::alloc(t->d_losses, (size_t)4));
+  NB_CUDA(cudaMemcpy(t->d_weights.get(), weights, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemset(t->d_m.get(), 0, (size_t)n_weights * sizeof(float)));
+  NB_CUDA(cudaMemset(t->d_v.get(), 0, (size_t)n_weights * sizeof(float)));
+  *out = t.release();
   return NB_OK;
 }
 
 int nb_dune_train_destroy(nb_dune_train_t* t) {
   if (!t) return NB_OK;
   cudaSetDevice(t->device);
-  void* bufs[] = {t->d_weights, t->d_m, t->d_v, t->d_thetas, t->d_losses};
-  for (void* b : bufs)
-    if (b) cudaFree(b);
   delete t;
   return NB_OK;
 }
@@ -129,15 +122,14 @@ int nb_dune_train_epoch(nb_dune_train_t* t, const float* pts, const float* mu, c
   cudaStream_t st = (cudaStream_t)stream;
   const size_t nbatch = (size_t)((n + batch - 1) / batch);
   if (nbatch > t->thetas_cap) {
-    if (t->d_thetas) cudaFree(t->d_thetas);
-    t->d_thetas = nullptr; t->thetas_cap = 0;
-    NB_CUDA(dalloc(&t->d_thetas, nbatch));
+    t->thetas_cap = 0;
+    NB_CUDA(nb::alloc(t->d_thetas, nbatch));
     t->thetas_cap = nbatch;
   }
-  NB_CUDA(cudaMemcpyAsync(t->d_thetas, thetas, nbatch * sizeof(float), cudaMemcpyHostToDevice, st));
+  NB_CUDA(cudaMemcpyAsync(t->d_thetas.get(), thetas, nbatch * sizeof(float), cudaMemcpyHostToDevice, st));
   nb::DuneTrainParams prm;
-  prm.pts = pts; prm.mu = mu; prm.dist = dist; prm.thetas = t->d_thetas;
-  prm.weights = t->d_weights; prm.adam_m = t->d_m; prm.adam_v = t->d_v; prm.losses = t->d_losses;
+  prm.pts = pts; prm.mu = mu; prm.dist = dist; prm.thetas = t->d_thetas.get();
+  prm.weights = t->d_weights.get(); prm.adam_m = t->d_m.get(); prm.adam_v = t->d_v.get(); prm.losses = t->d_losses.get();
   prm.n = (int)n; prm.batch = batch; prm.E = t->E; prm.validate = validate ? 1 : 0;
   prm.step0 = t->steps;
   prm.lr = lr; prm.beta1 = 0.9f; prm.beta2 = 0.999f; prm.eps = 1e-8f; prm.weight_decay = 1e-4f;  // Adam(lr, weight_decay=1e-4), dune_train.py:72
@@ -148,7 +140,7 @@ int nb_dune_train_epoch(nb_dune_train_t* t, const float* pts, const float* mu, c
   ++nb::launches;
   NB_CUDA(cudaGetLastError());
   double sums[4];
-  NB_CUDA(cudaMemcpyAsync(sums, t->d_losses, sizeof(sums), cudaMemcpyDeviceToHost, st));
+  NB_CUDA(cudaMemcpyAsync(sums, t->d_losses.get(), sizeof(sums), cudaMemcpyDeviceToHost, st));
   NB_CUDA(cudaStreamSynchronize(st));
   for (int i = 0; i < 4; ++i) losses[i] = sums[i] / (double)nbatch;  // mean over the batches, like train_one_epoch (:322-327)
   if (!validate) t->steps += (long long)nbatch;
@@ -158,7 +150,7 @@ int nb_dune_train_epoch(nb_dune_train_t* t, const float* pts, const float* mu, c
 int nb_dune_train_get_weights(nb_dune_train_t* t, float* weights) {
   if (!t || !weights) return fail(NB_ERR_INVALID, "nb_dune_train_get_weights: null argument");
   NB_CUDA(cudaSetDevice(t->device));
-  NB_CUDA(cudaMemcpy(weights, t->d_weights, (size_t)t->n_weights * sizeof(float), cudaMemcpyDeviceToHost));
+  NB_CUDA(cudaMemcpy(weights, t->d_weights.get(), (size_t)t->n_weights * sizeof(float), cudaMemcpyDeviceToHost));
   return NB_OK;
 }
 
@@ -173,27 +165,21 @@ int nb_ipath_create(const nb_ipath_config* cfg, nb_ipath_t** out) {
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cfg->device >= ndev)
     return fail(NB_ERR_NO_DEVICE, "no CUDA device available: neupan_b200 has no CPU fallback");
   NB_CUDA(cudaSetDevice(cfg->device));
-  nb_ipath* p = new nb_ipath();
+  std::unique_ptr<nb_ipath> p(new (std::nothrow) nb_ipath());
+  if (!p) return fail(NB_ERR_INVALID, "out of host memory");
   p->cfg = *cfg;
-  cudaError_t e = dalloc(&p->d_env_curve_begin, (size_t)cfg->max_envs + 1);
-  if (e == cudaSuccess) e = dalloc(&p->d_interval, (size_t)cfg->max_envs);
-  if (e == cudaSuccess) e = dalloc(&p->d_curve_index, (size_t)cfg->max_envs);
-  if (e == cudaSuccess) e = dalloc(&p->d_point_index, (size_t)cfg->max_envs);
-  if (e == cudaSuccess) e = dalloc(&p->d_arrive_flag, (size_t)cfg->max_envs);
-  if (e != cudaSuccess) {
-    nb_ipath_destroy(p);
-    return fail(NB_ERR_CUDA, "nb_ipath_create: %s", cudaGetErrorString(e));
-  }
-  *out = p;
+  NB_CUDA(nb::alloc(p->d_env_curve_begin, (size_t)cfg->max_envs + 1));
+  NB_CUDA(nb::alloc(p->d_interval, (size_t)cfg->max_envs));
+  NB_CUDA(nb::alloc(p->d_curve_index, (size_t)cfg->max_envs));
+  NB_CUDA(nb::alloc(p->d_point_index, (size_t)cfg->max_envs));
+  NB_CUDA(nb::alloc(p->d_arrive_flag, (size_t)cfg->max_envs));
+  *out = p.release();
   return NB_OK;
 }
 
 int nb_ipath_destroy(nb_ipath_t* p) {
   if (!p) return NB_OK;
   cudaSetDevice(p->cfg.device);
-  void* bufs[] = {p->d_pts, p->d_curve_begin, p->d_env_curve_begin, p->d_interval, p->d_curve_index, p->d_point_index, p->d_arrive_flag};
-  for (void* b : bufs)
-    if (b) cudaFree(b);
   delete p;
   return NB_OK;
 }
@@ -202,9 +188,9 @@ int nb_ipath_reset_async(nb_ipath_t* p, void* stream) {
   if (!p) return fail(NB_ERR_INVALID, "nb_ipath_reset: null handle");
   NB_CUDA(cudaSetDevice(p->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  NB_CUDA(cudaMemsetAsync(p->d_curve_index, 0, sizeof(int32_t) * p->cfg.max_envs, st));
-  NB_CUDA(cudaMemsetAsync(p->d_point_index, 0, sizeof(int32_t) * p->cfg.max_envs, st));
-  NB_CUDA(cudaMemsetAsync(p->d_arrive_flag, 0, sizeof(int32_t) * p->cfg.max_envs, st));
+  NB_CUDA(cudaMemsetAsync(p->d_curve_index.get(), 0, sizeof(int32_t) * p->cfg.max_envs, st));
+  NB_CUDA(cudaMemsetAsync(p->d_point_index.get(), 0, sizeof(int32_t) * p->cfg.max_envs, st));
+  NB_CUDA(cudaMemsetAsync(p->d_arrive_flag.get(), 0, sizeof(int32_t) * p->cfg.max_envs, st));
   return NB_OK;
 }
 
@@ -226,15 +212,14 @@ int nb_ipath_set_paths(nb_ipath_t* p, int32_t B, const double* points, int64_t P
   for (int c = 0; c < C; ++c)
     if (curve_begin[c + 1] <= curve_begin[c]) return fail(NB_ERR_INVALID, "curve %d is empty", c);
   NB_CUDA(cudaSetDevice(p->cfg.device));
-  if (p->d_pts) cudaFree(p->d_pts);
-  if (p->d_curve_begin) cudaFree(p->d_curve_begin);
-  p->d_pts = nullptr; p->d_curve_begin = nullptr;
-  NB_CUDA(dalloc(&p->d_pts, (size_t)P * 4));
-  NB_CUDA(dalloc(&p->d_curve_begin, (size_t)C + 1));
-  NB_CUDA(cudaMemcpy(p->d_pts, points, sizeof(double) * 4 * P, cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemcpy(p->d_curve_begin, curve_begin, sizeof(int32_t) * (C + 1), cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemcpy(p->d_env_curve_begin, env_curve_begin, sizeof(int32_t) * (B + 1), cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemcpy(p->d_interval, interval, sizeof(double) * B, cudaMemcpyHostToDevice));
+  p->d_pts.reset();
+  p->d_curve_begin.reset();
+  NB_CUDA(nb::alloc(p->d_pts, (size_t)P * 4));
+  NB_CUDA(nb::alloc(p->d_curve_begin, (size_t)C + 1));
+  NB_CUDA(cudaMemcpy(p->d_pts.get(), points, sizeof(double) * 4 * P, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(p->d_curve_begin.get(), curve_begin, sizeof(int32_t) * (C + 1), cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(p->d_env_curve_begin.get(), env_curve_begin, sizeof(int32_t) * (B + 1), cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(p->d_interval.get(), interval, sizeof(double) * B, cudaMemcpyHostToDevice));
   p->B = B; p->P = P;
   return nb_ipath_reset(p);
 }
@@ -253,8 +238,9 @@ int nb_ipath_step_ex(nb_ipath_t* p, int32_t B, const int32_t* env_index, const d
   prm.ind_range = p->cfg.ind_range; prm.arrive_index_threshold = p->cfg.arrive_index_threshold;
   prm.dt = p->cfg.step_time; prm.L = p->cfg.wheelbase; prm.arrive_threshold = p->cfg.arrive_threshold; prm.close_threshold = p->cfg.close_threshold;
   prm.ref_speed = ref_speed;
-  prm.pts = p->d_pts; prm.curve_begin = p->d_curve_begin; prm.env_curve_begin = p->d_env_curve_begin; prm.interval = p->d_interval;
-  prm.curve_index = p->d_curve_index; prm.point_index = p->d_point_index; prm.arrive_flag = p->d_arrive_flag;
+  prm.pts = p->d_pts.get(); prm.curve_begin = p->d_curve_begin.get(); prm.env_curve_begin = p->d_env_curve_begin.get();
+  prm.interval = p->d_interval.get(); prm.curve_index = p->d_curve_index.get(); prm.point_index = p->d_point_index.get();
+  prm.arrive_flag = p->d_arrive_flag.get();
   prm.states = states; prm.cur_vel = cur_vel; prm.nom_s = nom_s; prm.nom_u = nom_u; prm.ref_s = ref_s; prm.ref_us = ref_us; prm.arrived = arrived;
   prm.env_index = env_index; prm.n_env = p->B;
   auto* kernel = env_index ? nb::ipath_step_kernel<true> : nb::ipath_step_kernel<false>;
@@ -275,11 +261,11 @@ int nb_ipath_read_state(nb_ipath_t* p, int32_t B, int32_t* curve_index, int32_t*
   if (B != p->B) return fail(NB_ERR_INVALID, "B = %d but the paths were set for %d environments", B, p->B);
   NB_CUDA(cudaSetDevice(p->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  if (curve_index) NB_CUDA(cudaMemcpyAsync(curve_index, p->d_curve_index, sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
-  if (point_index) NB_CUDA(cudaMemcpyAsync(point_index, p->d_point_index, sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
-  if (arrive_flag) NB_CUDA(cudaMemcpyAsync(arrive_flag, p->d_arrive_flag, sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
+  if (curve_index) NB_CUDA(cudaMemcpyAsync(curve_index, p->d_curve_index.get(), sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
+  if (point_index) NB_CUDA(cudaMemcpyAsync(point_index, p->d_point_index.get(), sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
+  if (arrive_flag) NB_CUDA(cudaMemcpyAsync(arrive_flag, p->d_arrive_flag.get(), sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
   if (points_host) {
-    NB_CUDA(cudaMemcpyAsync(points_host, p->d_pts, sizeof(double) * 4 * p->P, cudaMemcpyDeviceToHost, st));
+    NB_CUDA(cudaMemcpyAsync(points_host, p->d_pts.get(), sizeof(double) * 4 * p->P, cudaMemcpyDeviceToHost, st));
     NB_CUDA(cudaStreamSynchronize(st));
   }
   return NB_OK;

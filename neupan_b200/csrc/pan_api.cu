@@ -7,6 +7,7 @@
 #include <cstdlib>
 #include <chrono>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -15,7 +16,6 @@
 #include "dune_table_kernel.cuh"
 #include "nrmp_common.cuh"
 
-using nb::dalloc;
 using nb::fail;
 
 struct nb_pan {
@@ -24,58 +24,63 @@ struct nb_pan {
   int sm_count = 0;
   int max_smem_optin = 0;
   // device buffers
-  float* d_weights = nullptr;
-  unsigned char* d_tc_image = nullptr;  // wgmma operand image of the warpgroup DUNE kernels
-  int tc_flags = 0;                     // build_tc_image(): bit 0 = bounded tanh arguments
-  unsigned char* d_tc_screen = nullptr; // operand image of the screening network (NB_OPT_DUNE_KERNEL = 4)
-  int32_t *cand_idx = nullptr, *cand_cnt = nullptr, *flag_list = nullptr, *flag_count = nullptr, *refine_list = nullptr;
-  float *cand_dt = nullptr, *cand_rad = nullptr;
-  unsigned* screen_stats = nullptr;
+  nb::DeviceArray<float> d_weights;
+  nb::DeviceArray<unsigned char> d_tc_image;  // wgmma operand image of the warpgroup DUNE kernels
+  int tc_flags = 0;                           // build_tc_image(): bit 0 = bounded tanh arguments
+  nb::DeviceArray<unsigned char> d_tc_screen; // operand image of the screening network (NB_OPT_DUNE_KERNEL = 4)
+  nb::DeviceArray<int32_t> cand_idx, cand_cnt, flag_list, flag_count, refine_list;
+  nb::DeviceArray<float> cand_dt, cand_rad;
+  nb::DeviceArray<unsigned> screen_stats;
   float c_mu = 0.012f;                  // bound on the screening network's |mu~ - mu|: set by calibrate_screen() to 4 x the largest error
                                         // measured for THIS checkpoint and polygon (NB_SCREEN_CMU overrides; DESIGN.md 3.1)
   bool screen_calibrated = false;
   float screen_cal_ratio = 0.f;
   bool cmu_override = false;            // NB_SCREEN_CMU is set: every point gets the radius c_mu sum_e |G_e p0 - h_e| + 1e-4 (network screen)
   int screen_table = 1;                 // NB_OPT_DUNE_SCREEN_TABLE: the mma.sync screen looks distances up in the table below
-  float4* tab_cell = nullptr;           // distance table (dune_table_kernel.cuh), built once per handle by build_screen_table()
-  float* tab_rad = nullptr;
+  nb::DeviceArray<float4> tab_cell;     // distance table (dune_table_kernel.cuh), built once per handle by build_screen_table()
+  nb::DeviceArray<float> tab_rad;
   int tab_n = 0;
   float tab_h = 0.f, tab_half = 0.f, tab_ratio = 0.f, tab_ms = 0.f;
-  bool tab_built = false;               // built (and kept, or freed as not accurate enough: tab_cell == nullptr)
+  bool tab_built = false;               // built (and kept, or freed as not accurate enough: tab_cell empty)
   int dune_variant = 2;              // NB_OPT_DUNE_KERNEL: 2 = the exact wgmma kernel on every point, 4 = screening pipeline
   int overlap = 1;                   // NB_OPT_OVERLAP: number of env sub-batches pipelined on internal streams
-  cudaStream_t streams[4] = {nullptr, nullptr, nullptr, nullptr};
-  cudaEvent_t ev_fork = nullptr, ev_join[4] = {nullptr, nullptr, nullptr, nullptr};
+  nb::Stream streams[4];
+  nb::Event ev_fork, ev_join[4];
   // host-input entry points: uploads run on copy_stream in env chunks; ev_chunk[c] = chunk c (and everything before it) has landed
   static constexpr int kMaxChunks = 8;
-  cudaStream_t copy_stream = nullptr;
-  cudaEvent_t ev_chunk[kMaxChunks] = {}, ev_inputs_free = nullptr;
+  nb::Stream copy_stream;
+  nb::Event ev_chunk[kMaxChunks], ev_inputs_free;
   int h2d_chunks = 4;               // NB_H2D_CHUNKS (developer switch, read at create); 1 = no overlap
-  float *sel_mu = nullptr, *sel_lam = nullptr, *sel_pts = nullptr, *sel_dist = nullptr;
-  int32_t* sel_count = nullptr;
-  float *prev_s = nullptr, *prev_u = nullptr, *prev_mu = nullptr, *prev_lam = nullptr;
-  int32_t *prev_count = nullptr, *prev_valid = nullptr, *active = nullptr, *iters = nullptr, *status = nullptr, *ipm_it = nullptr;
-  float* min_dist = nullptr;
-  // differentiable mode (NB_OPT_DIFFERENTIABLE): adjoint records of every (iteration, env) solve + gradient workspaces
-  int differentiable = 0, adj_iters = 0;
-  double *adj_rec = nullptr, *adj_gs = nullptr, *adj_gu = nullptr, *adj_gd = nullptr, *adj_gtheta = nullptr;
-  int32_t* adj_valid = nullptr;
-  int* work_counters = nullptr;     // dynamic env -> warp assignment of the NRMP kernel, one counter per internal stream
+  nb::DeviceArray<float> sel_mu, sel_lam, sel_pts, sel_dist;
+  nb::DeviceArray<int32_t> sel_count;
+  nb::DeviceArray<float> prev_s, prev_u, prev_mu, prev_lam;
+  nb::DeviceArray<int32_t> prev_count, prev_valid, active, iters, status, ipm_it;
+  nb::DeviceArray<float> min_dist;
+  // differentiable mode (NB_OPT_DIFFERENTIABLE): adjoint records of every (iteration, env) solve for `iters` iterations + gradient
+  // workspaces; allocated as a whole or not at all
+  struct Adjoint {
+    int iters = 0;
+    nb::DeviceArray<double> rec, gs, gu, gd, gtheta;
+    nb::DeviceArray<int32_t> valid;
+  };
+  int differentiable = 0;
+  Adjoint adj;
+  nb::DeviceArray<int> work_counters;  // dynamic env -> warp assignment of the NRMP kernel, one counter per internal stream
   int dune_skip_t0 = 1;             // NB_OPT_DUNE_SKIP_T0: PAN iterations k > 0 keep the step-0 items of iteration 0 (screening variant)
   int screen_mma = 1;               // NB_OPT_DUNE_SCREEN_MMA: screening pass on mma.sync (N <= 1024) instead of wgmma
   int nrmp_defer_stop_min = 256;    // NB_NRMP_DEFER_STOP_MIN (developer switch, read at create): smallest batch whose stop criterion runs as its own kernel
   int nrmp_dynamic = 1;             // NB_NRMP_STATIC=1 (developer switch, read at create) turns the persistent-warp schedule off
-  float* warm = nullptr;            // NRMP warm-start records, nrmp_warm_floats(T, M) per environment
-  int32_t* warm_valid = nullptr;
+  nb::DeviceArray<float> warm;      // NRMP warm-start records, nrmp_warm_floats(T, M) per environment
+  nb::DeviceArray<int32_t> warm_valid;
   int nrmp_warm = 0;                // NB_OPT_NRMP_WARM (off by default: see DESIGN.md 3.2)
   double nrmp_gap_tol = 1e-12;      // NB_NRMP_GAP_TOL (developer switch, read once at create)
   int warm_check_it = 12;           // NB_NRMP_RESTART_IT / NB_NRMP_RESTART_GAP (developer switches): early cold restart of a warm start
   double warm_check_gap = 1e-5;
   // staging for the host-pointer entry point
-  float *h_in = nullptr, *h_out = nullptr;  // device staging
+  nb::DeviceArray<float> h_in, h_out;  // device staging
   size_t h_in_floats = 0, h_out_floats = 0;
-  int32_t* h_np = nullptr;
-  int32_t* h_io = nullptr;
+  nb::DeviceArray<int32_t> h_np;
+  nb::DeviceArray<int32_t> h_io;
 };
 
 namespace {
@@ -94,12 +99,12 @@ int check_forward_args(const nb_pan* p, int B, int N) {
 nb::DuneParams dune_params(const nb_pan* p) {
   const nb_pan_config& c = p->cfg;
   nb::DuneParams d{};
-  d.weights = p->d_weights; d.geo = p->geo;
+  d.weights = p->d_weights.get(); d.geo = p->geo;
   d.T = c.receding; d.M = c.nrmp_max_num; d.dt = (float)c.step_time;
-  d.c_mu = p->c_mu; d.screen_stats = p->screen_stats; d.screen_mma = p->screen_mma;
-  d.sel_mu = p->sel_mu; d.sel_lam = p->sel_lam; d.sel_pts = p->sel_pts; d.sel_dist = p->sel_dist; d.sel_count = p->sel_count;
-  d.cand_idx = p->cand_idx; d.cand_dt = p->cand_dt; d.cand_cnt = p->cand_cnt; d.cand_rad = p->cand_rad;
-  d.flag_list = p->flag_list; d.flag_count = p->flag_count; d.refine_list = p->refine_list;
+  d.c_mu = p->c_mu; d.screen_stats = p->screen_stats.get(); d.screen_mma = p->screen_mma;
+  d.sel_mu = p->sel_mu.get(); d.sel_lam = p->sel_lam.get(); d.sel_pts = p->sel_pts.get(); d.sel_dist = p->sel_dist.get(); d.sel_count = p->sel_count.get();
+  d.cand_idx = p->cand_idx.get(); d.cand_dt = p->cand_dt.get(); d.cand_cnt = p->cand_cnt.get(); d.cand_rad = p->cand_rad.get();
+  d.flag_list = p->flag_list.get(); d.flag_count = p->flag_count.get(); d.refine_list = p->refine_list.get();
   return d;
 }
 
@@ -139,7 +144,7 @@ nb::NrmpParams nrmp_params(const nb_pan* p) {
 
 // what an NRMP launch on the internal stream `counter_slot` (0: the caller's stream) borrows from the handle
 nb::NrmpLaunch nrmp_launch(const nb_pan* p, int counter_slot) {
-  return {p->sm_count, p->max_smem_optin, p->nrmp_defer_stop_min, p->nrmp_dynamic, p->work_counters + counter_slot};
+  return {p->sm_count, p->max_smem_optin, p->nrmp_defer_stop_min, p->nrmp_dynamic, p->work_counters.get() + counter_slot};
 }
 
 // Screening bound of this handle: the screen and the exact network evaluate the same 32-point items (points uniform in the square the
@@ -151,15 +156,15 @@ int calibrate_screen(nb_pan* p, cudaStream_t st) {
   int Bc = c.max_envs < 512 ? c.max_envs : 512;
   const int rounds = (4096 + Bc * T1 - 1) / (Bc * T1) < 1 ? 1 : (4096 + Bc * T1 - 1) / (Bc * T1);
   std::vector<float> pts((size_t)Bc * 2 * N), ns((size_t)Bc * 3 * T1, 0.f);
-  float *d_pts = nullptr, *d_ns = nullptr, *d_md = nullptr;
-  NB_CUDA(dalloc(&d_pts, pts.size()));
-  NB_CUDA(dalloc(&d_ns, ns.size()));
-  NB_CUDA(dalloc(&d_md, (size_t)Bc));
-  NB_CUDA(cudaMemcpyAsync(d_ns, ns.data(), ns.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+  nb::DeviceArray<float> d_pts, d_ns, d_md;
+  NB_CUDA(nb::alloc(d_pts, pts.size()));
+  NB_CUDA(nb::alloc(d_ns, ns.size()));
+  NB_CUDA(nb::alloc(d_md, (size_t)Bc));
+  NB_CUDA(cudaMemcpyAsync(d_ns.get(), ns.data(), ns.size() * sizeof(float), cudaMemcpyHostToDevice, st));
   unsigned saved[4];
   NB_CUDA(cudaStreamSynchronize(st));
-  NB_CUDA(cudaMemcpy(saved, p->screen_stats, sizeof(saved), cudaMemcpyDeviceToHost));
-  NB_CUDA(cudaMemset(p->screen_stats, 0, sizeof(saved)));
+  NB_CUDA(cudaMemcpy(saved, p->screen_stats.get(), sizeof(saved), cudaMemcpyDeviceToHost));
+  NB_CUDA(cudaMemset(p->screen_stats.get(), 0, sizeof(saved)));
   unsigned long long rng = 0x9E3779B97F4A7C15ull;
   auto uni = [&]() { rng = rng * 6364136223846793005ull + 1442695040888963407ull; return (float)((rng >> 40) * (1.0 / 16777216.0)); };
   int rc = NB_OK;
@@ -168,20 +173,20 @@ int calibrate_screen(nb_pan* p, cudaStream_t st) {
       const float R = ((b + r) & 1) ? 25.f : 6.f;
       for (int i = 0; i < N; ++i) { pts[((size_t)b * 2) * N + i] = R * (2.f * uni() - 1.f); pts[((size_t)b * 2 + 1) * N + i] = R * (2.f * uni() - 1.f); }
     }
-    cudaError_t e = cudaMemcpyAsync(d_pts, pts.data(), pts.size() * sizeof(float), cudaMemcpyHostToDevice, st);
+    cudaError_t e = cudaMemcpyAsync(d_pts.get(), pts.data(), pts.size() * sizeof(float), cudaMemcpyHostToDevice, st);
     if (e != cudaSuccess) { rc = fail(NB_ERR_CUDA, "calibrate_screen: %s", cudaGetErrorString(e)); break; }
     nb::DuneParams prm = dune_params(p);  // no distance table: this measures the screening network
-    prm.nom_s = d_ns; prm.points = d_pts; prm.min_dist = d_md;
+    prm.nom_s = d_ns.get(); prm.points = d_pts.get(); prm.min_dist = d_md.get();
     prm.B = Bc; prm.N = N; prm.calibrate = 1;
     for (int shape = 0; shape < 2 && rc == NB_OK; ++shape) {  // both screening kernels (wgmma / mma.sync): the bound holds whichever option is set later
       prm.screen_mma = shape;
-      rc = nb::launch_dune_tc(prm, p->d_tc_image, p->d_tc_screen, p->tc_flags, true, p->sm_count, p->max_smem_optin, st);
+      rc = nb::launch_dune_tc(prm, p->d_tc_image.get(), p->d_tc_screen.get(), p->tc_flags, true, p->sm_count, p->max_smem_optin, st);
       if (rc == NB_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = fail(NB_ERR_CUDA, "calibrate_screen: kernel failed");
     }
   }
   if (rc == NB_OK) {
     unsigned h[4];
-    NB_CUDA(cudaMemcpy(h, p->screen_stats, sizeof(h), cudaMemcpyDeviceToHost));
+    NB_CUDA(cudaMemcpy(h, p->screen_stats.get(), sizeof(h), cudaMemcpyDeviceToHost));
     float ratio;
     memcpy(&ratio, &h[0], 4);
     p->screen_cal_ratio = ratio;
@@ -190,8 +195,7 @@ int calibrate_screen(nb_pan* p, cudaStream_t st) {
     if (const char* e = getenv("NB_SCREEN_CMU")) p->c_mu = (float)atof(e);
     p->screen_calibrated = true;
   }
-  cudaMemcpy(p->screen_stats, saved, sizeof(saved), cudaMemcpyHostToDevice);
-  cudaFree(d_pts); cudaFree(d_ns); cudaFree(d_md);
+  cudaMemcpy(p->screen_stats.get(), saved, sizeof(saved), cudaMemcpyHostToDevice);
   return rc;
 }
 
@@ -213,30 +217,27 @@ int build_screen_table(nb_pan* p) {
   const long long m = nb::kTableSub * n + 1;
   const auto t0 = std::chrono::steady_clock::now();
   NB_CUDA(cudaDeviceSynchronize());
-  float* fine = nullptr;
-  unsigned* d_ratio = nullptr;
-  NB_CUDA(dalloc(&fine, (size_t)(m * m)));
-  NB_CUDA(dalloc(&d_ratio, (size_t)1));
-  if (!p->tab_cell) NB_CUDA(dalloc(&p->tab_cell, (size_t)(n * n)));
-  if (!p->tab_rad) NB_CUDA(dalloc(&p->tab_rad, (size_t)(n * n)));
-  NB_CUDA(cudaMemset(d_ratio, 0, sizeof(unsigned)));
+  nb::DeviceArray<float> fine;
+  nb::DeviceArray<unsigned> d_ratio;
+  NB_CUDA(nb::alloc(fine, (size_t)(m * m)));
+  NB_CUDA(nb::alloc(d_ratio, (size_t)1));
+  if (!p->tab_cell) NB_CUDA(nb::alloc(p->tab_cell, (size_t)(n * n)));
+  if (!p->tab_rad) NB_CUDA(nb::alloc(p->tab_rad, (size_t)(n * n)));
+  NB_CUDA(cudaMemset(d_ratio.get(), 0, sizeof(unsigned)));
   const float hs = h / nb::kTableSub;
-  nb::dune_table_sample_kernel<<<p->sm_count * 16, 128>>>(p->d_weights, p->geo, (int)m, half, hs, fine);
-  nb::dune_table_cell_kernel<<<p->sm_count * 8, 128>>>(fine, (int)n, half, hs, p->geo, p->tab_cell, p->tab_rad, d_ratio);
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  nb::dune_table_sample_kernel<<<p->sm_count * 16, 128>>>(p->d_weights.get(), p->geo, (int)m, half, hs, fine.get());
+  nb::dune_table_cell_kernel<<<p->sm_count * 8, 128>>>(fine.get(), (int)n, half, hs, p->geo, p->tab_cell.get(), p->tab_rad.get(), d_ratio.get());
+  NB_CUDA(cudaGetLastError());
+  NB_CUDA(cudaDeviceSynchronize());
   unsigned r = 0;
-  if (e == cudaSuccess) e = cudaMemcpy(&r, d_ratio, sizeof(r), cudaMemcpyDeviceToHost);
-  cudaFree(fine);
-  cudaFree(d_ratio);
-  if (e != cudaSuccess) return fail(NB_ERR_CUDA, "build_screen_table: %s", cudaGetErrorString(e));
+  NB_CUDA(cudaMemcpy(&r, d_ratio.get(), sizeof(r), cudaMemcpyDeviceToHost));
+  fine.reset();
+  d_ratio.reset();
   memcpy(&p->tab_ratio, &r, 4);
   p->tab_n = (int)n; p->tab_h = h; p->tab_half = half; p->tab_built = true;
   if (!(2.f * p->tab_ratio <= p->c_mu)) {
-    cudaFree(p->tab_cell);
-    cudaFree(p->tab_rad);
-    p->tab_cell = nullptr;
-    p->tab_rad = nullptr;
+    p->tab_cell.reset();
+    p->tab_rad.reset();
   }
   p->tab_ms = (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   return NB_OK;
@@ -245,8 +246,8 @@ int build_screen_table(nb_pan* p) {
 // the table goes to the screen only where it is meant to be used; without it every point runs the screening network
 void set_screen_table(const nb_pan* p, nb::DuneParams& prm) {
   const bool on = p->screen_table && !p->cmu_override && p->tab_cell;
-  prm.tab_cell = on ? p->tab_cell : nullptr;
-  prm.tab_rad = p->tab_rad;
+  prm.tab_cell = on ? p->tab_cell.get() : nullptr;
+  prm.tab_rad = p->tab_rad.get();
   prm.tab_n = p->tab_n;
   prm.tab_half = p->tab_half;
   prm.tab_inv_h = on ? 1.f / p->tab_h : 0.f;
@@ -302,6 +303,7 @@ int64_t nb_weight_count(int32_t edge_dim) { return nb::WeightLayout::count(edge_
 int nb_version(void) { return NB_VERSION; }
 const char* nb_last_error(void) { return g_err; }
 int64_t nb_launch_count(void) { return nb::launches; }
+int64_t nb_buffer_count(void) { return nb::live_buffers; }
 
 int nb_pan_create(const nb_pan_config* cfg, const float* weights, int64_t n_weights, const float* G, const float* h, nb_pan_t** out) {
   if (!cfg || !out) return fail(NB_ERR_INVALID, "null argument");
@@ -327,7 +329,7 @@ int nb_pan_create(const nb_pan_config* cfg, const float* weights, int64_t n_weig
     return fail(NB_ERR_NO_DEVICE, "no CUDA device available: neupan_b200 has no CPU fallback");
   if (cfg->device < 0 || cfg->device >= ndev) return fail(NB_ERR_INVALID, "device %d out of range (%d devices)", cfg->device, ndev);
   NB_CUDA(cudaSetDevice(cfg->device));
-  nb_pan* p = new (std::nothrow) nb_pan();
+  std::unique_ptr<nb_pan> p(new (std::nothrow) nb_pan());  // every return below but the last frees what was built
   if (!p) return fail(NB_ERR_INVALID, "out of host memory");
   p->cfg = *cfg;
   NB_CUDA(cudaDeviceGetAttribute(&p->sm_count, cudaDevAttrMultiProcessorCount, cfg->device));
@@ -339,46 +341,46 @@ int nb_pan_create(const nb_pan_config* cfg, const float* weights, int64_t n_weig
     for (int e = 0; e < cfg->edge_dim; ++e) {
       p->geo.G[e][0] = G[2 * e]; p->geo.G[e][1] = G[2 * e + 1]; p->geo.h[e] = h[e];
     }
-    NB_CUDA(dalloc(&p->d_weights, (size_t)n_weights));
-    NB_CUDA(cudaMemcpy(p->d_weights, weights, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
+    NB_CUDA(nb::alloc(p->d_weights, (size_t)n_weights));
+    NB_CUDA(cudaMemcpy(p->d_weights.get(), weights, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
     std::vector<unsigned char> image;
     p->tc_flags = nb::build_tc_image(weights, cfg->edge_dim, image, false);
-    NB_CUDA(dalloc(&p->d_tc_image, image.size()));
-    NB_CUDA(cudaMemcpy(p->d_tc_image, image.data(), image.size(), cudaMemcpyHostToDevice));
+    NB_CUDA(nb::alloc(p->d_tc_image, image.size()));
+    NB_CUDA(cudaMemcpy(p->d_tc_image.get(), image.data(), image.size(), cudaMemcpyHostToDevice));
     nb::build_tc_image(weights, cfg->edge_dim, image, true);
-    NB_CUDA(dalloc(&p->d_tc_screen, image.size()));
-    NB_CUDA(cudaMemcpy(p->d_tc_screen, image.data(), image.size(), cudaMemcpyHostToDevice));
-    NB_CUDA(dalloc(&p->cand_idx, (size_t)cfg->max_envs * (cfg->receding + 1) * nb::kCandMax));
-    NB_CUDA(dalloc(&p->cand_dt, (size_t)cfg->max_envs * (cfg->receding + 1) * nb::kCandMax));
-    NB_CUDA(dalloc(&p->cand_rad, (size_t)cfg->max_envs * (cfg->receding + 1) * nb::kCandMax));
-    NB_CUDA(dalloc(&p->cand_cnt, (size_t)cfg->max_envs * (cfg->receding + 1)));
-    NB_CUDA(dalloc(&p->flag_list, (size_t)cfg->max_envs * (cfg->receding + 1)));
-    NB_CUDA(dalloc(&p->flag_count, (size_t)32));  // 4 words per internal stream: flagged items, the two refine list lengths
-    NB_CUDA(dalloc(&p->refine_list, (size_t)2 * cfg->max_envs * (cfg->receding + 1)));
-    NB_CUDA(dalloc(&p->screen_stats, (size_t)4));
-    NB_CUDA(cudaMemset(p->screen_stats, 0, 4 * sizeof(unsigned)));
+    NB_CUDA(nb::alloc(p->d_tc_screen, image.size()));
+    NB_CUDA(cudaMemcpy(p->d_tc_screen.get(), image.data(), image.size(), cudaMemcpyHostToDevice));
+    NB_CUDA(nb::alloc(p->cand_idx, (size_t)cfg->max_envs * (cfg->receding + 1) * nb::kCandMax));
+    NB_CUDA(nb::alloc(p->cand_dt, (size_t)cfg->max_envs * (cfg->receding + 1) * nb::kCandMax));
+    NB_CUDA(nb::alloc(p->cand_rad, (size_t)cfg->max_envs * (cfg->receding + 1) * nb::kCandMax));
+    NB_CUDA(nb::alloc(p->cand_cnt, (size_t)cfg->max_envs * (cfg->receding + 1)));
+    NB_CUDA(nb::alloc(p->flag_list, (size_t)cfg->max_envs * (cfg->receding + 1)));
+    NB_CUDA(nb::alloc(p->flag_count, (size_t)32));  // 4 words per internal stream: flagged items, the two refine list lengths
+    NB_CUDA(nb::alloc(p->refine_list, (size_t)2 * cfg->max_envs * (cfg->receding + 1)));
+    NB_CUDA(nb::alloc(p->screen_stats, (size_t)4));
+    NB_CUDA(cudaMemset(p->screen_stats.get(), 0, 4 * sizeof(unsigned)));
     if (const char* e = getenv("NB_SCREEN_CMU")) { p->c_mu = (float)atof(e); p->cmu_override = true; }
   }
-  NB_CUDA(dalloc(&p->sel_mu, B * T1 * M * E));
-  NB_CUDA(dalloc(&p->sel_lam, B * T1 * M * 2));
-  NB_CUDA(dalloc(&p->sel_pts, B * T1 * M * 2));
-  NB_CUDA(dalloc(&p->sel_dist, B * T1 * M));
-  NB_CUDA(dalloc(&p->sel_count, B));
-  NB_CUDA(dalloc(&p->prev_s, B * 3 * T1));
-  NB_CUDA(dalloc(&p->prev_u, B * 2 * T));
-  NB_CUDA(dalloc(&p->prev_mu, B * T1 * M * E));
-  NB_CUDA(dalloc(&p->prev_lam, B * T1 * M * 2));
-  NB_CUDA(dalloc(&p->prev_count, B));
-  NB_CUDA(dalloc(&p->prev_valid, B));
-  NB_CUDA(dalloc(&p->active, B));
-  NB_CUDA(dalloc(&p->iters, B));
-  NB_CUDA(dalloc(&p->status, B));
-  NB_CUDA(dalloc(&p->ipm_it, B));
-  NB_CUDA(cudaMemset(p->ipm_it, 0, B * sizeof(int32_t)));
-  NB_CUDA(dalloc(&p->min_dist, B));
-  NB_CUDA(dalloc(&p->warm, B * nb::nrmp_warm_floats(cfg->receding, cfg->nrmp_max_num)));
-  NB_CUDA(dalloc(&p->warm_valid, B));
-  NB_CUDA(dalloc(&p->work_counters, (size_t)8));
+  NB_CUDA(nb::alloc(p->sel_mu, B * T1 * M * E));
+  NB_CUDA(nb::alloc(p->sel_lam, B * T1 * M * 2));
+  NB_CUDA(nb::alloc(p->sel_pts, B * T1 * M * 2));
+  NB_CUDA(nb::alloc(p->sel_dist, B * T1 * M));
+  NB_CUDA(nb::alloc(p->sel_count, B));
+  NB_CUDA(nb::alloc(p->prev_s, B * 3 * T1));
+  NB_CUDA(nb::alloc(p->prev_u, B * 2 * T));
+  NB_CUDA(nb::alloc(p->prev_mu, B * T1 * M * E));
+  NB_CUDA(nb::alloc(p->prev_lam, B * T1 * M * 2));
+  NB_CUDA(nb::alloc(p->prev_count, B));
+  NB_CUDA(nb::alloc(p->prev_valid, B));
+  NB_CUDA(nb::alloc(p->active, B));
+  NB_CUDA(nb::alloc(p->iters, B));
+  NB_CUDA(nb::alloc(p->status, B));
+  NB_CUDA(nb::alloc(p->ipm_it, B));
+  NB_CUDA(cudaMemset(p->ipm_it.get(), 0, B * sizeof(int32_t)));
+  NB_CUDA(nb::alloc(p->min_dist, B));
+  NB_CUDA(nb::alloc(p->warm, B * nb::nrmp_warm_floats(cfg->receding, cfg->nrmp_max_num)));
+  NB_CUDA(nb::alloc(p->warm_valid, B));
+  NB_CUDA(nb::alloc(p->work_counters, (size_t)8));
   if (getenv("NB_NRMP_STATIC")) p->nrmp_dynamic = 0;
   if (const char* e = getenv("NB_NRMP_DEFER_STOP_MIN")) p->nrmp_defer_stop_min = atoi(e);
   if (const char* e = getenv("NB_H2D_CHUNKS")) { p->h2d_chunks = atoi(e); if (p->h2d_chunks < 1) p->h2d_chunks = 1; if (p->h2d_chunks > nb_pan::kMaxChunks) p->h2d_chunks = nb_pan::kMaxChunks; }
@@ -387,36 +389,20 @@ int nb_pan_create(const nb_pan_config* cfg, const float* weights, int64_t n_weig
   if (const char* e = getenv("NB_SCREEN_TABLE")) p->screen_table = atoi(e) != 0;
   if (const char* e = getenv("NB_NRMP_RESTART_IT")) p->warm_check_it = atoi(e);
   if (const char* e = getenv("NB_NRMP_RESTART_GAP")) p->warm_check_gap = atof(e);
-  NB_CUDA(cudaMemset(p->warm_valid, 0, B * sizeof(int32_t)));
+  NB_CUDA(cudaMemset(p->warm_valid.get(), 0, B * sizeof(int32_t)));
   if (const char* e = getenv("NB_NRMP_GAP_TOL")) p->nrmp_gap_tol = atof(e);
-  NB_CUDA(cudaMemset(p->prev_valid, 0, B * sizeof(int32_t)));
-  NB_CUDA(cudaMemset(p->prev_count, 0, B * sizeof(int32_t)));
-  NB_CUDA(cudaMemset(p->sel_count, 0, B * sizeof(int32_t)));
-  if (int rc = nb_pan_set_option(p, NB_OPT_OVERLAP, 2)) {  // the default: two sub-batches on internal streams (streams / events are made here)
-    nb_pan_destroy(p);
-    return rc;
-  }
-  *out = p;
+  NB_CUDA(cudaMemset(p->prev_valid.get(), 0, B * sizeof(int32_t)));
+  NB_CUDA(cudaMemset(p->prev_count.get(), 0, B * sizeof(int32_t)));
+  NB_CUDA(cudaMemset(p->sel_count.get(), 0, B * sizeof(int32_t)));
+  // the default: two sub-batches on internal streams (streams / events are made here)
+  if (int rc = nb_pan_set_option(p.get(), NB_OPT_OVERLAP, 2)) return rc;
+  *out = p.release();
   return NB_OK;
 }
 
 int nb_pan_destroy(nb_pan_t* p) {
   if (!p) return NB_OK;
   cudaSetDevice(p->cfg.device);
-  for (int i = 0; i < 4; ++i) {
-    if (p->streams[i]) cudaStreamDestroy(p->streams[i]);
-    if (p->ev_join[i]) cudaEventDestroy(p->ev_join[i]);
-  }
-  if (p->ev_fork) cudaEventDestroy(p->ev_fork);
-  if (p->copy_stream) cudaStreamDestroy(p->copy_stream);
-  if (p->ev_inputs_free) cudaEventDestroy(p->ev_inputs_free);
-  for (cudaEvent_t e : p->ev_chunk)
-    if (e) cudaEventDestroy(e);
-  void* bufs[] = {p->d_tc_image, p->d_weights, p->sel_mu, p->sel_lam, p->sel_pts, p->sel_dist, p->sel_count, p->prev_s, p->prev_u, p->prev_mu,
-                  p->prev_lam, p->prev_count, p->prev_valid, p->active, p->iters, p->status, p->ipm_it, p->min_dist, p->h_in, p->h_out, p->h_np, p->h_io,
-                  p->d_tc_screen, p->cand_idx, p->cand_cnt, p->cand_dt, p->cand_rad, p->tab_cell, p->tab_rad, p->screen_stats, p->flag_list, p->flag_count, p->refine_list, p->warm, p->warm_valid, p->work_counters, p->adj_rec, p->adj_gs, p->adj_gu, p->adj_gd, p->adj_gtheta, p->adj_valid};
-  for (void* b : bufs)
-    if (b) cudaFree(b);
   delete p;
   return NB_OK;
 }
@@ -461,10 +447,10 @@ int nb_pan_set_option(nb_pan_t* p, int32_t option, int32_t value) {
     if (value < 1 || value > 4) return fail(NB_ERR_INVALID, "NB_OPT_OVERLAP takes 1..4");
     NB_CUDA(cudaSetDevice(p->cfg.device));
     for (int i = 0; i < value && value > 1; ++i) {
-      if (!p->streams[i]) NB_CUDA(cudaStreamCreateWithFlags(&p->streams[i], cudaStreamNonBlocking));
-      if (!p->ev_join[i]) NB_CUDA(cudaEventCreateWithFlags(&p->ev_join[i], cudaEventDisableTiming));
+      if (!p->streams[i]) NB_CUDA(nb::create(p->streams[i]));
+      if (!p->ev_join[i]) NB_CUDA(nb::create(p->ev_join[i]));
     }
-    if (value > 1 && !p->ev_fork) NB_CUDA(cudaEventCreateWithFlags(&p->ev_fork, cudaEventDisableTiming));
+    if (value > 1 && !p->ev_fork) NB_CUDA(nb::create(p->ev_fork));
     p->overlap = value;
     return NB_OK;
   }
@@ -489,8 +475,8 @@ int nb_pan_set_option(nb_pan_t* p, int32_t option, int32_t value) {
 int nb_pan_reset_state_async(nb_pan_t* p, void* stream) {
   if (!p) return fail(NB_ERR_INVALID, "null handle");
   NB_CUDA(cudaSetDevice(p->cfg.device));
-  NB_CUDA(cudaMemsetAsync(p->prev_valid, 0, (size_t)p->cfg.max_envs * sizeof(int32_t), (cudaStream_t)stream));
-  NB_CUDA(cudaMemsetAsync(p->prev_count, 0, (size_t)p->cfg.max_envs * sizeof(int32_t), (cudaStream_t)stream));
+  NB_CUDA(cudaMemsetAsync(p->prev_valid.get(), 0, (size_t)p->cfg.max_envs * sizeof(int32_t), (cudaStream_t)stream));
+  NB_CUDA(cudaMemsetAsync(p->prev_count.get(), 0, (size_t)p->cfg.max_envs * sizeof(int32_t), (cudaStream_t)stream));
   return NB_OK;
 }
 
@@ -498,7 +484,7 @@ int nb_pan_reset_envs_async(nb_pan_t* p, int32_t B, const int32_t* mask, void* s
   if (!p || !mask) return fail(NB_ERR_INVALID, "nb_pan_reset_envs_async: null argument");
   if (B < 1 || B > p->cfg.max_envs) return fail(NB_ERR_CAPACITY, "B = %d outside [1, max_envs = %d]", B, p->cfg.max_envs);
   NB_CUDA(cudaSetDevice(p->cfg.device));
-  reset_envs_kernel<<<(B + 255) / 256, 256, 0, (cudaStream_t)stream>>>(B, mask, p->prev_valid, p->prev_count);
+  reset_envs_kernel<<<(B + 255) / 256, 256, 0, (cudaStream_t)stream>>>(B, mask, p->prev_valid.get(), p->prev_count.get());
   ++nb::launches;
   NB_CUDA(cudaGetLastError());
   return NB_OK;
@@ -522,7 +508,7 @@ int nb_dune_forward(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, const
   prm.min_dist = out_min_distance;
   prm.B = B; prm.N = N;
   set_screen_table(p, prm);
-  return nb::launch_dune_tc(prm, p->d_tc_image, p->d_tc_screen, p->tc_flags, p->dune_variant == 4, p->sm_count, p->max_smem_optin,
+  return nb::launch_dune_tc(prm, p->d_tc_image.get(), p->d_tc_screen.get(), p->tc_flags, p->dune_variant == 4, p->sm_count, p->max_smem_optin,
                             (cudaStream_t)stream);
 }
 
@@ -535,7 +521,7 @@ int nb_nrmp_forward(nb_pan_t* p, int32_t B, const float* nom_s, const float* nom
   nb::NrmpParams prm = nrmp_params(p);
   prm.nom_s = nom_s; prm.nom_u = nom_u; prm.ref_s = ref_s; prm.ref_us = ref_us; prm.fa = fa; prm.fb = fb;
   prm.out_s = out_s; prm.out_u = out_u; prm.out_d = out_d; prm.status = out_status;
-  prm.ipm_iters = p->ipm_it;  // nb_pan_read_diagnostics
+  prm.ipm_iters = p->ipm_it.get();  // nb_pan_read_diagnostics
   prm.B = B;
   return nb::launch_nrmp(prm, nrmp_launch(p, 0), (cudaStream_t)stream);
 }
@@ -571,24 +557,23 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
   const nb_pan_config& c = p->cfg;
   const int T = c.receding, T1 = T + 1;
   const bool with_dune = c.nrmp_max_num > 0 && points != nullptr && N > 0;  // pan.py:130
-  if (p->differentiable && (p->adj_rec == nullptr || p->adj_iters < c.iter_num)) {  // (re)allocate the adjoint records for K iterations
-    void* old[] = {p->adj_rec, p->adj_valid, p->adj_gs, p->adj_gu, p->adj_gd, p->adj_gtheta};
-    for (void* o : old)
-      if (o) cudaFree(o);
-    p->adj_rec = nullptr; p->adj_valid = nullptr; p->adj_gs = p->adj_gu = p->adj_gd = p->adj_gtheta = nullptr;
+  if (p->differentiable && (!p->adj.rec || p->adj.iters < c.iter_num)) {  // (re)allocate the adjoint records for K iterations
+    p->adj = {};  // the old set goes first; a failure below leaves none, never part of one
     const size_t Bm = c.max_envs, Ks = c.iter_num > 0 ? c.iter_num : 1;
-    NB_CUDA(dalloc(&p->adj_rec, Ks * Bm * nb::nrmp_adj_doubles(T, c.nrmp_max_num)));
-    NB_CUDA(dalloc(&p->adj_valid, Ks * Bm));
-    NB_CUDA(dalloc(&p->adj_gs, Bm * 3 * T1));
-    NB_CUDA(dalloc(&p->adj_gu, Bm * 2 * T));
-    NB_CUDA(dalloc(&p->adj_gd, Bm * T));
-    NB_CUDA(dalloc(&p->adj_gtheta, Bm * 7));
-    p->adj_iters = (int)Ks;
+    nb_pan::Adjoint a;
+    NB_CUDA(nb::alloc(a.rec, Ks * Bm * nb::nrmp_adj_doubles(T, c.nrmp_max_num)));
+    NB_CUDA(nb::alloc(a.valid, Ks * Bm));
+    NB_CUDA(nb::alloc(a.gs, Bm * 3 * T1));
+    NB_CUDA(nb::alloc(a.gu, Bm * 2 * T));
+    NB_CUDA(nb::alloc(a.gd, Bm * T));
+    NB_CUDA(nb::alloc(a.gtheta, Bm * 7));
+    a.iters = (int)Ks;
+    p->adj = std::move(a);
   }
-  if (p->differentiable) NB_CUDA(cudaMemsetAsync(p->adj_valid, 0, (size_t)p->adj_iters * c.max_envs * sizeof(int32_t), st));
+  if (p->differentiable) NB_CUDA(cudaMemsetAsync(p->adj.valid.get(), 0, (size_t)p->adj.iters * c.max_envs * sizeof(int32_t), st));
   if (plan && plan->n > 0) NB_CUDA(cudaStreamWaitEvent(st, plan->ev[0], 0));  // the small tensors travel ahead of chunk 0
   const int tb = 128, gb = (B + tb - 1) / tb;
-  init_run_kernel<<<gb, tb, 0, st>>>(B, p->active, p->iters, p->status, p->min_dist, p->sel_count, p->warm_valid);
+  init_run_kernel<<<gb, tb, 0, st>>>(B, p->active.get(), p->iters.get(), p->status.get(), p->min_dist.get(), p->sel_count.get(), p->warm_valid.get());
   ++nb::launches;
   // the nominal trajectory lives in the output buffers and is updated in place every iteration
   NB_CUDA(cudaMemcpyAsync(out_s, nom_s, (size_t)B * 3 * T1 * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -600,13 +585,13 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
     const size_t T1s = (size_t)T1, Ms = (size_t)c.nrmp_max_num, Es = (size_t)(c.edge_dim > 0 ? c.edge_dim : 1);
     const bool screen = p->dune_variant == 4;
     auto dune = [&](const nb::DuneParams& d) {
-      return nb::launch_dune_tc(d, p->d_tc_image, p->d_tc_screen, p->tc_flags, screen, p->sm_count, p->max_smem_optin, s);
+      return nb::launch_dune_tc(d, p->d_tc_image.get(), p->d_tc_screen.get(), p->tc_flags, screen, p->sm_count, p->max_smem_optin, s);
     };
     nb::DuneParams d{};  // the environments [lo, hi)
     if (with_dune) {
       d = dune_params(p);
       d.nom_s = out_s; d.points = points; d.velocities = velocities; d.num_points = num_points;
-      d.active = p->active; d.min_dist = p->min_dist;
+      d.active = p->active.get(); d.min_dist = p->min_dist.get();
       d.B = nb_; d.N = N;
       d.flag_count += 4 * counter_slot;
       set_screen_table(p, d);
@@ -635,17 +620,17 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
       n.nom_s = out_s + (size_t)lo * 3 * T1s; n.nom_u = out_u + (size_t)lo * 2 * T; n.ref_s = ref_s + (size_t)lo * 3 * T1s; n.ref_us = ref_us + (size_t)lo * T;
       if (with_dune) { n.sel_mu = d.sel_mu; n.sel_lam = d.sel_lam; n.sel_pts = d.sel_pts; n.sel_count = d.sel_count; }
       n.out_s = out_s + (size_t)lo * 3 * T1s; n.out_u = out_u + (size_t)lo * 2 * T; n.out_d = out_d + (size_t)lo * T;
-      n.status = p->status + lo; n.iters = p->iters + lo; n.active = p->active + lo; n.ipm_iters = p->ipm_it + lo;
-      n.prev_s = p->prev_s + (size_t)lo * 3 * T1s; n.prev_u = p->prev_u + (size_t)lo * 2 * T;
-      n.prev_mu = p->prev_mu + (size_t)lo * T1s * Ms * Es; n.prev_lam = p->prev_lam + (size_t)lo * T1s * Ms * 2;
-      n.prev_count = p->prev_count + lo; n.prev_valid = p->prev_valid + lo;
-      if (p->differentiable && p->adj_rec && k < p->adj_iters) {
-        n.adj_save = p->adj_rec + ((size_t)k * c.max_envs + lo) * nb::nrmp_adj_doubles(T, c.nrmp_max_num);
-        n.adj_valid = p->adj_valid + (size_t)k * c.max_envs + lo;
+      n.status = p->status.get() + lo; n.iters = p->iters.get() + lo; n.active = p->active.get() + lo; n.ipm_iters = p->ipm_it.get() + lo;
+      n.prev_s = p->prev_s.get() + (size_t)lo * 3 * T1s; n.prev_u = p->prev_u.get() + (size_t)lo * 2 * T;
+      n.prev_mu = p->prev_mu.get() + (size_t)lo * T1s * Ms * Es; n.prev_lam = p->prev_lam.get() + (size_t)lo * T1s * Ms * 2;
+      n.prev_count = p->prev_count.get() + lo; n.prev_valid = p->prev_valid.get() + lo;
+      if (p->differentiable && p->adj.rec && k < p->adj.iters) {
+        n.adj_save = p->adj.rec.get() + ((size_t)k * c.max_envs + lo) * nb::nrmp_adj_doubles(T, c.nrmp_max_num);
+        n.adj_valid = p->adj.valid.get() + (size_t)k * c.max_envs + lo;
       }
       if (p->nrmp_warm) {
-        n.warm = p->warm + (size_t)lo * nb::nrmp_warm_floats(T, c.nrmp_max_num);
-        n.warm_valid = p->warm_valid + lo;
+        n.warm = p->warm.get() + (size_t)lo * nb::nrmp_warm_floats(T, c.nrmp_max_num);
+        n.warm_valid = p->warm_valid.get() + lo;
       }
       n.B = nb_;
       if (int rc = nb::launch_nrmp(n, nrmp_launch(p, counter_slot), s)) return rc;
@@ -658,8 +643,8 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
   } else {
     // sub-batches on internal streams: the DUNE kernel of one part (issue / tensor / MUFU bound) shares the SMs with the
     // NRMP kernel of another (latency bound, few warps)
-    NB_CUDA(cudaEventRecord(p->ev_fork, st));
-    for (int i = 0; i < parts; ++i) NB_CUDA(cudaStreamWaitEvent(p->streams[i], p->ev_fork, 0));
+    NB_CUDA(cudaEventRecord(p->ev_fork.get(), st));
+    for (int i = 0; i < parts; ++i) NB_CUDA(cudaStreamWaitEvent(p->streams[i].get(), p->ev_fork.get(), 0));
     // enqueue order: iteration by iteration, alternating the streams (every sub-batch starts at once; NB_PAN_INTERLEAVE=0, a developer
     // switch, enqueues all K iterations of one sub-batch before the next)
     static int interleave = -1;
@@ -673,21 +658,21 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
         for (int i = 0; i < parts; ++i) {
           int lo, hi;
           range_of(i, lo, hi);
-          if (int rc = run_range(lo, hi, p->streams[i], 1 + i, k, k + 1)) return rc;
+          if (int rc = run_range(lo, hi, p->streams[i].get(), 1 + i, k, k + 1)) return rc;
         }
     } else {
       for (int i = 0; i < parts; ++i) {
         int lo, hi;
         range_of(i, lo, hi);
-        if (int rc = run_range(lo, hi, p->streams[i], 1 + i, 0, c.iter_num)) return rc;
+        if (int rc = run_range(lo, hi, p->streams[i].get(), 1 + i, 0, c.iter_num)) return rc;
       }
     }
     for (int i = 0; i < parts; ++i) {
-      NB_CUDA(cudaEventRecord(p->ev_join[i], p->streams[i]));
-      NB_CUDA(cudaStreamWaitEvent(st, p->ev_join[i], 0));
+      NB_CUDA(cudaEventRecord(p->ev_join[i].get(), p->streams[i].get()));
+      NB_CUDA(cudaStreamWaitEvent(st, p->ev_join[i].get(), 0));
     }
   }
-  finish_run_kernel<<<gb, tb, 0, st>>>(B, p->iters, p->status, p->min_dist, out_iters, out_status, out_min_distance);
+  finish_run_kernel<<<gb, tb, 0, st>>>(B, p->iters.get(), p->status.get(), p->min_dist.get(), out_iters, out_status, out_min_distance);
   ++nb::launches;
   NB_CUDA(cudaGetLastError());
   return NB_OK;
@@ -697,18 +682,18 @@ int pan_forward_impl(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, cons
 int nb_pan_backward(nb_pan_t* p, int32_t B, const float* ref_s, const float* ref_us, const float* grad_s, const float* grad_u, const float* grad_d,
                     float* grad_theta, void* stream) {
   if (int rc = check_forward_args(p, B, 0)) return rc;
-  if (!p->differentiable || !p->adj_rec) return fail(NB_ERR_INVALID, "nb_pan_backward needs a forward in differentiable mode (NB_OPT_DIFFERENTIABLE = 1) first");
+  if (!p->differentiable || !p->adj.rec) return fail(NB_ERR_INVALID, "nb_pan_backward needs a forward in differentiable mode (NB_OPT_DIFFERENTIABLE = 1) first");
   if (!ref_s || !ref_us || !grad_theta) return fail(NB_ERR_INVALID, "null tensor argument");
   NB_CUDA(cudaSetDevice(p->cfg.device));
   const nb_pan_config& c = p->cfg;
   nb::NrmpAdjParams a{};
-  a.rec = p->adj_rec; a.rec_valid = p->adj_valid;
-  a.iters = p->iters; a.ref_s = ref_s; a.ref_us = ref_us;
-  a.g_s = p->adj_gs; a.g_u = p->adj_gu; a.g_d = p->adj_gd; a.grad_theta = p->adj_gtheta;
+  a.rec = p->adj.rec.get(); a.rec_valid = p->adj.valid.get();
+  a.iters = p->iters.get(); a.ref_s = ref_s; a.ref_us = ref_us;
+  a.g_s = p->adj.gs.get(); a.g_u = p->adj.gu.get(); a.g_d = p->adj.gd.get(); a.grad_theta = p->adj.gtheta.get();
   a.B = B; a.T = c.receding; a.M = c.nrmp_max_num; a.kin = c.kinematics;
   for (int i = 0; i < 3; ++i) a.q[i] = c.q_s[i];
   a.p_u = c.p_u; a.d_min = c.d_min; a.bk = c.bk;
-  const int K = c.iter_num < p->adj_iters ? c.iter_num : p->adj_iters;
+  const int K = c.iter_num < p->adj.iters ? c.iter_num : p->adj.iters;
   return nb::launch_nrmp_backward(a, K, c.max_envs, grad_s, grad_u, grad_d, grad_theta, (cudaStream_t)stream);
 }
 
@@ -718,11 +703,11 @@ int nb_pan_read_selection(nb_pan_t* p, int32_t B, float* sel_mu, float* sel_lam,
   NB_CUDA(cudaSetDevice(p->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   const size_t T1 = p->cfg.receding + 1, M = p->cfg.nrmp_max_num, E = p->cfg.edge_dim;
-  if (sel_mu) NB_CUDA(cudaMemcpyAsync(sel_mu, p->sel_mu, (size_t)B * T1 * M * E * 4, cudaMemcpyDeviceToDevice, st));
-  if (sel_lam) NB_CUDA(cudaMemcpyAsync(sel_lam, p->sel_lam, (size_t)B * T1 * M * 2 * 4, cudaMemcpyDeviceToDevice, st));
-  if (sel_points) NB_CUDA(cudaMemcpyAsync(sel_points, p->sel_pts, (size_t)B * T1 * M * 2 * 4, cudaMemcpyDeviceToDevice, st));
-  if (sel_distance) NB_CUDA(cudaMemcpyAsync(sel_distance, p->sel_dist, (size_t)B * T1 * M * 4, cudaMemcpyDeviceToDevice, st));
-  if (sel_count) NB_CUDA(cudaMemcpyAsync(sel_count, p->sel_count, (size_t)B * 4, cudaMemcpyDeviceToDevice, st));
+  if (sel_mu) NB_CUDA(cudaMemcpyAsync(sel_mu, p->sel_mu.get(), (size_t)B * T1 * M * E * 4, cudaMemcpyDeviceToDevice, st));
+  if (sel_lam) NB_CUDA(cudaMemcpyAsync(sel_lam, p->sel_lam.get(), (size_t)B * T1 * M * 2 * 4, cudaMemcpyDeviceToDevice, st));
+  if (sel_points) NB_CUDA(cudaMemcpyAsync(sel_points, p->sel_pts.get(), (size_t)B * T1 * M * 2 * 4, cudaMemcpyDeviceToDevice, st));
+  if (sel_distance) NB_CUDA(cudaMemcpyAsync(sel_distance, p->sel_dist.get(), (size_t)B * T1 * M * 4, cudaMemcpyDeviceToDevice, st));
+  if (sel_count) NB_CUDA(cudaMemcpyAsync(sel_count, p->sel_count.get(), (size_t)B * 4, cudaMemcpyDeviceToDevice, st));
   return NB_OK;
 }
 
@@ -732,12 +717,12 @@ int nb_pan_read_screen_stats(nb_pan_t* p, float* max_error_ratio, int32_t* count
   NB_CUDA(cudaSetDevice(p->cfg.device));
   NB_CUDA(cudaDeviceSynchronize());
   unsigned h[4];
-  NB_CUDA(cudaMemcpy(h, p->screen_stats, sizeof(h), cudaMemcpyDeviceToHost));
+  NB_CUDA(cudaMemcpy(h, p->screen_stats.get(), sizeof(h), cudaMemcpyDeviceToHost));
   memcpy(max_error_ratio, &h[0], 4);
   max_error_ratio[1] = p->c_mu;
   max_error_ratio[2] = p->screen_cal_ratio;
   counts[0] = (int32_t)h[1]; counts[1] = (int32_t)h[2]; counts[2] = (int32_t)h[3];
-  if (reset) NB_CUDA(cudaMemset(p->screen_stats, 0, sizeof(h)));
+  if (reset) NB_CUDA(cudaMemset(p->screen_stats.get(), 0, sizeof(h)));
   return NB_OK;
 }
 
@@ -754,7 +739,7 @@ int nb_pan_read_screen_table(nb_pan_t* p, float* info) {
 int nb_pan_read_diagnostics(nb_pan_t* p, int32_t B, int32_t* ipm_iterations, void* stream) {
   if (int rc = check_forward_args(p, B, 0)) return rc;
   NB_CUDA(cudaSetDevice(p->cfg.device));
-  if (ipm_iterations) NB_CUDA(cudaMemcpyAsync(ipm_iterations, p->ipm_it, (size_t)B * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  if (ipm_iterations) NB_CUDA(cudaMemcpyAsync(ipm_iterations, p->ipm_it.get(), (size_t)B * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return NB_OK;
 }
 
@@ -767,35 +752,34 @@ int pan_forward_from_host(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s,
   const size_t T = p->cfg.receding, T1 = T + 1;
   const size_t n_s = (size_t)B * 3 * T1, n_u = (size_t)B * 2 * T, n_r = (size_t)B * T, n_p = (size_t)B * 2 * N;
   const size_t in_floats = 2 * n_s + n_u + n_r + 2 * n_p;
-  if (!p->copy_stream) NB_CUDA(cudaStreamCreateWithFlags(&p->copy_stream, cudaStreamNonBlocking));
-  if (!p->ev_inputs_free) NB_CUDA(cudaEventCreateWithFlags(&p->ev_inputs_free, cudaEventDisableTiming));
-  for (int i = 0; i < nb_pan::kMaxChunks; ++i)
-    if (!p->ev_chunk[i]) NB_CUDA(cudaEventCreateWithFlags(&p->ev_chunk[i], cudaEventDisableTiming));
+  if (!p->copy_stream) NB_CUDA(nb::create(p->copy_stream));
+  if (!p->ev_inputs_free) NB_CUDA(nb::create(p->ev_inputs_free));
+  for (nb::Event& ev : p->ev_chunk)
+    if (!ev) NB_CUDA(nb::create(ev));
+  cudaStream_t cs = p->copy_stream.get();
   // whatever `st` still does with the staging buffer (the previous call) must be over before it is overwritten
-  NB_CUDA(cudaEventRecord(p->ev_inputs_free, st));
-  NB_CUDA(cudaStreamWaitEvent(p->copy_stream, p->ev_inputs_free, 0));
+  NB_CUDA(cudaEventRecord(p->ev_inputs_free.get(), st));
+  NB_CUDA(cudaStreamWaitEvent(cs, p->ev_inputs_free.get(), 0));
   if (in_floats > p->h_in_floats) {
-    NB_CUDA(cudaStreamSynchronize(p->copy_stream));
-    if (p->h_in) cudaFree(p->h_in);
-    p->h_in = nullptr; p->h_in_floats = 0;
-    NB_CUDA(dalloc(&p->h_in, in_floats));
+    NB_CUDA(cudaStreamSynchronize(cs));
+    p->h_in_floats = 0;
+    NB_CUDA(nb::alloc(p->h_in, in_floats));
     p->h_in_floats = in_floats;
   }
-  if (!p->h_np) NB_CUDA(dalloc(&p->h_np, (size_t)p->cfg.max_envs));
-  float* d = p->h_in;
+  if (!p->h_np) NB_CUDA(nb::alloc(p->h_np, (size_t)p->cfg.max_envs));
+  float* d = p->h_in.get();
   float* d_nom_s = d; d += n_s;
   float* d_ref_s = d; d += n_s;
   float* d_nom_u = d; d += n_u;
   float* d_ref_us = d; d += n_r;
   float* d_pts = d; d += n_p;
   float* d_vel = d;
-  cudaStream_t cs = p->copy_stream;
   auto h2d = [&](void* dst, const void* src, size_t bytes) { return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, cs); };
   NB_CUDA(h2d(d_nom_s, nom_s, n_s * 4));
   NB_CUDA(h2d(d_ref_s, ref_s, n_s * 4));
   NB_CUDA(h2d(d_nom_u, nom_u, n_u * 4));
   NB_CUDA(h2d(d_ref_us, ref_us, n_r * 4));
-  if (num_points) NB_CUDA(h2d(p->h_np, num_points, (size_t)B * 4));
+  if (num_points) NB_CUDA(h2d(p->h_np.get(), num_points, (size_t)B * 4));
   const bool with_pts = points && N > 0;
   ChunkPlan plan;
   plan.n = (with_pts && B >= 64 * p->h2d_chunks) ? p->h2d_chunks : 1;
@@ -808,11 +792,11 @@ int pan_forward_from_host(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s,
     const size_t lo = (size_t)plan.bound[c] * 2 * N, cnt = (size_t)(plan.bound[c + 1] - plan.bound[c]) * 2 * N;
     if (with_pts && cnt) NB_CUDA(h2d(d_pts + lo, points + lo, cnt * 4));
     if (with_pts && velocities && cnt) NB_CUDA(h2d(d_vel + lo, velocities + lo, cnt * 4));
-    plan.ev[c] = p->ev_chunk[c];
+    plan.ev[c] = p->ev_chunk[c].get();
     NB_CUDA(cudaEventRecord(plan.ev[c], cs));
   }
   return pan_forward_impl(p, B, N, d_nom_s, d_nom_u, d_ref_s, d_ref_us, with_pts ? d_pts : nullptr, (with_pts && velocities) ? d_vel : nullptr,
-                          num_points ? p->h_np : nullptr, out_s, out_u, out_d, out_min_distance, out_iters, out_status, st, &plan);
+                          num_points ? p->h_np.get() : nullptr, out_s, out_u, out_d, out_min_distance, out_iters, out_status, st, &plan);
 }
 }  // namespace
 
@@ -837,27 +821,27 @@ int nb_pan_forward_host(nb_pan_t* p, int32_t B, int32_t N, const float* nom_s, c
   const size_t n_s = (size_t)B * 3 * T1, n_u = (size_t)B * 2 * T, n_r = (size_t)B * T;
   const size_t out_floats = n_s + n_u + n_r + (size_t)B;
   if (out_floats > p->h_out_floats) {
-    if (p->h_out) cudaFree(p->h_out);
-    p->h_out = nullptr; p->h_out_floats = 0;
-    NB_CUDA(dalloc(&p->h_out, out_floats));
+    p->h_out_floats = 0;
+    NB_CUDA(nb::alloc(p->h_out, out_floats));
     p->h_out_floats = out_floats;
   }
-  if (!p->h_io) NB_CUDA(dalloc(&p->h_io, 2 * (size_t)p->cfg.max_envs));
-  float* o = p->h_out;
+  if (!p->h_io) NB_CUDA(nb::alloc(p->h_io, 2 * (size_t)p->cfg.max_envs));
+  int32_t* io = p->h_io.get();
+  float* o = p->h_out.get();
   float* o_s = o; o += n_s;
   float* o_u = o; o += n_u;
   float* o_d = o; o += n_r;
   float* o_md = o;
-  int rc = pan_forward_from_host(p, B, N, nom_s, nom_u, ref_s, ref_us, points, velocities, num_points, o_s, o_u, o_d, o_md, p->h_io,
-                                 p->h_io + p->cfg.max_envs, st);
+  int rc = pan_forward_from_host(p, B, N, nom_s, nom_u, ref_s, ref_us, points, velocities, num_points, o_s, o_u, o_d, o_md, io,
+                                 io + p->cfg.max_envs, st);
   if (rc) return rc;
   auto d2h = [&](void* dst, const void* src, size_t bytes) { return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st); };
   NB_CUDA(d2h(out_s, o_s, n_s * 4));
   NB_CUDA(d2h(out_u, o_u, n_u * 4));
   NB_CUDA(d2h(out_d, o_d, n_r * 4));
   if (out_min_distance) NB_CUDA(d2h(out_min_distance, o_md, (size_t)B * 4));
-  if (out_iters) NB_CUDA(d2h(out_iters, p->h_io, (size_t)B * 4));
-  if (out_status) NB_CUDA(d2h(out_status, p->h_io + p->cfg.max_envs, (size_t)B * 4));
+  if (out_iters) NB_CUDA(d2h(out_iters, io, (size_t)B * 4));
+  if (out_status) NB_CUDA(d2h(out_status, io + p->cfg.max_envs, (size_t)B * 4));
   NB_CUDA(cudaStreamSynchronize(st));
   return NB_OK;
 }

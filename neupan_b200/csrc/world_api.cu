@@ -2,6 +2,7 @@
 // the world handle, and the launches of the scan, rvo and step kernels.
 #include <algorithm>
 #include <cmath>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -10,7 +11,6 @@
 #include "world_rvo_kernel.cuh"
 #include "world_episode_kernel.cuh"
 
-using nb::dalloc;
 using nb::fail;
 
 struct nb_world {
@@ -18,56 +18,64 @@ struct nb_world {
   int B = 0, O = 0, V = 0;
   int max_circ = 0, max_edges = 0, scan_threads = 0, scan_grid = 0;
   size_t scan_smem = 0;
-  int32_t *d_obs_begin = nullptr, *d_vert_begin = nullptr, *d_slot = nullptr, *d_counts = nullptr, *d_kind = nullptr;
-  int32_t *d_collided = nullptr, *d_arrived = nullptr;
-  double *d_vertices = nullptr, *d_env = nullptr, *d_obs = nullptr, *d_states = nullptr;
-  double* d_beam_cs = nullptr;  // (R, 2), fixed at creation
+  nb::DeviceArray<double> beam_cs;  // (R, 2), fixed at creation
+  // the scenes (nb_world_set_scenes_ex)
+  struct Scenes {
+    nb::DeviceArray<int32_t> obs_begin, vert_begin, slot, counts, kind;
+    nb::DeviceArray<double> vertices, env, obs;
+  } scenes;
   // host copies of the scene (nb_world_set_behaviors checks against them)
   std::vector<int32_t> h_obs_begin, h_vert_begin, h_kind;
   std::vector<double> h_vertices, h_env;
-  // obstacle behaviours (nb_world_set_behaviors; nb_world_set_scenes clears them): has_rvo false -> nb_world_step launches only
-  // world_step_kernel
-  bool has_rvo = false;
-  uint64_t seed = 0;
-  int rvo_cap = 0, rvo_grid = 0;
-  size_t rvo_smem = 0;
-  double *d_beh = nullptr, *d_rad = nullptr, *d_goal = nullptr;
-  int32_t* d_draws = nullptr;
-  int rvo_max_n = 0;  // the largest environment's obstacle count (rvo_cap = rvo_max_n + K)
-  // robots per environment (nb_world_set_fleet; nb_world_set_scenes makes it 1, from the env rows): the per-robot arrays
-  // (states, collided, arrived above, every robot's goal and the velocity of its last step) hold B K rows (world_set_robots)
+  // obstacle behaviours (nb_world_set_behaviors): has_rvo false -> nb_world_step launches only world_step_kernel
+  struct Behaviors {
+    bool has_rvo = false;
+    uint64_t seed = 0;
+    int cap = 0, grid = 0;
+    size_t smem = 0;
+    int max_n = 0;  // the largest environment's obstacle count (cap = max_n + K)
+    nb::DeviceArray<double> beh, rad, goal;
+    nb::DeviceArray<int32_t> draws;
+  } rvo;
+  // robots per environment (nb_world_set_fleet; nb_world_set_scenes makes it 1, from the env rows): the per-robot arrays hold B K
+  // rows (world_set_robots): states, flags, every robot's goal and the velocity of its last step; the robot types (type 0 is the
+  // config's robot): the table (T + 1 rows) and each robot's type (B K, zeros without a mix)
   int K = 1;
-  double *d_fgoal = nullptr, *d_fvel = nullptr;
-  // robot types (nb_world_set_fleet_ex; type 0 is the config's robot): the table (T + 1 rows), each robot's type (B K, zeros
-  // without a mix) and the largest environment's robot edge count (the scan's staging size; 0 with K = 1)
-  nb::WorldRobotType* d_types = nullptr;
-  int32_t* d_rtype = nullptr;
-  int max_redges = 0;
+  struct Robots {
+    nb::DeviceArray<double> states, goal, vel;
+    nb::DeviceArray<int32_t> collided, arrived, rtype;
+    nb::DeviceArray<nb::WorldRobotType> types;
+  } robots;
+  int max_redges = 0;  // the largest environment's robot edge count (the scan's staging size; 0 with K = 1)
   // host copies of the placed robots (nb_world_set_maps checks the start bodies against them): rows, types 1..T, each robot's type
   std::vector<double> h_robots;
   std::vector<nb_world_robot_type> h_types;
   std::vector<int32_t> h_rtype;
-  // occupancy maps (nb_world_set_maps; nb_world_set_scenes(_ex) and nb_world_set_fleet(_ex) drop them): has_map false -> the
-  // kernels' map-free instantiations
-  bool has_map = false;
-  nb::WorldMap* d_maps = nullptr;
-  uint32_t* d_bits = nullptr;
-  int32_t* d_env_map = nullptr;
-  double window = 0.0;
-  // host copies of the maps (nb_world_set_map_contact checks the obstacles' starts against them)
-  std::vector<nb::WorldMap> h_maps;
-  std::vector<uint32_t> h_bits;
-  std::vector<int32_t> h_env_map;
-  // maps that block obstacles (nb_world_set_map_contact; dropped with the maps and by nb_world_set_behaviors): has_block false -> the
-  // kernels' instantiations without it
-  bool has_block = false;
-  int32_t *d_block = nullptr, *d_bounces = nullptr, *d_bounced = nullptr;
-  // episode mode (nb_world_set_episodes; every other set call leaves it): ep_slots > 0 slots run the B = S scenes of the bank
-  int ep_slots = 0, ep_max_steps = 0;
-  int32_t *d_scene_of = nullptr, *d_live = nullptr, *d_reset = nullptr, *d_ep_t = nullptr, *d_ep_count = nullptr;  // count: next, finished
-  float* d_ep_clear = nullptr;
-  int32_t *d_r_col = nullptr, *d_r_arr = nullptr, *d_r_astep = nullptr, *d_r_end = nullptr, *d_r_reason = nullptr, *d_r_slot = nullptr;
-  float* d_r_minclr = nullptr;
+  // occupancy maps (nb_world_set_maps): has_map false -> the kernels' map-free instantiations; the host copies are what
+  // nb_world_set_map_contact checks the obstacles' starts against
+  struct Maps {
+    bool has_map = false;
+    nb::DeviceArray<nb::WorldMap> table;
+    nb::DeviceArray<uint32_t> bits;
+    nb::DeviceArray<int32_t> env_map;
+    double window = 0.0;
+    std::vector<nb::WorldMap> h_table;
+    std::vector<uint32_t> h_bits;
+    std::vector<int32_t> h_env_map;
+  } maps;
+  // maps that block obstacles (nb_world_set_map_contact): has_block false -> the kernels' instantiations without it
+  struct Contact {
+    bool has_block = false;
+    nb::DeviceArray<int32_t> block, bounces, bounced;
+  } contact;
+  // episode mode (nb_world_set_episodes): slots > 0 slots run the B = S scenes of the bank
+  struct Episodes {
+    int slots = 0, max_steps = 0;
+    nb::DeviceArray<int32_t> scene_of, live, reset, t, count;  // count: next, finished
+    nb::DeviceArray<float> clear;
+    nb::DeviceArray<int32_t> r_col, r_arr, r_astep, r_end, r_reason, r_slot;
+    nb::DeviceArray<float> r_minclr;
+  } ep;
 };
 
 namespace {
@@ -417,26 +425,6 @@ int world_check_maps(const nb_world_config* cfg, int32_t T, const nb_world_robot
   return NB_OK;
 }
 
-// Frees the map-contact arrays: obstacles pass over the maps from here on.
-void world_drop_contact(nb_world* w) {
-  void* old[] = {w->d_block, w->d_bounces, w->d_bounced};
-  for (void* p : old)
-    if (p) cudaFree(p);
-  w->d_block = w->d_bounces = w->d_bounced = nullptr;
-  w->has_block = false;
-}
-
-// Frees the maps (and their contact flags): the kernels' map-free instantiations from here on.
-void world_drop_maps(nb_world* w) {
-  void* old[] = {w->d_maps, w->d_bits, w->d_env_map};
-  for (void* p : old)
-    if (p) cudaFree(p);
-  w->d_maps = nullptr; w->d_bits = nullptr; w->d_env_map = nullptr;
-  w->has_map = false;
-  w->h_maps.clear(); w->h_bits.clear(); w->h_env_map.clear();
-  world_drop_contact(w);
-}
-
 // Does the footprint of obstacle o at its centre (row) overlap or touch cell [xa, xb] x [ya, yb]?  The host's reading of the
 // kernels' contact test: a circle by its centre's distance to the closed cell, a convex polygon by SAT, an outline by its edges,
 // its vertex 0 in the cell or the cell's corner in it.
@@ -506,18 +494,6 @@ int world_check_contact(const nb_world_config* cfg, int32_t B, const int32_t* ob
   return NB_OK;
 }
 
-// Leaves episode mode: frees the slot and result arrays (the scenes' own rows stay as they are).
-void world_drop_episodes(nb_world* w) {
-  void* old[] = {w->d_scene_of, w->d_live, w->d_reset, w->d_ep_t, w->d_ep_count, w->d_ep_clear, w->d_r_col, w->d_r_arr, w->d_r_astep,
-                 w->d_r_end, w->d_r_reason, w->d_r_slot, w->d_r_minclr};
-  for (void* p : old)
-    if (p) cudaFree(p);
-  w->d_scene_of = w->d_live = w->d_reset = w->d_ep_t = w->d_ep_count = nullptr;
-  w->d_r_col = w->d_r_arr = w->d_r_astep = w->d_r_end = w->d_r_reason = w->d_r_slot = nullptr;
-  w->d_ep_clear = w->d_r_minclr = nullptr;
-  w->ep_slots = 0; w->ep_max_steps = 0;
-}
-
 // Every check of nb_world_set_episodes on the host: S in 1..max_envs, slots in 1..S, max_steps >= 1, and (robot_type not NULL)
 // robot k of every scene of the type of robot k of scene 0.
 int world_check_episodes(const nb_world_config* cfg, int32_t S, int32_t K, const int32_t* robot_type, int32_t slots, int32_t max_steps) {
@@ -535,8 +511,12 @@ int world_check_episodes(const nb_world_config* cfg, int32_t S, int32_t K, const
   return NB_OK;
 }
 
-nb::WorldMapParams world_map_params(const nb_world* w) { return nb::WorldMapParams{w->d_maps, w->d_bits, w->d_env_map, w->window}; }
-nb::WorldBlockParams world_block_params(const nb_world* w) { return nb::WorldBlockParams{w->d_block, w->d_bounces, w->d_bounced}; }
+nb::WorldMapParams world_map_params(const nb_world* w) {
+  return nb::WorldMapParams{w->maps.table.get(), w->maps.bits.get(), w->maps.env_map.get(), w->maps.window};
+}
+nb::WorldBlockParams world_block_params(const nb_world* w) {
+  return nb::WorldBlockParams{w->contact.block.get(), w->contact.bounces.get(), w->contact.bounced.get()};
+}
 
 template <bool kMap>
 int world_scan_occupancy(nb_world* w, int* per_sm) {
@@ -554,7 +534,7 @@ int world_scan_shape(nb_world* w, int B) {
                  (size_t)nre * (4 * sizeof(double) + sizeof(int32_t));
   w->scan_threads = std::min(256, std::max(32, (w->K * w->cfg.num_beams + 31) / 32 * 32));
   int per_sm = 0, sms = 0;
-  if (int rc = w->has_map ? world_scan_occupancy<true>(w, &per_sm) : world_scan_occupancy<false>(w, &per_sm)) return rc;
+  if (int rc = w->maps.has_map ? world_scan_occupancy<true>(w, &per_sm) : world_scan_occupancy<false>(w, &per_sm)) return rc;
   NB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->cfg.device));
   if (per_sm < 1) return fail(NB_ERR_CUDA, "world_scan_kernel: %zu B of shared memory do not fit", w->scan_smem);
   w->scan_grid = std::min(B, per_sm * sms);
@@ -563,14 +543,15 @@ int world_scan_shape(nb_world* w, int B) {
 
 // rvo launch shape: the largest environment's rows (+ the K robots) and one cone list per warp in shared memory
 int world_rvo_shape(nb_world* w, int B) {
-  w->rvo_cap = w->rvo_max_n + w->K;
-  w->rvo_smem = (size_t)w->rvo_cap * (5 * sizeof(double) + nb::kWorldRvoWarps * (6 * sizeof(double) + sizeof(int32_t)));
-  NB_CUDA(cudaFuncSetAttribute(nb::world_rvo_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
+  nb_world::Behaviors& r = w->rvo;
+  r.cap = r.max_n + w->K;
+  r.smem = (size_t)r.cap * (5 * sizeof(double) + nb::kWorldRvoWarps * (6 * sizeof(double) + sizeof(int32_t)));
+  NB_CUDA(cudaFuncSetAttribute(nb::world_rvo_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)r.smem));
   int per_sm = 0, sms = 0;
-  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_rvo_kernel<false>, 32 * nb::kWorldRvoWarps, w->rvo_smem));
+  NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nb::world_rvo_kernel<false>, 32 * nb::kWorldRvoWarps, r.smem));
   NB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->cfg.device));
-  if (per_sm < 1) return fail(NB_ERR_CUDA, "world_rvo_kernel: %zu B of shared memory do not fit", w->rvo_smem);
-  w->rvo_grid = std::min(B, per_sm * sms);
+  if (per_sm < 1) return fail(NB_ERR_CUDA, "world_rvo_kernel: %zu B of shared memory do not fit", r.smem);
+  r.grid = std::min(B, per_sm * sms);
   return NB_OK;
 }
 
@@ -591,26 +572,22 @@ int world_set_robots(nb_world* w, int B, int K, const double* robots, int T, con
     for (int k = 0; k < K; ++k) e += table[rtype[(size_t)b * K + k]].nv;
     max_redges = std::max(max_redges, e);
   }
-  void* old[] = {w->d_states, w->d_collided, w->d_arrived, w->d_fgoal, w->d_fvel, w->d_types, w->d_rtype};
-  for (void* p : old)
-    if (p) cudaFree(p);
-  w->d_states = w->d_fgoal = w->d_fvel = nullptr;
-  w->d_collided = w->d_arrived = w->d_rtype = nullptr;
-  w->d_types = nullptr;
-  NB_CUDA(dalloc(&w->d_states, 3 * N));
-  NB_CUDA(dalloc(&w->d_collided, N));
-  NB_CUDA(dalloc(&w->d_arrived, N));
-  NB_CUDA(dalloc(&w->d_fgoal, 3 * N));
-  NB_CUDA(dalloc(&w->d_fvel, 2 * N));
-  NB_CUDA(dalloc(&w->d_types, table.size()));
-  NB_CUDA(dalloc(&w->d_rtype, N));
-  NB_CUDA(cudaMemcpy(w->d_states, states.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemcpy(w->d_fgoal, goal.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemcpy(w->d_types, table.data(), sizeof(nb::WorldRobotType) * table.size(), cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemcpy(w->d_rtype, rtype.data(), sizeof(int32_t) * N, cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemset(w->d_collided, 0, sizeof(int32_t) * N));
-  NB_CUDA(cudaMemset(w->d_arrived, 0, sizeof(int32_t) * N));
-  NB_CUDA(cudaMemset(w->d_fvel, 0, sizeof(double) * 2 * N));
+  nb_world::Robots& r = w->robots;
+  r = {};
+  NB_CUDA(nb::alloc(r.states, 3 * N));
+  NB_CUDA(nb::alloc(r.collided, N));
+  NB_CUDA(nb::alloc(r.arrived, N));
+  NB_CUDA(nb::alloc(r.goal, 3 * N));
+  NB_CUDA(nb::alloc(r.vel, 2 * N));
+  NB_CUDA(nb::alloc(r.types, table.size()));
+  NB_CUDA(nb::alloc(r.rtype, N));
+  NB_CUDA(cudaMemcpy(r.states.get(), states.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(r.goal.get(), goal.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(r.types.get(), table.data(), sizeof(nb::WorldRobotType) * table.size(), cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(r.rtype.get(), rtype.data(), sizeof(int32_t) * N, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemset(r.collided.get(), 0, sizeof(int32_t) * N));
+  NB_CUDA(cudaMemset(r.arrived.get(), 0, sizeof(int32_t) * N));
+  NB_CUDA(cudaMemset(r.vel.get(), 0, sizeof(double) * 2 * N));
   w->K = K;
   w->max_redges = max_redges;
   w->h_robots.assign(robots, robots + 6 * N);
@@ -622,15 +599,17 @@ int world_set_robots(nb_world* w, int B, int K, const double* robots, int T, con
 nb::WorldParams world_params(const nb_world* w) {
   nb::WorldParams prm;
   const nb_world_config& c = w->cfg;
-  prm.B = w->ep_slots ? w->ep_slots : w->B; prm.R = c.num_beams;
-  prm.dt = c.step_time; prm.range_max = c.range_max; prm.beam_cs = w->d_beam_cs;
+  const nb_world::Scenes& s = w->scenes;
+  const nb_world::Robots& r = w->robots;
+  prm.B = w->ep.slots ? w->ep.slots : w->B; prm.R = c.num_beams;
+  prm.dt = c.step_time; prm.range_max = c.range_max; prm.beam_cs = w->beam_cs.get();
   prm.off_x = c.scan_offset[0]; prm.off_y = c.scan_offset[1]; prm.off_th = c.scan_offset[2];
-  prm.types = w->d_types; prm.rtype = w->d_rtype;
-  prm.obs_begin = w->d_obs_begin; prm.vert_begin = w->d_vert_begin; prm.slot = w->d_slot; prm.counts = w->d_counts; prm.kind = w->d_kind;
-  prm.vertices = w->d_vertices; prm.env = w->d_env; prm.obs = w->d_obs; prm.states = w->d_states;
-  prm.collided = w->d_collided; prm.arrived = w->d_arrived;
-  prm.K = w->K; prm.fgoal = w->d_fgoal; prm.fvel = w->d_fvel;
-  prm.scene_of = w->d_scene_of; prm.live = w->d_live; prm.ep_clear = w->d_ep_clear;
+  prm.types = r.types.get(); prm.rtype = r.rtype.get();
+  prm.obs_begin = s.obs_begin.get(); prm.vert_begin = s.vert_begin.get(); prm.slot = s.slot.get(); prm.counts = s.counts.get(); prm.kind = s.kind.get();
+  prm.vertices = s.vertices.get(); prm.env = s.env.get(); prm.obs = s.obs.get(); prm.states = r.states.get();
+  prm.collided = r.collided.get(); prm.arrived = r.arrived.get();
+  prm.K = w->K; prm.fgoal = r.goal.get(); prm.fvel = r.vel.get();
+  prm.scene_of = w->ep.scene_of.get(); prm.live = w->ep.live.get(); prm.ep_clear = w->ep.clear.get();
   return prm;
 }
 
@@ -639,10 +618,10 @@ nb::WorldParams world_params(const nb_world* w) {
 int world_ready(const nb_world* w, int32_t B, const char* what, bool per_robot = false) {
   if (!w) return fail(NB_ERR_INVALID, "%s: null handle", what);
   if (!w->B) return fail(NB_ERR_INVALID, "%s: no scenes set (nb_world_set_scenes)", what);
-  if (per_robot && w->ep_slots) {
-    if (B != w->ep_slots * w->K)
-      return fail(NB_ERR_INVALID, "%s: count = %d but the world runs episodes in %d slots x %d robots (N = %d)", what, B, w->ep_slots, w->K,
-                  w->ep_slots * w->K);
+  if (per_robot && w->ep.slots) {
+    if (B != w->ep.slots * w->K)
+      return fail(NB_ERR_INVALID, "%s: count = %d but the world runs episodes in %d slots x %d robots (N = %d)", what, B, w->ep.slots, w->K,
+                  w->ep.slots * w->K);
     return NB_OK;
   }
   if (per_robot && w->K > 1) {
@@ -656,8 +635,8 @@ int world_ready(const nb_world* w, int32_t B, const char* what, bool per_robot =
 
 nb::WorldRvoParams world_rvo_params(const nb_world* w, const float* action) {
   nb::WorldRvoParams rp;
-  rp.beh = w->d_beh; rp.radius = w->d_rad; rp.goal = w->d_goal; rp.draws = w->d_draws; rp.action = action;
-  rp.seed = w->seed; rp.cap = w->rvo_cap;
+  rp.beh = w->rvo.beh.get(); rp.radius = w->rvo.rad.get(); rp.goal = w->rvo.goal.get(); rp.draws = w->rvo.draws.get(); rp.action = action;
+  rp.seed = w->rvo.seed; rp.cap = w->rvo.cap;
   return rp;
 }
 
@@ -673,7 +652,7 @@ int nb_world_create(const nb_world_config* cfg, nb_world_t** out) {
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cfg->device < 0 || cfg->device >= ndev)
     return fail(NB_ERR_NO_DEVICE, "no CUDA device available: neupan_b200 has no CPU fallback");
   NB_CUDA(cudaSetDevice(cfg->device));
-  nb_world* w = new (std::nothrow) nb_world();
+  std::unique_ptr<nb_world> w(new (std::nothrow) nb_world());
   if (!w) return fail(NB_ERR_INVALID, "out of host memory");
   w->cfg = *cfg;
   // cos / sin of the beam angles a_i = numpy.linspace(angle_min, angle_max, R)[i] (i * step + start, the last one = stop)
@@ -685,25 +664,15 @@ int nb_world_create(const nb_world_config* cfg, nb_world_t** out) {
     cs[2 * i] = std::cos(a);
     cs[2 * i + 1] = std::sin(a);
   }
-  cudaError_t e = dalloc(&w->d_beam_cs, cs.size());
-  if (e == cudaSuccess) e = cudaMemcpy(w->d_beam_cs, cs.data(), sizeof(double) * cs.size(), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) {
-    nb_world_destroy(w);
-    return fail(NB_ERR_CUDA, "nb_world_create: %s", cudaGetErrorString(e));
-  }
-  *out = w;
+  NB_CUDA(nb::alloc(w->beam_cs, cs.size()));
+  NB_CUDA(cudaMemcpy(w->beam_cs.get(), cs.data(), sizeof(double) * cs.size(), cudaMemcpyHostToDevice));
+  *out = w.release();
   return NB_OK;
 }
 
 int nb_world_destroy(nb_world_t* w) {
   if (!w) return NB_OK;
   cudaSetDevice(w->cfg.device);
-  world_drop_episodes(w);
-  void* bufs[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_collided, w->d_arrived, w->d_vertices, w->d_env, w->d_obs,
-                  w->d_states, w->d_beam_cs, w->d_beh, w->d_rad, w->d_goal, w->d_draws, w->d_fgoal, w->d_fvel, w->d_types, w->d_rtype,
-                  w->d_maps, w->d_bits, w->d_env_map, w->d_block, w->d_bounces, w->d_bounced};
-  for (void* b : bufs)
-    if (b) cudaFree(b);
   delete w;
   return NB_OK;
 }
@@ -730,39 +699,34 @@ int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, c
   for (int b = 0; b < B; ++b)
     for (int c = 0; c < 6; ++c) robots[6 * (size_t)b + c] = envs[(size_t)nb::kWorldEnvCols * b + 4 + c];
   NB_CUDA(cudaSetDevice(w->cfg.device));
-  void* old[] = {w->d_obs_begin, w->d_vert_begin, w->d_slot, w->d_counts, w->d_kind, w->d_vertices, w->d_env, w->d_obs,
-                 w->d_beh, w->d_rad, w->d_goal, w->d_draws};
-  for (void* b : old)
-    if (b) cudaFree(b);
-  w->d_obs_begin = w->d_vert_begin = w->d_slot = w->d_counts = w->d_kind = w->d_draws = nullptr;
-  w->d_vertices = w->d_env = w->d_obs = w->d_beh = w->d_rad = w->d_goal = nullptr;
   w->B = 0;
-  w->has_rvo = false;  // new scenes: every obstacle keeps a constant velocity until nb_world_set_behaviors
-  world_drop_maps(w);  // and has no map until nb_world_set_maps
-  world_drop_episodes(w);  // and runs as a plain world until nb_world_set_episodes
+  // new scenes: every obstacle keeps a constant velocity until nb_world_set_behaviors, has no map until nb_world_set_maps, and the
+  // world runs as a plain world until nb_world_set_episodes
+  w->scenes = {}; w->rvo = {}; w->maps = {}; w->contact = {}; w->ep = {};
   w->h_obs_begin.assign(obs_begin, obs_begin + B + 1);
   w->h_vert_begin.assign(vert_begin, vert_begin + O + 1);
   w->h_vertices.assign(vertices, vertices + 2 * (size_t)V);
   if (obs_kind) w->h_kind.assign(obs_kind, obs_kind + O);
   else w->h_kind.assign(O, 0);
   w->h_env.assign(envs, envs + (size_t)nb::kWorldEnvCols * B);
-  NB_CUDA(dalloc(&w->d_obs_begin, (size_t)B + 1));
-  NB_CUDA(dalloc(&w->d_vert_begin, (size_t)O + 1));
-  NB_CUDA(dalloc(&w->d_slot, (size_t)O));
-  NB_CUDA(dalloc(&w->d_counts, 2 * (size_t)B));
-  NB_CUDA(dalloc(&w->d_kind, (size_t)O));
-  if (O && obs_kind) NB_CUDA(cudaMemcpy(w->d_kind, obs_kind, sizeof(int32_t) * O, cudaMemcpyHostToDevice));
-  else if (O) NB_CUDA(cudaMemset(w->d_kind, 0, sizeof(int32_t) * O));
-  NB_CUDA(dalloc(&w->d_vertices, 2 * (size_t)V));
-  NB_CUDA(dalloc(&w->d_env, (size_t)nb::kWorldEnvCols * B));
-  NB_CUDA(dalloc(&w->d_obs, (size_t)nb::kWorldObsCols * O));
-  NB_CUDA(cudaMemcpy(w->d_obs_begin, obs_begin, sizeof(int32_t) * (B + 1), cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemcpy(w->d_vert_begin, vert_begin, sizeof(int32_t) * (O + 1), cudaMemcpyHostToDevice));
-  if (O) NB_CUDA(cudaMemcpy(w->d_slot, slot.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemcpy(w->d_counts, counts.data(), sizeof(int32_t) * 2 * B, cudaMemcpyHostToDevice));
-  if (V) NB_CUDA(cudaMemcpy(w->d_vertices, vertices, sizeof(double) * 2 * V, cudaMemcpyHostToDevice));
-  NB_CUDA(cudaMemcpy(w->d_env, envs, sizeof(double) * nb::kWorldEnvCols * B, cudaMemcpyHostToDevice));
-  if (O) NB_CUDA(cudaMemcpy(w->d_obs, obstacles, sizeof(double) * nb::kWorldObsCols * O, cudaMemcpyHostToDevice));
+  nb_world::Scenes& s = w->scenes;
+  NB_CUDA(nb::alloc(s.obs_begin, (size_t)B + 1));
+  NB_CUDA(nb::alloc(s.vert_begin, (size_t)O + 1));
+  NB_CUDA(nb::alloc(s.slot, (size_t)O));
+  NB_CUDA(nb::alloc(s.counts, 2 * (size_t)B));
+  NB_CUDA(nb::alloc(s.kind, (size_t)O));
+  if (O && obs_kind) NB_CUDA(cudaMemcpy(s.kind.get(), obs_kind, sizeof(int32_t) * O, cudaMemcpyHostToDevice));
+  else if (O) NB_CUDA(cudaMemset(s.kind.get(), 0, sizeof(int32_t) * O));
+  NB_CUDA(nb::alloc(s.vertices, 2 * (size_t)V));
+  NB_CUDA(nb::alloc(s.env, (size_t)nb::kWorldEnvCols * B));
+  NB_CUDA(nb::alloc(s.obs, (size_t)nb::kWorldObsCols * O));
+  NB_CUDA(cudaMemcpy(s.obs_begin.get(), obs_begin, sizeof(int32_t) * (B + 1), cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(s.vert_begin.get(), vert_begin, sizeof(int32_t) * (O + 1), cudaMemcpyHostToDevice));
+  if (O) NB_CUDA(cudaMemcpy(s.slot.get(), slot.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(s.counts.get(), counts.data(), sizeof(int32_t) * 2 * B, cudaMemcpyHostToDevice));
+  if (V) NB_CUDA(cudaMemcpy(s.vertices.get(), vertices, sizeof(double) * 2 * V, cudaMemcpyHostToDevice));
+  NB_CUDA(cudaMemcpy(s.env.get(), envs, sizeof(double) * nb::kWorldEnvCols * B, cudaMemcpyHostToDevice));
+  if (O) NB_CUDA(cudaMemcpy(s.obs.get(), obstacles, sizeof(double) * nb::kWorldObsCols * O, cudaMemcpyHostToDevice));
   if (int rc = world_set_robots(w, B, 1, robots.data(), 0, nullptr, nullptr)) return rc;
   w->max_circ = max_circ; w->max_edges = max_edges;
   if (int rc = world_scan_shape(w, B)) return rc;
@@ -788,10 +752,9 @@ int nb_world_set_behaviors(nb_world_t* w, int32_t B, const double* behaviors, ui
   NB_CUDA(cudaSetDevice(w->cfg.device));
   const int O = w->O;
   std::vector<double> obs((size_t)nb::kWorldObsCols * O);
-  if (O) NB_CUDA(cudaMemcpy(obs.data(), w->d_obs, sizeof(double) * obs.size(), cudaMemcpyDeviceToHost));  // the current centres
+  if (O) NB_CUDA(cudaMemcpy(obs.data(), w->scenes.obs.get(), sizeof(double) * obs.size(), cudaMemcpyDeviceToHost));  // the current centres
   if (int rc = world_check_behaviors(&w->cfg, B, w->h_obs_begin.data(), obs.data(), w->h_env.data(), behaviors)) return rc;
-  world_drop_episodes(w);
-  world_drop_contact(w);  // which obstacles move has changed: the contact flags need their checks again
+  w->contact = {}; w->ep = {};  // which obstacles move has changed: the contact flags need their checks again
   // radii (circle: its own; polygon: the largest vertex norm), initial goals (NaN: draw 0) and draw counters
   std::vector<double> rad(O), goal(2 * (size_t)O, 0.0);
   std::vector<int32_t> draws(O, 0);
@@ -822,37 +785,33 @@ int nb_world_set_behaviors(nb_world_t* w, int32_t B, const double* behaviors, ui
       }
     }
   }
-  void* old[] = {w->d_beh, w->d_rad, w->d_goal, w->d_draws};
-  for (void* p : old)
-    if (p) cudaFree(p);
-  w->d_beh = w->d_rad = w->d_goal = nullptr;
-  w->d_draws = nullptr;
-  w->has_rvo = false;
-  NB_CUDA(dalloc(&w->d_beh, (size_t)nb::kWorldBehCols * O));
-  NB_CUDA(dalloc(&w->d_rad, (size_t)O));
-  NB_CUDA(dalloc(&w->d_goal, 2 * (size_t)O));
-  NB_CUDA(dalloc(&w->d_draws, (size_t)O));
+  nb_world::Behaviors& r = w->rvo;
+  r = {};
+  NB_CUDA(nb::alloc(r.beh, (size_t)nb::kWorldBehCols * O));
+  NB_CUDA(nb::alloc(r.rad, (size_t)O));
+  NB_CUDA(nb::alloc(r.goal, 2 * (size_t)O));
+  NB_CUDA(nb::alloc(r.draws, (size_t)O));
   if (O) {
-    NB_CUDA(cudaMemcpy(w->d_beh, behaviors, sizeof(double) * nb::kWorldBehCols * O, cudaMemcpyHostToDevice));
-    NB_CUDA(cudaMemcpy(w->d_rad, rad.data(), sizeof(double) * O, cudaMemcpyHostToDevice));
-    NB_CUDA(cudaMemcpy(w->d_goal, goal.data(), sizeof(double) * 2 * O, cudaMemcpyHostToDevice));
-    NB_CUDA(cudaMemcpy(w->d_draws, draws.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemcpy(r.beh.get(), behaviors, sizeof(double) * nb::kWorldBehCols * O, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemcpy(r.rad.get(), rad.data(), sizeof(double) * O, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemcpy(r.goal.get(), goal.data(), sizeof(double) * 2 * O, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemcpy(r.draws.get(), draws.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice));
   }
-  w->seed = seed;
-  w->rvo_max_n = max_n;
+  r.seed = seed;
+  r.max_n = max_n;
   if (int rc = world_rvo_shape(w, B)) return rc;
-  w->has_rvo = any;
+  r.has_rvo = any;
   NB_CUDA(cudaDeviceSynchronize());
   return NB_OK;
 }
 
 int nb_world_read_behaviors(nb_world_t* w, int32_t B, double* goals, int32_t* draws, void* stream) {
   if (int rc = world_ready(w, B, "nb_world_read_behaviors")) return rc;
-  if (!w->d_goal) return fail(NB_ERR_INVALID, "nb_world_read_behaviors: no behaviours set (nb_world_set_behaviors)");
+  if (!w->rvo.goal) return fail(NB_ERR_INVALID, "nb_world_read_behaviors: no behaviours set (nb_world_set_behaviors)");
   NB_CUDA(cudaSetDevice(w->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  if (goals && w->O) NB_CUDA(cudaMemcpyAsync(goals, w->d_goal, sizeof(double) * 2 * w->O, cudaMemcpyDeviceToDevice, st));
-  if (draws && w->O) NB_CUDA(cudaMemcpyAsync(draws, w->d_draws, sizeof(int32_t) * w->O, cudaMemcpyDeviceToDevice, st));
+  if (goals && w->O) NB_CUDA(cudaMemcpyAsync(goals, w->rvo.goal.get(), sizeof(double) * 2 * w->O, cudaMemcpyDeviceToDevice, st));
+  if (draws && w->O) NB_CUDA(cudaMemcpyAsync(draws, w->rvo.draws.get(), sizeof(int32_t) * w->O, cudaMemcpyDeviceToDevice, st));
   return NB_OK;
 }
 
@@ -862,8 +821,9 @@ int nb_world_scan(nb_world_t* w, int32_t B, float* ranges, float* velocity, int3
   NB_CUDA(cudaSetDevice(w->cfg.device));
   // the dynamic shared-memory limit is an attribute of the kernel, shared by every handle of the process: set this handle's
   // size before each launch (another handle's nb_world_set_scenes may have set a smaller one)
-  auto* kernel = w->ep_slots ? (w->has_map ? nb::world_scan_kernel<true, true> : nb::world_scan_kernel<false, true>)
-                             : (w->has_map ? nb::world_scan_kernel<true, false> : nb::world_scan_kernel<false, false>);
+  const bool map = w->maps.has_map;
+  auto* kernel = w->ep.slots ? (map ? nb::world_scan_kernel<true, true> : nb::world_scan_kernel<false, true>)
+                             : (map ? nb::world_scan_kernel<true, false> : nb::world_scan_kernel<false, false>);
   NB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
   kernel<<<w->scan_grid, w->scan_threads, w->scan_smem, (cudaStream_t)stream>>>(world_params(w), world_map_params(w), w->max_circ, w->max_edges,
                                                                                 w->max_redges, ranges, velocity, hit);
@@ -877,16 +837,18 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
   if (!action) return fail(NB_ERR_INVALID, "nb_world_step: null action");
   NB_CUDA(cudaSetDevice(w->cfg.device));
   const nb::WorldParams prm = world_params(w);  // prm.B: the environments, or the slots in episode mode
-  if (w->has_rvo) {  // reactive obstacles choose their velocities from the states at the start of the step
-    const int grid = std::min(w->rvo_grid, prm.B);
-    if (w->has_block) {
-      auto* rvo = w->ep_slots ? nb::world_rvo_block_kernel<true> : nb::world_rvo_block_kernel<false>;
-      NB_CUDA(cudaFuncSetAttribute(rvo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
-      rvo<<<grid, 32 * nb::kWorldRvoWarps, w->rvo_smem, (cudaStream_t)stream>>>(prm, world_rvo_params(w, action), world_map_params(w), world_block_params(w));
+  const bool ep = w->ep.slots > 0, map = w->maps.has_map, blocking = w->contact.has_block;
+  if (w->rvo.has_rvo) {  // reactive obstacles choose their velocities from the states at the start of the step
+    const int grid = std::min(w->rvo.grid, prm.B);
+    const size_t smem = w->rvo.smem;
+    if (blocking) {
+      auto* rvo = ep ? nb::world_rvo_block_kernel<true> : nb::world_rvo_block_kernel<false>;
+      NB_CUDA(cudaFuncSetAttribute(rvo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      rvo<<<grid, 32 * nb::kWorldRvoWarps, smem, (cudaStream_t)stream>>>(prm, world_rvo_params(w, action), world_map_params(w), world_block_params(w));
     } else {
-      auto* rvo = w->ep_slots ? nb::world_rvo_kernel<true> : nb::world_rvo_kernel<false>;
-      NB_CUDA(cudaFuncSetAttribute(rvo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w->rvo_smem));
-      rvo<<<grid, 32 * nb::kWorldRvoWarps, w->rvo_smem, (cudaStream_t)stream>>>(prm, world_rvo_params(w, action));
+      auto* rvo = ep ? nb::world_rvo_kernel<true> : nb::world_rvo_kernel<false>;
+      NB_CUDA(cudaFuncSetAttribute(rvo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      rvo<<<grid, 32 * nb::kWorldRvoWarps, smem, (cudaStream_t)stream>>>(prm, world_rvo_params(w, action));
     }
     ++nb::launches;
     NB_CUDA(cudaGetLastError());
@@ -894,25 +856,26 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
   // a CTA of up to 8 warps per E environments, a warp per robot
   const int E = nb::world_step_envs(w->K);
   const dim3 grid((prm.B + E - 1) / E), block(32 * std::min(E * w->K, nb::kWorldStepMaxWarps));
-  if (w->has_block) {
-    auto* kernel = w->ep_slots ? nb::world_step_block_kernel<true> : nb::world_step_block_kernel<false>;
+  if (blocking) {
+    auto* kernel = ep ? nb::world_step_block_kernel<true> : nb::world_step_block_kernel<false>;
     kernel<<<grid, block, 0, (cudaStream_t)stream>>>(prm, world_map_params(w), world_block_params(w), action, collided, arrived, clearance);
   } else {
-    auto* kernel = w->ep_slots ? (w->has_map ? nb::world_step_ep_kernel<true> : nb::world_step_ep_kernel<false>)
-                               : (w->has_map ? nb::world_step_kernel<true> : nb::world_step_kernel<false>);
+    auto* kernel = ep ? (map ? nb::world_step_ep_kernel<true> : nb::world_step_ep_kernel<false>)
+                      : (map ? nb::world_step_kernel<true> : nb::world_step_kernel<false>);
     kernel<<<grid, block, 0, (cudaStream_t)stream>>>(prm, world_map_params(w), action, collided, arrived, clearance);
   }
   ++nb::launches;
   NB_CUDA(cudaGetLastError());
-  if (w->ep_slots) {  // end the episodes of this step and hand out the next scenes
-    nb::WorldEpisodeParams ep;
-    ep.S = w->B; ep.slots = w->ep_slots; ep.K = w->K; ep.max_steps = w->ep_max_steps;
-    ep.scene_of = w->d_scene_of; ep.live = w->d_live; ep.reset = w->d_reset; ep.t = w->d_ep_t;
-    ep.next = w->d_ep_count; ep.finished = w->d_ep_count + 1;
-    ep.collided = w->d_collided; ep.arrived = w->d_arrived; ep.clear = w->d_ep_clear;
-    ep.r_col = w->d_r_col; ep.r_arr = w->d_r_arr; ep.r_astep = w->d_r_astep; ep.r_minclr = w->d_r_minclr;
-    ep.r_end = w->d_r_end; ep.r_reason = w->d_r_reason; ep.r_slot = w->d_r_slot;
-    nb::world_advance_kernel<<<1, nb::kWorldAdvanceThreads, 0, (cudaStream_t)stream>>>(ep);
+  if (ep) {  // end the episodes of this step and hand out the next scenes
+    const nb_world::Episodes& e = w->ep;
+    nb::WorldEpisodeParams a;
+    a.S = w->B; a.slots = e.slots; a.K = w->K; a.max_steps = e.max_steps;
+    a.scene_of = e.scene_of.get(); a.live = e.live.get(); a.reset = e.reset.get(); a.t = e.t.get();
+    a.next = e.count.get(); a.finished = e.count.get() + 1;
+    a.collided = w->robots.collided.get(); a.arrived = w->robots.arrived.get(); a.clear = e.clear.get();
+    a.r_col = e.r_col.get(); a.r_arr = e.r_arr.get(); a.r_astep = e.r_astep.get(); a.r_minclr = e.r_minclr.get();
+    a.r_end = e.r_end.get(); a.r_reason = e.r_reason.get(); a.r_slot = e.r_slot.get();
+    nb::world_advance_kernel<<<1, nb::kWorldAdvanceThreads, 0, (cudaStream_t)stream>>>(a);
     ++nb::launches;
     NB_CUDA(cudaGetLastError());
   }
@@ -921,24 +884,26 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
 
 int nb_world_read_state(nb_world_t* w, int32_t B, double* states, double* obstacles, int32_t* collided, int32_t* arrived, void* stream) {
   // episode mode: B = slots K reads the slot rows (a gather), B = S K the scenes' own rows (copies, like a plain world)
-  const bool scenes = w && w->ep_slots && B == w->B * w->K;
+  const bool scenes = w && w->ep.slots && B == w->B * w->K;
   if (!scenes)
     if (int rc = world_ready(w, B, "nb_world_read_state", true)) return rc;
   NB_CUDA(cudaSetDevice(w->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  if (w->ep_slots && !scenes) {
-    if (obstacles && w->O) NB_CUDA(cudaMemcpyAsync(obstacles, w->d_obs, sizeof(double) * nb::kWorldObsCols * w->O, cudaMemcpyDeviceToDevice, st));
+  const nb_world::Robots& r = w->robots;
+  const double* obs = w->scenes.obs.get();
+  if (w->ep.slots && !scenes) {
+    if (obstacles && w->O) NB_CUDA(cudaMemcpyAsync(obstacles, obs, sizeof(double) * nb::kWorldObsCols * w->O, cudaMemcpyDeviceToDevice, st));
     if (!states && !collided && !arrived) return NB_OK;
-    nb::world_gather_kernel<<<(B + 255) / 256, 256, 0, st>>>(w->ep_slots, w->K, w->d_scene_of, w->d_states, w->d_collided, w->d_arrived, states,
-                                                             collided, arrived);
+    nb::world_gather_kernel<<<(B + 255) / 256, 256, 0, st>>>(w->ep.slots, w->K, w->ep.scene_of.get(), r.states.get(), r.collided.get(), r.arrived.get(),
+                                                             states, collided, arrived);
     ++nb::launches;
     NB_CUDA(cudaGetLastError());
     return NB_OK;
   }
-  if (states) NB_CUDA(cudaMemcpyAsync(states, w->d_states, sizeof(double) * 3 * B, cudaMemcpyDeviceToDevice, st));
-  if (obstacles && w->O) NB_CUDA(cudaMemcpyAsync(obstacles, w->d_obs, sizeof(double) * nb::kWorldObsCols * w->O, cudaMemcpyDeviceToDevice, st));
-  if (collided) NB_CUDA(cudaMemcpyAsync(collided, w->d_collided, sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
-  if (arrived) NB_CUDA(cudaMemcpyAsync(arrived, w->d_arrived, sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
+  if (states) NB_CUDA(cudaMemcpyAsync(states, r.states.get(), sizeof(double) * 3 * B, cudaMemcpyDeviceToDevice, st));
+  if (obstacles && w->O) NB_CUDA(cudaMemcpyAsync(obstacles, obs, sizeof(double) * nb::kWorldObsCols * w->O, cudaMemcpyDeviceToDevice, st));
+  if (collided) NB_CUDA(cudaMemcpyAsync(collided, r.collided.get(), sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
+  if (arrived) NB_CUDA(cudaMemcpyAsync(arrived, r.arrived.get(), sizeof(int32_t) * B, cudaMemcpyDeviceToDevice, st));
   return NB_OK;
 }
 
@@ -957,11 +922,10 @@ int nb_world_set_fleet_ex(nb_world_t* w, int32_t T, const nb_world_robot_type* t
   if (int rc = world_check_fleet(&w->cfg, T, types, B, K, robots, robot_type)) return rc;
   NB_CUDA(cudaSetDevice(w->cfg.device));
   w->B = 0;  // unusable until the new arrays are in place
-  world_drop_maps(w);  // the new starts need a new map check
-  world_drop_episodes(w);
+  w->maps = {}; w->contact = {}; w->ep = {};  // the new starts need a new map check
   if (int rc = world_set_robots(w, B, K, robots, T, types, robot_type)) return rc;
   if (int rc = world_scan_shape(w, B)) return rc;
-  if (w->d_beh)
+  if (w->rvo.beh)
     if (int rc = world_rvo_shape(w, B)) return rc;
   w->B = B;
   NB_CUDA(cudaDeviceSynchronize());
@@ -986,26 +950,29 @@ int nb_world_set_maps(nb_world_t* w, int32_t P, const nb_world_map* maps, const 
                                 bits, env_map, window, &table))
     return rc;
   NB_CUDA(cudaSetDevice(w->cfg.device));
-  world_drop_maps(w);
-  world_drop_episodes(w);
+  w->maps = {}; w->contact = {}; w->ep = {};
   const size_t words = (size_t)(table.back().off + (int64_t)table.back().H * table.back().words);
-  cudaError_t e = nb::dalloc(&w->d_maps, table.size());
-  if (e == cudaSuccess) e = nb::dalloc(&w->d_bits, words);
-  if (e == cudaSuccess) e = nb::dalloc(&w->d_env_map, (size_t)w->B);
-  if (e == cudaSuccess) e = cudaMemcpy(w->d_maps, table.data(), sizeof(nb::WorldMap) * table.size(), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(w->d_bits, bits, sizeof(uint32_t) * words, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(w->d_env_map, env_map, sizeof(int32_t) * w->B, cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) {  // the handle stays usable, without maps
+  nb_world::Maps m;
+  auto upload = [&]() -> int {
+    NB_CUDA(nb::alloc(m.table, table.size()));
+    NB_CUDA(nb::alloc(m.bits, words));
+    NB_CUDA(nb::alloc(m.env_map, (size_t)w->B));
+    NB_CUDA(cudaMemcpy(m.table.get(), table.data(), sizeof(nb::WorldMap) * table.size(), cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemcpy(m.bits.get(), bits, sizeof(uint32_t) * words, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemcpy(m.env_map.get(), env_map, sizeof(int32_t) * w->B, cudaMemcpyHostToDevice));
+    return NB_OK;
+  };
+  if (int rc = upload()) {  // the handle stays usable, without maps
     cudaGetLastError();
-    world_drop_maps(w);
-    if (int rc = world_scan_shape(w, w->B)) return rc;
-    return fail(NB_ERR_CUDA, "nb_world_set_maps: %zu words of maps: %s", words, cudaGetErrorString(e));
+    if (int rc2 = world_scan_shape(w, w->B)) return rc2;
+    return rc;
   }
-  w->has_map = std::any_of(env_map, env_map + w->B, [](int32_t m) { return m >= 0; });
-  w->window = window;
-  w->h_maps = table;
-  w->h_bits.assign(bits, bits + words);
-  w->h_env_map.assign(env_map, env_map + w->B);
+  m.has_map = std::any_of(env_map, env_map + w->B, [](int32_t e) { return e >= 0; });
+  m.window = window;
+  m.h_table = std::move(table);
+  m.h_bits.assign(bits, bits + words);
+  m.h_env_map.assign(env_map, env_map + w->B);
+  w->maps = std::move(m);
   if (int rc = world_scan_shape(w, w->B)) return rc;
   NB_CUDA(cudaDeviceSynchronize());
   return NB_OK;
@@ -1021,63 +988,63 @@ int nb_world_set_episodes(nb_world_t* w, int32_t slots, int32_t max_steps) {
   const int S = w->B, K = w->K;
   if (int rc = world_check_episodes(&w->cfg, S, K, w->h_rtype.data(), slots, max_steps)) return rc;
   NB_CUDA(cudaSetDevice(w->cfg.device));
-  world_drop_episodes(w);
+  w->ep = {};
   const size_t SK = (size_t)S * K, BK = (size_t)slots * K;
-  std::vector<int32_t> scene_of(slots), slot(S, -1), minus(SK, -1);
+  std::vector<int32_t> scene_of(slots), slot(S, -1), minus(SK, -1), ones(slots, 1);
   for (int b = 0; b < slots; ++b) scene_of[b] = slot[b] = b;
   const int32_t count[2] = {slots, 0};  // the next scene, episodes finished
   std::vector<float> inf(SK, INFINITY);
-  cudaError_t e = cudaSuccess;
-  auto alloc = [&](auto** p, size_t n) { if (e == cudaSuccess) e = dalloc(p, std::max<size_t>(n, 1)); };
-  alloc(&w->d_scene_of, slots); alloc(&w->d_live, slots); alloc(&w->d_reset, slots); alloc(&w->d_ep_t, slots); alloc(&w->d_ep_count, 2);
-  alloc(&w->d_ep_clear, BK);
-  alloc(&w->d_r_col, SK); alloc(&w->d_r_arr, SK); alloc(&w->d_r_astep, SK); alloc(&w->d_r_minclr, SK);
-  alloc(&w->d_r_end, S); alloc(&w->d_r_reason, S); alloc(&w->d_r_slot, S);
-  auto up = [&](void* d, const void* h, size_t bytes) { if (e == cudaSuccess) e = cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice); };
-  auto one = [&](void* d, size_t n) {  // int32 ones
-    std::vector<int32_t> v(n, 1);
-    up(d, v.data(), n * sizeof(int32_t));
+  nb_world::Episodes ep;
+  auto upload = [&]() -> int {
+    NB_CUDA(nb::alloc(ep.scene_of, slots)); NB_CUDA(nb::alloc(ep.live, slots)); NB_CUDA(nb::alloc(ep.reset, slots));
+    NB_CUDA(nb::alloc(ep.t, slots)); NB_CUDA(nb::alloc(ep.count, 2));
+    NB_CUDA(nb::alloc(ep.clear, BK));
+    NB_CUDA(nb::alloc(ep.r_col, SK)); NB_CUDA(nb::alloc(ep.r_arr, SK)); NB_CUDA(nb::alloc(ep.r_astep, SK)); NB_CUDA(nb::alloc(ep.r_minclr, SK));
+    NB_CUDA(nb::alloc(ep.r_end, S)); NB_CUDA(nb::alloc(ep.r_reason, S)); NB_CUDA(nb::alloc(ep.r_slot, S));
+    auto up = [](auto& d, const auto* h, size_t n) { return cudaMemcpy(d.get(), h, n * sizeof(*h), cudaMemcpyHostToDevice); };
+    NB_CUDA(up(ep.scene_of, scene_of.data(), slots));
+    NB_CUDA(up(ep.live, ones.data(), slots));
+    NB_CUDA(up(ep.reset, ones.data(), slots));  // every slot has just taken its first scene
+    NB_CUDA(cudaMemset(ep.t.get(), 0, slots * sizeof(int32_t)));
+    NB_CUDA(up(ep.count, count, 2));
+    NB_CUDA(cudaMemset(ep.r_col.get(), 0, SK * sizeof(int32_t)));
+    NB_CUDA(cudaMemset(ep.r_arr.get(), 0, SK * sizeof(int32_t)));
+    NB_CUDA(up(ep.r_astep, minus.data(), SK));
+    NB_CUDA(up(ep.r_minclr, inf.data(), SK));
+    NB_CUDA(cudaMemset(ep.r_end.get(), 0, S * sizeof(int32_t)));
+    NB_CUDA(cudaMemset(ep.r_reason.get(), 0, S * sizeof(int32_t)));
+    NB_CUDA(up(ep.r_slot, slot.data(), S));
+    NB_CUDA(cudaDeviceSynchronize());
+    return NB_OK;
   };
-  up(w->d_scene_of, scene_of.data(), slots * sizeof(int32_t));
-  one(w->d_live, slots);
-  one(w->d_reset, slots);  // every slot has just taken its first scene
-  if (e == cudaSuccess) e = cudaMemset(w->d_ep_t, 0, slots * sizeof(int32_t));
-  up(w->d_ep_count, count, sizeof(count));
-  if (e == cudaSuccess) e = cudaMemset(w->d_r_col, 0, SK * sizeof(int32_t));
-  if (e == cudaSuccess) e = cudaMemset(w->d_r_arr, 0, SK * sizeof(int32_t));
-  up(w->d_r_astep, minus.data(), SK * sizeof(int32_t));
-  up(w->d_r_minclr, inf.data(), SK * sizeof(float));
-  if (e == cudaSuccess) e = cudaMemset(w->d_r_end, 0, S * sizeof(int32_t));
-  if (e == cudaSuccess) e = cudaMemset(w->d_r_reason, 0, S * sizeof(int32_t));
-  up(w->d_r_slot, slot.data(), S * sizeof(int32_t));
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) {  // the handle stays usable as a plain world
+  if (int rc = upload()) {  // the handle stays usable as a plain world
     cudaGetLastError();
-    world_drop_episodes(w);
-    return fail(NB_ERR_CUDA, "nb_world_set_episodes: %s", cudaGetErrorString(e));
+    return rc;
   }
-  w->ep_slots = slots; w->ep_max_steps = max_steps;
+  ep.slots = slots; ep.max_steps = max_steps;
+  w->ep = std::move(ep);
   return NB_OK;
 }
 
 int nb_world_read_episodes(nb_world_t* w, int32_t S, int32_t* collided, int32_t* arrived, int32_t* arrive_step, float* min_clearance, int32_t* end_step,
                            int32_t* reason, int32_t* slot, int32_t* scene_of, int32_t* reset, int32_t* finished, void* stream) {
   if (int rc = world_ready(w, S, "nb_world_read_episodes")) return rc;
-  if (!w->ep_slots) return fail(NB_ERR_INVALID, "nb_world_read_episodes: not in episode mode (nb_world_set_episodes)");
+  const nb_world::Episodes& ep = w->ep;
+  if (!ep.slots) return fail(NB_ERR_INVALID, "nb_world_read_episodes: not in episode mode (nb_world_set_episodes)");
   NB_CUDA(cudaSetDevice(w->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   const size_t SK = (size_t)S * w->K;
   auto cp = [&](void* dst, const void* src, size_t bytes) { return dst ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) : cudaSuccess; };
-  NB_CUDA(cp(collided, w->d_r_col, SK * sizeof(int32_t)));
-  NB_CUDA(cp(arrived, w->d_r_arr, SK * sizeof(int32_t)));
-  NB_CUDA(cp(arrive_step, w->d_r_astep, SK * sizeof(int32_t)));
-  NB_CUDA(cp(min_clearance, w->d_r_minclr, SK * sizeof(float)));
-  NB_CUDA(cp(end_step, w->d_r_end, S * sizeof(int32_t)));
-  NB_CUDA(cp(reason, w->d_r_reason, S * sizeof(int32_t)));
-  NB_CUDA(cp(slot, w->d_r_slot, S * sizeof(int32_t)));
-  NB_CUDA(cp(scene_of, w->d_scene_of, w->ep_slots * sizeof(int32_t)));
-  NB_CUDA(cp(reset, w->d_reset, w->ep_slots * sizeof(int32_t)));
-  NB_CUDA(cp(finished, w->d_ep_count + 1, sizeof(int32_t)));
+  NB_CUDA(cp(collided, ep.r_col.get(), SK * sizeof(int32_t)));
+  NB_CUDA(cp(arrived, ep.r_arr.get(), SK * sizeof(int32_t)));
+  NB_CUDA(cp(arrive_step, ep.r_astep.get(), SK * sizeof(int32_t)));
+  NB_CUDA(cp(min_clearance, ep.r_minclr.get(), SK * sizeof(float)));
+  NB_CUDA(cp(end_step, ep.r_end.get(), S * sizeof(int32_t)));
+  NB_CUDA(cp(reason, ep.r_reason.get(), S * sizeof(int32_t)));
+  NB_CUDA(cp(slot, ep.r_slot.get(), S * sizeof(int32_t)));
+  NB_CUDA(cp(scene_of, ep.scene_of.get(), ep.slots * sizeof(int32_t)));
+  NB_CUDA(cp(reset, ep.reset.get(), ep.slots * sizeof(int32_t)));
+  NB_CUDA(cp(finished, ep.count.get() + 1, sizeof(int32_t)));
   return NB_OK;
 }
 
@@ -1094,20 +1061,20 @@ int nb_world_check_map_contact(const nb_world_config* cfg, int32_t B, const int3
 
 int nb_world_set_map_contact(nb_world_t* w, int32_t B, const int32_t* flags) {
   if (int rc = world_ready(w, B, "nb_world_set_map_contact")) return rc;
-  if (!w->d_maps) return fail(NB_ERR_INVALID, "nb_world_set_map_contact: no maps set (nb_world_set_maps)");
+  if (!w->maps.table) return fail(NB_ERR_INVALID, "nb_world_set_map_contact: no maps set (nb_world_set_maps)");
   NB_CUDA(cudaSetDevice(w->cfg.device));
   const int O = w->O;
+  nb_world::Behaviors& rvo = w->rvo;
   std::vector<double> obs((size_t)nb::kWorldObsCols * O), beh;
-  if (O) NB_CUDA(cudaMemcpy(obs.data(), w->d_obs, sizeof(double) * obs.size(), cudaMemcpyDeviceToHost));  // the current centres
-  if (w->d_beh && O) {
+  if (O) NB_CUDA(cudaMemcpy(obs.data(), w->scenes.obs.get(), sizeof(double) * obs.size(), cudaMemcpyDeviceToHost));  // the current centres
+  if (rvo.beh && O) {
     beh.resize((size_t)nb::kWorldBehCols * O);
-    NB_CUDA(cudaMemcpy(beh.data(), w->d_beh, sizeof(double) * beh.size(), cudaMemcpyDeviceToHost));
+    NB_CUDA(cudaMemcpy(beh.data(), rvo.beh.get(), sizeof(double) * beh.size(), cudaMemcpyDeviceToHost));
   }
   if (int rc = world_check_contact(&w->cfg, B, w->h_obs_begin.data(), obs.data(), w->h_vert_begin.data(), w->h_vertices.data(), w->h_kind.data(),
-                                   beh.empty() ? nullptr : beh.data(), w->h_maps, w->h_bits.data(), w->h_env_map.data(), flags))
+                                   beh.empty() ? nullptr : beh.data(), w->maps.h_table, w->maps.h_bits.data(), w->maps.h_env_map.data(), flags))
     return rc;
-  world_drop_contact(w);
-  world_drop_episodes(w);
+  w->contact = {}; w->ep = {};
   // a wandering obstacle without an explicit goal in a blocking environment starts from goal = its centre and draw 0, so that its
   // first goal is drawn on the device through the map test
   std::vector<double> goal;
@@ -1115,8 +1082,8 @@ int nb_world_set_map_contact(nb_world_t* w, int32_t B, const int32_t* flags) {
   bool reset = false;
   if (!beh.empty()) {
     goal.resize(2 * (size_t)O); draws.resize(O);
-    NB_CUDA(cudaMemcpy(goal.data(), w->d_goal, sizeof(double) * goal.size(), cudaMemcpyDeviceToHost));
-    NB_CUDA(cudaMemcpy(draws.data(), w->d_draws, sizeof(int32_t) * O, cudaMemcpyDeviceToHost));
+    NB_CUDA(cudaMemcpy(goal.data(), rvo.goal.get(), sizeof(double) * goal.size(), cudaMemcpyDeviceToHost));
+    NB_CUDA(cudaMemcpy(draws.data(), rvo.draws.get(), sizeof(int32_t) * O, cudaMemcpyDeviceToHost));
     for (int b = 0; b < B; ++b) {
       if (!flags[b]) continue;
       for (int o = w->h_obs_begin[b]; o < w->h_obs_begin[b + 1]; ++o) {
@@ -1128,31 +1095,35 @@ int nb_world_set_map_contact(nb_world_t* w, int32_t B, const int32_t* flags) {
       }
     }
   }
-  cudaError_t e = nb::dalloc(&w->d_block, (size_t)B);
-  if (e == cudaSuccess) e = nb::dalloc(&w->d_bounces, std::max<size_t>(O, 1));
-  if (e == cudaSuccess) e = nb::dalloc(&w->d_bounced, std::max<size_t>(O, 1));
-  if (e == cudaSuccess) e = cudaMemcpy(w->d_block, flags, sizeof(int32_t) * B, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemset(w->d_bounces, 0, sizeof(int32_t) * std::max(O, 1));
-  if (e == cudaSuccess) e = cudaMemset(w->d_bounced, 0, sizeof(int32_t) * std::max(O, 1));
-  if (e == cudaSuccess && reset) e = cudaMemcpy(w->d_goal, goal.data(), sizeof(double) * goal.size(), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && reset) e = cudaMemcpy(w->d_draws, draws.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) {
+  nb_world::Contact c;
+  auto upload = [&]() -> int {
+    NB_CUDA(nb::alloc(c.block, (size_t)B));
+    NB_CUDA(nb::alloc(c.bounces, (size_t)O));
+    NB_CUDA(nb::alloc(c.bounced, (size_t)O));
+    NB_CUDA(cudaMemcpy(c.block.get(), flags, sizeof(int32_t) * B, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemset(c.bounces.get(), 0, sizeof(int32_t) * std::max(O, 1)));
+    NB_CUDA(cudaMemset(c.bounced.get(), 0, sizeof(int32_t) * std::max(O, 1)));
+    if (reset) NB_CUDA(cudaMemcpy(rvo.goal.get(), goal.data(), sizeof(double) * goal.size(), cudaMemcpyHostToDevice));
+    if (reset) NB_CUDA(cudaMemcpy(rvo.draws.get(), draws.data(), sizeof(int32_t) * O, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaDeviceSynchronize());
+    return NB_OK;
+  };
+  if (int rc = upload()) {  // no contact flags
     cudaGetLastError();
-    world_drop_contact(w);
-    return fail(NB_ERR_CUDA, "nb_world_set_map_contact: %s", cudaGetErrorString(e));
+    return rc;
   }
-  w->has_block = std::any_of(flags, flags + B, [](int32_t f) { return f != 0; });
+  c.has_block = std::any_of(flags, flags + B, [](int32_t f) { return f != 0; });
+  w->contact = std::move(c);
   return NB_OK;
 }
 
 int nb_world_read_map_contact(nb_world_t* w, int32_t O, int32_t* bounces, void* stream) {
   if (!w) return fail(NB_ERR_INVALID, "nb_world_read_map_contact: null handle");
-  if (!w->d_bounces) return fail(NB_ERR_INVALID, "nb_world_read_map_contact: no map contact set (nb_world_set_map_contact)");
+  if (!w->contact.bounces) return fail(NB_ERR_INVALID, "nb_world_read_map_contact: no map contact set (nb_world_set_map_contact)");
   if (O != w->O) return fail(NB_ERR_INVALID, "nb_world_read_map_contact: O = %d but the scenes have %d obstacles", O, w->O);
   if (!bounces) return fail(NB_ERR_INVALID, "nb_world_read_map_contact: null bounces");
   NB_CUDA(cudaSetDevice(w->cfg.device));
-  if (O) NB_CUDA(cudaMemcpyAsync(bounces, w->d_bounces, sizeof(int32_t) * O, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  if (O) NB_CUDA(cudaMemcpyAsync(bounces, w->contact.bounces.get(), sizeof(int32_t) * O, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return NB_OK;
 }
 
