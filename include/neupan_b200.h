@@ -495,12 +495,47 @@ int nb_world_set_maps(nb_world_t* w, int32_t P, const nb_world_map* maps, const 
  * still be crossed by a footprint smaller than one step.  nb_world_check_map_contact performs them on the host without a handle or a
  * device (behaviors NULL: every obstacle keeps its constant velocity).
  * nb_world_read_map_contact enqueues a device-to-device copy of the O per-obstacle bounce counts on `stream` and does not synchronise.
- * Not modelled: walls as RVO neighbours (ORCA lines), obstacle-obstacle collisions, moving maps, swept or continuous collision. */
+ * Not modelled: walls as RVO neighbours (ORCA lines), moving maps, swept or continuous collision; obstacle-obstacle contact is the
+ * separate nb_world_set_obstacle_contact below. */
 int nb_world_check_map_contact(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
                                const double* vertices, const double* envs, const int32_t* obs_kind, const double* behaviors, int32_t P,
                                const nb_world_map* maps, const uint32_t* bits, const int32_t* env_map, const int32_t* flags);
 int nb_world_set_map_contact(nb_world_t* w, int32_t B, const int32_t* flags);
 int nb_world_read_map_contact(nb_world_t* w, int32_t O, int32_t* bounces, void* stream);
+
+/* Obstacle contact (semantics in csrc/world_contact_kernel.cuh): flags (B) int32 HOST, 1 where an environment's obstacles block each
+ * other, 0 (the default, and every environment without this call) where they pass through each other.  Where it is 1:
+ *   touch     two footprints touch when their clearance is <= 0: circle-circle by centre distance - (r_i + r_j); circle-convex by the
+ *             circle test of the robot clearance; circle-outline by even-odd or centre-edge distance <= r; convex-convex and
+ *             convex-outline by the robot clearance tests; outline-outline when two edges meet or vertex 0 of either lies inside the
+ *             other.  A pair is tested only when the boxes of the two footprints, each widened by 1e-6 m, meet.  The test is symmetric
+ *             bit for bit.
+ *   move      the obstacles move in ascending row order.  Every moving obstacle (v != 0 after the rvo kernel) takes, after its move and
+ *             rectangle mirror (c', v') from (c, v), the first of A (c'x, c'y) with (v'x, v'y), B (c'x, cy) with (v'x, -v'y), C
+ *             (cx, c'y) with (-v'x, v'y), D (cx, cy) with (-v'x, -v'y) whose footprint touches no other obstacle of its environment (the
+ *             earlier rows at their new centres, the later rows at their old ones, static obstacles included) and, where the map
+ *             blocks obstacles, not the map either.  D always (the start is clear), so no moving obstacle ever touches another
+ *             obstacle.  A step whose A touches another obstacle is an obstacle bounce (nb_world_read_obstacle_contact counts them per
+ *             obstacle); the map's bounce count and a reactive obstacle's reaction to it keep their meaning (A touched the map).
+ *             Reactive obstacles choose their velocity as before.  Robots do not block obstacles (an obstacle may still move into a
+ *             robot, which then collides).
+ * nb_world_set_obstacle_contact comes after nb_world_set_scenes(_ex), nb_world_set_behaviors, nb_world_set_fleet(_ex),
+ * nb_world_set_maps and nb_world_set_map_contact, which all drop it; it leaves episode mode (nb_world_set_episodes comes after it:
+ * then scene s's flag and bounce counts hold for its obstacle rows in whatever slot runs it).  It zeroes the bounce counts and
+ * synchronises the device.  With a flag set nb_world_step launches one more kernel (the obstacles move there, one warp per
+ * environment); without one the kernels launched are those of a world without this call.
+ * Checks (NB_ERR_INVALID, naming the environment and obstacle rows): B is the handle's environment count; every flag is 0 or 1; no
+ * obstacle that can move (v != 0, or reactive) of an environment with the flag set starts touching another obstacle of it, by the
+ * same test on the host.  Static obstacles may overlap each other.  nb_world_check_obstacle_contact performs them on the host
+ * without a handle or a device (behaviors NULL: every obstacle keeps its constant velocity).
+ * nb_world_read_obstacle_contact enqueues a device-to-device copy of the O per-obstacle bounce counts on `stream` and does not
+ * synchronise.
+ * Limits: no swept test (a step longer than the thinner of two footprints can pass through it; dyna_obs's circles move at most
+ * 0.05 m per step at step_time 0.1 s), no contact with robots, no momentum or elastic response, and earlier rows move first. */
+int nb_world_check_obstacle_contact(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                                    const double* vertices, const double* envs, const int32_t* obs_kind, const double* behaviors, const int32_t* flags);
+int nb_world_set_obstacle_contact(nb_world_t* w, int32_t B, const int32_t* flags);
+int nb_world_read_obstacle_contact(nb_world_t* w, int32_t O, int32_t* bounces, void* stream);
 
 /* Continuous episodes (semantics in csrc/world_episode_kernel.cuh): a bank of S scenes runs through `slots` slots, and a slot starts
  * the next unstarted scene on the device when its episode ends.  The bank is uploaded as a world of B = S environments

@@ -130,6 +130,9 @@ SYMBOLS = {
     "nb_world_check_map_contact": (C.c_int, [C.POINTER(WorldConfig), C.c_int32] + [_FP] * 7 + [C.c_int32, _FP, _FP, _FP, _FP]),
     "nb_world_set_map_contact": (C.c_int, [C.c_void_p, C.c_int32, _FP]),
     "nb_world_read_map_contact": (C.c_int, [C.c_void_p, C.c_int32, _FP, C.c_void_p]),
+    "nb_world_check_obstacle_contact": (C.c_int, [C.POINTER(WorldConfig), C.c_int32] + [_FP] * 8),
+    "nb_world_set_obstacle_contact": (C.c_int, [C.c_void_p, C.c_int32, _FP]),
+    "nb_world_read_obstacle_contact": (C.c_int, [C.c_void_p, C.c_int32, _FP, C.c_void_p]),
     "nb_world_check_episodes": (C.c_int, [C.POINTER(WorldConfig), C.c_int32, C.c_int32, _FP, C.c_int32, C.c_int32]),
     "nb_world_set_episodes": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "nb_world_read_episodes": (C.c_int, [C.c_void_p, C.c_int32] + [_FP] * 10 + [C.c_void_p]),

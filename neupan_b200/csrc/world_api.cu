@@ -10,6 +10,7 @@
 #include "world_kernel.cuh"
 #include "world_rvo_kernel.cuh"
 #include "world_episode_kernel.cuh"
+#include "world_contact_kernel.cuh"
 
 using nb::fail;
 
@@ -68,6 +69,12 @@ struct nb_world {
     bool has_block = false;
     nb::DeviceArray<int32_t> block, bounces, bounced;
   } contact;
+  // obstacles that block each other (nb_world_set_obstacle_contact): has_contact false -> the kernels of a world without it
+  struct ObstacleContact {
+    bool has_contact = false;
+    int max_n = 0;  // the largest environment's obstacle count (world_contact_kernel's staging)
+    nb::DeviceArray<int32_t> flag, bounces;
+  } ocontact;
   // episode mode (nb_world_set_episodes): slots > 0 slots run the B = S scenes of the bank
   struct Episodes {
     int slots = 0, max_steps = 0;
@@ -494,6 +501,118 @@ int world_check_contact(const nb_world_config* cfg, int32_t B, const int32_t* ob
   return NB_OK;
 }
 
+// ---- obstacle contact on the host (the start check of nb_world_set_obstacle_contact) ------------------------------------------
+
+double host_seg_dist(double px, double py, const double* a, const double* b) {
+  const double ex = b[0] - a[0], ey = b[1] - a[1], wx = px - a[0], wy = py - a[1];
+  double t = (host_dmul(wx, ex) + host_dmul(wy, ey)) / (host_dmul(ex, ex) + host_dmul(ey, ey));
+  t = t < 0.0 ? 0.0 : (t > 1.0 ? 1.0 : t);
+  const double qx = wx - host_dmul(t, ex), qy = wy - host_dmul(t, ey);
+  return std::sqrt(host_dmul(qx, qx) + host_dmul(qy, qy));
+}
+
+double host_cross(const double* a, const double* b, double px, double py) {
+  return host_dmul(b[0] - a[0], py - a[1]) - host_dmul(b[1] - a[1], px - a[0]);
+}
+
+// even-odd test of (px, py) against the polygon v of n vertices
+bool host_inside_outline(const double* v, int n, double px, double py) {
+  bool in = false;
+  for (int k = 0; k < n; ++k) {
+    const double* a = v + 2 * k;
+    const double* b = v + 2 * ((k + 1) % n);
+    if ((a[1] > py) != (b[1] > py)) {
+      const double cr = host_cross(a, b, px, py);
+      if (b[1] > a[1] ? cr > 0.0 : cr < 0.0) in = !in;
+    }
+  }
+  return in;
+}
+
+// (px, py) is not strictly outside the convex polygon v (the edge cross products do not take both signs)
+bool host_inside_convex(const double* v, int n, double px, double py) {
+  bool pos = false, neg = false;
+  for (int k = 0; k < n; ++k) {
+    const double cr = host_cross(v + 2 * k, v + 2 * ((k + 1) % n), px, py);
+    pos |= cr > 0.0; neg |= cr < 0.0;
+  }
+  return !(pos && neg);
+}
+
+// An obstacle footprint at its centre: rank 0 circle, 1 convex polygon, 2 outline; world vertices; the box widened by the pad
+struct HostShape {
+  double cx, cy, r;
+  int nv, rank;
+  double v[2 * nb::kWorldMaxOutlineVertices];
+  double box[4];
+};
+
+HostShape host_shape(const double* row, const double* rel, int nv, int kind) {
+  HostShape s{};
+  s.cx = row[0]; s.cy = row[1]; s.r = row[4]; s.nv = nv;
+  s.rank = nv == 0 ? 0 : (kind != 0 ? 2 : 1);
+  double x0 = -s.r, y0 = -s.r, x1 = s.r, y1 = s.r;
+  if (nv > 0) {
+    x0 = x1 = rel[0]; y0 = y1 = rel[1];
+    for (int k = 0; k < nv; ++k) {
+      s.v[2 * k] = s.cx + rel[2 * k]; s.v[2 * k + 1] = s.cy + rel[2 * k + 1];
+      x0 = std::min(x0, rel[2 * k]); x1 = std::max(x1, rel[2 * k]);
+      y0 = std::min(y0, rel[2 * k + 1]); y1 = std::max(y1, rel[2 * k + 1]);
+    }
+  }
+  s.box[0] = s.cx + x0 - nb::kWorldContactPad; s.box[1] = s.cy + y0 - nb::kWorldContactPad;
+  s.box[2] = s.cx + x1 + nb::kWorldContactPad; s.box[3] = s.cy + y1 + nb::kWorldContactPad;
+  return s;
+}
+
+// world_footprints_touch on the host, behind the same broad phase
+bool host_shapes_touch(const HostShape& f, const HostShape& g) {
+  if (f.box[2] < g.box[0] || g.box[2] < f.box[0] || f.box[3] < g.box[1] || g.box[3] < f.box[1]) return false;
+  const HostShape& a = f.rank <= g.rank ? f : g;
+  const HostShape& b = f.rank <= g.rank ? g : f;
+  if (b.rank == 0) {
+    const double dx = a.cx - b.cx, dy = a.cy - b.cy;
+    return std::sqrt(host_dmul(dx, dx) + host_dmul(dy, dy)) - (a.r + b.r) <= 0.0;
+  }
+  if (a.rank == 0) {
+    double d = INFINITY;
+    for (int k = 0; k < b.nv; ++k) d = std::min(d, host_seg_dist(a.cx, a.cy, b.v + 2 * k, b.v + 2 * ((k + 1) % b.nv)));
+    return b.rank == 1 ? (host_inside_convex(b.v, b.nv, a.cx, a.cy) || d - a.r <= 0.0) : (host_inside_outline(b.v, b.nv, a.cx, a.cy) || d <= a.r);
+  }
+  if (b.rank == 1) return world_bodies_meet(a.v, a.nv, b.v, b.nv);
+  for (int k = 0; k < a.nv; ++k)
+    for (int i = 0; i < b.nv; ++i)
+      if (world_segs_meet(a.v + 2 * k, a.v + 2 * ((k + 1) % a.nv), b.v + 2 * i, b.v + 2 * ((i + 1) % b.nv))) return true;
+  if (host_inside_outline(b.v, b.nv, a.v[0], a.v[1])) return true;
+  return a.rank == 1 ? host_inside_convex(a.v, a.nv, b.v[0], b.v[1]) : host_inside_outline(a.v, a.nv, b.v[0], b.v[1]);
+}
+
+// Every check of nb_world_set_obstacle_contact on valid scenes and behaviours (NULL: every obstacle constant); obs holds the
+// obstacles' current centres and velocities.
+int world_check_obstacle_contact(int32_t B, const int32_t* obs_begin, const double* obs, const int32_t* vert_begin, const double* vertices,
+                                 const int32_t* kind, const double* beh, const int32_t* flags) {
+  if (!flags) return fail(NB_ERR_INVALID, "nb_world obstacle contact: null flags");
+  std::vector<HostShape> shapes;
+  for (int b = 0; b < B; ++b) {
+    if (flags[b] != 0 && flags[b] != 1) return fail(NB_ERR_INVALID, "environment %d: obstacle contact flag %d (0 or 1)", b, flags[b]);
+    if (flags[b] == 0) continue;
+    const int o0 = obs_begin[b], o1 = obs_begin[b + 1];
+    shapes.clear();
+    for (int o = o0; o < o1; ++o)
+      shapes.push_back(host_shape(obs + (size_t)nb::kWorldObsCols * o, vertices + 2 * (size_t)vert_begin[o], vert_begin[o + 1] - vert_begin[o],
+                                  kind ? kind[o] : 0));
+    for (int o = o0; o < o1; ++o) {
+      const double* row = obs + (size_t)nb::kWorldObsCols * o;
+      const bool reactive = beh && beh[(size_t)nb::kWorldBehCols * o] == 1.0;
+      if (!reactive && row[2] == 0.0 && row[3] == 0.0) continue;  // static obstacles may overlap each other
+      for (int p = o0; p < o1; ++p)
+        if (p != o && host_shapes_touch(shapes[o - o0], shapes[p - o0]))
+          return fail(NB_ERR_INVALID, "environment %d, obstacle %d: moves but its start footprint overlaps or touches obstacle %d", b, o, p);
+    }
+  }
+  return NB_OK;
+}
+
 // Every check of nb_world_set_episodes on the host: S in 1..max_envs, slots in 1..S, max_steps >= 1, and (robot_type not NULL)
 // robot k of every scene of the type of robot k of scene 0.
 int world_check_episodes(const nb_world_config* cfg, int32_t S, int32_t K, const int32_t* robot_type, int32_t slots, int32_t max_steps) {
@@ -516,6 +635,9 @@ nb::WorldMapParams world_map_params(const nb_world* w) {
 }
 nb::WorldBlockParams world_block_params(const nb_world* w) {
   return nb::WorldBlockParams{w->contact.block.get(), w->contact.bounces.get(), w->contact.bounced.get()};
+}
+nb::WorldContactParams world_contact_params(const nb_world* w) {
+  return nb::WorldContactParams{w->ocontact.flag.get(), w->ocontact.bounces.get(), w->ocontact.max_n};
 }
 
 template <bool kMap>
@@ -702,7 +824,7 @@ int nb_world_set_scenes_ex(nb_world_t* w, int32_t B, const int32_t* obs_begin, c
   w->B = 0;
   // new scenes: every obstacle keeps a constant velocity until nb_world_set_behaviors, has no map until nb_world_set_maps, and the
   // world runs as a plain world until nb_world_set_episodes
-  w->scenes = {}; w->rvo = {}; w->maps = {}; w->contact = {}; w->ep = {};
+  w->scenes = {}; w->rvo = {}; w->maps = {}; w->contact = {}; w->ocontact = {}; w->ep = {};
   w->h_obs_begin.assign(obs_begin, obs_begin + B + 1);
   w->h_vert_begin.assign(vert_begin, vert_begin + O + 1);
   w->h_vertices.assign(vertices, vertices + 2 * (size_t)V);
@@ -754,7 +876,7 @@ int nb_world_set_behaviors(nb_world_t* w, int32_t B, const double* behaviors, ui
   std::vector<double> obs((size_t)nb::kWorldObsCols * O);
   if (O) NB_CUDA(cudaMemcpy(obs.data(), w->scenes.obs.get(), sizeof(double) * obs.size(), cudaMemcpyDeviceToHost));  // the current centres
   if (int rc = world_check_behaviors(&w->cfg, B, w->h_obs_begin.data(), obs.data(), w->h_env.data(), behaviors)) return rc;
-  w->contact = {}; w->ep = {};  // which obstacles move has changed: the contact flags need their checks again
+  w->contact = {}; w->ocontact = {}; w->ep = {};  // which obstacles move has changed: the contact flags need their checks again
   // radii (circle: its own; polygon: the largest vertex norm), initial goals (NaN: draw 0) and draw counters
   std::vector<double> rad(O), goal(2 * (size_t)O, 0.0);
   std::vector<int32_t> draws(O, 0);
@@ -837,7 +959,7 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
   if (!action) return fail(NB_ERR_INVALID, "nb_world_step: null action");
   NB_CUDA(cudaSetDevice(w->cfg.device));
   const nb::WorldParams prm = world_params(w);  // prm.B: the environments, or the slots in episode mode
-  const bool ep = w->ep.slots > 0, map = w->maps.has_map, blocking = w->contact.has_block;
+  const bool ep = w->ep.slots > 0, map = w->maps.has_map, blocking = w->contact.has_block, contact = w->ocontact.has_contact;
   if (w->rvo.has_rvo) {  // reactive obstacles choose their velocities from the states at the start of the step
     const int grid = std::min(w->rvo.grid, prm.B);
     const size_t smem = w->rvo.smem;
@@ -856,7 +978,18 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
   // a CTA of up to 8 warps per E environments, a warp per robot
   const int E = nb::world_step_envs(w->K);
   const dim3 grid((prm.B + E - 1) / E), block(32 * std::min(E * w->K, nb::kWorldStepMaxWarps));
-  if (blocking) {
+  if (contact) {  // the obstacles move one environment per warp, in row order; the step then leaves them where they are
+    const int units = (prm.B + nb::kWorldContactWarps - 1) / nb::kWorldContactWarps;
+    const size_t smem = sizeof(double) * nb::kWorldContactWarps * 6 * w->ocontact.max_n;
+    auto* move = blocking ? (ep ? nb::world_contact_kernel<true, true> : nb::world_contact_kernel<true, false>)
+                          : (ep ? nb::world_contact_kernel<false, true> : nb::world_contact_kernel<false, false>);
+    move<<<units, 32 * nb::kWorldContactWarps, smem, (cudaStream_t)stream>>>(prm, world_map_params(w), world_block_params(w), world_contact_params(w));
+    ++nb::launches;
+    NB_CUDA(cudaGetLastError());
+    auto* kernel = ep ? (map ? nb::world_step_contact_kernel<true, true> : nb::world_step_contact_kernel<false, true>)
+                      : (map ? nb::world_step_contact_kernel<true, false> : nb::world_step_contact_kernel<false, false>);
+    kernel<<<grid, block, 0, (cudaStream_t)stream>>>(prm, world_map_params(w), action, collided, arrived, clearance);
+  } else if (blocking) {
     auto* kernel = ep ? nb::world_step_block_kernel<true> : nb::world_step_block_kernel<false>;
     kernel<<<grid, block, 0, (cudaStream_t)stream>>>(prm, world_map_params(w), world_block_params(w), action, collided, arrived, clearance);
   } else {
@@ -922,7 +1055,7 @@ int nb_world_set_fleet_ex(nb_world_t* w, int32_t T, const nb_world_robot_type* t
   if (int rc = world_check_fleet(&w->cfg, T, types, B, K, robots, robot_type)) return rc;
   NB_CUDA(cudaSetDevice(w->cfg.device));
   w->B = 0;  // unusable until the new arrays are in place
-  w->maps = {}; w->contact = {}; w->ep = {};  // the new starts need a new map check
+  w->maps = {}; w->contact = {}; w->ocontact = {}; w->ep = {};  // the new starts need a new map check
   if (int rc = world_set_robots(w, B, K, robots, T, types, robot_type)) return rc;
   if (int rc = world_scan_shape(w, B)) return rc;
   if (w->rvo.beh)
@@ -950,7 +1083,7 @@ int nb_world_set_maps(nb_world_t* w, int32_t P, const nb_world_map* maps, const 
                                 bits, env_map, window, &table))
     return rc;
   NB_CUDA(cudaSetDevice(w->cfg.device));
-  w->maps = {}; w->contact = {}; w->ep = {};
+  w->maps = {}; w->contact = {}; w->ocontact = {}; w->ep = {};
   const size_t words = (size_t)(table.back().off + (int64_t)table.back().H * table.back().words);
   nb_world::Maps m;
   auto upload = [&]() -> int {
@@ -1074,7 +1207,7 @@ int nb_world_set_map_contact(nb_world_t* w, int32_t B, const int32_t* flags) {
   if (int rc = world_check_contact(&w->cfg, B, w->h_obs_begin.data(), obs.data(), w->h_vert_begin.data(), w->h_vertices.data(), w->h_kind.data(),
                                    beh.empty() ? nullptr : beh.data(), w->maps.h_table, w->maps.h_bits.data(), w->maps.h_env_map.data(), flags))
     return rc;
-  w->contact = {}; w->ep = {};
+  w->contact = {}; w->ocontact = {}; w->ep = {};
   // a wandering obstacle without an explicit goal in a blocking environment starts from goal = its centre and draw 0, so that its
   // first goal is drawn on the device through the map test
   std::vector<double> goal;
@@ -1124,6 +1257,58 @@ int nb_world_read_map_contact(nb_world_t* w, int32_t O, int32_t* bounces, void* 
   if (!bounces) return fail(NB_ERR_INVALID, "nb_world_read_map_contact: null bounces");
   NB_CUDA(cudaSetDevice(w->cfg.device));
   if (O) NB_CUDA(cudaMemcpyAsync(bounces, w->contact.bounces.get(), sizeof(int32_t) * O, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return NB_OK;
+}
+
+
+int nb_world_check_obstacle_contact(const nb_world_config* cfg, int32_t B, const int32_t* obs_begin, const double* obstacles, const int32_t* vert_begin,
+                                    const double* vertices, const double* envs, const int32_t* obs_kind, const double* behaviors, const int32_t* flags) {
+  if (int rc = world_check_scenes(cfg, B, obs_begin, obstacles, vert_begin, vertices, envs, obs_kind, nullptr, nullptr, nullptr, nullptr)) return rc;
+  if (behaviors)
+    if (int rc = world_check_behaviors(cfg, B, obs_begin, obstacles, envs, behaviors)) return rc;
+  return world_check_obstacle_contact(B, obs_begin, obstacles, vert_begin, vertices, obs_kind, behaviors, flags);
+}
+
+int nb_world_set_obstacle_contact(nb_world_t* w, int32_t B, const int32_t* flags) {
+  if (int rc = world_ready(w, B, "nb_world_set_obstacle_contact")) return rc;
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  const int O = w->O;
+  std::vector<double> obs((size_t)nb::kWorldObsCols * O), beh;
+  if (O) NB_CUDA(cudaMemcpy(obs.data(), w->scenes.obs.get(), sizeof(double) * obs.size(), cudaMemcpyDeviceToHost));  // the current centres
+  if (w->rvo.beh && O) {
+    beh.resize((size_t)nb::kWorldBehCols * O);
+    NB_CUDA(cudaMemcpy(beh.data(), w->rvo.beh.get(), sizeof(double) * beh.size(), cudaMemcpyDeviceToHost));
+  }
+  if (int rc = world_check_obstacle_contact(B, w->h_obs_begin.data(), obs.data(), w->h_vert_begin.data(), w->h_vertices.data(), w->h_kind.data(),
+                                            beh.empty() ? nullptr : beh.data(), flags))
+    return rc;
+  w->ocontact = {}; w->ep = {};
+  nb_world::ObstacleContact c;
+  auto upload = [&]() -> int {
+    NB_CUDA(nb::alloc(c.flag, (size_t)B));
+    NB_CUDA(nb::alloc(c.bounces, (size_t)O));
+    NB_CUDA(cudaMemcpy(c.flag.get(), flags, sizeof(int32_t) * B, cudaMemcpyHostToDevice));
+    NB_CUDA(cudaMemset(c.bounces.get(), 0, sizeof(int32_t) * std::max(O, 1)));
+    NB_CUDA(cudaDeviceSynchronize());
+    return NB_OK;
+  };
+  if (int rc = upload()) {  // no contact flags
+    cudaGetLastError();
+    return rc;
+  }
+  for (int b = 0; b < B; ++b) c.max_n = std::max(c.max_n, w->h_obs_begin[b + 1] - w->h_obs_begin[b]);
+  c.has_contact = std::any_of(flags, flags + B, [](int32_t f) { return f != 0; });
+  w->ocontact = std::move(c);
+  return NB_OK;
+}
+
+int nb_world_read_obstacle_contact(nb_world_t* w, int32_t O, int32_t* bounces, void* stream) {
+  if (!w) return fail(NB_ERR_INVALID, "nb_world_read_obstacle_contact: null handle");
+  if (!w->ocontact.bounces) return fail(NB_ERR_INVALID, "nb_world_read_obstacle_contact: no obstacle contact set (nb_world_set_obstacle_contact)");
+  if (O != w->O) return fail(NB_ERR_INVALID, "nb_world_read_obstacle_contact: O = %d but the scenes have %d obstacles", O, w->O);
+  if (!bounces) return fail(NB_ERR_INVALID, "nb_world_read_obstacle_contact: null bounces");
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  if (O) NB_CUDA(cudaMemcpyAsync(bounces, w->ocontact.bounces.get(), sizeof(int32_t) * O, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return NB_OK;
 }
 

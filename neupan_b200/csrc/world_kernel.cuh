@@ -46,6 +46,13 @@
 //         <= window; the robot's clearance is min(obstacles, robots, m) and m <= 0 sets collided.
 // There is no sub-cell geometry.
 //
+// Obstacle contact (nb_world_set_obstacle_contact; semantics, predicates and limits in world_contact_kernel.cuh): where an
+// environment's flag is 1 its obstacles block each other.  They move one at a time in row order, each taking the first of the
+// candidates A (the move), B (x only), C (y only), D (stay) whose footprint touches no other obstacle where it stands at that moment
+// (nor a map that blocks obstacles), so no moving obstacle ever touches another.  Robots are not blockers.  A handle with a flag set
+// moves its obstacles in world_contact_kernel and steps with world_step_body<..., kMove = false>; a handle without one launches the
+// kernels above unchanged.
+//
 // All arithmetic is FP64 with explicit rounding (__dmul_rn / __dadd_rn / __dsub_rn: no FMA contraction), so that oracle/world.py,
 // which performs the same operations in the same order in numpy, agrees to the last bit wherever the inputs agree (the only
 // differences come from CUDA's sin / cos / tan vs libm).
@@ -482,13 +489,13 @@ __device__ __forceinline__ void world_integrate(int kinematics, double L, double
   x = dadd(x, dmul(vx, dt)); y = dadd(y, dmul(vy, dt)); th = dadd(th, dmul(dth, dt));
 }
 
-// Obstacle o moves by v dt; a moving centre that left the rectangle is mirrored back and its velocity component reversed.  Writes
-// the row and returns the new centre.
-__device__ __forceinline__ void world_move_obstacle(const WorldParams& prm, const double* env, int o, double& cx, double& cy) {
-  double* row = prm.obs + (size_t)kWorldObsCols * o;
-  double vx = row[2], vy = row[3];
-  cx = dadd(row[0], dmul(vx, prm.dt));
-  cy = dadd(row[1], dmul(vy, prm.dt));
+// The move of an obstacle row by v dt; a moving centre that left the rectangle env is mirrored back and its velocity component
+// reversed: the new centre (cx, cy) and velocity (vx, vy).
+__device__ __forceinline__ void world_obstacle_move(const double* row, const double* env, double dt, double& cx, double& cy, double& vx,
+                                                    double& vy) {
+  vx = row[2]; vy = row[3];
+  cx = dadd(row[0], dmul(vx, dt));
+  cy = dadd(row[1], dmul(vy, dt));
   if (vx != 0.0) {
     if (cx < env[0]) { cx = dsub(dmul(2.0, env[0]), cx); vx = -vx; }
     else if (cx > env[2]) { cx = dsub(dmul(2.0, env[2]), cx); vx = -vx; }
@@ -497,6 +504,13 @@ __device__ __forceinline__ void world_move_obstacle(const WorldParams& prm, cons
     if (cy < env[1]) { cy = dsub(dmul(2.0, env[1]), cy); vy = -vy; }
     else if (cy > env[3]) { cy = dsub(dmul(2.0, env[3]), cy); vy = -vy; }
   }
+}
+
+// Obstacle o moves by world_obstacle_move.  Writes the row and returns the new centre.
+__device__ __forceinline__ void world_move_obstacle(const WorldParams& prm, const double* env, int o, double& cx, double& cy) {
+  double* row = prm.obs + (size_t)kWorldObsCols * o;
+  double vx, vy;
+  world_obstacle_move(row, env, prm.dt, cx, cy, vx, vy);
   row[0] = cx; row[1] = cy; row[2] = vx; row[3] = vy;
 }
 
@@ -732,7 +746,9 @@ __device__ __forceinline__ void world_move_obstacle_blocked(const WorldParams& p
 // kEp (episode mode): the CTA's units are slots b0 .. b0 + E - 1; a live slot steps the robots and obstacles of scene scene_of[b]
 // (the scene's rows) and writes its outputs to slot rows q = b K + k, its clearances also to ep_clear; an idle slot's scene is not
 // touched, and its outputs are the frozen flags and clearance +inf.
-template <bool kMap, bool kEp, bool kBlock>
+// kMove false (obstacle contact, nb_world_set_obstacle_contact): world_contact_kernel has already moved the obstacles, so phase 1
+// integrates the robots only.
+template <bool kMap, bool kEp, bool kBlock, bool kMove = true>
 __device__ __forceinline__ void world_step_body(const WorldParams& prm, const WorldMapParams& mp, const WorldBlockParams& bp, const float* __restrict__ action,
                                                 int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived, float* __restrict__ clearance) {
   __shared__ double f_x[kWorldMaxFleet][kWorldMaxVertices], f_y[kWorldMaxFleet][kWorldMaxVertices];  // E K <= 8 or K <= 16 slots
@@ -770,7 +786,9 @@ __device__ __forceinline__ void world_step_body(const WorldParams& prm, const Wo
     f_v[s][0] = vx; f_v[s][1] = vy;
     f_nv[s] = ty->nv;
   }
-  if constexpr (kEp) {  // the slots' scenes are anywhere in the obstacle rows: one live scene after the other
+  if constexpr (!kMove) {
+    // the obstacles have moved
+  } else if constexpr (kEp) {  // the slots' scenes are anywhere in the obstacle rows: one live scene after the other
     for (int j = 0; j < nslot / K; ++j) {
       if (prm.live[b0 + j] == 0) continue;
       const int e = prm.scene_of[b0 + j];

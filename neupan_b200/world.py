@@ -35,7 +35,18 @@ velocity reversed), else stays in place with both reversed -- a bounce, counted 
 obstacle's wander goal must have a clear footprint and a straight segment to it that keeps more than the obstacle's circumradius from
 every occupied cell (at most 16 draws per step, else it waits a step); after a bounce it draws a new goal.  Every moving obstacle of
 such a scene must start clear of the map, and its top speed times step_time must be below the map's resolution.  Walls are not RVO
-neighbours, obstacles do not collide with each other, and motion is not swept (csrc/world_kernel.cuh states the rules).
+neighbours, obstacles pass through each other unless the scene has obstacle contact (below), and motion is not swept
+(csrc/world_kernel.cuh states the rules).
+
+Obstacle contact (a scene's ``"obstacle_contact": True``, nb_world_set_obstacle_contact): the scene's obstacles block each other.
+They move one after another in list order, each tested against the others where they stand at that moment (the earlier ones already
+moved), which is how IR-SIM moves its objects.  A moving obstacle whose move would make its footprint touch another obstacle (or a map
+that blocks obstacles) takes instead the x move alone (y velocity reversed), else the y move alone (x velocity reversed), else stays in
+place with both reversed -- an obstacle bounce, counted per obstacle by ``obstacle_bounces()``.  So no moving obstacle ever touches
+another obstacle.  Every moving obstacle of such a scene must start clear of the others; static obstacles may overlap each other.
+Robots do not block obstacles, motion is not swept (a step longer than the thinner of two footprints can pass through it), and there
+is no momentum or elastic response (csrc/world_contact_kernel.cuh states the rules).  The builders ``dyna_obs``, ``dyna_non_obs``,
+``maze`` and ``cave`` take ``contact=True`` to place their obstacles clear of each other and set the key.
 
 An obstacle's "behavior" is {"name": "constant"} (the default) or {"name": "rvo", "vxmax", "vymax", ...} (keys and defaults in
 ``RVO_DEFAULTS``): a reactive obstacle that heads for a goal at ``speed`` and steers around the other obstacles and the robot with a
@@ -253,6 +264,11 @@ def pack_map_contact(scenes) -> np.ndarray:
     return np.ascontiguousarray([1 if (sc.get("map") or {}).get("blocks_obstacles", False) else 0 for sc in scenes], np.int32)
 
 
+def pack_obstacle_contact(scenes) -> np.ndarray:
+    """Scenes -> the (B) int32 flags of nb_world_set_obstacle_contact: 1 where the scene has ``"obstacle_contact": True``."""
+    return np.ascontiguousarray([1 if sc.get("obstacle_contact", False) else 0 for sc in scenes], np.int32)
+
+
 def _host_ptrs(packed):
     return [C.c_void_p(a.ctypes.data) for a in packed]
 
@@ -321,6 +337,9 @@ class WorldBatch:
         contact = pack_map_contact(scenes) if maps is not None else None
         if contact is not None and not contact.any():
             contact = None
+        ocontact = pack_obstacle_contact(scenes) if any("obstacle_contact" in sc for sc in scenes) else None
+        if ocontact is not None and not ocontact.any():
+            ocontact = None
         with torch.cuda.device(self.device):
             lib = _lib.load()
             fleet_args = (B, K, C.c_void_p(fleet.ctypes.data)) if fleet is not None else None
@@ -340,6 +359,10 @@ class WorldBatch:
                 bptr = C.c_void_p(beh.ctypes.data) if beh is not None else C.c_void_p(0)
                 _lib.check(lib.nb_world_check_map_contact(C.byref(self.config), B, *_host_ptrs(packed), bptr, *map_args[:4],
                                                           C.c_void_p(contact.ctypes.data)))
+            if ocontact is not None:
+                bptr = C.c_void_p(beh.ctypes.data) if beh is not None else C.c_void_p(0)
+                _lib.check(lib.nb_world_check_obstacle_contact(C.byref(self.config), B, *_host_ptrs(packed), bptr,
+                                                               C.c_void_p(ocontact.ctypes.data)))
             _lib.check(lib.nb_world_set_scenes_ex(self._handle, B, *_host_ptrs(packed)))
             self.O, self.K, self.N = int(packed[0][-1]), 1, B
             self._envs, self.S, self.slots = B, None, None
@@ -356,7 +379,10 @@ class WorldBatch:
                 _lib.check(lib.nb_world_set_maps(self._handle, *map_args))
             if contact is not None:
                 _lib.check(lib.nb_world_set_map_contact(self._handle, B, C.c_void_p(contact.ctypes.data)))
+            if ocontact is not None:
+                _lib.check(lib.nb_world_set_obstacle_contact(self._handle, B, C.c_void_p(ocontact.ctypes.data)))
         self.map_contact = contact is not None
+        self.obstacle_contact = ocontact is not None
         self.robot_types = rtype
         self._rows = [torch.from_numpy(np.flatnonzero(rtype == i)).to(self.device) for i in range(len(self.robots))]
 
@@ -384,6 +410,17 @@ class WorldBatch:
         out = torch.empty(self.O, dtype=torch.int32, device=self.device)
         with torch.cuda.device(self.device):
             _lib.check(_lib.load().nb_world_read_map_contact(self._handle, self.O, C.c_void_p(out.data_ptr()), self._stream()))
+        return out
+
+    def obstacle_bounces(self) -> torch.Tensor:
+        """(O,) int32 on the device: per obstacle, the steps in which its move would have touched another obstacle and was turned
+        back (0 for obstacles of scenes without obstacle contact).  Needs scenes with ``"obstacle_contact": True``; a copy enqueued on
+        the current stream."""
+        if not getattr(self, "obstacle_contact", False):
+            raise ValueError("no scene has obstacle contact (\"obstacle_contact\": True)")
+        out = torch.empty(self.O, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nb_world_read_obstacle_contact(self._handle, self.O, C.c_void_p(out.data_ptr()), self._stream()))
         return out
 
     def _read(self, states=None, obstacles=None, collided=None, arrived=None, rows=None):
@@ -685,12 +722,44 @@ def _apply_behavior(obs, behavior: str):
     return [dict(ob, velocity=(0.0, 0.0), behavior=dict(EXAMPLE_RVO)) for ob in obs]
 
 
-def dyna_obs(num_envs: int, seed: int = 0, count: int = 20, behavior: str = "constant"):
+def _circumradius(ob) -> float:
+    if "radius" in ob:
+        return float(ob["radius"])
+    v = np.asarray(ob.get("vertices", ob.get("outline")), np.float64)
+    return float(np.hypot(v[:, 0], v[:, 1]).max())
+
+
+CONTACT_GAP = 0.05  # m kept between the circumcircles of two obstacles placed with contact=True
+
+
+def _separate(obs, b: int, seed: int, draw):
+    """The ``contact=True`` placement of a builder: in list order, an obstacle whose circumcircle about its centre comes within
+    CONTACT_GAP of that of an earlier one takes a new centre ``draw(rng)`` until it is clear (at most 1000 draws), from environment
+    b's own contact stream (apart from the builder's streams, so the other draws do not change).  Circumcircles apart mean footprints
+    apart, whatever the shapes."""
+    rng = np.random.Generator(np.random.PCG64(np.random.SeedSequence(seed, spawn_key=(b, 2))))
+    placed = []
+    for ob in obs:
+        r = _circumradius(ob)
+        for _ in range(1000):
+            c = ob["center"]
+            if all(math.hypot(c[0] - p["center"][0], c[1] - p["center"][1]) > r + _circumradius(p) + CONTACT_GAP for p in placed):
+                break
+            ob = dict(ob, center=tuple(float(v) for v in draw(rng)))
+        else:
+            raise ValueError(f"environment {b}: no place clear of the other obstacles after 1000 draws")
+        placed.append(ob)
+    return placed
+
+
+def dyna_obs(num_envs: int, seed: int = 0, count: int = 20, behavior: str = "constant", contact: bool = False):
     """example/dyna_obs/diff/env.yaml: ``count`` (20) circles of radius 0.4..1.0 m placed at random in the box [10, 40]^2, goal
     threshold 0.4.  ``behavior="constant"``: each moves at a constant speed of at most 0.5 m/s in a random direction and bounces
     inside that box.  ``behavior="rvo"``: the example's reactive obstacles (EXAMPLE_RVO: vxmax = vymax = 0.5, wander, goal threshold
     0.3), starting at rest at the same centres.  The robot crosses the box: it starts at (6, y0) facing the goal (44, y1), y0, y1 in
-    15..35 m, on a straight path."""
+    15..35 m, on a straight path.  ``contact=True``: the circles block each other (``"obstacle_contact": True``) and start apart, an
+    overlapping circle drawn again in the box (``_separate``); at 0.5 m/s and step_time 0.1 a circle moves at most 0.05 m per step,
+    well below the thinnest footprint (no swept test is needed)."""
     scenes = []
     for b in range(num_envs):
         rng = _rng(seed, b)
@@ -702,9 +771,13 @@ def dyna_obs(num_envs: int, seed: int = 0, count: int = 20, behavior: str = "con
         speed, heading = rng.uniform(0.0, 0.5, count), rng.uniform(-math.pi, math.pi, count)
         obs = [dict(center=(c[i, 0], c[i, 1]), radius=r[i], velocity=(speed[i] * math.cos(heading[i]), speed[i] * math.sin(heading[i])))
                for i in range(count)]
+        if contact:
+            obs = _separate(obs, b, seed, lambda g: g.uniform(10.0, 40.0, 2))
         obs = _apply_behavior(obs, behavior)
         scenes.append(dict(obstacles=obs, bounds=(10.0, 10.0, 40.0, 40.0), start=start, goal=goal, goal_threshold=0.4,
                            path=line_path(start, goal)))
+        if contact:
+            scenes[-1]["obstacle_contact"] = True
     return scenes
 
 
@@ -736,13 +809,14 @@ def _example_outline(rng, avg_radius: float, irregularity: float) -> np.ndarray:
     return random_outline(rng, avg_radius, irregularity, spikeyness, n)
 
 
-def dyna_non_obs(num_envs: int, seed: int = 0, behavior: str = "constant"):
+def dyna_non_obs(num_envs: int, seed: int = 0, behavior: str = "constant", contact: bool = False):
     """example/dyna_non_obs/diff/{env,planner}.yaml: 11 obstacles, each one of the example's four shapes drawn uniformly -- the
     2 x 2 m square, a circle of r = 1.5, a circle of r = 1.0, or an outline of average radius U(0.5, 1.5) and irregularity 0.9 (how
     IR-SIM assigns a 4-entry shape list to 11 obstacles is a stated choice here).  Centres uniform in [5, 45] x [15, 35].
     ``behavior="constant"``: constant velocities (vx, vy) in U(-1, 1)^2, bouncing in that box.  ``behavior="rvo"``: the example's
     reactive obstacles (EXAMPLE_RVO), circles, squares and outlines alike, starting at rest at the same centres.  The robot starts
-    at (-1, 25, 0) on the planner's line path to (50, 25), its goal, with threshold 0.4."""
+    at (-1, 25, 0) on the planner's line path to (50, 25), its goal, with threshold 0.4.  ``contact=True``: the obstacles block each
+    other (``"obstacle_contact": True``) and start apart, an overlapping one drawn again in the box (``_separate``)."""
     square = [[-1.0, -1.0], [1.0, -1.0], [1.0, 1.0], [-1.0, 1.0]]
     start, goal = (-1.0, 25.0, 0.0), (50.0, 25.0)
     scenes = []
@@ -759,9 +833,13 @@ def dyna_non_obs(num_envs: int, seed: int = 0, behavior: str = "constant"):
             else:
                 ob["outline"] = _example_outline(rng, rng.uniform(0.5, 1.5), 0.9)
             obs.append(ob)
+        if contact:
+            obs = _separate(obs, b, seed, lambda g: g.uniform((5.0, 15.0), (45.0, 35.0)))
         obs = _apply_behavior(obs, behavior)
         scenes.append(dict(obstacles=obs, bounds=(5.0, 15.0, 45.0, 35.0), start=start, goal=goal, goal_threshold=0.4,
                            path=line_path(start, goal)))
+        if contact:
+            scenes[-1]["obstacle_contact"] = True
     return scenes
 
 
@@ -875,10 +953,11 @@ def _maze_layout(rng, nx: int, ny: int):
     return open_, sol[::-1]
 
 
-def _movers(b: int, seed: int, centres, count: int, behavior: str):
+def _movers(b: int, seed: int, centres, count: int, behavior: str, contact: bool = False):
     """``count`` circles of radius U(0.3, 0.6) at centres drawn from ``centres`` (distinct while there are enough), from
     environment b's own movers stream (apart from the layout streams, so the maps do not change): behavior "constant" moves each at
-    a speed U(0, 0.5) m/s in a random direction, "rvo" starts it at rest with EXAMPLE_RVO."""
+    a speed U(0, 0.5) m/s in a random direction, "rvo" starts it at rest with EXAMPLE_RVO.  ``contact``: a circle that would overlap
+    an earlier one takes another of ``centres`` (``_separate``)."""
     rng = np.random.Generator(np.random.PCG64(np.random.SeedSequence(seed, spawn_key=(b, 1))))
     if not len(centres):
         raise ValueError("no free place for a moving obstacle")
@@ -887,11 +966,13 @@ def _movers(b: int, seed: int, centres, count: int, behavior: str):
     speed, heading = rng.uniform(0.0, 0.5, count), rng.uniform(-math.pi, math.pi, count)
     obs = [dict(center=tuple(float(v) for v in centres[pick[i]]), radius=float(r[i]),
                 velocity=(speed[i] * math.cos(heading[i]), speed[i] * math.sin(heading[i]))) for i in range(count)]
+    if contact:
+        obs = _separate(obs, b, seed, lambda g: centres[int(g.integers(len(centres)))])
     return _apply_behavior(obs, behavior)
 
 
 def maze(num_envs: int, cells=(6, 6), cell_size: float = 5.0, wall: float = 0.3, resolution: float = 0.1, seed: int = 0, layouts=None,
-         movers: int = 0, behavior: str = "constant"):
+         movers: int = 0, behavior: str = "constant", contact: bool = False):
     """Perfect mazes on an occupancy map: ``cells`` (nx, ny) maze cells of ``cell_size`` m, carved by a randomised depth-first search
     (every cell reachable by exactly one route), rasterised at ``resolution`` with walls ``wall`` m thick centred on the closed cell
     boundaries, the outer border included.  Maze cell (a, c) is [a s, (a + 1) s] x [c s, (c + 1) s]; the map covers that area plus
@@ -902,7 +983,8 @@ def maze(num_envs: int, cells=(6, 6), cell_size: float = 5.0, wall: float = 0.3,
     ``movers`` > 0: that many circles of radius U(0.3, 0.6) m at the centres of maze cells other than the start cell and its eight
     neighbours, moving at U(0, 0.5) m/s in a random direction (``behavior="constant"``) or starting at rest as the examples' reactive
     obstacles (``"rvo"``, EXAMPLE_RVO: wander in the maze's rectangle), drawn per environment; the map then blocks obstacles
-    (``"blocks_obstacles": True``).  The speeds need step_time * 0.5 m/s (constant) or * 0.71 m/s (rvo) below ``resolution``."""
+    (``"blocks_obstacles": True``).  The speeds need step_time * 0.5 m/s (constant) or * 0.71 m/s (rvo) below ``resolution``.
+    ``contact=True`` (with movers): the movers also block each other (``"obstacle_contact": True``) and start apart."""
     nx, ny = (int(v) for v in cells)
     if nx < 1 or ny < 1 or not (0.0 < wall < cell_size):
         raise ValueError("maze needs cells >= 1 and 0 < wall < cell_size")
@@ -935,8 +1017,10 @@ def maze(num_envs: int, cells=(6, 6), cell_size: float = 5.0, wall: float = 0.3,
                            goal_threshold=0.3, path=path, map=dict(occupancy=occ, origin=origin, resolution=resolution)))
         if movers > 0:
             free = [((a + 0.5) * cell_size, (c + 0.5) * cell_size) for c in range(ny) for a in range(nx) if max(a, c) > 1]
-            scenes[-1]["obstacles"] = _movers(b, seed, free, int(movers), behavior)
+            scenes[-1]["obstacles"] = _movers(b, seed, free, int(movers), behavior, contact)
             scenes[-1]["map"]["blocks_obstacles"] = True
+            if contact:
+                scenes[-1]["obstacle_contact"] = True
     return scenes
 
 
@@ -980,7 +1064,7 @@ def _bfs(free, start):
 
 
 def cave(num_envs: int, size=(40.0, 40.0), resolution: float = 0.1, fill: float = 0.45, seed: int = 0, layouts=None,
-         coarse: float = 1.0, clearance: float = 2.0, movers: int = 0, behavior: str = "constant"):
+         coarse: float = 1.0, clearance: float = 2.0, movers: int = 0, behavior: str = "constant", contact: bool = False):
     """Caves on an occupancy map: a cellular automaton on a coarse grid of ``coarse`` m cells over ``size`` (m) -- each cell a wall
     with probability ``fill``, the border always a wall, then 5 rounds of the 4-5 rule (a cell becomes a wall when at least 5 of
     its 8 neighbours are walls, free when at most 3 are, cells past the border counting as walls) -- of which only the largest
@@ -990,7 +1074,7 @@ def cave(num_envs: int, size=(40.0, 40.0), resolution: float = 0.1, fill: float 
     them, the goal the cell of that group farthest from it by breadth-first search; ``path`` is that breadth-first path through the
     cell centres at 0.1 m spacing, the start facing along it, goal threshold 0.3.  ``layouts`` as in ``maze``.  ``movers`` and
     ``behavior`` as in ``maze``, the circles at the centres of free coarse cells whose eight neighbours are free too and that lie at
-    least 4 m from the start (wander in the cave's rectangle)."""
+    least 4 m from the start (wander in the cave's rectangle).  ``contact`` as in ``maze``."""
     sx, sy = float(size[0]), float(size[1])
     nx, ny = int(round(sx / coarse)), int(round(sy / coarse))
     up = int(round(coarse / resolution))
@@ -1046,6 +1130,8 @@ def cave(num_envs: int, size=(40.0, 40.0), resolution: float = 0.1, fill: float 
         scenes.append(dict(obstacles=[], bounds=(0.0, 0.0, sx, sy), start=(pts[0][0], pts[0][1], th), goal=pts[-1], goal_threshold=0.3,
                            path=_polyline_path(pts), map=dict(occupancy=occ, origin=(0.0, 0.0), resolution=resolution)))
         if movers > 0:
-            scenes[-1]["obstacles"] = _movers(b, seed, free, int(movers), behavior)
+            scenes[-1]["obstacles"] = _movers(b, seed, free, int(movers), behavior, contact)
             scenes[-1]["map"]["blocks_obstacles"] = True
+            if contact:
+                scenes[-1]["obstacle_contact"] = True
     return scenes

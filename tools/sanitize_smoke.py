@@ -111,6 +111,18 @@ if "world" in SECTIONS:
         torch.cuda.synchronize()
         assert torch.isfinite(w.obstacles()).all() and (w.map_bounces() >= 0).all()
         w.close()
+    # obstacle contact: the contact kernel and the step without obstacle motion, plain and over blocking maps, constant and reactive
+    from neupan_b200.world import dyna_non_obs
+    for scenes in (dyna_non_obs(3, seed=1, behavior="rvo", contact=True) + dyna_obs(1, seed=1),
+                   maze(4, cells=(4, 4), seed=1, layouts=2, movers=6, behavior="rvo", contact=True)):
+        w = WorldBatch(4, rb, lidar, 0.1)
+        w.set_scenes(scenes)
+        for _ in range(30):
+            w.scan()
+            w.step(torch.full((4, 2), 0.5, device="cuda"))
+        torch.cuda.synchronize()
+        assert torch.isfinite(w.obstacles()).all() and (w.obstacle_bounces() >= 0).all()
+        w.close()
     # continuous episodes: the episode instantiations of the scan, rvo and step kernels, the advance and slot gather kernels, and the
     # per-slot ipath and PAN calls, through run_episodes over a bank of 7 scenes in 3 slots (some slots go idle); then a maze bank
     # with its map through 2 slots, stepped until every slot is idle

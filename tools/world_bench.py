@@ -1,6 +1,6 @@
 """Times the batched world (csrc/world_kernel.cuh) against the planner it serves, on the device, and prints one JSON line.
 
-    python tools/world_bench.py [--scene dyna_obs|dyna_non_obs|circle_swap|maze|cave] [--behavior constant|rvo] [--movers 0] [--envs 4096] [--robots 1]
+    python tools/world_bench.py [--scene dyna_obs|dyna_non_obs|circle_swap|maze|cave] [--behavior constant|rvo] [--movers 0] [--contact] [--envs 4096] [--robots 1]
                                 [--beams 1080] [--steps 20] [--warmup 3]
     python tools/world_bench.py --mixed [--envs 4096] [--robots 6] [--beams 1080] [--steps 20] [--warmup 3]
 
@@ -18,7 +18,8 @@ inputs change every step (robots move, some arrive or stop), so the two planner 
 limit are read in the same run.  --mixed: mixed_swap (diff, acker and omni robots in turn, types 0, 1, 2: C4's, C2's and C5's bodies)
 against circle_swap of C4's robot at the same B and K, world alone and closed loop, each kind driven by its own config's PlannerBatch
 through MixedPlanner (circle_swap: one C4 PlannerBatch of N planners).  With --behavior rvo, one more closed-loop window of --steps iterations runs under torch.profiler,
-which gives the device time of world_rvo_kernel per step and its share of the closed-loop step timed with events.
+which gives the device time of world_rvo_kernel per step and its share of the closed-loop step timed with events.  --contact: the
+builders' contact=True scenes, whose obstacles block each other (csrc/world_contact_kernel.cuh).
 """
 import argparse
 import json
@@ -47,6 +48,7 @@ def main():
     ap.add_argument("--robots", type=int, default=1, help="robots per environment (circle_swap only)")
     ap.add_argument("--behavior", choices=("constant", "rvo"), default="constant")
     ap.add_argument("--movers", type=int, default=0, help="moving obstacles that the map blocks (maze and cave only)")
+    ap.add_argument("--contact", action="store_true", help="obstacles block each other (dyna_obs, dyna_non_obs, and maze / cave movers)")
     ap.add_argument("--envs", type=int, default=4096)
     ap.add_argument("--beams", type=int, default=1080)
     ap.add_argument("--steps", type=int, default=20)
@@ -74,9 +76,12 @@ def main():
     elif args.robots != 1:
         raise SystemExit("--robots needs --scene circle_swap")
     elif args.scene in ("maze", "cave"):
-        scenes = (maze if args.scene == "maze" else cave)(B, seed=2024, layouts=min(B, 64), movers=args.movers, behavior=args.behavior)
+        scenes = (maze if args.scene == "maze" else cave)(B, seed=2024, layouts=min(B, 64), movers=args.movers, behavior=args.behavior,
+                                                          contact=args.contact)
     else:
-        scenes = (dyna_obs if args.scene == "dyna_obs" else dyna_non_obs)(B, seed=2024, behavior=args.behavior)
+        scenes = (dyna_obs if args.scene == "dyna_obs" else dyna_non_obs)(B, seed=2024, behavior=args.behavior, contact=args.contact)
+    if args.contact and args.scene == "circle_swap":
+        raise SystemExit("--contact needs dyna_obs, dyna_non_obs, maze or cave")
     N = B * args.robots
     packed = pack_scenes_ex(scenes)
     n_obs, n_edges = int(packed[0][-1]), int(packed[2][-1])
@@ -148,7 +153,8 @@ def main():
     if args.scene in ("maze", "cave"):
         occ = scenes[0]["map"]["occupancy"]
         maps = dict(map_cells=int(occ.size), map_occupied=float(occ.mean()), map_resolution=scenes[0]["map"]["resolution"], map_layouts=min(B, 64))
-    print(json.dumps(dict(metric="batched world: scan + step vs PlannerBatch.forward", scene=args.scene, behavior=args.behavior, envs=B,
+    print(json.dumps(dict(metric="batched world: scan + step vs PlannerBatch.forward", scene=args.scene, behavior=args.behavior,
+                          contact=args.contact, envs=B,
                           robots_per_env=args.robots, planners=N, beams=R,
                           obstacles_per_env=n_obs / B, circles_per_env=n_circles / B, edges_per_env=n_edges / B,
                           steps=args.steps, warmup=args.warmup, ms_scan=ms_scan, ms_world_scan_step=ms_world, ms_planner_forward=ms_planner,
