@@ -187,6 +187,11 @@ int nb_pan_read_selection(nb_pan_t* pan, int32_t B, float* sel_mu, float* sel_la
  * (4 x the error measured at calibration, when NB_OPT_DUNE_KERNEL = 4 is first selected), [2] = that calibration measurement;
  * counts[0] = items sent to the exact kernel, counts[1] = candidates refined, counts[2] = items screened. */
 int nb_pan_read_screen_stats(nb_pan_t* pan, float* max_error_ratio, int32_t* counts, int32_t reset);
+/* The two-level table path of the one-warp-per-item screen since the last reset: counts[0] = points that survived the coarse bound
+ * table (summed over the items that took the path), counts[1] = items that tried the path and took the one-level path instead (a
+ * point outside the table, or more survivors than the path holds); both stay 0 with NB_SCREEN_COARSE=0.  Reset separately from
+ * nb_pan_read_screen_stats. */
+int nb_pan_read_screen_coarse(nb_pan_t* pan, int32_t counts[2], int32_t reset);
 /* The screen's distance table (all zero while none is built): info[0] = cell side h (m), [1] = half-width of the covered square (m),
  * [2] = device bytes (0: built, but not kept: [4] > c_mu / 2), [3] = build time (ms, host clock around the synchronised build), [4] = the largest |table - network| /
  * sum_e |G_e p - h_e| on the 4 x 4 sub-grid of every cell. */

@@ -96,6 +96,7 @@ SYMBOLS = {
     "nb_pan_read_selection": (C.c_int, [C.c_void_p, C.c_int32] + [_FP] * 5 + [C.c_void_p]),
     "nb_pan_read_screen_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_float * 3), C.POINTER(C.c_int32 * 3), C.c_int32]),
     "nb_pan_read_screen_table": (C.c_int, [C.c_void_p, C.POINTER(C.c_float * 5)]),
+    "nb_pan_read_screen_coarse": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32 * 2), C.c_int32]),
     "nb_pan_read_diagnostics": (C.c_int, [C.c_void_p, C.c_int32, _FP, C.c_void_p]),
     "nb_dune_forward": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32] + [_FP] * 5 + [C.c_void_p]),
     "nb_nrmp_forward": (C.c_int, [C.c_void_p, C.c_int32] + [_FP] * 10 + [C.c_void_p]),

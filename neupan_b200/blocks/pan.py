@@ -327,12 +327,18 @@ class PAN(torch.nn.Module):
         return out
 
     def screen_stats(self, reset=True):
-        """Screening statistics (dune_kernel = 4) since the last reset: dict(max_error_ratio, exact_items, candidates, screened_items)."""
+        """Screening statistics (dune_kernel = 4) since the last reset: dict(max_error_ratio, exact_items, candidates, screened_items,
+        coarse_survivors, coarse_fallback_items).  The last two count the two-level table path of the one-warp-per-item screen: the
+        points that survived its coarse bounds, and the items that took the one-level path instead (a point outside the table, or too
+        many survivors)."""
         if self._handle is None or self.no_obs:
             return None
-        r, c = (C.c_float * 3)(), (C.c_int32 * 3)()
-        _lib.check(_lib.load().nb_pan_read_screen_stats(self._handle, C.byref(r), C.byref(c), int(reset)))
-        return dict(max_error_ratio=float(r[0]), c_mu=float(r[1]), calibration_ratio=float(r[2]), exact_items=int(c[0]), candidates=int(c[1]), screened_items=int(c[2]))
+        r, c, k = (C.c_float * 3)(), (C.c_int32 * 3)(), (C.c_int32 * 2)()
+        lib = _lib.load()
+        _lib.check(lib.nb_pan_read_screen_stats(self._handle, C.byref(r), C.byref(c), int(reset)))
+        _lib.check(lib.nb_pan_read_screen_coarse(self._handle, C.byref(k), int(reset)))
+        return dict(max_error_ratio=float(r[0]), c_mu=float(r[1]), calibration_ratio=float(r[2]), exact_items=int(c[0]), candidates=int(c[1]), screened_items=int(c[2]),
+                    coarse_survivors=int(k[0]), coarse_fallback_items=int(k[1]))
 
     def screen_table(self):
         """The screen's distance table: dict(h, half, bytes, build_ms, max_error_ratio); all zero while none is built."""

@@ -44,6 +44,12 @@ struct DuneParams {
   const float* tab_rad;     // (n, n) the cell's error radius
   int tab_n;                // cells per side
   float tab_half, tab_inv_h;  // the table covers [-tab_half, tab_half]^2 of the robot frame with cells of 1 / tab_inv_h metres
+  // coarse bound table of dune_screen_warp_kernel (dune_table_kernel.cuh): coarse cell (ix >> kCoarseLog, iy >> kCoarseLog) of fine cell
+  // (ix, iy) holds {LB, UB} as fp16 (low, high half) with LB <= table_bilerp - rad and UB >= table_bilerp + rad of every point of its fine
+  // cells; nullptr: every item takes the one-level table path (NB_SCREEN_COARSE=0)
+  const uint32_t* tab_coarse;
+  int tab_cn;               // coarse cells per side
+  unsigned* coarse_stats;   // [0] survivors of the coarse pass, [1] table items that took the one-level path (nb_pan_read_screen_coarse)
   int32_t* flag_list;       // (B (T+1)) the items with cand_cnt == -1, in the order the screen kernel met them
   int32_t* flag_count;      // (3) [0] their number, [1] / [2] the lengths of the two refine lists; zeroed by the launcher before the screen kernel
   int32_t* refine_list;     // (2 B (T+1)) work lists of dune_refine_kernel, appended by the screen kernels: [0, B (T+1)) the items with 1..16
@@ -64,14 +70,24 @@ __device__ __forceinline__ float table_bilerp(const float4& c, float a, float b)
   return fmaf(b, d1 - d0, d0);
 }
 
-// the table cell c of the robot-frame point (x, y) and the point's position (a, b) in it; false when the point lies outside the table
-__device__ __forceinline__ bool table_cell(const DuneParams& prm, float x, float y, int& c, float& a, float& b) {
+constexpr int kCoarseLog = 4;  // a coarse bound cell covers 16 x 16 fine cells of the distance table
+
+// the table cell (ix, iy) of the robot-frame point (x, y) and the point's position (a, b) in it; false when the point lies outside the table
+__device__ __forceinline__ bool table_cell_xy(const DuneParams& prm, float x, float y, int& ix, int& iy, float& a, float& b) {
   const float fx = (x + prm.tab_half) * prm.tab_inv_h, fy = (y + prm.tab_half) * prm.tab_inv_h, nf = (float)prm.tab_n;
   if (!(fx >= 0.f && fx < nf && fy >= 0.f && fy < nf)) return false;  // NaN coordinates are outside as well
-  const int ix = (int)fx, iy = (int)fy;
-  c = iy * prm.tab_n + ix;
+  ix = (int)fx;
+  iy = (int)fy;
   a = fx - (float)ix;
   b = fy - (float)iy;
+  return true;
+}
+
+// the same as table_cell_xy with the cell as one index c = iy n + ix
+__device__ __forceinline__ bool table_cell(const DuneParams& prm, float x, float y, int& c, float& a, float& b) {
+  int ix, iy;
+  if (!table_cell_xy(prm, x, y, ix, iy, a, b)) return false;
+  c = iy * prm.tab_n + ix;
   return true;
 }
 

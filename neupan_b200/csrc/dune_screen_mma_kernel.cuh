@@ -27,7 +27,9 @@ namespace sm {
 using tc::f2;
 
 #ifndef NB_WHATIF
-#define NB_WHATIF 0  // timing experiments only (wrong results): 1 = no MUFU.TANH, 2 = no HMMA, 4 = no selection, 8 = no LayerNorm scale math
+#define NB_WHATIF 0  // timing experiments only (wrong results): 1 = no MUFU.TANH, 2 = no HMMA, 4 = no selection, 8 = no LayerNorm scale math,
+                     // 16 = every point of dune_screen_warp_kernel's table branch gathers cell 0 (a broadcast: no L2 traffic) and takes
+                     // |x| + |y| in the robot frame as its distance, so that the candidate lists keep a realistic length
 #endif
 
 constexpr int kFragBytes = 5 * 2 * 2 * 32 * 16;  // B fragments, [layer][k-step][n-tile pair][lane] uint4 = {b0,b1 (tile 2jp), b0,b1 (2jp+1)}
@@ -528,6 +530,24 @@ __global__ void __launch_bounds__(128, 4) dune_screen_mma_kernel(const DuneParam
 // then runs the network.  tau = the M-th smallest key of the warp (M REDUX rounds), the candidates are compacted by ballot: no merge
 // stage, no block barrier, no shared-memory atomics per item.  Candidate and item counts, and the refine lists, are collected in
 // shared memory and reach global memory once per environment (refine lists: one atomic per size class) or once per CTA (statistics).
+//
+// Two-level table path.  Of the ~500 points of an item only about M become candidates, so an item whose points all lie in the table
+// first bounds every point from the coarse bound table (dune_table_coarse_kernel: one 4-byte load per point from a ~11 KB table that
+// stays in L1, no fine-table gather) and gathers the fine cell only for the points that survive:
+//   coarse pass: key_c = unique_key(orderable(UB_c), i); tau_c = the M-th smallest key_c (M REDUX rounds, as below);
+//   survivors:   orderable(LB_c) <= tau_c, compacted by ballot in (tile j, lane) order (at most kSurvMax, 2 per lane);
+//   fine pass:   the fine bounds of the survivors with the one-level path's arithmetic; tau_f = the M-th smallest fine key among them;
+//                candidates: the survivors with orderable(d - rad) <= tau_f, written in survivor order.
+// Why the candidates are the one-level path's, bit for bit (LB_f, UB_f: a point's fine bounds fl(d - rad), fl(d + rad); tau: the
+// one-level path's M-th smallest fine key over all points):
+//   - LB_c <= LB_f and UB_c >= UB_f at every point, and unique_key is monotone, so key_c >= key_f point by point and tau_c >= tau.
+//   - A culled point has orderable(LB_f) >= orderable(LB_c) > tau_c >= tau: the one-level path rejects it as well.
+//   - A point with key_f <= tau has orderable(LB_c) <= orderable(LB_f) <= orderable(UB_f) < key_f <= tau <= tau_c (unique_key rounds
+//     up past the low 9 bits), so it survives: the M smallest fine keys are all survivors' and tau_f = tau.
+//   - So survivors and one-level path take the same candidates, and the survivor order is the one-level order restricted to them.
+// cand_idx / cand_dt / cand_rad / cand_cnt, the refine lists and the statistics are therefore those of the one-level path.  An item
+// with a point outside the table (NaN included) or more than kSurvMax survivors takes the one-level path, as does every item when
+// the handle has no coarse table (NB_SCREEN_COARSE=0).
 constexpr int kWarpTiles = 16;  // 32-point tiles of an item: N <= 512, 9 index bits in the key (tc::unique_key)
 // warps per CTA and CTAs per SM the register allocation is made for (128 registers).  Measured on C4 (H100 80GB HBM3, 700 W, bench.py
 // 10 steps, 3 runs each): 4 warps x 4 CTAs 16.27-16.41 ms per step, 5 x 3 16.54-16.59 ms, 8 x 2 16.61-16.64 ms.
@@ -542,6 +562,7 @@ constexpr int kScreenWarps = NB_SCREEN_WARPS;
 #define NB_SCREEN_GATHER 4
 #endif
 constexpr int kGather = NB_SCREEN_GATHER;  // table gathers in flight per lane
+constexpr int kSurvMax = 64;  // survivors of the coarse pass the two-level path holds: two per lane, their indices in the warp's net area
 
 // shared memory: B fragments | permuted vectors | bias fragments | two clouds (x | y | vx | vy, N floats each) | per-warp network
 // results (kWarpTiles x 32 float2) | refine lists of two environments ([parity][size class][T+1] items)
@@ -563,12 +584,13 @@ __global__ void __launch_bounds__(32 * kScreenWarps, NB_SCREEN_WARP_BLOCKS)
   float2* net = reinterpret_cast<float2*>(cloud + (size_t)8 * N) + (size_t)warp * kWarpTiles * 32;
   int* rlist = reinterpret_cast<int*>(cloud + (size_t)8 * N + (size_t)W * kWarpTiles * 64);
   __shared__ int rcnt_s[2][2];   // [parity][size class] lengths of the refine lists in rlist
-  __shared__ unsigned stat_s[2];  // candidates and items screened by this CTA (screen_stats[2], [3])
+  __shared__ unsigned stat_s[4];  // candidates and items screened by this CTA (screen_stats[2], [3]), coarse survivors and items of the
+                                 // one-level table path (coarse_stats[0], [1])
   __shared__ float4 frame_s[W][32];  // per warp: {sx, sy, cos, sin} of the steps of its next <= 32 items
 
   sm::stage_operands(image, wfrag, vec, biasq, tid, kThreads);
   if (tid < 4) rcnt_s[tid >> 1][tid & 1] = 0;
-  if (tid < 2) stat_s[tid] = 0;
+  if (tid < 4) stat_s[tid] = 0;
   const uint4* wl = wfrag + lane;
   const float* vq = vec + 8 * tq;
   const float4* bqq = biasq + 4 * tq;
@@ -683,9 +705,133 @@ __global__ void __launch_bounds__(32 * kScreenWarps, NB_SCREEN_WARP_BLOCKS)
           }
         };
 
-        // the bounds of the lane's points, d~ and its error radius, collect in net[32 j + lane] (tile j): from the table where it covers
-        // the point, then from the network for the tiles with a point outside it (netm; every tile when there is no table)
         const int tiles = (n + 31) >> 5;
+        int32_t* out_idx = prm.cand_idx + (size_t)item * kCandMax;
+        float* out_dt = prm.cand_dt + (size_t)item * kCandMax;
+        const uint32_t below = (1u << lane) - 1u;
+        // lane 0: the item's candidate count, refine list and statistics (nc <= kCandMax), or the item to the exact kernel
+        auto finish = [&](int nc) {
+          if (lane != 0) return;
+          if (nc <= kCandMax) {
+            prm.cand_cnt[item] = nc;
+            refine_push(par, item, nc);
+            atomicAdd(&stat_s[0], (unsigned)nc);
+            atomicAdd(&stat_s[1], 1u);
+          } else {
+            prm.cand_cnt[item] = -1;  // too many candidates: the exact kernel evaluates this item in full
+            atomicAdd(&prm.screen_stats[1], 1u);
+            prm.flag_list[atomicAdd(prm.flag_count, 1)] = item;
+          }
+        };
+        // candidate p: point i with screened distance d and error radius r
+        auto put = [&](int p, int i, float d, float r) {
+          const float lb = d - r;
+          out_idx[p] = i;
+          out_dt[p] = d;
+          prm.cand_rad[(size_t)item * kCandMax + p] = d - lb;
+        };
+        if (prm.tab_coarse && n > kCandMax && NB_WHATIF == 0) {  // the two-level table path (see above the kernel)
+          bool inside = true;
+          uint32_t kc[kWarpTiles];
+#pragma unroll
+          for (int j = 0; j < kWarpTiles; ++j) {
+            kc[j] = 0xFFFFFFFFu;
+            const int i = 32 * j + own;
+            if (j < tiles && i < n) {
+              float x0, y0, a, bq;
+              int ix, iy;
+              local(i, x0, y0);
+              if (table_cell_xy(prm, x0, y0, ix, iy, a, bq)) {
+                const uint32_t lu = __ldg(prm.tab_coarse + (iy >> kCoarseLog) * prm.tab_cn + (ix >> kCoarseLog));
+                net[32 * j + lane].x = __half2float(__ushort_as_half((unsigned short)(lu & 0xFFFFu)));
+                kc[j] = tc::unique_key(orderable(__half2float(__ushort_as_half((unsigned short)(lu >> 16)))), i);
+              } else {
+                inside = false;
+              }
+            }
+          }
+          if (__all_sync(0xffffffffu, inside)) {
+            uint32_t tau = 0u;
+#pragma unroll 1
+            for (int m = 0; m < M; ++m) {
+              uint32_t mine = 0xFFFFFFFFu;
+#pragma unroll
+              for (int j = 0; j < kWarpTiles; ++j) mine = min(mine, kc[j] > tau ? kc[j] : 0xFFFFFFFFu);
+              tau = __reduce_min_sync(0xffffffffu, mine);
+            }
+            uint32_t survm = 0u;
+#pragma unroll
+            for (int j = 0; j < kWarpTiles; ++j)
+              if (kc[j] != 0xFFFFFFFFu && orderable(net[32 * j + lane].x) <= tau) survm |= 1u << j;
+            __syncwarp();  // every lane has read its coarse bounds: the survivor list overwrites the start of the warp's net area
+            int* surv = reinterpret_cast<int*>(net);
+            int ns = 0;
+#pragma unroll
+            for (int j = 0; j < kWarpTiles; ++j) {
+              const bool sv = (survm >> j) & 1u;
+              const uint32_t bal = __ballot_sync(0xffffffffu, sv);
+              const int p = ns + __popc(bal & below);
+              if (sv && p < kSurvMax) surv[p] = 32 * j + own;
+              ns += __popc(bal);
+            }
+            if (ns <= kSurvMax) {
+              __syncwarp();
+              int si[2];
+              float4 cell[2];
+              float rad[2], ca[2], cb[2];
+#pragma unroll
+              for (int r = 0; r < 2; ++r) {
+                const int p = 32 * r + lane;
+                si[r] = p < ns ? surv[p] : -1;
+                int c = 0;
+                ca[r] = 0.f; cb[r] = 0.f;
+                if (si[r] >= 0) {
+                  float x0, y0;
+                  local(si[r], x0, y0);
+                  table_cell(prm, x0, y0, c, ca[r], cb[r]);
+                }
+                cell[r] = __ldg(prm.tab_cell + c);
+                rad[r] = __ldg(prm.tab_rad + c);
+              }
+              __syncwarp();  // the survivor list is read: the next item may write the net area
+              float d[2];
+              uint32_t kf[2];
+#pragma unroll
+              for (int r = 0; r < 2; ++r) {
+                d[r] = table_bilerp(cell[r], ca[r], cb[r]);
+                kf[r] = si[r] >= 0 ? tc::unique_key(orderable(d[r] + rad[r]), si[r]) : 0xFFFFFFFFu;
+              }
+              tau = 0u;
+#pragma unroll 1
+              for (int m = 0; m < M; ++m) {
+                const uint32_t mine = min(kf[0] > tau ? kf[0] : 0xFFFFFFFFu, kf[1] > tau ? kf[1] : 0xFFFFFFFFu);
+                tau = __reduce_min_sync(0xffffffffu, mine);
+              }
+              bool tk[2];
+              int nc = 0;
+#pragma unroll
+              for (int r = 0; r < 2; ++r) {
+                tk[r] = kf[r] != 0xFFFFFFFFu && orderable(d[r] - rad[r]) <= tau;
+                nc += __popc(__ballot_sync(0xffffffffu, tk[r]));
+              }
+              if (nc <= kCandMax) {
+                int pos = 0;
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                  const uint32_t bal = __ballot_sync(0xffffffffu, tk[r]);
+                  if (tk[r]) put(pos + __popc(bal & below), si[r], d[r], rad[r]);
+                  pos += __popc(bal);
+                }
+              }
+              finish(nc);
+              if (lane == 0) atomicAdd(&stat_s[2], (unsigned)ns);
+              continue;
+            }
+          }
+          if (lane == 0) atomicAdd(&stat_s[3], 1u);
+        }
+        // one-level path: the bounds of the lane's points, d~ and its error radius, collect in net[32 j + lane] (tile j): from the table
+        // where it covers the point, then from the network for the tiles with a point outside it (netm; every tile when there is no table)
         uint32_t netm = 0u;
         if (prm.tab_cell) {
           uint32_t hitm = 0u;  // bit j: the point of tile j lies in the table or beyond n
@@ -703,6 +849,7 @@ __global__ void __launch_bounds__(32 * kScreenWarps, NB_SCREEN_WARP_BLOCKS)
                 int c = 0;  // a point outside the table, or beyond n, reads cell 0
                 ca[q] = 0.f; cb[q] = 0.f;
                 const bool hit = i >= n || table_cell(prm, x0, y0, c, ca[q], cb[q]);
+                if (NB_WHATIF & 16) { c = 0; ca[q] = fabsf(x0) + fabsf(y0); }
                 hitm |= hit ? 1u << j : 0u;
                 if (!__all_sync(0xffffffffu, hit)) netm |= 1u << j;
                 cell[q] = __ldg(prm.tab_cell + c);
@@ -711,7 +858,9 @@ __global__ void __launch_bounds__(32 * kScreenWarps, NB_SCREEN_WARP_BLOCKS)
             }
 #pragma unroll
             for (int q = 0; q < kGather; ++q)
-              if (h + q < tiles) net[32 * (h + q) + lane] = make_float2(table_bilerp(cell[q], ca[q], cb[q]), rad[q]);
+              if (h + q < tiles)
+                net[32 * (h + q) + lane] = (NB_WHATIF & 16) ? make_float2(ca[q] + 0.f * cell[q].x, fminf(rad[q], 0.05f))
+                                                            : make_float2(table_bilerp(cell[q], ca[q], cb[q]), rad[q]);
           }
 #pragma unroll 1
           for (uint32_t m = netm; m != 0u; m &= m - 1u) {
@@ -745,8 +894,6 @@ __global__ void __launch_bounds__(32 * kScreenWarps, NB_SCREEN_WARP_BLOCKS)
           if (lane == 0) prm.cand_cnt[item] = (key[0] ^ key[kWarpTiles - 1]) == 12345u ? 1 : 0;
           continue;
         }
-        int32_t* out_idx = prm.cand_idx + (size_t)item * kCandMax;
-        float* out_dt = prm.cand_dt + (size_t)item * kCandMax;
         if (n <= kCandMax) {  // calibration mode: all points (tile 0), with their screened distance
           if (key[0] != 0xFFFFFFFFu) { out_idx[own] = own; out_dt[own] = net[lane].x; }
           if (lane == 0) { prm.cand_cnt[item] = n; refine_push(par, item, n); }
@@ -776,33 +923,19 @@ __global__ void __launch_bounds__(32 * kScreenWarps, NB_SCREEN_WARP_BLOCKS)
           nc += __popc(__ballot_sync(0xffffffffu, tk));
         }
         if (nc <= kCandMax) {
-          const uint32_t below = (1u << lane) - 1u;
           int pos = 0;
 #pragma unroll
           for (int j = 0; j < kWarpTiles; ++j) {
             const bool tk = (takem >> j) & 1u;
             const uint32_t bal = __ballot_sync(0xffffffffu, tk);
             if (tk) {
-              const int p = pos + __popc(bal & below);
               const float2 v = net[32 * j + lane];
-              const float lb = v.x - v.y;
-              out_idx[p] = 32 * j + own;
-              out_dt[p] = v.x;
-              prm.cand_rad[(size_t)item * kCandMax + p] = v.x - lb;
+              put(pos + __popc(bal & below), 32 * j + own, v.x, v.y);
             }
             pos += __popc(bal);
           }
-          if (lane == 0) {
-            prm.cand_cnt[item] = nc;
-            refine_push(par, item, nc);
-            atomicAdd(&stat_s[0], (unsigned)nc);
-            atomicAdd(&stat_s[1], 1u);
-          }
-        } else if (lane == 0) {
-          prm.cand_cnt[item] = -1;  // too many candidates: the exact kernel evaluates this item in full
-          atomicAdd(&prm.screen_stats[1], 1u);
-          prm.flag_list[atomicAdd(prm.flag_count, 1)] = item;
         }
+        finish(nc);
       }
     }
   }
@@ -815,6 +948,10 @@ __global__ void __launch_bounds__(32 * kScreenWarps, NB_SCREEN_WARP_BLOCKS)
   if (tid == 0 && stat_s[1]) {
     atomicAdd(&prm.screen_stats[2], stat_s[0]);
     atomicAdd(&prm.screen_stats[3], stat_s[1]);
+  }
+  if (tid == 0 && (stat_s[2] || stat_s[3])) {
+    atomicAdd(&prm.coarse_stats[0], stat_s[2]);
+    atomicAdd(&prm.coarse_stats[1], stat_s[3]);
   }
 }
 

@@ -14,6 +14,8 @@
 // every radius positive.  The radius is checked at run time like the network's: the refine
 // kernel compares every candidate's |screened - exact| with half of that candidate's radius.
 #pragma once
+#include <cuda_fp16.h>
+
 #include "dune_common.cuh"
 
 namespace nb {
@@ -135,6 +137,44 @@ __global__ void __launch_bounds__(128) dune_table_cell_kernel(const float* __res
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) worst = fmaxf(worst, __shfl_xor_sync(0xffffffffu, worst, o));
   if ((threadIdx.x & 31) == 0 && worst > 0.f) atomicMax(max_ratio, __float_as_uint(worst));
+}
+
+// Coarse bound table of dune_screen_warp_kernel: coarse cell (u, v) of cn x cn covers the fine cells (ix, iy) with ix >> kCoarseLog = u,
+// iy >> kCoarseLog = v (the last row and column cover what is left of the n fine cells) and holds {LB, UB} in fp16 with
+//   LB <= fl(table_bilerp(cell, a, b) - rad)  and  UB >= fl(table_bilerp(cell, a, b) + rad)
+// for every fine cell it covers and every (a, b) in [0, 1)^2, in the kernel's float arithmetic.
+// Margin of table_bilerp: with corners in [lo, hi], X = max |corner| and u = 2^-24, each of d0, d1 = fl(a (c1 - c0) + c0) lies in
+// [lo - e, hi + e] with e <= 3.01 u X fused (difference 2 u X, FMA 1.01 u X) or 5.1 u X unfused (+ the product's rounding); the final
+// fl(b (d1 - d0) + d0) adds <= 2.01 u X (difference) + 1.01 u X (rounding), + 2.02 u X unfused: at most 10.2 u X in all, so
+// m = 16 u X = 2^-20 X, plus FLT_MIN for subnormal results, bounds table_bilerp to [lo - m, hi + m] with or without contraction.
+// The bounds then round outward: LB = rd(rd(lo - m) - rad), UB = ru(ru(hi + m) + rad), since fl(d - rad) >= rd(d' - rad) for every d >= d'
+// (rounding to nearest is monotone and rd(...) is a float), and the conversion to fp16 rounds down for LB and up for UB.  A zero LB is
+// stored as -0 and a zero UB as +0, because orderable() puts -0 below +0.  A fine cell with a non-finite corner or a NaN radius makes
+// its coarse cell {-inf, NaN}: every point survives and its key sorts last.
+__global__ void __launch_bounds__(128) dune_table_coarse_kernel(const float4* __restrict__ cell, const float* __restrict__ rad, int n, int cn,
+                                                                uint32_t* __restrict__ coarse) {
+  for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < cn * cn; q += gridDim.x * blockDim.x) {
+    const int v = q / cn, u = q - v * cn;
+    const int x0 = u << kCoarseLog, y0 = v << kCoarseLog;
+    const int x1 = min(x0 + (1 << kCoarseLog), n), y1 = min(y0 + (1 << kCoarseLog), n);
+    float lb = __int_as_float(0x7f800000), ub = -__int_as_float(0x7f800000);
+    bool bad = false;
+    for (int iy = y0; iy < y1; ++iy)
+      for (int ix = x0; ix < x1; ++ix) {
+        const float4 c = cell[(size_t)iy * n + ix];
+        const float r = rad[(size_t)iy * n + ix];
+        const float lo = fminf(fminf(c.x, c.y), fminf(c.z, c.w)), hi = fmaxf(fmaxf(c.x, c.y), fmaxf(c.z, c.w));
+        if (!(isfinite(c.x) && isfinite(c.y) && isfinite(c.z) && isfinite(c.w)) || r != r) { bad = true; continue; }
+        const float m = fmaf(fmaxf(fabsf(lo), fabsf(hi)), 0x1p-20f, 0x1p-126f);
+        lb = fminf(lb, __fsub_rd(__fsub_rd(lo, m), r));
+        ub = fmaxf(ub, __fadd_ru(__fadd_ru(hi, m), r));
+      }
+    __half hl = __float2half_rd(lb), hu = __float2half_ru(ub);
+    if (bad) { hl = __float2half_rd(-__int_as_float(0x7f800000)); hu = __float2half(__int_as_float(0x7fc00000)); }
+    if (__half2float(hl) == 0.f) hl = __float2half(-0.f);
+    if (__half2float(hu) == 0.f) hu = __float2half(0.f);
+    coarse[q] = (uint32_t)__half_as_ushort(hl) | ((uint32_t)__half_as_ushort(hu) << 16);
+  }
 }
 
 }  // namespace nb

@@ -39,7 +39,10 @@ struct nb_pan {
   int screen_table = 1;                 // NB_OPT_DUNE_SCREEN_TABLE: the mma.sync screen looks distances up in the table below
   nb::DeviceArray<float4> tab_cell;     // distance table (dune_table_kernel.cuh), built once per handle by build_screen_table()
   nb::DeviceArray<float> tab_rad;
-  int tab_n = 0;
+  nb::DeviceArray<uint32_t> tab_coarse; // its coarse bound table (dune_table_coarse_kernel), tab_cn x tab_cn
+  int tab_n = 0, tab_cn = 0;
+  int screen_coarse = 1;                // NB_SCREEN_COARSE=0 (developer switch, read at create): every item takes the one-level table path
+  nb::DeviceArray<unsigned> coarse_stats;  // survivors of the coarse pass and items that took the one-level path (nb_pan_read_screen_coarse)
   float tab_h = 0.f, tab_half = 0.f, tab_ratio = 0.f, tab_ms = 0.f;
   bool tab_built = false;               // built (and kept, or freed as not accurate enough: tab_cell empty)
   int dune_variant = 2;              // NB_OPT_DUNE_KERNEL: 2 = the exact wgmma kernel on every point, 4 = screening pipeline
@@ -101,7 +104,7 @@ nb::DuneParams dune_params(const nb_pan* p) {
   nb::DuneParams d{};
   d.weights = p->d_weights.get(); d.geo = p->geo;
   d.T = c.receding; d.M = c.nrmp_max_num; d.dt = (float)c.step_time;
-  d.c_mu = p->c_mu; d.screen_stats = p->screen_stats.get(); d.screen_mma = p->screen_mma;
+  d.c_mu = p->c_mu; d.screen_stats = p->screen_stats.get(); d.screen_mma = p->screen_mma; d.coarse_stats = p->coarse_stats.get();
   d.sel_mu = p->sel_mu.get(); d.sel_lam = p->sel_lam.get(); d.sel_pts = p->sel_pts.get(); d.sel_dist = p->sel_dist.get(); d.sel_count = p->sel_count.get();
   d.cand_idx = p->cand_idx.get(); d.cand_dt = p->cand_dt.get(); d.cand_cnt = p->cand_cnt.get(); d.cand_rad = p->cand_rad.get();
   d.flag_list = p->flag_list.get(); d.flag_count = p->flag_count.get(); d.refine_list = p->refine_list.get();
@@ -223,10 +226,13 @@ int build_screen_table(nb_pan* p) {
   NB_CUDA(nb::alloc(d_ratio, (size_t)1));
   if (!p->tab_cell) NB_CUDA(nb::alloc(p->tab_cell, (size_t)(n * n)));
   if (!p->tab_rad) NB_CUDA(nb::alloc(p->tab_rad, (size_t)(n * n)));
+  const long long cn = (n + (1 << nb::kCoarseLog) - 1) >> nb::kCoarseLog;
+  if (!p->tab_coarse) NB_CUDA(nb::alloc(p->tab_coarse, (size_t)(cn * cn)));
   NB_CUDA(cudaMemset(d_ratio.get(), 0, sizeof(unsigned)));
   const float hs = h / nb::kTableSub;
   nb::dune_table_sample_kernel<<<p->sm_count * 16, 128>>>(p->d_weights.get(), p->geo, (int)m, half, hs, fine.get());
   nb::dune_table_cell_kernel<<<p->sm_count * 8, 128>>>(fine.get(), (int)n, half, hs, p->geo, p->tab_cell.get(), p->tab_rad.get(), d_ratio.get());
+  nb::dune_table_coarse_kernel<<<p->sm_count, 128>>>(p->tab_cell.get(), p->tab_rad.get(), (int)n, (int)cn, p->tab_coarse.get());
   NB_CUDA(cudaGetLastError());
   NB_CUDA(cudaDeviceSynchronize());
   unsigned r = 0;
@@ -234,10 +240,11 @@ int build_screen_table(nb_pan* p) {
   fine.reset();
   d_ratio.reset();
   memcpy(&p->tab_ratio, &r, 4);
-  p->tab_n = (int)n; p->tab_h = h; p->tab_half = half; p->tab_built = true;
+  p->tab_n = (int)n; p->tab_cn = (int)cn; p->tab_h = h; p->tab_half = half; p->tab_built = true;
   if (!(2.f * p->tab_ratio <= p->c_mu)) {
     p->tab_cell.reset();
     p->tab_rad.reset();
+    p->tab_coarse.reset();
   }
   p->tab_ms = (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   return NB_OK;
@@ -251,6 +258,8 @@ void set_screen_table(const nb_pan* p, nb::DuneParams& prm) {
   prm.tab_n = p->tab_n;
   prm.tab_half = p->tab_half;
   prm.tab_inv_h = on ? 1.f / p->tab_h : 0.f;
+  prm.tab_coarse = on && p->screen_coarse ? p->tab_coarse.get() : nullptr;
+  prm.tab_cn = p->tab_cn;
 }
 
 __global__ void init_run_kernel(int B, int32_t* active, int32_t* iters, int32_t* status, float* min_dist, int32_t* sel_count, int32_t* warm_valid) {
@@ -359,6 +368,8 @@ int nb_pan_create(const nb_pan_config* cfg, const float* weights, int64_t n_weig
     NB_CUDA(nb::alloc(p->refine_list, (size_t)2 * cfg->max_envs * (cfg->receding + 1)));
     NB_CUDA(nb::alloc(p->screen_stats, (size_t)4));
     NB_CUDA(cudaMemset(p->screen_stats.get(), 0, 4 * sizeof(unsigned)));
+    NB_CUDA(nb::alloc(p->coarse_stats, (size_t)2));
+    NB_CUDA(cudaMemset(p->coarse_stats.get(), 0, 2 * sizeof(unsigned)));
     if (const char* e = getenv("NB_SCREEN_CMU")) { p->c_mu = (float)atof(e); p->cmu_override = true; }
   }
   NB_CUDA(nb::alloc(p->sel_mu, B * T1 * M * E));
@@ -387,6 +398,7 @@ int nb_pan_create(const nb_pan_config* cfg, const float* weights, int64_t n_weig
   if (const char* e = getenv("NB_DUNE_SKIP_T0")) p->dune_skip_t0 = atoi(e) != 0;  // developer overrides of the option defaults
   if (const char* e = getenv("NB_SCREEN_MMA")) p->screen_mma = atoi(e) != 0;
   if (const char* e = getenv("NB_SCREEN_TABLE")) p->screen_table = atoi(e) != 0;
+  if (const char* e = getenv("NB_SCREEN_COARSE")) p->screen_coarse = atoi(e) != 0;
   if (const char* e = getenv("NB_NRMP_RESTART_IT")) p->warm_check_it = atoi(e);
   if (const char* e = getenv("NB_NRMP_RESTART_GAP")) p->warm_check_gap = atof(e);
   NB_CUDA(cudaMemset(p->warm_valid.get(), 0, B * sizeof(int32_t)));
@@ -726,11 +738,23 @@ int nb_pan_read_screen_stats(nb_pan_t* p, float* max_error_ratio, int32_t* count
   return NB_OK;
 }
 
+int nb_pan_read_screen_coarse(nb_pan_t* p, int32_t* counts, int32_t reset) {
+  if (!p || !counts) return fail(NB_ERR_INVALID, "nb_pan_read_screen_coarse: null argument");
+  if (!p->coarse_stats) return fail(NB_ERR_INVALID, "handle was created in no_obs mode");
+  NB_CUDA(cudaSetDevice(p->cfg.device));
+  NB_CUDA(cudaDeviceSynchronize());
+  unsigned h[2];
+  NB_CUDA(cudaMemcpy(h, p->coarse_stats.get(), sizeof(h), cudaMemcpyDeviceToHost));
+  counts[0] = (int32_t)h[0]; counts[1] = (int32_t)h[1];
+  if (reset) NB_CUDA(cudaMemset(p->coarse_stats.get(), 0, sizeof(h)));
+  return NB_OK;
+}
+
 int nb_pan_read_screen_table(nb_pan_t* p, float* info) {
   if (!p || !info) return fail(NB_ERR_INVALID, "nb_pan_read_screen_table: null argument");
   info[0] = p->tab_h;
   info[1] = p->tab_half;
-  info[2] = p->tab_cell ? (float)((double)p->tab_n * p->tab_n * (sizeof(float4) + sizeof(float))) : 0.f;
+  info[2] = p->tab_cell ? (float)((double)p->tab_n * p->tab_n * (sizeof(float4) + sizeof(float)) + (double)p->tab_cn * p->tab_cn * sizeof(uint32_t)) : 0.f;
   info[3] = p->tab_ms;
   info[4] = p->tab_ratio;
   return NB_OK;

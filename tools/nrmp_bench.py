@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Times the NRMP solve alone (nb_nrmp_forward) at the shapes of a benchmark workload, on obstacle coefficients made once per input set.
 
-    python tools/nrmp_bench.py [--workload C4] [--envs B] [--reps 20] [--warmup 3] [--dump DIR] [--split] [--phases]
+    python tools/nrmp_bench.py [--workload C4] [--envs B] [--reps 20] [--warmup 3] [--dump DIR] [--split [--overlap 2]] [--phases]
 
 The inputs are bench.py's (tests/helpers.make_inputs, two sets of distinct environments).  For each set, nb_dune_forward runs once
 and the obstacle coefficients of the NRMP program are formed on the device from its selection (nrmp.py:220-261, as
@@ -11,7 +11,7 @@ launches alternate between the sets with a 256 MiB L2 flush before each, outside
 Prints one JSON line: ms per launch (mean, min, max), mean / max interior point iterations (nb_pan_read_diagnostics), status
 count, the card's name, power limit and SM clock.  --dump DIR writes S, U, D, ipm_iters and status of set 0 as DIR/<name>.npy, so
 two builds can be compared output for output.  --split adds a second JSON line: torch.profiler's per-kernel device time of a
-bench.py-shaped control step (K PAN iterations, two overlapped sub-batches) of the same workload.  --phases times a build of the
+bench.py-shaped control step (K PAN iterations, two overlapped sub-batches; --overlap 1: one stream, each kernel's time its own) of the same workload.  --phases times a build of the
 library with -DNB_NRMP_PHASES=1 instead (made and cached under neupan_b200/lib/phases/ when its sources changed) and adds the mean
 clock64() cycles per warp of the setup (per solve) and of the phases (a)-(e) of the interior point iteration (per iteration) to the
 line; the timers' atomics lengthen that build's launch a little.
@@ -97,6 +97,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--dump", default=None, metavar="DIR")
     ap.add_argument("--split", action="store_true", help="also print torch.profiler's per-kernel split of a bench.py-shaped step")
+    ap.add_argument("--overlap", type=int, default=2, help="sub-batch streams of the --split step (1: kernels do not overlap)")
     ap.add_argument("--phases", action="store_true", help="time the NB_NRMP_PHASES build and report cycles per phase")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "nrmp_bench.py times the device"
@@ -184,12 +185,12 @@ def main():
 
 
 def split(cfg, B, args, dev):
-    """Per-kernel device time of a bench.py-shaped step: K iterations forced, overlap 2, L2 flushed between steps."""
+    """Per-kernel device time of a bench.py-shaped step: K iterations forced, --overlap sub-batches, L2 flushed between steps."""
     from gpu_helpers import make_pan
     from helpers import make_inputs
     from torch.profiler import ProfilerActivity, profile
 
-    pan = make_pan(cfg, K=cfg.K, max_envs=B, overlap=2)
+    pan = make_pan(cfg, K=cfg.K, max_envs=B, overlap=args.overlap)
     inp = make_inputs(cfg, B=B)
     d = {k: (None if v is None else torch.from_numpy(v).to(dev)) for k, v in inp.items()}
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
@@ -215,7 +216,7 @@ def split(cfg, B, args, dev):
         name = e.key.replace("void ", "").split("(")[0]
         per[name] = per.get(name, 0.0) + t / 1e3 / steps
     tot = sum(per.values())
-    line = dict(metric="per-kernel device ms per control step (torch.profiler)", workload=f"{args.workload} {cfg.name}: B={B} T={cfg.T} K={cfg.K}, overlap 2",
+    line = dict(metric="per-kernel device ms per control step (torch.profiler)", workload=f"{args.workload} {cfg.name}: B={B} T={cfg.T} K={cfg.K}, overlap {args.overlap}",
                 steps=steps, kernel_ms_per_step=dict(sorted(per.items(), key=lambda kv: -kv[1])), kernel_ms_sum=tot,
                 note="the two sub-batches run on two streams, so kernel times overlap and their sum exceeds the step time", **gpu_info())
     print(json.dumps(line), flush=True)
