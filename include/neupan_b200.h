@@ -578,6 +578,39 @@ int nb_world_read_episodes(nb_world_t* w, int32_t S, int32_t* collided, int32_t*
                            int32_t* end_step, int32_t* reason, int32_t* slot, int32_t* scene_of, int32_t* reset, int32_t* finished,
                            void* stream);
 
+/* Actuation limits and noise (semantics in csrc/world_kernel.cuh; this project's reading of IR-SIM's vel_min / vel_max / acce and
+ * its motion and lidar `noise` switches, not a claim of parity).  Both are off until these calls; a handle without them launches the
+ * kernels of a world without them.
+ *   nb_world_set_actuation: per_type (num_types, HOST) one row per robot type of the handle (type 0 the config's robot, then the
+ *           types of nb_world_set_fleet_ex), in the action's own convention (diff (v, omega), acker (v, steering), omni (vx, vy)):
+ *           vel_min / vel_max (-inf / +inf: no bound), acce (+inf: no rate limit), alpha (0: no motion noise).  In a step robot n
+ *           with action a takes, per component, c = min(max(a, max(vel_min, cmd_prev - acce dt)), min(vel_max, cmd_prev + acce dt)),
+ *           stores cmd_prev = c, and integrates u = c + (s0 z0, s1 z1) with s0 = sqrt(alpha0 c0^2 + alpha1 c1^2), s1 = sqrt(alpha2 c0^2
+ *           + alpha3 c1^2) and standard normal z from the motion stream (`seed`); the scan's velocity of the robot is that of u.  A
+ *           collided robot stays frozen and its cmd_prev becomes 0.  Reactive obstacles still see the action as given.  From this
+ *           call on nb_world_step launches the step's actuation variant.
+ *           Checks (NB_ERR_INVALID, naming the type and component): num_types is the handle's type count, no NaN, vel_min <= vel_max
+ *           (vel_min < +inf, vel_max > -inf), acce > 0, alpha finite and >= 0, an acker type's finite steering limits in (-pi/2, pi/2).
+ *   nb_world_set_lidar_noise: a beam that hits something reports clamp(t + range_std z, range_min, range_max) (FP64, then the float
+ *           cast); a miss (range_max), the hit index and the velocity are unchanged; z from the lidar stream (`seed`).  range_std 0
+ *           turns it off.  Checks (NB_ERR_INVALID): range_std finite and >= 0, range_min in [0, range_max).
+ *   streams z is keyed by (seed, environment e, robot k within it, the scene's step n, component or beam j), with a domain tag per
+ *           use (motion, lidar), independent of the reactive obstacles' goal draws.  n counts the nb_world_step calls since the
+ *           robots were placed in a plain world, and is the slot's episode step in episode mode (e the scene there); the first scan
+ *           and step use n = 0.  So environment e's noise does not depend on B, two scans without a step between them are equal, and
+ *           an episode is bitwise the plain run of its scene.
+ * The settings are kept by nb_world_set_scenes(_ex), nb_world_set_fleet(_ex) and nb_world_set_episodes, which zero cmd_prev (so
+ * does a slot taking a new scene); types past num_types (a later fleet with more types) take the defaults.
+ * nb_world_read_commands enqueues on `stream` a device-to-device copy of cmd_prev (N, 2) float64, N = B*K (S*K, the scenes' rows, in
+ * episode mode), without synchronising. */
+typedef struct nb_world_actuation {
+  double vel_min[2], vel_max[2], acce[2], alpha[4];
+} nb_world_actuation;
+
+int nb_world_set_actuation(nb_world_t* w, int32_t num_types, const nb_world_actuation* per_type, uint64_t seed);
+int nb_world_set_lidar_noise(nb_world_t* w, double range_min, double range_std, uint64_t seed);
+int nb_world_read_commands(nb_world_t* w, int32_t N, double* cmd_prev, void* stream);
+
 /* ---- DUNE training on the device (SURVEY 8f "next" row 4) ------------------------------------------------------------ */
 
 /* DUNETrain.generate_data_set / prob_solve (neupan/blocks/dune_train.py:100-140): labels of n sampled points -- the solution of the

@@ -76,6 +76,11 @@ class WorldMap(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("origin", C.c_double * 2), ("resolution", C.c_double)]
 
 
+class WorldActuation(C.Structure):
+    """struct nb_world_actuation (include/neupan_b200.h)."""
+    _fields_ = [("vel_min", C.c_double * 2), ("vel_max", C.c_double * 2), ("acce", C.c_double * 2), ("alpha", C.c_double * 4)]
+
+
 _FP = C.c_void_p  # device or host float* / int32*: passed as raw addresses
 
 # name -> (restype, argtypes); every symbol include/neupan_b200.h declares
@@ -137,6 +142,9 @@ SYMBOLS = {
     "nb_world_check_episodes": (C.c_int, [C.POINTER(WorldConfig), C.c_int32, C.c_int32, _FP, C.c_int32, C.c_int32]),
     "nb_world_set_episodes": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "nb_world_read_episodes": (C.c_int, [C.c_void_p, C.c_int32] + [_FP] * 10 + [C.c_void_p]),
+    "nb_world_set_actuation": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(WorldActuation), C.c_uint64]),
+    "nb_world_set_lidar_noise": (C.c_int, [C.c_void_p, C.c_double, C.c_double, C.c_uint64]),
+    "nb_world_read_commands": (C.c_int, [C.c_void_p, C.c_int32, _FP, C.c_void_p]),
     "nb_dune_labels": (C.c_int, [C.c_int32, _FP, _FP, C.c_int64, _FP, _FP, _FP, _FP, C.c_void_p]),
     "nb_dune_train_create": (C.c_int, [C.c_int32, _FP, _FP, _FP, C.c_int64, C.c_int32, C.POINTER(C.c_void_p)]),
     "nb_dune_train_destroy": (C.c_int, [C.c_void_p]),

@@ -43,7 +43,7 @@ struct nb_world {
   // config's robot): the table (T + 1 rows) and each robot's type (B K, zeros without a mix)
   int K = 1;
   struct Robots {
-    nb::DeviceArray<double> states, goal, vel;
+    nb::DeviceArray<double> states, goal, vel, cmd;  // cmd: cmd_prev (B K, 2), the last limited command (nb_world_set_actuation)
     nb::DeviceArray<int32_t> collided, arrived, rtype;
     nb::DeviceArray<nb::WorldRobotType> types;
   } robots;
@@ -83,6 +83,17 @@ struct nb_world {
     nb::DeviceArray<int32_t> r_col, r_arr, r_astep, r_end, r_reason, r_slot;
     nb::DeviceArray<float> r_minclr;
   } ep;
+  // actuation limits and motion noise (nb_world_set_actuation): on false -> the step kernels without the actuation stage; act holds
+  // kWorldMaxRobotTypes rows (defaults past num_types).  Kept by nb_world_set_scenes / _fleet / _episodes, which zero cmd_prev.
+  struct Actuation {
+    bool on = false;
+    uint64_t seed = 0;
+    nb::DeviceArray<double> act;
+  } act;
+  // lidar range noise (nb_world_set_lidar_noise): range_std 0 -> the scan kernels without it
+  double range_min = 0.0, range_std = 0.0;
+  uint64_t lidar_seed = 0;
+  uint64_t steps = 0;  // plain world: nb_world_step calls since the robots were placed (the noise streams' step n)
 };
 
 namespace {
@@ -701,6 +712,7 @@ int world_set_robots(nb_world* w, int B, int K, const double* robots, int T, con
   NB_CUDA(nb::alloc(r.arrived, N));
   NB_CUDA(nb::alloc(r.goal, 3 * N));
   NB_CUDA(nb::alloc(r.vel, 2 * N));
+  NB_CUDA(nb::alloc(r.cmd, 2 * N));
   NB_CUDA(nb::alloc(r.types, table.size()));
   NB_CUDA(nb::alloc(r.rtype, N));
   NB_CUDA(cudaMemcpy(r.states.get(), states.data(), sizeof(double) * 3 * N, cudaMemcpyHostToDevice));
@@ -710,7 +722,9 @@ int world_set_robots(nb_world* w, int B, int K, const double* robots, int T, con
   NB_CUDA(cudaMemset(r.collided.get(), 0, sizeof(int32_t) * N));
   NB_CUDA(cudaMemset(r.arrived.get(), 0, sizeof(int32_t) * N));
   NB_CUDA(cudaMemset(r.vel.get(), 0, sizeof(double) * 2 * N));
+  NB_CUDA(cudaMemset(r.cmd.get(), 0, sizeof(double) * 2 * N));
   w->K = K;
+  w->steps = 0;
   w->max_redges = max_redges;
   w->h_robots.assign(robots, robots + 6 * N);
   w->h_types.assign(types, types + T);
@@ -760,6 +774,44 @@ nb::WorldRvoParams world_rvo_params(const nb_world* w, const float* action) {
   rp.beh = w->rvo.beh.get(); rp.radius = w->rvo.rad.get(); rp.goal = w->rvo.goal.get(); rp.draws = w->rvo.draws.get(); rp.action = action;
   rp.seed = w->rvo.seed; rp.cap = w->rvo.cap;
   return rp;
+}
+
+// the actuation (step) or lidar (scan) noise parameters
+nb::WorldNoiseParams world_noise_params(const nb_world* w, bool lidar) {
+  nb::WorldNoiseParams nz;
+  nz.act = w->act.act.get(); nz.cmd = w->robots.cmd.get(); nz.ep_t = w->ep.t.get(); nz.n = w->steps;
+  nz.seed = lidar ? w->lidar_seed : w->act.seed;
+  nz.range_min = w->range_min; nz.range_std = w->range_std;
+  return nz;
+}
+
+// Every check of nb_world_set_actuation: one row per robot type of the handle, no NaN, vel_min <= vel_max with vel_min < +inf and
+// vel_max > -inf, acce > 0 (+inf: no rate limit), finite alpha >= 0, and an acker type's finite steering limits in (-pi/2, pi/2).
+int world_check_actuation(const nb_world* w, int32_t num_types, const nb_world_actuation* per_type) {
+  const int T = 1 + (int)w->h_types.size();
+  if (num_types != T) return fail(NB_ERR_INVALID, "nb_world_set_actuation: num_types = %d but the handle has %d robot types", num_types, T);
+  if (!per_type) return fail(NB_ERR_INVALID, "nb_world_set_actuation: null per_type");
+  for (int t = 0; t < T; ++t) {
+    const nb_world_actuation& a = per_type[t];
+    const int kin = t == 0 ? w->cfg.kinematics : w->h_types[t - 1].kinematics;
+    for (int j = 0; j < 2; ++j) {
+      if (std::isnan(a.vel_min[j]) || std::isnan(a.vel_max[j]) || std::isnan(a.acce[j]))
+        return fail(NB_ERR_INVALID, "nb_world_set_actuation: type %d, component %d: NaN limit", t, j);
+      if (!(a.vel_min[j] <= a.vel_max[j]) || a.vel_min[j] == INFINITY || a.vel_max[j] == -INFINITY)
+        return fail(NB_ERR_INVALID, "nb_world_set_actuation: type %d, component %d: vel_min = %g, vel_max = %g (need vel_min <= vel_max, "
+                    "vel_min < inf, vel_max > -inf)", t, j, a.vel_min[j], a.vel_max[j]);
+      if (!(a.acce[j] > 0.0)) return fail(NB_ERR_INVALID, "nb_world_set_actuation: type %d, component %d: acce = %g must be > 0", t, j, a.acce[j]);
+    }
+    for (int j = 0; j < 4; ++j)
+      if (!std::isfinite(a.alpha[j]) || a.alpha[j] < 0.0)
+        return fail(NB_ERR_INVALID, "nb_world_set_actuation: type %d: alpha[%d] = %g must be finite and >= 0", t, j, a.alpha[j]);
+    const double h = 1.5707963267948966;
+    if (kin == NB_KIN_ACKER)
+      for (const double s : {a.vel_min[1], a.vel_max[1]})
+        if (std::isfinite(s) && !(-h < s && s < h))
+          return fail(NB_ERR_INVALID, "nb_world_set_actuation: type %d (acker): steering limit %g outside (-pi/2, pi/2)", t, s);
+  }
+  return NB_OK;
 }
 
 }  // namespace
@@ -944,11 +996,14 @@ int nb_world_scan(nb_world_t* w, int32_t B, float* ranges, float* velocity, int3
   // the dynamic shared-memory limit is an attribute of the kernel, shared by every handle of the process: set this handle's
   // size before each launch (another handle's nb_world_set_scenes may have set a smaller one)
   const bool map = w->maps.has_map;
-  auto* kernel = w->ep.slots ? (map ? nb::world_scan_kernel<true, true> : nb::world_scan_kernel<false, true>)
-                             : (map ? nb::world_scan_kernel<true, false> : nb::world_scan_kernel<false, false>);
+  auto* kernel = w->range_std > 0.0
+                     ? (w->ep.slots ? (map ? nb::world_scan_kernel<true, true, true> : nb::world_scan_kernel<false, true, true>)
+                                    : (map ? nb::world_scan_kernel<true, false, true> : nb::world_scan_kernel<false, false, true>))
+                     : (w->ep.slots ? (map ? nb::world_scan_kernel<true, true> : nb::world_scan_kernel<false, true>)
+                                    : (map ? nb::world_scan_kernel<true, false> : nb::world_scan_kernel<false, false>));
   NB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(w->scan_smem, 1)));
   kernel<<<w->scan_grid, w->scan_threads, w->scan_smem, (cudaStream_t)stream>>>(world_params(w), world_map_params(w), w->max_circ, w->max_edges,
-                                                                                w->max_redges, ranges, velocity, hit);
+                                                                                w->max_redges, ranges, velocity, hit, world_noise_params(w, true));
   ++nb::launches;
   NB_CUDA(cudaGetLastError());
   return NB_OK;
@@ -978,6 +1033,8 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
   // a CTA of up to 8 warps per E environments, a warp per robot
   const int E = nb::world_step_envs(w->K);
   const dim3 grid((prm.B + E - 1) / E), block(32 * std::min(E * w->K, nb::kWorldStepMaxWarps));
+  const bool act = w->act.on;
+  const nb::WorldNoiseParams nz = world_noise_params(w, false);
   if (contact) {  // the obstacles move one environment per warp, in row order; the step then leaves them where they are
     const int units = (prm.B + nb::kWorldContactWarps - 1) / nb::kWorldContactWarps;
     const size_t smem = sizeof(double) * nb::kWorldContactWarps * 6 * w->ocontact.max_n;
@@ -986,9 +1043,20 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
     move<<<units, 32 * nb::kWorldContactWarps, smem, (cudaStream_t)stream>>>(prm, world_map_params(w), world_block_params(w), world_contact_params(w));
     ++nb::launches;
     NB_CUDA(cudaGetLastError());
-    auto* kernel = ep ? (map ? nb::world_step_contact_kernel<true, true> : nb::world_step_contact_kernel<false, true>)
-                      : (map ? nb::world_step_contact_kernel<true, false> : nb::world_step_contact_kernel<false, false>);
-    kernel<<<grid, block, 0, (cudaStream_t)stream>>>(prm, world_map_params(w), action, collided, arrived, clearance);
+    if (act) {
+      auto* kernel = ep ? (map ? nb::world_step_act_kernel<true, true, false, false> : nb::world_step_act_kernel<false, true, false, false>)
+                        : (map ? nb::world_step_act_kernel<true, false, false, false> : nb::world_step_act_kernel<false, false, false, false>);
+      kernel<<<grid, block, 0, (cudaStream_t)stream>>>(prm, world_map_params(w), nb::WorldBlockParams{}, nz, action, collided, arrived, clearance);
+    } else {
+      auto* kernel = ep ? (map ? nb::world_step_contact_kernel<true, true> : nb::world_step_contact_kernel<false, true>)
+                        : (map ? nb::world_step_contact_kernel<true, false> : nb::world_step_contact_kernel<false, false>);
+      kernel<<<grid, block, 0, (cudaStream_t)stream>>>(prm, world_map_params(w), action, collided, arrived, clearance);
+    }
+  } else if (act) {  // the step with the actuation stage: blocking maps, or the plain and episode kernels' variants
+    auto* kernel = blocking ? (ep ? nb::world_step_act_kernel<true, true, true, true> : nb::world_step_act_kernel<true, false, true, true>)
+                            : (ep ? (map ? nb::world_step_act_kernel<true, true, false, true> : nb::world_step_act_kernel<false, true, false, true>)
+                                  : (map ? nb::world_step_act_kernel<true, false, false, true> : nb::world_step_act_kernel<false, false, false, true>));
+    kernel<<<grid, block, 0, (cudaStream_t)stream>>>(prm, world_map_params(w), world_block_params(w), nz, action, collided, arrived, clearance);
   } else if (blocking) {
     auto* kernel = ep ? nb::world_step_block_kernel<true> : nb::world_step_block_kernel<false>;
     kernel<<<grid, block, 0, (cudaStream_t)stream>>>(prm, world_map_params(w), world_block_params(w), action, collided, arrived, clearance);
@@ -1008,10 +1076,12 @@ int nb_world_step(nb_world_t* w, int32_t B, const float* action, int32_t* collid
     a.collided = w->robots.collided.get(); a.arrived = w->robots.arrived.get(); a.clear = e.clear.get();
     a.r_col = e.r_col.get(); a.r_arr = e.r_arr.get(); a.r_astep = e.r_astep.get(); a.r_minclr = e.r_minclr.get();
     a.r_end = e.r_end.get(); a.r_reason = e.r_reason.get(); a.r_slot = e.r_slot.get();
+    a.cmd = act ? w->robots.cmd.get() : nullptr;
     nb::world_advance_kernel<<<1, nb::kWorldAdvanceThreads, 0, (cudaStream_t)stream>>>(a);
     ++nb::launches;
     NB_CUDA(cudaGetLastError());
   }
+  ++w->steps;
   return NB_OK;
 }
 
@@ -1147,6 +1217,7 @@ int nb_world_set_episodes(nb_world_t* w, int32_t slots, int32_t max_steps) {
     NB_CUDA(cudaMemset(ep.r_end.get(), 0, S * sizeof(int32_t)));
     NB_CUDA(cudaMemset(ep.r_reason.get(), 0, S * sizeof(int32_t)));
     NB_CUDA(up(ep.r_slot, slot.data(), S));
+    NB_CUDA(cudaMemset(w->robots.cmd.get(), 0, SK * 2 * sizeof(double)));  // every scene starts from a zero command
     NB_CUDA(cudaDeviceSynchronize());
     return NB_OK;
   };
@@ -1156,6 +1227,7 @@ int nb_world_set_episodes(nb_world_t* w, int32_t slots, int32_t max_steps) {
   }
   ep.slots = slots; ep.max_steps = max_steps;
   w->ep = std::move(ep);
+  w->steps = 0;
   return NB_OK;
 }
 
@@ -1309,6 +1381,53 @@ int nb_world_read_obstacle_contact(nb_world_t* w, int32_t O, int32_t* bounces, v
   if (!bounces) return fail(NB_ERR_INVALID, "nb_world_read_obstacle_contact: null bounces");
   NB_CUDA(cudaSetDevice(w->cfg.device));
   if (O) NB_CUDA(cudaMemcpyAsync(bounces, w->ocontact.bounces.get(), sizeof(int32_t) * O, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return NB_OK;
+}
+
+int nb_world_set_actuation(nb_world_t* w, int32_t num_types, const nb_world_actuation* per_type, uint64_t seed) {
+  if (!w) return fail(NB_ERR_INVALID, "nb_world_set_actuation: null handle");
+  if (int rc = world_check_actuation(w, num_types, per_type)) return rc;
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  const double inf = INFINITY;
+  const double def[nb::kWorldActCols] = {-inf, -inf, inf, inf, inf, inf, 0.0, 0.0, 0.0, 0.0};
+  std::vector<double> table((size_t)nb::kWorldMaxRobotTypes * nb::kWorldActCols);
+  for (int t = 0; t < nb::kWorldMaxRobotTypes; ++t) {
+    double* row = table.data() + (size_t)t * nb::kWorldActCols;
+    if (t < num_types) {
+      const nb_world_actuation& a = per_type[t];
+      const double r[nb::kWorldActCols] = {a.vel_min[0], a.vel_min[1], a.vel_max[0], a.vel_max[1], a.acce[0], a.acce[1],
+                                           a.alpha[0], a.alpha[1], a.alpha[2], a.alpha[3]};
+      std::copy(r, r + nb::kWorldActCols, row);
+    } else {
+      std::copy(def, def + nb::kWorldActCols, row);
+    }
+  }
+  if (!w->act.act) NB_CUDA(nb::alloc(w->act.act, table.size()));
+  NB_CUDA(cudaMemcpy(w->act.act.get(), table.data(), sizeof(double) * table.size(), cudaMemcpyHostToDevice));
+  w->act.seed = seed;
+  w->act.on = true;
+  return NB_OK;
+}
+
+int nb_world_set_lidar_noise(nb_world_t* w, double range_min, double range_std, uint64_t seed) {
+  if (!w) return fail(NB_ERR_INVALID, "nb_world_set_lidar_noise: null handle");
+  if (!(std::isfinite(range_std) && range_std >= 0.0))
+    return fail(NB_ERR_INVALID, "nb_world_set_lidar_noise: range_std = %g must be finite and >= 0", range_std);
+  if (!(range_min >= 0.0 && range_min < w->cfg.range_max))
+    return fail(NB_ERR_INVALID, "nb_world_set_lidar_noise: range_min = %g outside [0, range_max = %g)", range_min, w->cfg.range_max);
+  w->range_min = range_min; w->range_std = range_std; w->lidar_seed = seed;
+  return NB_OK;
+}
+
+int nb_world_read_commands(nb_world_t* w, int32_t N, double* cmd_prev, void* stream) {
+  if (!w) return fail(NB_ERR_INVALID, "nb_world_read_commands: null handle");
+  if (!w->B) return fail(NB_ERR_INVALID, "nb_world_read_commands: no scenes set (nb_world_set_scenes)");
+  if (N != w->B * w->K)
+    return fail(NB_ERR_INVALID, "nb_world_read_commands: N = %d but the world has %d %s x %d robots (N = %d)", N, w->B, w->ep.slots ? "scenes" : "environments",
+                w->K, w->B * w->K);
+  if (!cmd_prev) return fail(NB_ERR_INVALID, "nb_world_read_commands: null cmd_prev");
+  NB_CUDA(cudaSetDevice(w->cfg.device));
+  NB_CUDA(cudaMemcpyAsync(cmd_prev, w->robots.cmd.get(), sizeof(double) * 2 * (size_t)N, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return NB_OK;
 }
 

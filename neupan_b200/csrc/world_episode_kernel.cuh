@@ -8,7 +8,8 @@
 //            and the smallest clearance over the episode's steps (accumulated every step), per scene the end step and the reason.
 //   next     the slots whose episode ended in this step, in ascending slot order, take the next unstarted scenes in ascending scene
 //            order (one block-wide exclusive scan over the slots); a slot for which none is left goes idle: its scene is frozen and
-//            no kernel touches its rows again.  reset[b] = 1 for a slot that has just taken a new scene, else 0.
+//            no kernel touches its rows again.  reset[b] = 1 for a slot that has just taken a new scene, else 0.  With actuation
+//            set (nb_world_set_actuation) the new scene's cmd_prev rows are zeroed.
 //
 // Every scene runs once, so nothing needs restoring at a reset: a scene's own rows hold its start until its slot takes it and its
 // final state after its episode.
@@ -37,6 +38,7 @@ struct WorldEpisodeParams {
   int32_t* r_end;           // (S) results per scene: end step (0 while running), reason (0 while running), the slot that ran it
   int32_t* r_reason;
   int32_t* r_slot;
+  double* cmd;              // (S K, 2) cmd_prev of the scenes' robots (nb_world_set_actuation), or NULL
 };
 
 // One CTA: thread i takes the contiguous slots [i c, (i + 1) c), c = ceil(slots / blockDim), so that ascending threads are
@@ -104,6 +106,8 @@ __global__ void __launch_bounds__(kWorldAdvanceThreads) world_advance_kernel(con
       ep.scene_of[b] = s;
       ep.t[b] = 0;
       ep.r_slot[s] = b;
+      if (ep.cmd)  // the new scene's robots start from a zero command
+        for (int k = 0; k < 2 * K; ++k) ep.cmd[2 * (size_t)s * K + k] = 0.0;
     } else {
       ep.live[b] = 0;
       ep.reset[b] = 0;

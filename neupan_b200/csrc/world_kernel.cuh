@@ -53,6 +53,24 @@
 // moves its obstacles in world_contact_kernel and steps with world_step_body<..., kMove = false>; a handle without one launches the
 // kernels above unchanged.
 //
+// Actuation limits and noise (nb_world_set_actuation, nb_world_set_lidar_noise; this project's reading of IR-SIM's vel_min /
+// vel_max / acce and its motion and lidar `noise` switches, not a claim of parity).  Each robot type t has vel_min[2], vel_max[2],
+// acce[2] and alpha[4] (defaults -inf, +inf, +inf, 0), in the action's own convention (diff (v, omega), acker (v, steering), omni
+// (vx, vy)); each robot row n has cmd_prev[2], its last limited command (0 after nb_world_set_scenes / _fleet / _episodes and when a
+// slot takes a new scene).  In a step, robot n of type t with action a (converted to double), per component j:
+//   lo_j = max(vel_min_j, cmd_prev_j - acce_j dt)   hi_j = min(vel_max_j, cmd_prev_j + acce_j dt)   c_j = min(max(a_j, lo_j), hi_j)
+//   cmd_prev <- c;  s0 = sqrt(alpha0 c0^2 + alpha1 c1^2), s1 = sqrt(alpha2 c0^2 + alpha3 c1^2);  u = (c0 + s0 z0, c1 + s1 z1)
+// and the robot integrates u (world_integrate); the velocity the scan reports for it is that of u.  The noise is added after the
+// limits and not clipped again (IR-SIM's order); a type whose alpha are all 0 draws nothing (u = c).  A collided robot stays frozen
+// and its cmd_prev becomes 0.  Reactive obstacles still see the action as given.  Lidar: a beam that hits something (hit >= 0)
+// reports clamp(t + range_std z, range_min, range_max), in FP64 before the float cast; a miss, the hit index and the velocity are
+// unchanged.  z is a standard normal draw from the counter-based streams below, keyed by (seed, tag, e, k, n, j): e the environment
+// (the scene in episode mode), k the robot within it, n the steps that scene has taken (the host's count in a plain world, the
+// slot's episode step t in episode mode; the first scan and step use n = 0), j the component (0, 1) or the beam.  So a run is
+// reproducible from its seeds, environment e's noise does not depend on B, two scans without a step between them are equal, and an
+// episode is bitwise the plain run of its scene.  Both are compile-time variants (kAct of world_step_body, kNoise of
+// world_scan_kernel) launched only when the handle has actuation set or range_std > 0.
+//
 // All arithmetic is FP64 with explicit rounding (__dmul_rn / __dadd_rn / __dsub_rn: no FMA contraction), so that oracle/world.py,
 // which performs the same operations in the same order in numpy, agrees to the last bit wherever the inputs agree (the only
 // differences come from CUDA's sin / cos / tan vs libm).
@@ -128,11 +146,58 @@ struct WorldMapParams {
   double window;            // the step's search distance (0, 10] m
 };
 
+constexpr int kWorldActCols = 10;  // actuation row of a robot type: vel_min[2], vel_max[2], acce[2], alpha[4]
+
+// Actuation limits, motion noise and lidar noise (read by the kAct / kNoise instantiations only)
+struct WorldNoiseParams {
+  const double* act;    // (kWorldMaxRobotTypes, kWorldActCols) per robot type (step)
+  double* cmd;          // (B K, 2) cmd_prev of every robot row (step)
+  const int32_t* ep_t;  // (slots) the steps of each slot's current episode (episode mode)
+  uint64_t n;           // plain world: the steps taken since the robots were placed
+  uint64_t seed;        // the motion seed (step) or the lidar seed (scan)
+  double range_min, range_std;  // scan
+};
+
 __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
 __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
 __device__ __forceinline__ double ddot(double ax, double ay, double bx, double by) { return dadd(dmul(ax, bx), dmul(ay, by)); }
 __device__ __forceinline__ double dcross(double ax, double ay, double bx, double by) { return dsub(dmul(ax, by), dmul(ay, bx)); }
+
+// ---- counter-based random streams ------------------------------------------------------------------------------------------
+
+constexpr uint64_t kSplitMixGamma = 0x9E3779B97F4A7C15ull;
+// domain tags of the noise streams, so that they are independent of each other and of the reactive obstacles' goal draws
+constexpr uint64_t kNoiseTagMotion = 0x6D6F74696F6E0001ull;
+constexpr uint64_t kNoiseTagLidar = 0x6C69646172000002ull;
+
+// SplitMix64 (Steele, Lea and Flood 2014): output n of the generator seeded with s is mix(s + (n + 1) gamma), so any draw is
+// computed directly from its counter.
+__host__ __device__ __forceinline__ uint64_t splitmix64_mix(uint64_t z) {
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+__host__ __device__ __forceinline__ uint64_t splitmix64_at(uint64_t s, uint64_t n) { return splitmix64_mix(s + (n + 1) * kSplitMixGamma); }
+// the stream of obstacle i (index within its environment) of environment b
+__host__ __device__ __forceinline__ uint64_t world_rvo_key(uint64_t seed, int b, int i) {
+  return splitmix64_mix(splitmix64_mix(seed + kSplitMixGamma) ^ (((uint64_t)(uint32_t)b << 32) | (uint64_t)(uint32_t)i));
+}
+// (x >> 11) 2^-53: uniform in [0, 1), exact
+__host__ __device__ __forceinline__ double world_u01(uint64_t x) { return (double)(x >> 11) * 0x1.0p-53; }
+
+// The noise stream of robot k of environment e at step n under a domain tag: the robot's goal-draw style key with the tag mixed in,
+// then output n of it as the seed of the step's draws
+__host__ __device__ __forceinline__ uint64_t world_noise_key(uint64_t seed, uint64_t tag, int e, int k, uint64_t n) {
+  return splitmix64_at(splitmix64_mix(world_rvo_key(seed, e, k) ^ tag), n);
+}
+
+// Draw j of a step's stream: Box-Muller from outputs 2j and 2j + 1, z = sqrt(-2 log(1 - u1)) cos(2 pi u2) (1 - u1 >= 2^-53, so
+// z is finite).  Only log and cos are not correctly rounded.
+__device__ __forceinline__ double world_normal(uint64_t key, int j) {
+  const double u1 = world_u01(splitmix64_at(key, 2 * (uint64_t)j)), u2 = world_u01(splitmix64_at(key, 2 * (uint64_t)j + 1));
+  return dmul(sqrt(dmul(-2.0, log(dsub(1.0, u1)))), cos(dmul(6.283185307179586, u2)));
+}
 
 // ---- occupancy maps ---------------------------------------------------------------------------------------------------------
 
@@ -212,10 +277,12 @@ __device__ __forceinline__ double world_map_cast(const WorldMap& m, const uint32
 // max_redges: the largest environment's robot edge count (the sum of its robots' vertex counts with K > 1, else 0); robot k's edges
 // follow those of robots 0 .. k - 1, each robot's polygon that of its own type.  kMap: then the environment's map (world_map_cast,
 // index O_b + K, velocity 0); mp is not read without it.  kEp (episode mode): the CTA's unit b is a slot, which scans the robots of
-// scene scene_of[b] (an idle slot its frozen scene) into slot rows b K + k.
-template <bool kMap, bool kEp>
+// scene scene_of[b] (an idle slot its frozen scene) into slot rows b K + k.  kNoise (range_std > 0): a hit's range gets the lidar
+// noise of the header, draw i of robot k's lidar stream at the scene's step n; nz is not read without it.
+template <bool kMap, bool kEp, bool kNoise = false>
 __global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, const WorldMapParams mp, int max_circ, int max_edges, int max_redges,
-                                                         float* __restrict__ ranges, float* __restrict__ velocity, int32_t* __restrict__ hit) {
+                                                         float* __restrict__ ranges, float* __restrict__ velocity, int32_t* __restrict__ hit,
+                                                         const WorldNoiseParams nz) {
   extern __shared__ double wsm[];
   __shared__ double s_sx[kWorldMaxFleet], s_sy[kWorldMaxFleet], s_hc[kWorldMaxFleet], s_hs[kWorldMaxFleet];  // sensor poses
   __shared__ int s_nre;  // the environment's robot edges
@@ -333,6 +400,13 @@ __global__ void __launch_bounds__(256) world_scan_kernel(const WorldParams prm, 
         }
       }
       if (!(best < prm.range_max)) { best = prm.range_max; bid = -1; }
+      if constexpr (kNoise) {
+        if (bid >= 0) {
+          const uint64_t step = kEp ? (uint64_t)nz.ep_t[b] : nz.n;
+          const double r = dadd(best, dmul(nz.range_std, world_normal(world_noise_key(nz.seed, kNoiseTagLidar, e, k, step), i)));
+          best = fmin(fmax(r, nz.range_min), prm.range_max);
+        }
+      }
       const size_t n = (size_t)b * K + k;
       ranges[n * R + i] = (float)best;
       if (velocity) {
@@ -487,6 +561,30 @@ __device__ __forceinline__ void world_integrate(int kinematics, double L, double
   // omni: no turn; acker: v tan(phi) / L; diff: omega
   const double dth = kinematics == 2 ? 0.0 : (kinematics == 1 ? dmul(a0, tan(a1)) / L : a1);
   x = dadd(x, dmul(vx, dt)); y = dadd(y, dmul(vy, dt)); th = dadd(th, dmul(dth, dt));
+}
+
+// The actuation stage of the header for robot row n (robot k of scene e) of type t at the scene's step n_step: the action (a0, a1)
+// becomes the limited command c, written to cmd_prev, plus the motion noise (none when the type's alpha are all 0).
+__device__ __forceinline__ void world_actuate(const WorldNoiseParams& nz, double dt, int t, size_t n, int e, int k, uint64_t n_step, double& a0,
+                                              double& a1) {
+  const double* A = nz.act + (size_t)kWorldActCols * t;
+  double* cmd = nz.cmd + 2 * n;
+  double c[2] = {a0, a1};
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const double r = dmul(A[4 + j], dt);
+    const double lo = fmax(A[j], dsub(cmd[j], r)), hi = fmin(A[2 + j], dadd(cmd[j], r));
+    c[j] = fmin(fmax(c[j], lo), hi);
+    cmd[j] = c[j];
+  }
+  a0 = c[0]; a1 = c[1];
+  if (A[6] != 0.0 || A[7] != 0.0 || A[8] != 0.0 || A[9] != 0.0) {
+    const double q0 = dmul(c[0], c[0]), q1 = dmul(c[1], c[1]);
+    const double s0 = sqrt(dadd(dmul(A[6], q0), dmul(A[7], q1))), s1 = sqrt(dadd(dmul(A[8], q0), dmul(A[9], q1)));
+    const uint64_t key = world_noise_key(nz.seed, kNoiseTagMotion, e, k, n_step);
+    a0 = dadd(c[0], dmul(s0, world_normal(key, 0)));
+    a1 = dadd(c[1], dmul(s1, world_normal(key, 1)));
+  }
 }
 
 // The move of an obstacle row by v dt; a moving centre that left the rectangle env is mirrored back and its velocity component
@@ -748,9 +846,12 @@ __device__ __forceinline__ void world_move_obstacle_blocked(const WorldParams& p
 // touched, and its outputs are the frozen flags and clearance +inf.
 // kMove false (obstacle contact, nb_world_set_obstacle_contact): world_contact_kernel has already moved the obstacles, so phase 1
 // integrates the robots only.
-template <bool kMap, bool kEp, bool kBlock, bool kMove = true>
+// kAct (nb_world_set_actuation): phase 1 limits the action and adds the motion noise first (world_actuate); nz is not read
+// without it.
+template <bool kMap, bool kEp, bool kBlock, bool kMove = true, bool kAct = false>
 __device__ __forceinline__ void world_step_body(const WorldParams& prm, const WorldMapParams& mp, const WorldBlockParams& bp, const float* __restrict__ action,
-                                                int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived, float* __restrict__ clearance) {
+                                                int32_t* __restrict__ out_collided, int32_t* __restrict__ out_arrived, float* __restrict__ clearance,
+                                                const WorldNoiseParams& nz = WorldNoiseParams{}) {
   __shared__ double f_x[kWorldMaxFleet][kWorldMaxVertices], f_y[kWorldMaxFleet][kWorldMaxVertices];  // E K <= 8 or K <= 16 slots
   __shared__ double f_v[kWorldMaxFleet][2];
   __shared__ int f_nv[kWorldMaxFleet];  // each slot's vertex count (its type's)
@@ -768,7 +869,18 @@ __device__ __forceinline__ void world_step_body(const WorldParams& prm, const Wo
     double x = prm.states[3 * n], y = prm.states[3 * n + 1], th = prm.states[3 * n + 2];
     double vx = 0.0, vy = 0.0;
     const WorldRobotType* ty = prm.types + prm.rtype[n];
-    if (prm.collided[n] == 0) world_integrate(ty->kinematics, ty->L, prm.dt, (double)action[2 * q], (double)action[2 * q + 1], x, y, th, vx, vy);
+    if constexpr (kAct) {
+      if (prm.collided[n] == 0) {
+        double a0 = (double)action[2 * q], a1 = (double)action[2 * q + 1];
+        const uint64_t step = kEp ? (uint64_t)nz.ep_t[b0 + s / K] : nz.n;
+        world_actuate(nz, prm.dt, prm.rtype[n], n, (int)(n / K), (int)(n % K), step, a0, a1);
+        world_integrate(ty->kinematics, ty->L, prm.dt, a0, a1, x, y, th, vx, vy);
+      } else {
+        nz.cmd[2 * n] = 0.0; nz.cmd[2 * n + 1] = 0.0;
+      }
+    } else if (prm.collided[n] == 0) {
+      world_integrate(ty->kinematics, ty->L, prm.dt, (double)action[2 * q], (double)action[2 * q + 1], x, y, th, vx, vy);
+    }
     prm.states[3 * n] = x; prm.states[3 * n + 1] = y; prm.states[3 * n + 2] = th;
     const double* g = prm.fgoal + 3 * n;
     const double gx = dsub(x, g[0]), gy = dsub(y, g[1]);
@@ -878,6 +990,15 @@ __global__ void __maxnreg__(128) world_step_block_kernel(const WorldParams prm, 
                                                                                  const float* __restrict__ action, int32_t* __restrict__ out_collided,
                                                                                  int32_t* __restrict__ out_arrived, float* __restrict__ clearance) {
   world_step_body<true, kEp, true>(prm, mp, bp, action, out_collided, out_arrived, clearance);
+}
+
+// Actuation limits and noise (nb_world_set_actuation): the step of any of the kernels above (kMap, kEp, kBlock; kMove false after
+// world_contact_kernel) with the actuation stage.  __maxnreg__(128) as in world_step_ep_kernel.
+template <bool kMap, bool kEp, bool kBlock, bool kMove>
+__global__ void __maxnreg__(128) world_step_act_kernel(const WorldParams prm, const WorldMapParams mp, const WorldBlockParams bp, const WorldNoiseParams nz,
+                                                       const float* __restrict__ action, int32_t* __restrict__ out_collided,
+                                                       int32_t* __restrict__ out_arrived, float* __restrict__ clearance) {
+  world_step_body<kMap, kEp, kBlock, kMove, true>(prm, mp, bp, action, out_collided, out_arrived, clearance, nz);
 }
 
 }  // namespace nb

@@ -45,7 +45,6 @@ constexpr int kWorldBehCols = 13;  // kind, vxmax, vymax, acce, factor, speed, w
 constexpr int kWorldRvoWarps = 8;
 constexpr int kWorldRvoMaxAxis = 64;  // candidates per axis
 constexpr int kWorldRvoMaxDraws = 16;  // wander goal draws per obstacle and step in an environment whose map blocks obstacles
-constexpr uint64_t kSplitMixGamma = 0x9E3779B97F4A7C15ull;
 
 struct WorldRvoParams {
   const double* beh;     // (O, kWorldBehCols)
@@ -57,20 +56,7 @@ struct WorldRvoParams {
   int cap;               // shared rows per environment: the largest obstacle count + K (the robots)
 };
 
-// SplitMix64 (Steele, Lea and Flood 2014): output n of the generator seeded with s is mix(s + (n + 1) gamma), so any draw is
-// computed directly from its counter.
-__host__ __device__ __forceinline__ uint64_t splitmix64_mix(uint64_t z) {
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-__host__ __device__ __forceinline__ uint64_t splitmix64_at(uint64_t s, uint64_t n) { return splitmix64_mix(s + (n + 1) * kSplitMixGamma); }
-// the stream of obstacle i (index within its environment) of environment b
-__host__ __device__ __forceinline__ uint64_t world_rvo_key(uint64_t seed, int b, int i) {
-  return splitmix64_mix(splitmix64_mix(seed + kSplitMixGamma) ^ (((uint64_t)(uint32_t)b << 32) | (uint64_t)(uint32_t)i));
-}
-// (x >> 11) 2^-53: uniform in [0, 1), exact
-__host__ __device__ __forceinline__ double world_u01(uint64_t x) { return (double)(x >> 11) * 0x1.0p-53; }
+// The goal draws use the counter-based SplitMix64 streams of world_kernel.cuh (world_rvo_key, splitmix64_at, world_u01).
 
 __device__ __forceinline__ int world_rvo_count(double lo, double hi, double grid) {
   if (!(hi > lo)) return 0;

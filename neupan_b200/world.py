@@ -84,6 +84,25 @@ exhausted a slot goes idle and its scene is frozen.  Each scene runs once in its
 its scene truncated at its end.  The per-scene results are read with ``episodes()``.  Limits: one ``max_steps`` per world, no
 differentiable mode, a single GPU, the bank within ``num_envs`` and device memory, a fixed type per robot index.
 
+Actuation limits and noise (``WorldBatch.set_actuation``, ``set_lidar_noise``; nb_world_set_actuation, nb_world_set_lidar_noise):
+both off by default, and a world without them runs the kernels it ran before.  This is this project's reading of IR-SIM's
+``vel_min`` / ``vel_max`` / ``acce`` and of the ``noise`` switches of its motion model and ``lidar2d``, not a claim of parity.
+``set_actuation`` takes one dict per robot type with the keys ``vel_min``, ``vel_max`` (2 values each, default -inf / +inf),
+``acce`` (2, default +inf) and ``alpha`` (4, default 0), in the action's own convention: diff (v, omega), acker (v, steering), omni
+(vx, vy).  Each robot carries cmd_prev, its last limited command (``commands()``; 0 after set_scenes / set_episodes and when a slot
+takes a new scene).  In a step, per component, lo = max(vel_min, cmd_prev - acce dt), hi = min(vel_max, cmd_prev + acce dt),
+c = min(max(a, lo), hi) and cmd_prev = c; then s0 = sqrt(alpha0 c0^2 + alpha1 c1^2), s1 = sqrt(alpha2 c0^2 + alpha3 c1^2) and the
+robot integrates u = c + (s0 z0, s1 z1) with its type's motion model; the velocity the lidar reports for it is that of u.  Noise comes
+after the limits and is not clipped again (IR-SIM's order).  A collided robot stays frozen and its cmd_prev becomes 0.  Reactive
+obstacles still see the action as given.  ``set_lidar_noise(range_std, range_min)``: a beam that hits something reports
+clamp(t + range_std z, range_min, range_max), computed in FP64 and rounded to float; a miss still reports range_max, and the hit
+index and velocity do not change.  z are standard normal draws (Box-Muller from SplitMix64 counter streams, one domain tag for motion
+and one for the lidar, apart from the goal draws) keyed by (seed, environment -- the scene in episode mode --, robot within it, the
+steps that scene has taken, component or beam), so a run is reproducible from its seeds, environment b's noise does not depend on B,
+a scan repeated without a step is the same scan, and an episode stays bitwise the plain run of its scene.  The settings survive
+set_scenes and set_episodes.  Refused (ValueError): NaN, vel_min > vel_max, acce <= 0, negative or non-finite alpha, and an acker
+type's finite steering limits outside (-pi/2, pi/2).
+
 There is no CPU implementation here: the CUDA library is the product (oracle/world.py restates it for the tests).
 """
 from __future__ import annotations
@@ -104,6 +123,8 @@ BEH_COLS = 13  # kind, vxmax, vymax, acce, factor, speed, wander, goal x, y, goa
 # the keys of an "rvo" behaviour besides vxmax and vymax (required); speed None: min(vxmax, vymax); goal None: drawn
 RVO_DEFAULTS = dict(acce=1.0, factor=1.0, speed=None, wander=False, goal=None, goal_threshold=0.3, neighbor_range=10.0, grid=0.05,
                     min_speed=0.3)
+# the keys of a robot type's actuation (WorldBatch.set_actuation) and their defaults: no bound, no rate limit, no motion noise
+ACTUATION_DEFAULTS = dict(vel_min=(-math.inf, -math.inf), vel_max=(math.inf, math.inf), acce=(math.inf, math.inf), alpha=(0.0, 0.0, 0.0, 0.0))
 
 
 def _robot_vertices(robot):
@@ -269,6 +290,47 @@ def pack_obstacle_contact(scenes) -> np.ndarray:
     return np.ascontiguousarray([1 if sc.get("obstacle_contact", False) else 0 for sc in scenes], np.int32)
 
 
+def pack_actuation(limits, robots) -> np.ndarray:
+    """(T, 10) float64 rows [vel_min (2), vel_max (2), acce (2), alpha (4)] from one dict per robot type (``robots``: the world's
+    robot types, whose kinematics decide the acker check), with the refusals of nb_world_set_actuation as ValueError naming the type."""
+    if len(limits) != len(robots):
+        raise ValueError(f"{len(limits)} actuation dicts for {len(robots)} robot types")
+    rows = []
+    for t, (lim, robot) in enumerate(zip(limits, robots)):
+        unknown = set(lim) - set(ACTUATION_DEFAULTS)
+        if unknown:
+            raise ValueError(f"robot type {t}: unknown actuation keys {sorted(unknown)}")
+        v = {k: np.asarray(lim.get(k, d), np.float64).reshape(-1) for k, d in ACTUATION_DEFAULTS.items()}
+        for k, d in ACTUATION_DEFAULTS.items():
+            if v[k].shape != (len(d),):
+                raise ValueError(f"robot type {t}: {k} needs {len(d)} values, got {v[k].size}")
+            if np.isnan(v[k]).any():
+                raise ValueError(f"robot type {t}: {k} = {v[k].tolist()} has a NaN")
+        lo, hi = v["vel_min"], v["vel_max"]
+        if (lo > hi).any() or (lo == math.inf).any() or (hi == -math.inf).any():
+            raise ValueError(f"robot type {t}: vel_min = {lo.tolist()} and vel_max = {hi.tolist()} need vel_min <= vel_max (vel_min < inf, "
+                             "vel_max > -inf)")
+        if (v["acce"] <= 0.0).any():
+            raise ValueError(f"robot type {t}: acce = {v['acce'].tolist()} must be > 0 (inf: no rate limit)")
+        if not np.isfinite(v["alpha"]).all() or (v["alpha"] < 0.0).any():
+            raise ValueError(f"robot type {t}: alpha = {v['alpha'].tolist()} must be finite and >= 0")
+        if robot.kinematics == "acker":
+            steer = np.array([lo[1], hi[1]])
+            fin = steer[np.isfinite(steer)]
+            if (np.abs(fin) >= math.pi / 2).any():
+                raise ValueError(f"robot type {t} (acker): steering limits {steer.tolist()} outside (-pi/2, pi/2)")
+        rows.append(np.concatenate([lo, hi, v["acce"], v["alpha"]]))
+    return np.asarray(rows, np.float64).reshape(len(robots), 10)
+
+
+def check_lidar_noise(range_std: float, range_min: float, range_max: float):
+    """The refusals of nb_world_set_lidar_noise as ValueError: range_std finite and >= 0, range_min in [0, range_max)."""
+    if not (math.isfinite(range_std) and range_std >= 0.0):
+        raise ValueError(f"range_std = {range_std} must be finite and >= 0")
+    if not 0.0 <= range_min < range_max:
+        raise ValueError(f"range_min = {range_min} outside [0, range_max = {range_max})")
+
+
 def _host_ptrs(packed):
     return [C.c_void_p(a.ctypes.data) for a in packed]
 
@@ -421,6 +483,41 @@ class WorldBatch:
         out = torch.empty(self.O, dtype=torch.int32, device=self.device)
         with torch.cuda.device(self.device):
             _lib.check(_lib.load().nb_world_read_obstacle_contact(self._handle, self.O, C.c_void_p(out.data_ptr()), self._stream()))
+        return out
+
+    # ---- actuation limits and noise -----------------------------------------------------------------------------------------
+    def set_actuation(self, limits, seed: int = 0):
+        """Actuation limits and motion noise per robot type (module docstring): ``limits`` one dict per robot type with the keys
+        vel_min, vel_max, acce, alpha (defaults ACTUATION_DEFAULTS), ``seed`` the motion noise's.  Needs scenes; kept by
+        set_scenes and set_episodes, which zero every robot's cmd_prev."""
+        rows = pack_actuation(limits, self.robots)
+        if self._rows is None:
+            raise ValueError("set_actuation needs scenes (set_scenes or set_episodes first)")
+        per_type = (_lib.WorldActuation * len(rows))()
+        for t, r in enumerate(rows):
+            per_type[t].vel_min[:] = r[0:2].tolist(); per_type[t].vel_max[:] = r[2:4].tolist()
+            per_type[t].acce[:] = r[4:6].tolist(); per_type[t].alpha[:] = r[6:10].tolist()
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nb_world_set_actuation(self._handle, len(rows), per_type, C.c_uint64(int(seed))))
+        self.actuation = rows
+
+    def set_lidar_noise(self, range_std: float, range_min: float = None, seed: int = 0):
+        """Lidar range noise (module docstring): a hit reports clamp(t + range_std z, range_min, range_max); ``range_min`` defaults
+        to the lidar's.  range_std 0 turns it off.  Kept by set_scenes and set_episodes."""
+        range_min = self.scan_dict["range_min"] if range_min is None else float(range_min)
+        check_lidar_noise(float(range_std), range_min, self.scan_dict["range_max"])
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nb_world_set_lidar_noise(self._handle, C.c_double(range_min), C.c_double(float(range_std)),
+                                                            C.c_uint64(int(seed))))
+
+    def commands(self) -> torch.Tensor:
+        """(rows, 2) float64 on the device: every robot's cmd_prev, the last command after the actuation limits (zeros without
+        set_actuation).  Rows are the environments' robots (N), in episode mode the scenes' own rows (S K).  A copy enqueued on the
+        current stream."""
+        rows = self.N if self.S is None else self.S * self.K
+        out = torch.empty((rows, 2), dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nb_world_read_commands(self._handle, rows, C.c_void_p(out.data_ptr()), self._stream()))
         return out
 
     def _read(self, states=None, obstacles=None, collided=None, arrived=None, rows=None):
